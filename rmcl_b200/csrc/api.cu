@@ -389,6 +389,7 @@ struct b2_rcc {
     bool pdl_next = false, pdl_armed = false;   // the next find is followed by k_icp_loop launched with programmatic stream serialization / the find let it start early
     DevBuf<uint32_t> d_tile_cost; DevBuf<uint16_t> d_tile_perm; uint32_t perm_tiles = 0, cost_tiles = 0;    // tile schedule of k_rcc_find: warp durations of the last launch (cost_tiles of them if it recorded any), order for the next (always a permutation of perm_tiles tiles)
     unsigned long long n_reruns = 0;                            // calls that were run again through the cooperative launch (exchange abort: co-residency or range)
+    uint32_t loop_geom[2 + 4 * B2_MAX_SENSORS] = {};            // last fused call: sensors, grid, per sensor {n, blk0, nblk, smem_u} (b2_rcc_debug_loop_geometry)
     DevBuf<unsigned int> d_bar; unsigned int zc_seq = 0;        // [0] = "scan copy complete" flag (value: zc_seq of the call), [1] = abort word of the ICP loop
     DevBuf<unsigned long long> d_slots; unsigned int tag_base = 0; // exchange buffers of the ICP loop (icp_loop.cuh: accumulators, base, FP64 slots); round number of the next launch
     unsigned int seq = 0;               // sequence number of the last k_icp_loop launch (carried by every result chunk)
@@ -536,6 +537,16 @@ extern "C" __attribute__((visibility("default"))) int b2_rcc_debug_reruns(b2_rcc
 {
     NOTNULL(h); NOTNULL(out);
     *out = h->n_reruns;
+    return B2_OK;
+}
+// test aid (not part of the public header): the launch shape of k_icp_loop, so that tests can place pair counts on its tier boundaries.
+// out[0] = blocks of a full grid, out[1] = pairs per thread shared memory can hold, out[2] = sensors of this handle's last fused call (0: none yet),
+// out[3] = its grid, out[4 + 4k ..] = sensor k's {pairs, first block, blocks, pairs per thread in shared memory}; 4 + 4 * B2_MAX_SENSORS words
+extern "C" __attribute__((visibility("default"))) int b2_rcc_debug_loop_geometry(b2_rcc* h, uint32_t* out)
+{
+    NOTNULL(h); NOTNULL(out);
+    out[0] = (uint32_t)h->fused_grid; out[1] = (uint32_t)h->smem_u_cap;
+    memcpy(out + 2, h->loop_geom, sizeof(h->loop_geom));
     return B2_OK;
 }
 // test aid (not part of the public header): the tile order the next find of this handle will use (host copy; *n_tiles = 0 when the schedule is off)
@@ -817,7 +828,6 @@ extern "C" int b2_rcc_cross_statistics(b2_rcc* h, const b2_transform* T, double 
     NOTNULL(h); NOTNULL(T); NOTNULL(out);
     CU(cudaSetDevice(h->map->device));
     if (!h->found) return fail(B2_ERR_INVALID, "computeCrossStatistics before find");
-    if (h->n_dataset == 0) return fail(B2_ERR_INVALID, "computeCrossStatistics without a dataset");
     RES(launch_reduce(h, T, adaptive_max_dist(h, cp), nullptr, h->d_stats.p));
     CU(cudaMemcpyAsync(&h->pin->S[0], h->d_stats.p, sizeof(b2_cross_stats), cudaMemcpyDeviceToHost, h->stream));
     CU(cudaStreamSynchronize(h->stream));
@@ -1012,12 +1022,22 @@ static int micp_enqueue(SensorCall* sc, uint32_t ns, const b2_transform* Tom, ui
     IcpLaunch& L = pc.launch;
     memset(&L, 0, sizeof(L));
     L.Tom = *Tom; L.n_sensors = ns; L.iterations = iterations;
-    int grid = std::min<int>(H->fused_grid, (int)std::max<uint64_t>((total + B2_ICP_BLOCK - 1) / B2_ICP_BLOCK, ns));
-    // blocks per sensor in proportion to the pairs, at least one each
+    uint32_t ns_busy = 0;
+    for (uint32_t k = 0; k < ns; k++) if (sc[k].h->work_n() > 0) ns_busy++;
+    int grid = std::min<int>(H->fused_grid, (int)std::max<uint64_t>((total + B2_ICP_BLOCK - 1) / B2_ICP_BLOCK, ns_busy));
+    // blocks per sensor in proportion to the pairs, at least one for each sensor with pairs.  A sensor without pairs gets none, so the
+    // other sensors' pairs are summed by exactly the blocks a call without it would use: its presence cannot change a bit of the result.
     uint32_t nblk[B2_MAX_SENSORS]; int assigned = 0;
-    for (uint32_t k = 0; k < ns; k++) { nblk[k] = std::max<uint32_t>(1u, (uint32_t)((uint64_t)grid * sc[k].h->work_n() / total)); assigned += (int)nblk[k]; }
+    for (uint32_t k = 0; k < ns; k++) {
+        const uint32_t nw = sc[k].h->work_n();
+        nblk[k] = nw ? std::max<uint32_t>(1u, (uint32_t)((uint64_t)grid * nw / total)) : 0u; assigned += (int)nblk[k];
+    }
     while (assigned > grid) { uint32_t big = 0; for (uint32_t k = 1; k < ns; k++) if (nblk[k] > nblk[big]) big = k; nblk[big]--; assigned--; }
-    while (assigned < grid) { uint32_t best = 0; double load = -1.0; for (uint32_t k = 0; k < ns; k++) { const double l = (double)sc[k].h->work_n() / nblk[k]; if (l > load) { load = l; best = k; } } nblk[best]++; assigned++; }
+    while (assigned < grid) {
+        uint32_t best = 0; double load = -1.0;
+        for (uint32_t k = 0; k < ns; k++) { if (!nblk[k]) continue; const double l = (double)sc[k].h->work_n() / nblk[k]; if (l > load) { load = l; best = k; } }
+        nblk[best]++; assigned++;
+    }
     bool aux_any = false;
     uint32_t blk0 = 0, smem_u_max = 0, sort_tiles_max = 0;
     if (H->timing) CU(cudaEventRecord(H->ev[0], H->stream));
@@ -1027,7 +1047,7 @@ static int micp_enqueue(SensorCall* sc, uint32_t ns, const b2_transform* Tom, ui
         const uint32_t nw = h->work_n();
         S.n = nw; S.blk0 = blk0; S.nblk = nblk[k]; blk0 += nblk[k];
         const uint32_t stride = S.nblk * B2_ICP_BLOCK;
-        const uint32_t per_thread = (nw + stride - 1) / stride;
+        const uint32_t per_thread = stride ? (nw + stride - 1) / stride : 0u;
         S.smem_u = per_thread > B2_ICP_REG_PAIRS ? std::min<uint32_t>(per_thread - B2_ICP_REG_PAIRS, (uint32_t)H->smem_u_cap) : 0u;
         smem_u_max = std::max(smem_u_max, S.smem_u);
         S.max_dist = (float)(h->max_dist * (1.0 - cp) + h->adaptive_max_dist_min * cp);       // CorrespondencesCPU.cpp:21-23
@@ -1108,6 +1128,11 @@ static int micp_enqueue(SensorCall* sc, uint32_t ns, const b2_transform* Tom, ui
     sc[ns - 1].h->pdl_armed = false;
     pc.slot = (int)(H->slot_counter++ % B2_RING);
     RES(launch_icp_loop(H, L, grid, smem, mode, pdl, pc.slot));
+    H->loop_geom[0] = ns; H->loop_geom[1] = (uint32_t)grid;
+    for (uint32_t k = 0; k < B2_MAX_SENSORS; k++) {
+        uint32_t* g = H->loop_geom + 2 + 4 * k;
+        if (k < ns) { g[0] = L.s[k].n; g[1] = L.s[k].blk0; g[2] = L.s[k].nblk; g[3] = L.s[k].smem_u; } else g[0] = g[1] = g[2] = g[3] = 0u;
+    }
     if (H->timing) { CU(cudaEventRecord(H->ev[2], H->stream)); H->timing_valid = true; }
     for (uint32_t k = 1; k < ns; k++) {        // later work on the other sensors' own streams sees the model buffers this call wrote
         CU(cudaEventRecord(sc[k].h->ev_join, H->stream));

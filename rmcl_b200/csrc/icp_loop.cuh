@@ -455,6 +455,7 @@ __global__ void __launch_bounds__(B2_ICP_BLOCK) k_icp_loop(const __grid_constant
     }
     if (!COOP) asm volatile("griddepcontrol.wait;" ::: "memory");
     // ---- load this thread's pairs once: validity is folded into the dataset point (NaN fails the P2L gate like a masked pair) ----
+    // Slots beyond the sensor's pairs read pair 0 (and are then masked): every sensor that is given blocks has at least one pair (micp_enqueue).
     for (uint32_t u = 0; u < n_cached; u++) {
         const uint32_t i = lid + u * stride;
         const bool in = i < n;
