@@ -1469,6 +1469,7 @@ struct b2_pf {
     // was faster when last timed -- both are timed on the first updates and the loser again every 64 updates (particle sets converge and spread out)
     int map_mode = 3, map_cur = 0, map_best = 0; unsigned int map_updates = 0; float map_ms[2] = {0.f, 0.f}; bool map_timed = false;
     cudaEvent_t ev_m0 = nullptr, ev_m1 = nullptr;
+    uint32_t launch_geom[12] = {};      // launch shape of the last sensor update that launched (b2_pf_debug_launch_geometry)
     DevBuf<uint32_t> d_keys, d_keys2, d_idx, d_idx2; DevBuf<unsigned char> d_sort_tmp;
     // sharded resampling over NVLink peer memory (b2_pf_p2p_*): own exchange buffers (cudaMalloc: exportable through CUDA IPC) + the peers' mappings
     b2_transform* x_poses = nullptr; b2_particle_attr* x_attrs = nullptr; uint32_t x_cap = 0;
@@ -1576,6 +1577,13 @@ static int pf_prepare_beams(b2_pf* h, const b2_range_meas* beams, uint32_t n_bea
     *ppb_out = std::min(ppb, (uint32_t)B2_PF_BLOCK);
     return B2_OK;
 }
+// host-side record of an update's launch shape (b2_pf_debug_launch_geometry); pf_launch fills in the kernel's mapping, ppb, blocks and shared memory
+static void pf_geom_begin(b2_pf* h, uint32_t n, uint32_t n_beams, int map, uint32_t n_chunks, uint32_t per)
+{
+    uint32_t* g = h->launch_geom;
+    memset(g, 0, sizeof(h->launch_geom));
+    g[0] = (uint32_t)h->smem_optin; g[1] = (uint32_t)h->map_mode; g[2] = (uint32_t)map; g[8] = n_chunks; g[9] = per; g[10] = n; g[11] = n_beams;
+}
 static int pf_launch(b2_pf* h, const b2_transform* poses_dev, b2_particle_attr* attrs_dev, uint32_t n, const b2_transform* Tsb, uint32_t n_beams, const b2_pf_params* prm,
                      uint32_t ppb, cudaStream_t stream, int map = 0, const uint32_t* order = nullptr)
 {
@@ -1584,6 +1592,8 @@ static int pf_launch(b2_pf* h, const b2_transform* poses_dev, b2_particle_attr* 
     const uint32_t grid = (n + ppb - 1) / ppb;
     const size_t smem = bytes_per_particle * ppb;
     const bool cp = prm->correspondence_type == 1;
+    uint32_t* g = h->launch_geom;
+    g[3] = (uint32_t)map; g[4] = order != nullptr; g[5] = ppb; g[6] += grid; g[7] = (uint32_t)smem;
     if (map) {
         if (cp) k_pf_update<1, 1><<<grid, B2_PF_BLOCK, smem, stream>>>(h->map->view(), poses_dev, attrs_dev, n, *Tsb, h->d_beams.p, n_beams, *prm, ppb, order);
         else    k_pf_update<0, 1><<<grid, B2_PF_BLOCK, smem, stream>>>(h->map->view(), poses_dev, attrs_dev, n, *Tsb, h->d_beams.p, n_beams, *prm, ppb, order);
@@ -1633,6 +1643,7 @@ static int pf_update_impl(b2_pf* h, const b2_transform* poses_dev, b2_particle_a
         h->map_cur = map;
         CU(cudaEventRecord(h->ev_m0, h->stream));
     }
+    pf_geom_begin(h, n, n_beams, map, 0, 0);
     const uint32_t* order = nullptr;
     if (map == 2) { RES(pf_sort_particles(h, poses_dev, n, h->stream)); order = h->d_idx2.p; }
     RES(pf_launch(h, poses_dev, attrs_dev, n, Tsb, n_beams, prm, ppb, h->stream, map != 0, order));
@@ -1652,6 +1663,19 @@ extern "C" int b2_pf_get_mapping(b2_pf* h, int* mode, int* current)
     NOTNULL(h);
     if (mode) *mode = h->map_mode;
     if (current) *current = h->map_mode == 3 ? h->map_cur : h->map_mode;
+    return B2_OK;
+}
+// test aid (not part of the public header): the launch shape of the handle's last sensor update that launched k_pf_update, so that tests can
+// place beam and particle counts on its regime boundaries.  out[0] = dynamic shared memory a block may use (opt-in limit less the 1 KiB
+// reserve), out[1] = requested mapping (b2_pf_set_mapping), out[2] = mapping chosen for the update (0 / 1 / 2; the host path always 0),
+// out[3] = mapping of the kernel launched (0 lanes = beams, 1 lanes = particles; 0 where MAP 1 does not fit in shared memory),
+// out[4] = 1 if the particles ran in sorted order, out[5] = particles per block, out[6] = blocks launched (all chunks), out[7] = dynamic
+// shared memory per block in bytes, out[8] = chunks of the host path (0: device-resident call), out[9] = particles per chunk,
+// out[10] = particles, out[11] = beams; 12 words
+extern "C" __attribute__((visibility("default"))) int b2_pf_debug_launch_geometry(b2_pf* h, uint32_t* out)
+{
+    NOTNULL(h); NOTNULL(out);
+    memcpy(out, h->launch_geom, sizeof(h->launch_geom));
     return B2_OK;
 }
 
@@ -1682,6 +1706,7 @@ extern "C" int b2_pf_sensor_update_host(b2_pf* h, const b2_transform* poses, b2_
     // plus one chunk's transfers instead of kernel + all transfers.
     const uint32_t n_chunks = n >= 32768u ? 8u : 1u;
     const uint32_t per = ((n + n_chunks - 1) / n_chunks + ppb - 1) / ppb * ppb;          // whole blocks per chunk
+    pf_geom_begin(h, n, n_beams, 0, n_chunks, per);
     if (n_chunks > 1) {
         if (!h->side) { CU(cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking)); CU(cudaEventCreateWithFlags(&h->ev_beams, cudaEventDisableTiming)); CU(cudaEventCreateWithFlags(&h->ev_side, cudaEventDisableTiming)); }
         CU(cudaEventRecord(h->ev_beams, h->stream));                  // beam table (and whatever the caller had queued on the stream before)
