@@ -202,6 +202,24 @@ B2_API int b2_rcc_correct_once_wait(b2_rcc* h, b2_transform* Tom_new, b2_transfo
 B2_API int b2_micp_correct_once(b2_rcc* const* sensors, const b2_transform* Tbo, const double* merge_weights, const float* const* ranges_host, uint32_t n_sensors,
                                 const b2_transform* Tom, uint32_t iterations, double convergence_progress,
                                 b2_transform* Tom_new, b2_transform* T_onew_oold, b2_cross_stats* Cmerged_o);
+/* What one correctOnce of a chain leaves behind: what MICPSensorStats needs per correction (micp_localization.cpp:1009-1015). */
+typedef struct {
+    b2_transform   Tom_new, T_onew_oold;     /* as b2_micp_correct_once */
+    b2_cross_stats Cmerged_o;
+    double         convergence_progress;     /* after this step (:988-1007) */
+    uint32_t       valid_measurements;       /* mask ones of all sensors' datasets (MICPSensor.hpp:110, counted as unpackMessage counts them) */
+    uint32_t       total_measurements;       /* sum of the dataset sizes (MICPSensor.hpp:109) */
+} b2_micp_step;                              /* 144 B */
+/* n_corrections x MICPLocalizationNode::correctOnce (micp_localization.cpp:856-1007) back to back on the RESIDENT datasets of 1..4 sensors
+ * (upload the scans first: b2_rcc_set_ranges / set_dataset / bind_dataset); n_corrections = 3 is correct() (:847-854), and the body of
+ * correctionLoop (:1086-1171) is one call per scan.  Every step traces at the Tom the previous one left in device memory and gates with the
+ * max_dist its convergence progress gives (CorrespondencesCPU.cpp:21-23); the host is not involved between the steps.  At the end, one copy to
+ * the host: *Tom_inout and *convergence_progress_inout are updated (Tom only when a step had n_meas > 0, :974-984) and steps_out (NULL or
+ * n_corrections records) receives each step's outcome.  adaptive_max_dist == 0: the progress stays 0 (:988-990).  Arguments are checked as in
+ * b2_micp_correct_once; refused while calls are in flight on the lead handle; handles in exec mode 0 run the chain through mode 1. */
+B2_API int b2_micp_correct(b2_rcc* const* sensors, const b2_transform* Tbo, const double* merge_weights, uint32_t n_sensors,
+                           b2_transform* Tom_inout, double* convergence_progress_inout, int adaptive_max_dist,
+                           uint32_t n_corrections, uint32_t iterations, b2_micp_step* steps_out);
 /* How b2_rcc_correct_once* runs the inner iterations: 2 (default) one kernel for all of them, launched programmatically behind find; the block
  * sums cross the grid as 64-bit fixed-point atomics (every block must be co-resident: one block per SM).  1 the same kernel through a cooperative
  * launch, the sums as FP64 slots behind a grid sync.  0 one reduction launch per inner iteration in the reference's own frame-algebra order

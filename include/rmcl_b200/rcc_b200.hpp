@@ -168,6 +168,9 @@ public:
     }
     void setStream(void* cuda_stream) { b2_check(b2_rcc_set_stream(h_, cuda_stream), "setStream"); }
     b2_rcc* handle() const { return h_; }
+    friend void micp_correct(const std::vector<CorrespondencesB200*>& sensors, const std::vector<rm::Transform>& Tbo, const std::vector<double>& merge_weights,
+                             rm::Transform& Tom, double& convergence_progress, bool adaptive_max_dist, unsigned n_corrections, unsigned iterations,
+                             std::vector<b2_micp_step>* steps);
     void noteModelSize(uint32_t width, uint32_t height) { note_model(width, height); }      // for model tables set through the C ABI directly (rmcl_msgs_adapters.hpp)
 
 protected:
@@ -291,6 +294,23 @@ inline rm::Transform umeyama_transform(const rm::CrossStatistics& s, int device 
     rm::Transform T;
     b2_check(b2_umeyama_batch(reinterpret_cast<const b2_cross_stats*>(&s), 1, reinterpret_cast<b2_transform*>(&T), 0, device, nullptr), "umeyama_transform");
     return T;
+}
+
+// MICPLocalizationNode::correct() (micp_localization.cpp:847-854) / the body of correctionLoop (:1086-1171): n_corrections x correctOnce on the
+// device for all sensors of the node, Tom_ and convergence_progress_ (:988-1007) carried between the steps on the device and updated here at the
+// end.  merge_weights empty = all 1.0; steps (may be null) receives one record per correction (the fields of MICPSensorStats, :1009-1015).
+inline void micp_correct(const std::vector<CorrespondencesB200*>& sensors, const std::vector<rm::Transform>& Tbo, const std::vector<double>& merge_weights,
+                         rm::Transform& Tom, double& convergence_progress, bool adaptive_max_dist = true, unsigned n_corrections = 3, unsigned iterations = 5,
+                         std::vector<b2_micp_step>* steps = nullptr)
+{
+    if (sensors.size() != Tbo.size() || (!merge_weights.empty() && merge_weights.size() != sensors.size())) throw std::invalid_argument("micp_correct: one Tbo / weight per sensor");
+    std::vector<b2_rcc*> h;
+    for (CorrespondencesB200* s : sensors) { s->sync_params(); s->bind_members(); h.push_back(s->h_); }
+    if (steps) steps->resize(n_corrections);
+    b2_check(b2_micp_correct(h.data(), reinterpret_cast<const b2_transform*>(Tbo.data()), merge_weights.empty() ? nullptr : merge_weights.data(), (uint32_t)h.size(),
+                             reinterpret_cast<b2_transform*>(&Tom), &convergence_progress, adaptive_max_dist ? 1 : 0, n_corrections, iterations,
+                             steps ? steps->data() : nullptr), "micp_correct");
+    for (CorrespondencesB200* s : sensors) s->outdated = false;
 }
 
 // --- particle filter sensor update ------------------------------------------------------------------------------------------------

@@ -75,6 +75,7 @@ EXPORTS = [
     "b2_pf_set_stream", "b2_pf_sensor_update", "b2_pf_sensor_update_host", "b2_kernel_launch_count", "b2_rcc_enable_timing", "b2_rcc_last_timing", "b2_pf_motion_update", "b2_pf_likelihood_stats",
     "b2_rcc_set_correspondence_type", "b2_pf_resample_gladiator", "b2_pf_gladiator_randoms", "b2_rcc_segment", "b2_mesh_create_from_file", "b2_mesh_file_load", "b2_mesh_file_free", "b2_peek_cuda_error", "b2_mesh_blob_size", "b2_mesh_export_blob", "b2_mesh_create_from_blob", "b2_mesh_refit",
     "b2_rcc_correct_once_async", "b2_rcc_correct_once_wait", "b2_micp_correct_once", "b2_rcc_set_exec_mode", "b2_debug_read_bandwidth", "b2_rcc_set_sim_options", "b2_rcc_bind_dataset", "b2_rcc_bind_model_buffers", "b2_rcc_benchmark_batch", "b2_pf_p2p_init", "b2_pf_p2p_connect", "b2_pf_p2p_publish", "b2_pf_resample_gladiator_p2p", "b2_pf_p2p_connect_local", "b2_rcc_set_cpc_options", "b2_pf_set_mapping", "b2_pf_get_mapping",
+    "b2_micp_correct",
 ]
 
 
@@ -532,6 +533,31 @@ def micp_correct_once(sensors, Tbo, Tom, iterations=5, convergence_progress=0.0,
     for s in sensors:
         s.outdated = False
     return Tn, Td, Cm
+
+
+# b2_micp_step (rmcl_b200.h): one correction of a chain, what MICPSensorStats needs (micp_localization.cpp:1009-1015)
+MICP_STEP_DTYPE = np.dtype([("Tom_new", TRANSFORM_DTYPE), ("T_onew_oold", TRANSFORM_DTYPE), ("Cmerged_o", CROSS_STATS_DTYPE),
+                            ("convergence_progress", np.float64), ("valid_measurements", np.uint32), ("total_measurements", np.uint32)])
+assert MICP_STEP_DTYPE.itemsize == 144
+
+
+def micp_correct(sensors, Tbo, Tom, n_corrections=3, iterations=5, convergence_progress=0.0, merge_weights=None, adaptive_max_dist=True):
+    """`n_corrections` x MICPLocalizationNode::correctOnce back to back on the device (micp_localization.cpp:856-1007; 3 is correct(), :847-854):
+    each step traces at the pose the previous one produced and gates with the max_dist its convergence progress gives, without the host in
+    between.  Runs on the sensors' resident datasets (setRanges / setDataset / bindDataset first).  -> (Tom, convergence_progress, steps) with
+    `steps` a MICP_STEP_DTYPE record array, one per correction."""
+    n = len(sensors)
+    hs = (C.c_void_p * n)(*[s._h for s in sensors])
+    Tb = np.ascontiguousarray(np.asarray(Tbo, TRANSFORM_DTYPE).reshape(n))
+    w = None if merge_weights is None else np.ascontiguousarray(merge_weights, np.float64).reshape(n)
+    T = np.array(_tf(Tom), copy=True)
+    cp = C.c_double(float(convergence_progress))
+    steps = np.zeros(int(n_corrections), MICP_STEP_DTYPE)
+    _chk(load_library().b2_micp_correct(hs, _p(Tb), _p(w), C.c_uint32(n), _p(T), C.byref(cp), C.c_int(int(bool(adaptive_max_dist))),
+                                        C.c_uint32(int(n_corrections)), C.c_uint32(int(iterations)), _p(steps) if len(steps) else None))
+    for s in sensors:
+        s.outdated = False
+    return T, cp.value, steps
 
 
 def umeyama_transform(stats, device=0):

@@ -395,6 +395,7 @@ struct b2_rcc {
     unsigned int seq = 0;               // sequence number of the last k_icp_loop launch (carried by every result chunk)
     std::deque<PendingCall> pending;    // enqueued, not yet collected (oldest first), at most B2_RING
     unsigned int slot_counter = 0;
+    DevBuf<unsigned char> d_chain;      // b2_micp_correct with this handle in the lead: IcpChainState, then one b2_micp_step per correction
     bool timing = false; cudaEvent_t ev[3] = {nullptr, nullptr, nullptr}; bool timing_valid = false;
     cudaStream_t aux = nullptr; cudaEvent_t ev_aux = nullptr;     // side stream: scan upload + unpack overlap the find kernel
     cudaEvent_t ev_join = nullptr;      // multi-sensor correctOnce: orders this handle's stream against the lead handle's
@@ -488,6 +489,7 @@ extern "C" int b2_rcc_destroy(b2_rcc* h)
     h->d_dirs.release(); h->d_origs.release(); h->d_dpts.release(); h->d_dmask.release(); h->d_ranges_in.release();
     h->d_mpts.release(); h->d_mnrm.release(); h->d_mranges.release(); h->d_mhits.release(); h->d_mfaces.release();
     h->d_partials.release(); h->d_ticket.release(); h->d_stats.release(); h->d_icp.release(); h->d_bar.release(); h->d_res.release(); h->d_dbg.release(); h->d_slots.release(); h->d_tile_cost.release(); h->d_tile_perm.release();
+    h->d_chain.release();
     { DeviceCtx& dc = g_dev[h->map->device & 63]; std::lock_guard<std::mutex> lk(dc.m); dc.n_handles--; if (dc.last == h) { dc.last = nullptr; dc.recorded = false; } }
     h->d_poses.release(); h->d_tdelta.release(); h->d_ncorr.release(); h->d_bstats.release();
     if (h->pin) cudaFreeHost(h->pin);
@@ -919,9 +921,10 @@ static void fill_sensor_frames(IcpSensor& S, const b2_transform& Tbo, const b2_t
     tf_store(&S.Tos, Tos); tf_store(&S.Tso, tf_inv(Tos)); quat_to_mat(Tos.R, S.Ros);
 }
 
+// slot < 0: no result chunks in mapped host memory (chain steps: their results stay on the device)
 static int launch_icp_loop(b2_rcc* H, const IcpLaunch& L, int grid, size_t smem, int mode, bool pdl, int slot)
 {
-    unsigned long long* parts = H->d_slots.p; IcpResult* res_dev = H->d_res.p; uint4* host_out = H->pin_chunks_dev + (size_t)slot * (B2_ICP_RESULT_CHUNKS + 1);
+    unsigned long long* parts = H->d_slots.p; IcpResult* res_dev = H->d_res.p; uint4* host_out = slot >= 0 ? H->pin_chunks_dev + (size_t)slot * (B2_ICP_RESULT_CHUNKS + 1) : nullptr;
     unsigned int tag_base = H->tag_base; unsigned int* bar_abort = H->d_bar.p + 1; unsigned long long* dbg = H->d_dbg.p;
     H->tag_base += L.iterations;                                  // tags tag_base + 1 .. tag_base + iterations belong to this launch
     if (H->tag_base > 0xfffffff0u - 64u) H->tag_base = 0;          // wrap far away from anything a live slot can still hold
@@ -956,13 +959,41 @@ static int launch_icp_loop(b2_rcc* H, const IcpLaunch& L, int grid, size_t smem,
     return B2_OK;
 }
 
+// k_icp_loop launched programmatically behind the last find (B2_PDL, default 1)
+static bool pdl_enabled()
+{
+    static const int use_pdl = [] { const char* e = getenv("B2_PDL"); return e ? atoi(e) : 1; }();
+    return use_pdl != 0;
+}
+
+// Grid of k_icp_loop and blocks per sensor: in proportion to the pairs, at least one for each sensor with pairs.  A sensor without pairs gets
+// none, so the other sensors' pairs are summed by exactly the blocks a call without it would use: its presence cannot change a bit of the result.
+static int loop_blocks(const b2_rcc* H, const SensorCall* sc, uint32_t ns, uint64_t total, uint32_t* nblk)
+{
+    uint32_t ns_busy = 0;
+    for (uint32_t k = 0; k < ns; k++) if (sc[k].h->work_n() > 0) ns_busy++;
+    const int grid = std::min<int>(H->fused_grid, (int)std::max<uint64_t>((total + B2_ICP_BLOCK - 1) / B2_ICP_BLOCK, ns_busy));
+    int assigned = 0;
+    for (uint32_t k = 0; k < ns; k++) {
+        const uint32_t nw = sc[k].h->work_n();
+        nblk[k] = nw ? std::max<uint32_t>(1u, (uint32_t)((uint64_t)grid * nw / total)) : 0u; assigned += (int)nblk[k];
+    }
+    while (assigned > grid) { uint32_t big = 0; for (uint32_t k = 1; k < ns; k++) if (nblk[k] > nblk[big]) big = k; nblk[big]--; assigned--; }
+    while (assigned < grid) {
+        uint32_t best = 0; double load = -1.0;
+        for (uint32_t k = 0; k < ns; k++) { if (!nblk[k]) continue; const double l = (double)sc[k].h->work_n() / nblk[k]; if (l > load) { load = l; best = k; } }
+        nblk[best]++; assigned++;
+    }
+    return grid;
+}
+
 static int micp_enqueue(SensorCall* sc, uint32_t ns, const b2_transform* Tom, uint32_t iterations, double cp)
 {
     b2_rcc* H = sc[0].h;
     if (H->pending.size() >= B2_RING) return fail(B2_ERR_INVALID, "correctOnce: %d asynchronous calls are in flight already, collect one first (b2_rcc_correct_once_wait)", B2_RING);
     static const int use_zc = [] { const char* e = getenv("B2_ZEROCOPY"); return e ? atoi(e) : 1; }();
     static const int use_spin = [] { const char* e = getenv("B2_SPIN"); return e ? atoi(e) : 1; }();
-    static const int use_pdl = [] { const char* e = getenv("B2_PDL"); return e ? atoi(e) : 1; }();
+    const bool use_pdl = pdl_enabled();
     int mode = H->exec_mode;
     if (H->fused_grid <= 0) mode = 0;
     if (ns > 1 && mode == 0) mode = H->fused_grid > 0 ? 1 : 0;
@@ -1022,22 +1053,8 @@ static int micp_enqueue(SensorCall* sc, uint32_t ns, const b2_transform* Tom, ui
     IcpLaunch& L = pc.launch;
     memset(&L, 0, sizeof(L));
     L.Tom = *Tom; L.n_sensors = ns; L.iterations = iterations;
-    uint32_t ns_busy = 0;
-    for (uint32_t k = 0; k < ns; k++) if (sc[k].h->work_n() > 0) ns_busy++;
-    int grid = std::min<int>(H->fused_grid, (int)std::max<uint64_t>((total + B2_ICP_BLOCK - 1) / B2_ICP_BLOCK, ns_busy));
-    // blocks per sensor in proportion to the pairs, at least one for each sensor with pairs.  A sensor without pairs gets none, so the
-    // other sensors' pairs are summed by exactly the blocks a call without it would use: its presence cannot change a bit of the result.
-    uint32_t nblk[B2_MAX_SENSORS]; int assigned = 0;
-    for (uint32_t k = 0; k < ns; k++) {
-        const uint32_t nw = sc[k].h->work_n();
-        nblk[k] = nw ? std::max<uint32_t>(1u, (uint32_t)((uint64_t)grid * nw / total)) : 0u; assigned += (int)nblk[k];
-    }
-    while (assigned > grid) { uint32_t big = 0; for (uint32_t k = 1; k < ns; k++) if (nblk[k] > nblk[big]) big = k; nblk[big]--; assigned--; }
-    while (assigned < grid) {
-        uint32_t best = 0; double load = -1.0;
-        for (uint32_t k = 0; k < ns; k++) { if (!nblk[k]) continue; const double l = (double)sc[k].h->work_n() / nblk[k]; if (l > load) { load = l; best = k; } }
-        nblk[best]++; assigned++;
-    }
+    uint32_t nblk[B2_MAX_SENSORS];
+    const int grid = loop_blocks(H, sc, ns, total, nblk);
     bool aux_any = false;
     uint32_t blk0 = 0, smem_u_max = 0, sort_tiles_max = 0;
     if (H->timing) CU(cudaEventRecord(H->ev[0], H->stream));
@@ -1298,6 +1315,165 @@ extern "C" int b2_micp_correct_once(b2_rcc* const* sensors, const b2_transform* 
     if (!sc[0].h->pending.empty()) return fail(B2_ERR_INVALID, "correctOnce: asynchronous calls are still in flight on the lead handle, collect them first");
     RES(micp_enqueue(sc, n_sensors, Tom, iterations, cp));
     return micp_collect(sc[0].h, Tom_new, T_onew_oold, Cmerged);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// b2_micp_correct: correctOnce after correctOnce (correct(), micp_localization.cpp:847-854) with the state between them -- Tom_, convergence_progress_
+// -- in device memory (IcpChainState, icp_loop.cuh).  Per step the finds read Tom * Tbo from the state through their device-pose argument, the
+// loop gates with the state's progress, and block 0 of the loop writes the next state and the step's record.  The lead handle's d_chain holds the
+// state followed by the records; the host reads both once, at the end.
+// ---------------------------------------------------------------------------------------------------------------------
+static IcpChainState* chain_state(const b2_rcc* H) { return reinterpret_cast<IcpChainState*>(H->d_chain.p); }
+static b2_micp_step* chain_records(const b2_rcc* H) { return reinterpret_cast<b2_micp_step*>(H->d_chain.p + sizeof(IcpChainState)); }
+
+// one step: every sensor's find (the last one arms the programmatic launch, as in micp_enqueue), then the loop writing record `step`
+static int chain_step(SensorCall* sc, uint32_t ns, IcpLaunch& L, int grid, int mode, uint32_t step)
+{
+    b2_rcc* H = sc[0].h;
+    uint32_t sort_tiles_max = 0;
+    for (uint32_t k = 0; k < ns; k++) {
+        b2_rcc* h = sc[k].h;
+        const cudaStream_t own = h->stream;
+        h->stream = H->stream;                                                        // all launches of the chain ride the lead stream
+        h->pdl_next = (k + 1 == ns) && mode == 2 && pdl_enabled() && h->corr_type == B2_CORR_RCC;
+        const int rc = launch_find(h, nullptr, &chain_state(H)->find[k]);
+        h->pdl_next = false; h->stream = own;
+        RES(rc);
+        IcpSensor& S = L.s[k];
+        S.mpts = h->mpts(); S.mnrm = h->mnrm(); S.mmask = h->mhits();                 // find may have grown the model buffers
+        S.tile_cost = nullptr; S.tile_perm = nullptr; S.n_tiles = 0;
+        if (h->corr_type == B2_CORR_RCC && h->cost_tiles && L.iterations >= 3u) {
+            S.tile_cost = h->d_tile_cost.p; S.tile_perm = h->d_tile_perm.p; S.n_tiles = h->cost_tiles;
+            sort_tiles_max = std::max(sort_tiles_max, h->cost_tiles);
+        }
+    }
+    size_t smem = (size_t)L.smem_u_max * 9 * B2_ICP_BLOCK * sizeof(float);
+    if (sort_tiles_max) {
+        const size_t want = smem + 2 * (size_t)sort_tiles_max;
+        if (want <= (size_t)H->smem_u_cap * 9 * B2_ICP_BLOCK * sizeof(float)) smem = want;
+        else for (uint32_t k = 0; k < ns; k++) { L.s[k].tile_cost = nullptr; L.s[k].tile_perm = nullptr; L.s[k].n_tiles = 0; }
+    }
+    const bool pdl = mode == 2 && sc[ns - 1].h->pdl_armed;
+    sc[ns - 1].h->pdl_armed = false;
+    unsigned int seq = ++H->seq; if (seq == 0) seq = ++H->seq;
+    L.seq = seq; L.step_out = chain_records(H) + step;
+    return launch_icp_loop(H, L, grid, smem, mode, pdl, -1);
+}
+
+extern "C" int b2_micp_correct(b2_rcc* const* sensors, const b2_transform* Tbo, const double* merge_weights, uint32_t n_sensors,
+                               b2_transform* Tom_inout, double* cp_inout, int adaptive_max_dist, uint32_t n_corrections, uint32_t iterations, b2_micp_step* steps_out)
+{
+    NOTNULL(sensors); NOTNULL(Tbo); NOTNULL(Tom_inout); NOTNULL(cp_inout);
+    if (n_sensors == 0 || n_sensors > B2_MAX_SENSORS) return fail(B2_ERR_INVALID, "correct: %u sensors (1..%d supported per call)", n_sensors, B2_MAX_SENSORS);
+    SensorCall sc[B2_MAX_SENSORS];
+    for (uint32_t k = 0; k < n_sensors; k++) {
+        NOTNULL(sensors[k]);
+        for (uint32_t j = 0; j < k; j++) if (sensors[j] == sensors[k]) return fail(B2_ERR_INVALID, "correct: sensor %u given twice", k);
+        sc[k].h = sensors[k]; sc[k].Tbo = Tbo[k]; sc[k].weight = merge_weights ? merge_weights[k] : 1.0; sc[k].ranges_host = nullptr; sc[k].n_ranges = 0;
+    }
+    b2_rcc* H = sc[0].h;
+    const uint32_t ns = n_sensors;
+    CU(cudaSetDevice(H->map->device));
+    if (!H->pending.empty()) return fail(B2_ERR_INVALID, "correct: asynchronous calls are still in flight on the lead handle, collect them first");
+    if (H->fused_grid <= 0) return fail(B2_ERR_UNSUPPORTED, "correct: a chain of corrections needs a device with cooperative launch");
+    const int mode = H->exec_mode == 0 ? 1 : H->exec_mode;           // exec mode 0 keeps its state on the host between reductions: the chain runs the fused loop
+    uint64_t pairs = 0; uint32_t total_meas = 0;
+    for (uint32_t k = 0; k < ns; k++) {
+        const b2_rcc* h = sc[k].h;
+        if (h->map->device != H->map->device) return fail(B2_ERR_INVALID, "correct: all sensors must live on the same device");
+        if (h->corr_type != B2_CORR_CPC && !h->has_model) return fail(B2_ERR_INVALID, "correct before setModel");
+        if (h->n_dataset != h->work_n()) return fail(B2_ERR_INVALID, "dataset size %u != model size %u", h->n_dataset, h->n);
+        pairs += h->work_n(); total_meas += h->n_dataset;
+    }
+    if (n_corrections == 0) return B2_OK;
+    const size_t bytes = sizeof(IcpChainState) + sizeof(b2_micp_step) * (size_t)n_corrections;
+    RES(H->d_chain.reserve(bytes));
+    for (uint32_t k = 1; k < ns; k++) {        // order the lead stream behind the other sensors' own streams (pending set_ranges / set_dataset copies)
+        CU(cudaEventRecord(sc[k].h->ev_join, sc[k].h->stream));
+        CU(cudaStreamWaitEvent(H->stream, sc[k].h->ev_join, 0));
+    }
+    {
+        IcpChainState st; memset(&st, 0, sizeof(st));
+        for (uint32_t k = 0; k < ns; k++) { st.find[k].Tom = *Tom_inout; st.find[k].Tbo = sc[k].Tbo; }
+        st.cp = *cp_inout; st.total = total_meas;
+        CU(cudaMemcpyAsync(H->d_chain.p, &st, sizeof(st), cudaMemcpyHostToDevice, H->stream));      // pageable source: staged before the call returns
+        for (uint32_t k = 0; k < ns; k++) {
+            const b2_rcc* h = sc[k].h;
+            if (!h->n_dataset) continue;
+            const int g = (int)std::min<uint32_t>((uint32_t)H->red_grid * 4u, (h->n_dataset + 255u) / 256u);
+            k_mask_count<<<g, 256, 0, H->stream>>>(h->dmask(), h->n_dataset, &chain_state(H)->valid);
+            LAUNCHED();
+        }
+    }
+    std::vector<unsigned char> out(bytes);
+    IcpChainState* got = reinterpret_cast<IcpChainState*>(out.data());
+    b2_micp_step* rec = reinterpret_cast<b2_micp_step*>(out.data() + sizeof(IcpChainState));
+    if (pairs == 0 || iterations == 0) {
+        // Tom stays and the progress becomes 0 (micp_localization.cpp:974, :988-990); the finds still run (:900-908), at the same pose every step
+        for (uint32_t k = 0; k < ns && pairs > 0; k++) {
+            b2_rcc* h = sc[k].h;
+            b2_transform Tbm; memset(&Tbm, 0, sizeof(Tbm)); tf_store(&Tbm, tf_mul(tf_from_pod(*Tom_inout), tf_from_pod(sc[k].Tbo)));
+            const cudaStream_t own = h->stream; h->stream = H->stream;
+            const int rc = launch_find(h, &Tbm, nullptr);
+            h->stream = own;
+            RES(rc);
+        }
+        CU(cudaMemcpyAsync(out.data(), H->d_chain.p, sizeof(IcpChainState), cudaMemcpyDeviceToHost, H->stream));
+        CU(cudaStreamSynchronize(H->stream));
+        for (uint32_t s = 0; s < n_corrections; s++) {
+            memset(&rec[s], 0, sizeof(b2_micp_step));
+            rec[s].Tom_new = *Tom_inout; rec[s].T_onew_oold = tf_identity_pod(); rec[s].valid_measurements = got->valid; rec[s].total_measurements = total_meas;
+        }
+        got->find[0].Tom = *Tom_inout; got->cp = 0.0; got->done = n_corrections;
+    } else {
+        IcpLaunch L; memset(&L, 0, sizeof(L));
+        L.Tom = *Tom_inout; L.n_sensors = ns; L.iterations = iterations; L.chain = chain_state(H); L.adaptive = adaptive_max_dist ? 1u : 0u;
+        uint32_t nblk[B2_MAX_SENSORS];
+        const int grid = loop_blocks(H, sc, ns, pairs, nblk);
+        uint32_t blk0 = 0;
+        for (uint32_t k = 0; k < ns; k++) {
+            const b2_rcc* h = sc[k].h;
+            IcpSensor& S = L.s[k];
+            S.n = h->work_n(); S.blk0 = blk0; S.nblk = nblk[k]; blk0 += nblk[k];
+            const uint32_t stride = S.nblk * B2_ICP_BLOCK, per_thread = stride ? (S.n + stride - 1) / stride : 0u;
+            S.smem_u = per_thread > B2_ICP_REG_PAIRS ? std::min<uint32_t>(per_thread - B2_ICP_REG_PAIRS, (uint32_t)H->smem_u_cap) : 0u;
+            L.smem_u_max = std::max(L.smem_u_max, S.smem_u);
+            S.max_dist = h->max_dist; S.max_dist_min = h->adaptive_max_dist_min;      // the loop interpolates with the progress (CorrespondencesCPU.cpp:21-23)
+            S.merge_weight = sc[k].weight; S.range_min = h->range_min; S.range_max = h->range_max;
+            fill_sensor_frames(S, sc[k].Tbo, h->Tsb);
+            S.dpts = h->dpts(); S.dmask = h->dmask();
+        }
+        for (uint32_t s = 0; s < n_corrections; s++) RES(chain_step(sc, ns, L, grid, mode, s));
+        H->loop_geom[0] = ns; H->loop_geom[1] = (uint32_t)grid;
+        for (uint32_t k = 0; k < B2_MAX_SENSORS; k++) {
+            uint32_t* g = H->loop_geom + 2 + 4 * k;
+            if (k < ns) { g[0] = L.s[k].n; g[1] = L.s[k].blk0; g[2] = L.s[k].nblk; g[3] = L.s[k].smem_u; } else g[0] = g[1] = g[2] = g[3] = 0u;
+        }
+        CU(cudaMemcpyAsync(out.data(), H->d_chain.p, bytes, cudaMemcpyDeviceToHost, H->stream));
+        CU(cudaStreamSynchronize(H->stream));
+        if (got->done < n_corrections) {
+            // A mode-2 exchange gave up (micp_collect: co-residency or fixed-point range); the steps behind it saw the abort word and left.  The
+            // device state is the last completed step's: reset the abort and accumulator words and run the rest of the chain cooperatively.
+            unsigned int bar_state[2] = {0u, 0u};
+            CU(cudaMemcpy(bar_state, H->d_bar.p, sizeof(bar_state), cudaMemcpyDeviceToHost));
+            if (mode != 2 || bar_state[1] == 0u) return fail(B2_ERR_CUDA, "correct: step %u of %u left no record", got->done + 1, n_corrections);
+            CU(cudaMemset(H->d_bar.p + 1, 0, sizeof(unsigned int)));
+            CU(cudaMemset(H->d_slots.p, 0, ((size_t)B2_ICP_ACC_WORDS + B2_ICP_BASE_WORDS) * sizeof(unsigned long long)));
+            H->n_reruns++;
+            for (uint32_t s = got->done; s < n_corrections; s++) RES(chain_step(sc, ns, L, grid, 1, s));
+            CU(cudaMemcpyAsync(out.data(), H->d_chain.p, bytes, cudaMemcpyDeviceToHost, H->stream));
+            CU(cudaStreamSynchronize(H->stream));
+            if (got->done != n_corrections) return fail(B2_ERR_CUDA, "correct: the cooperative re-run left %u of %u records", got->done, n_corrections);
+        }
+    }
+    for (uint32_t k = 1; k < ns; k++) {        // later work on the other sensors' own streams sees the model buffers the chain wrote
+        CU(cudaEventRecord(sc[k].h->ev_join, H->stream));
+        CU(cudaStreamWaitEvent(sc[k].h->stream, sc[k].h->ev_join, 0));
+    }
+    *Tom_inout = got->find[0].Tom;
+    *cp_inout = got->cp;
+    if (steps_out) memcpy(steps_out, rec, sizeof(b2_micp_step) * (size_t)n_corrections);
+    return B2_OK;
 }
 
 extern "C" int b2_rcc_correct_batch(b2_rcc* h, const b2_transform* Tbm, uint32_t n_poses, int poses_on_device,

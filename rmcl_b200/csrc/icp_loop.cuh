@@ -39,12 +39,23 @@ struct IcpSensor {
     uint32_t n, blk0, nblk, zc_n_origs, smem_u;                 // pairs; blocks [blk0, blk0+nblk); pairs per thread kept in shared memory
     uint32_t zc_seq;
     const uint32_t* tile_cost; uint16_t* tile_perm;             // != nullptr: the idle warps of this sensor's first block turn the warp durations of the find
-    uint32_t n_tiles, pad_;                                     //   kernel into the tile order of the NEXT find (kernels.cuh: tile schedule)
+    uint32_t n_tiles;                                           //   kernel into the tile order of the NEXT find (kernels.cuh: tile schedule)
+    float max_dist_min;                                         // chain steps only: adaptive_max_dist_min (Correspondences.hpp:23); max_dist is then params.max_dist
+};
+// Device state of a chain of corrections (b2_micp_correct): what step k+1 reads from step k, so that the host is not involved between them.
+struct alignas(16) IcpChainState {
+    IcpState find[B2_MAX_SENSORS];     // Tom (the pose of the next find, written by block 0 of each loop) and Tbo of sensor k; the find kernels' `icp` argument
+    double cp;                         // convergence_progress_ after the last completed step (micp_localization.cpp:988-1007)
+    uint32_t valid, total;             // stats.valid_measurements / total_measurements over all sensors (:866-871): mask ones, dataset sizes
+    uint32_t done, pad_;               // steps completed
 };
 struct IcpLaunch {
     IcpSensor s[B2_MAX_SENSORS];
     b2_transform Tom;
     uint32_t n_sensors, iterations, seq, smem_u_max;
+    IcpChainState* chain;              // != nullptr: one step of a chain -- Tom and the progress come from here and block 0 writes the step's outcome back
+    b2_micp_step* step_out;            //   the record of this step
+    uint32_t adaptive, pad_;           //   adaptive_max_dist_ (micp_localization.hpp:157)
 };
 struct IcpResult { b2_transform Tom_new, T_onew_oold; b2_cross_stats Cmerged_o; };                  // 128 bytes
 static_assert(sizeof(IcpResult) == 128, "IcpResult must be 128 bytes");
@@ -211,8 +222,8 @@ B2_DEV Tf icp_umeyama(const CStats& s, long long* st = nullptr)
 // place, Tpre_out[s] receives the pre-transform of sensor s for the NEXT pass (T_snew_sold = Tso * T_onew_oold * Tos: MICPSensor.hpp:178 with
 // the constant frame chain pre-composed) for the sensors [k0, k1) -- on the device lane k of the warp computes sensor k --, `res` is filled
 // after the last iteration (micp_localization.cpp:972-984).
-B2_DEV void icp_tail_rest(const IcpLaunch& L, const float (*odo)[16], const uint32_t* cnt, Tf& T_onew_oold, Tf* Tpre_out, uint32_t k0, uint32_t k1, bool last,
-                          IcpResult* res, long long* st = nullptr)
+B2_DEV void icp_tail_rest(const IcpLaunch& L, const b2_transform& Tom_pod, const float (*odo)[16], const uint32_t* cnt, Tf& T_onew_oold, Tf* Tpre_out, uint32_t k0, uint32_t k1,
+                          bool last, IcpResult* res, long long* st = nullptr)
 {
     CStats merged = cs_identity(), merged_w = cs_identity();
     for (uint32_t k = 0; k < L.n_sensors; k++) {
@@ -231,7 +242,7 @@ B2_DEV void icp_tail_rest(const IcpLaunch& L, const float (*odo)[16], const uint
     for (uint32_t k = k0; k < k1; k++) Tpre_out[k] = tf_mul(tf_mul(tf_from_pod(L.s[k].Tso), T_onew_oold), tf_from_pod(L.s[k].Tos));
     B2_TAIL_STAMP(st, 7);
     if (last && res) {
-        const Tf Tom = tf_from_pod(L.Tom);
+        const Tf Tom = tf_from_pod(Tom_pod);
         Tf Tn = tf_mul(Tom, T_onew_oold);                                                             // :972
         if (merged.n > 0) Tn.R = q_normalize(Tn.R); else Tn = Tom;                                    // :974-984
         tf_store(&res->Tom_new, Tn); tf_store(&res->T_onew_oold, T_onew_oold); cs_store(&res->Cmerged_o, merged);
@@ -242,7 +253,32 @@ B2_DEV void icp_tail(const IcpLaunch& L, const double (*sums)[B2_NACC + 1], Tf& 
 {
     float odo[B2_MAX_SENSORS][16]; uint32_t cnt[B2_MAX_SENSORS];
     for (uint32_t k = 0; k < L.n_sensors; k++) cnt[k] = icp_sensor_stats(L.s[k], sums[k], odo[k]);
-    icp_tail_rest(L, odo, cnt, T_onew_oold, Tpre_out, 0, L.n_sensors, last, res);
+    icp_tail_rest(L, L.Tom, odo, cnt, T_onew_oold, Tpre_out, 0, L.n_sensors, last, res);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Between two corrections (host+device so that tests/emul runs the same code)
+// ---------------------------------------------------------------------------------------------------------------------
+// params.max_dist interpolated towards adaptive_max_dist_min by the progress (CorrespondencesCPU.cpp:21-23): float * double + float * double
+// in double, rounded to float -- the host's expression (api.cu: micp_enqueue), so that a chain step gates exactly like a host-fed call
+B2_DEV float icp_adaptive_max_dist(float max_dist, float max_dist_min, double cp)
+{
+    return (float)((double)max_dist * (1.0 - cp) + (double)max_dist_min * cp);
+}
+// convergence_progress_ after one correctOnce (micp_localization.cpp:988-1007), with the reference's types statement by statement.  T_onew_map =
+// Tom * T_onew_oold before the normalisation of :983 (:972); valid = stats.valid_measurements (:870).  Quirk: trans_force is the norm of the
+// ABSOLUTE translation of T_odom_map, so the progress is about 0 unless the odom origin lies within ~0.3 m of the map origin (SURVEY.md D12).
+B2_DEV double micp_progress(const b2_transform& Tom, const b2_transform& T_onew_oold, uint32_t n_meas, uint32_t valid, bool adaptive)
+{
+    if (n_meas == 0 || !adaptive) return 0.0;                                                        // :988-991
+    const Tf T = tf_mul(tf_from_pod(Tom), tf_from_pod(T_onew_oold));                                 // :972
+    const float trans_force = v_l2norm(T.t);                                                         // :994
+    const float trans_progress = (float)(1.0 / exp(10.0 * (double)trans_force));                     // :995
+    const float qscalar = add(add(add(mul(T.R.x, 0.0f), mul(T.R.y, 0.0f)), mul(T.R.z, 0.0f)), mul(T.R.w, 1.0f));   // :997-998, R.dot(Identity)
+    const float rot_progress = mul(qscalar, qscalar);                                                // :999
+    const double match_ratio = (double)n_meas / (double)valid;                                       // :1001
+    const float adaption_rate = (float)((double)mul(trans_progress, rot_progress) * match_ratio);   // :1002
+    return (double)adaption_rate;                                                                    // :1006
 }
 
 #if defined(__CUDACC__)
@@ -401,10 +437,13 @@ __global__ void __launch_bounds__(B2_ICP_BLOCK) k_icp_loop(const __grid_constant
     __shared__ uint32_t s_bin[1 + 16 * 15];                        // tile schedule of the next find (first block of each sensor)
     __shared__ Tf s_Tpre[B2_MAX_SENSORS];
     __shared__ Tf s_T;                                             // T_onew_oold
+    __shared__ b2_transform s_Tom;                                 // Tom of this correctOnce (micp_localization.cpp:860)
     __shared__ IcpResult s_res;
     const long long k0 = clock64();
     const unsigned long long g0 = globaltimer_ns();
     const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    // a chain step behind a step that gave up (abort word still set) does nothing: the host re-runs the chain from the first step without a record
+    if (L.chain && __syncthreads_or(tid == 0u && *reinterpret_cast<volatile unsigned int*>(bar_abort) != 0u)) return;
     uint32_t si = 0;
     for (uint32_t k = 1; k < L.n_sensors; k++) if (blockIdx.x >= L.s[k].blk0) si = k;
     const IcpSensor& S = L.s[si];
@@ -413,7 +452,7 @@ __global__ void __launch_bounds__(B2_ICP_BLOCK) k_icp_loop(const __grid_constant
     if (tid < L.n_sensors) {
         // pre-transform of the first pass: T_onew_oold = I  ->  Tso * I * Tos with the same individually rounded ops as later iterations
         s_Tpre[tid] = tf_mul(tf_mul(tf_from_pod(L.s[tid].Tso), tf_identity()), tf_from_pod(L.s[tid].Tos));
-        if (tid == 0) s_T = tf_identity();
+        if (tid == 0) { s_T = tf_identity(); s_Tom = L.chain ? L.chain->find[0].Tom : L.Tom; }
     }
     if (tid >= 32u && tid < 32u + 12u * L.n_sensors) {
         const uint32_t k = (tid - 32u) / 12u, e = (tid - 32u) - 12u * k;
@@ -483,11 +522,12 @@ __global__ void __launch_bounds__(B2_ICP_BLOCK) k_icp_loop(const __grid_constant
     ulonglong2* const slots = reinterpret_cast<ulonglong2*>(xbuf + B2_ICP_ACC_WORDS + B2_ICP_BASE_WORDS);
     if (!COOP && tid < 2u * B2_MAX_SENSORS * 32u) (&s_prev[0][0][0])[tid] = __ldcg(base_w + tid);     // written by block 0 of the previous launch
     __syncthreads();
+    // a chain step gates with the progress the previous step left (written before this grid's find was launched)
+    const float max_dist = L.chain ? icp_adaptive_max_dist(S.max_dist, S.max_dist_min, L.chain->cp) : S.max_dist;
     const long long k1 = clock64();
     for (uint32_t it = 0; it < L.iterations; it++) {
         const long long c0 = clock64();
         const Tf Tpre = s_Tpre[si];
-        const float max_dist = S.max_dist;
         P2LAcc acc; acc_zero(acc);
         #pragma unroll
         for (int u = 0; u < B2_ICP_REG_PAIRS; u++) {
@@ -607,7 +647,7 @@ __global__ void __launch_bounds__(B2_ICP_BLOCK) k_icp_loop(const __grid_constant
             long long st[8] = {0, 0, 0, 0, 0, 0, 0, 0};
             const bool prof = it == 1 && blockIdx.x == 0 && dbg && lane == 0;
             const bool mine = lane < L.n_sensors;                                                    // lane k prepares sensor k's next pre-transform
-            if (ok) icp_tail_rest(L, s_odo, s_n, T, s_Tpre, mine ? lane : 0u, mine ? lane + 1u : 0u, it + 1 == L.iterations, lane == 0 ? &s_res : nullptr, prof ? st : nullptr);
+            if (ok) icp_tail_rest(L, s_Tom, s_odo, s_n, T, s_Tpre, mine ? lane : 0u, mine ? lane + 1u : 0u, it + 1 == L.iterations, lane == 0 ? &s_res : nullptr, prof ? st : nullptr);
             __syncwarp();                                           // every lane has read s_T (and the statistics) before lane 0 replaces it
             if (lane == 0) s_T = T;
             if (prof) {
@@ -633,7 +673,31 @@ __global__ void __launch_bounds__(B2_ICP_BLOCK) k_icp_loop(const __grid_constant
             uint4 c; c.x = w[3 * tid]; c.y = 3 * tid + 1 < 32u ? w[3 * tid + 1] : 0u; c.z = 3 * tid + 2 < 32u ? w[3 * tid + 2] : 0u; c.w = L.seq;
             asm volatile("st.volatile.global.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(host_out + tid), "r"(c.x), "r"(c.y), "r"(c.z), "r"(c.w) : "memory");
         }
+        if (L.chain && tid == 0) {
+            // chain step: the progress (micp_localization.cpp:988-1007), then the state the next step reads -- the next find's pose (Tom_ after
+            // :983) and the progress its loop gates with -- and this step's record.  Every block has read the previous state before it
+            // contributed to this grid's first exchange, so nothing reads what is overwritten here.
+            IcpChainState* c = L.chain;
+            const uint32_t valid = c->valid;
+            const double cp = micp_progress(s_Tom, s_res.T_onew_oold, s_res.Cmerged_o.n_meas, valid, L.adaptive != 0u);
+            for (uint32_t k = 0; k < L.n_sensors; k++) c->find[k].Tom = s_res.Tom_new;
+            c->cp = cp;
+            b2_micp_step* r = L.step_out;
+            r->Tom_new = s_res.Tom_new; r->T_onew_oold = s_res.T_onew_oold; r->Cmerged_o = s_res.Cmerged_o;
+            r->convergence_progress = cp; r->valid_measurements = valid; r->total_measurements = c->total;
+            c->done++;
+        }
         if (tid == 0 && dbg) { dbg[4] = (unsigned long long)(k1 - k0); dbg[5] = (unsigned long long)(clock64() - k0); dbg[6] = g0; dbg[7] = globaltimer_ns(); }
     }
+}
+
+// stats.valid_measurements of a chain (micp_localization.cpp:866-871): the mask ones of one sensor's dataset (mask > 0, as unpackMessage
+// counts them), added to *out; once per sensor at the start of the chain, the dataset is fixed for the whole call
+__global__ void k_mask_count(const uint8_t* __restrict__ mask, uint32_t n, uint32_t* __restrict__ out)
+{
+    uint32_t c = 0;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) c += mask[i] > 0 ? 1u : 0u;
+    c = __reduce_add_sync(0xffffffffu, c);
+    if ((threadIdx.x & 31u) == 0u && c) atomicAdd(out, c);
 }
 #endif
