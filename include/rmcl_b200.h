@@ -300,6 +300,21 @@ B2_API int b2_pf_p2p_connect_local(b2_pf* h, const b2_transform* poses_all_dev, 
 /* the draws b2_pf_resample_gladiator would use (replaces init_curand / curand(), resampling.cu:13-30,134-143): raw u32 + 6 normals per particle */
 B2_API int b2_pf_gladiator_randoms(b2_pf* h, uint64_t seed, uint32_t step, uint32_t first, uint32_t n, uint32_t* raw_dev, float* normals_dev);
 
+/* Particle set initialisation on the device: writes particles first .. first+n-1 of the set into poses_dev / attrs_dev (n entries each; DEVICE
+ * pointers) with likelihood {1, 0, 0} and state_sigma 0.  Draws are Philox4x32-10 keyed by (seed, global particle index), so initialising
+ * [first, first+n) on each rank and concatenating equals one call for the whole set, bit for bit.  Launches on the handle's stream, no host
+ * synchronisation; n == 0 launches nothing.  A bad box or covariance and first + n > 2^32 are refused before any launch.
+ * RmclNode::initSamplesUniform (rmcl_ros/src/nodes/rmcl_localization.cpp:277-342): t and the Euler angles uniform in [bb_min, bb_max]
+ * (x, y, z, roll, pitch, yaw; doubles narrowed to float; min == max gives exactly that value; min > max or non-finite is refused). */
+B2_API int b2_pf_init_uniform(b2_pf* h, b2_transform* poses_dev, b2_particle_attr* attrs_dev, uint32_t first, uint32_t n, const double bb_min[6], const double bb_max[6],
+                              uint64_t seed);
+/* RmclNode::initSamples(PoseWithCovarianceStamped) (rmcl_localization.cpp:165-275): x = chol(C) N(0, I6) with C the message's 36 doubles
+ * (row-major, narrowed to float, lower triangle read), pose = *pose * Transform{EulerAngles{x3, x4, x5}, {x0, x1, x2}} -- the covariance
+ * acts in the pose frame.  A zero variance whose covariances are zero gives that component no noise; a negative or NaN pivot, or a zero
+ * variance with a non-zero covariance, is refused with a message naming the column. */
+B2_API int b2_pf_init_gaussian(b2_pf* h, b2_transform* poses_dev, b2_particle_attr* attrs_dev, uint32_t first, uint32_t n, const b2_transform* pose,
+                               const double cov_rowmajor[36], uint64_t seed);
+
 /* ---------------------------------------------------------------- introspection ------------------------------ */
 /* CUDA-event timing of the kernels inside b2_rcc_correct_once*(): when enabled, events are recorded on the handle's stream around the
  * find kernel and around the reduction/Umeyama kernels; b2_rcc_last_timing returns the two durations of the most recent call (ms). */

@@ -7,6 +7,7 @@
 //   rmcl::{Sphere,Pinhole,O1Dn,OnDn}CorrectorB200  v1 API used by rmcl_ros/src/benchmarks/lidar_corrector_{embree,optix}_benchmark.cpp:86-155
 //   rmcl::PCDSensorUpdaterB200              rmcl_ros/include/rmcl_ros/rmcl/ParticleUpdater.hpp:39-43 + PCDSensorUpdaterEmbree.cpp:244-352
 #pragma once
+#include <array>
 #include <memory>
 #include <stdexcept>
 #include <string>
@@ -377,6 +378,24 @@ public:
         b2_check(b2_pf_resample_gladiator(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<const b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(),
                                           first, (uint32_t)poses_new.size(), reinterpret_cast<b2_transform*>(poses_new.raw()), reinterpret_cast<b2_particle_attr*>(attrs_new.raw()),
                                           &resampler_config, seed, step, nullptr, nullptr), "resample");
+    }
+    // RmclNode::initSamplesUniform (rmcl_localization.cpp:277-342) on the device: particles first .. first+poses.size()-1 of a set drawn
+    // uniformly from [bb_min, bb_max] (x, y, z, roll, pitch, yaw).  Draws keyed by (seed, global index): shards concatenate to the whole set.
+    void initSamplesUniform(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs,
+                            const std::array<double, 6>& bb_min, const std::array<double, 6>& bb_max, uint64_t seed, uint32_t first = 0)
+    {
+        if (poses.size() != attrs.size()) throw std::invalid_argument("initSamplesUniform: poses and attrs differ in size");
+        b2_check(b2_pf_init_uniform(h_, reinterpret_cast<b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), first, (uint32_t)poses.size(),
+                                    bb_min.data(), bb_max.data(), seed), "initSamplesUniform");
+    }
+    // RmclNode::initSamples(PoseWithCovarianceStamped) (rmcl_localization.cpp:165-275) on the device: `pose` and the 36 row-major covariance
+    // entries of the message; the noise acts in the pose frame.
+    void initSamples(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs,
+                     const rm::Transform& pose, const std::array<double, 36>& covariance, uint64_t seed, uint32_t first = 0)
+    {
+        if (poses.size() != attrs.size()) throw std::invalid_argument("initSamples: poses and attrs differ in size");
+        b2_check(b2_pf_init_gaussian(h_, reinterpret_cast<b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), first, (uint32_t)poses.size(),
+                                     reinterpret_cast<const b2_transform*>(&pose), covariance.data(), seed), "initSamples");
     }
 private:
     B200MapPtr map_;

@@ -75,7 +75,7 @@ EXPORTS = [
     "b2_pf_set_stream", "b2_pf_sensor_update", "b2_pf_sensor_update_host", "b2_kernel_launch_count", "b2_rcc_enable_timing", "b2_rcc_last_timing", "b2_pf_motion_update", "b2_pf_likelihood_stats",
     "b2_rcc_set_correspondence_type", "b2_pf_resample_gladiator", "b2_pf_gladiator_randoms", "b2_rcc_segment", "b2_mesh_create_from_file", "b2_mesh_file_load", "b2_mesh_file_free", "b2_peek_cuda_error", "b2_mesh_blob_size", "b2_mesh_export_blob", "b2_mesh_create_from_blob", "b2_mesh_refit",
     "b2_rcc_correct_once_async", "b2_rcc_correct_once_wait", "b2_micp_correct_once", "b2_rcc_set_exec_mode", "b2_debug_read_bandwidth", "b2_rcc_set_sim_options", "b2_rcc_bind_dataset", "b2_rcc_bind_model_buffers", "b2_rcc_benchmark_batch", "b2_pf_p2p_init", "b2_pf_p2p_connect", "b2_pf_p2p_publish", "b2_pf_resample_gladiator_p2p", "b2_pf_p2p_connect_local", "b2_rcc_set_cpc_options", "b2_pf_set_mapping", "b2_pf_get_mapping",
-    "b2_micp_correct",
+    "b2_micp_correct", "b2_pf_init_uniform", "b2_pf_init_gaussian",
 ]
 
 
@@ -650,6 +650,32 @@ class PCDSensorUpdaterB200:
             s, m = float(ts[0]), float(tm[0])
         return s, m
 
+
+    @staticmethod
+    def _init_count(particle_poses, particle_attrs):
+        n = particle_poses.numel() * particle_poses.element_size() // 32
+        if particle_attrs.numel() * particle_attrs.element_size() != 36 * n:
+            raise ValueError(f"initSamples: {n} poses but {particle_attrs.numel() * particle_attrs.element_size() / 36:g} attrs")
+        return n
+
+    def initSamplesUniform(self, particle_poses, particle_attrs, bb_min, bb_max, seed, first=0):
+        """RmclNode::initSamplesUniform (rmcl_ros/src/nodes/rmcl_localization.cpp:277-342) on the device: fills the caller's (n, 8) / (n, 9)
+        float32 CUDA tensors in place with particles first .. first+n-1 of a set drawn uniformly from the box (x, y, z, roll, pitch, yaw)."""
+        lo, hi = np.ascontiguousarray(bb_min, np.float64).reshape(6), np.ascontiguousarray(bb_max, np.float64).reshape(6)
+        n = self._init_count(particle_poses, particle_attrs)
+        _chk(load_library().b2_pf_init_uniform(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(first), C.c_uint32(n), _p(lo), _p(hi),
+                                               C.c_uint64(seed)))
+        return particle_poses, particle_attrs
+
+    def initSamples(self, particle_poses, particle_attrs, pose, cov, seed, first=0):
+        """RmclNode::initSamples(PoseWithCovarianceStamped) (rmcl_localization.cpp:165-275) on the device: `pose` is the message pose (a
+        Transform record), `cov` its 36 covariance entries (row-major); the noise acts in the pose frame.  Fills the tensors in place."""
+        T = _tf(pose).reshape(())
+        c = np.ascontiguousarray(cov, np.float64).reshape(36)
+        n = self._init_count(particle_poses, particle_attrs)
+        _chk(load_library().b2_pf_init_gaussian(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(first), C.c_uint32(n), _p(T), _p(c),
+                                                C.c_uint64(seed)))
+        return particle_poses, particle_attrs
 
     def gladiatorRandoms(self, seed, step, first, n, device=None):
         """The draws resample() uses for champions first..first+n-1 (raw u32 opponent word + 6 normals each), as torch CUDA tensors."""

@@ -2035,6 +2035,81 @@ extern "C" int b2_pf_gladiator_randoms(b2_pf* h, uint64_t seed, uint32_t step, u
     return B2_OK;
 }
 
+// ---- particle set initialisation ------------------------------------------------------------------------------------------------------------
+static int pf_init_range(uint32_t first, uint32_t n)
+{
+    if ((uint64_t)first + n > (1ull << 32)) return fail(B2_ERR_INVALID, "particle range %u+%u exceeds 2^32 global indices", first, n);
+    return B2_OK;
+}
+
+extern "C" int b2_pf_init_uniform(b2_pf* h, b2_transform* poses_dev, b2_particle_attr* attrs_dev, uint32_t first, uint32_t n, const double* bb_min, const double* bb_max,
+                                  uint64_t seed)
+{
+    NOTNULL(h); NOTNULL(bb_min); NOTNULL(bb_max);
+    static const char* dim[6] = {"x", "y", "z", "roll", "pitch", "yaw"};
+    PfInitBox box;
+    for (int k = 0; k < 6; k++) {
+        box.lo[k] = (float)bb_min[k]; box.hi[k] = (float)bb_max[k];           // uniform_real_distribution<float> of the double parameters
+        if (!std::isfinite(box.lo[k]) || !std::isfinite(box.hi[k]))
+            return fail(B2_ERR_INVALID, "init uniform: %s bounds [%g, %g] are not finite in float", dim[k], bb_min[k], bb_max[k]);
+        if (box.lo[k] > box.hi[k]) return fail(B2_ERR_INVALID, "init uniform: %s bounds [%g, %g] have min > max", dim[k], bb_min[k], bb_max[k]);
+        if (!std::isfinite(box.hi[k] - box.lo[k])) return fail(B2_ERR_INVALID, "init uniform: the %s extent %g overflows float", dim[k], bb_max[k] - bb_min[k]);
+    }
+    RES(pf_init_range(first, n));
+    if (n == 0) return B2_OK;
+    NOTNULL(poses_dev); NOTNULL(attrs_dev);
+    CU(cudaSetDevice(h->map->device));
+    k_pf_init_uniform<<<(n + 255) / 256, 256, 0, h->stream>>>(poses_dev, attrs_dev, first, n, box, seed);
+    LAUNCHED();
+    return B2_OK;
+}
+
+// rm::chol (Cholesky-Banachiewicz in float, sums over k in order) of the covariance narrowed to float (convert, rmcl_localization.cpp:154-163),
+// lower triangle only.  A zero pivot whose column numerators are all exactly zero gives a zero column (a component without noise, as in rviz's
+// /initialpose and any 2-D robot's covariance) where the reference divides 0 by 0 (SURVEY quirk D14); any other non-positive pivot is refused.
+static int pf_chol6(const double* cov, float L[36])
+{
+    float A[36];
+    for (int i = 0; i < 36; i++) { A[i] = (float)cov[i]; L[i] = 0.0f; }
+    for (int i = 0; i < 6; i++)
+        for (int j = 0; j <= i; j++)
+            if (!std::isfinite(A[6 * i + j])) return fail(B2_ERR_INVALID, "init gaussian: covariance entry (%d,%d) = %g is not finite in float", i, j, cov[6 * i + j]);
+    for (int i = 0; i < 6; i++)                                                    // row by row; column j's pivot is row j's diagonal
+        for (int j = 0; j <= i; j++) {
+            float s = 0.0f;
+            for (int k = 0; k < j; k++) s += L[6 * i + k] * L[6 * j + k];
+            const float num = A[6 * i + j] - s;
+            if (i == j) {
+                if (!(num >= 0.0f) || !std::isfinite(num))
+                    return fail(B2_ERR_INVALID, "init gaussian: covariance is not positive semi-definite at column %d (pivot %g)", j, (double)num);
+                L[6 * i + i] = std::sqrt(num);
+            } else if (L[6 * j + j] == 0.0f) {
+                if (num != 0.0f) return fail(B2_ERR_INVALID, "init gaussian: column %d has zero variance but a non-zero covariance at (%d,%d)", j, i, j);
+                // zero column: no noise on this component
+            } else {
+                L[6 * i + j] = num / L[6 * j + j];
+                if (!std::isfinite(L[6 * i + j])) return fail(B2_ERR_INVALID, "init gaussian: Cholesky factor (%d,%d) of column %d overflows float", i, j, j);
+            }
+        }
+    return B2_OK;
+}
+
+extern "C" int b2_pf_init_gaussian(b2_pf* h, b2_transform* poses_dev, b2_particle_attr* attrs_dev, uint32_t first, uint32_t n, const b2_transform* pose,
+                                   const double* cov_rowmajor, uint64_t seed)
+{
+    NOTNULL(h); NOTNULL(pose); NOTNULL(cov_rowmajor);
+    PfInitGauss g;
+    RES(pf_chol6(cov_rowmajor, g.L));
+    g.Tlm = *pose;                                                                 // Tpm = Identity (:222-225), so Tlm = Tlp
+    RES(pf_init_range(first, n));
+    if (n == 0) return B2_OK;
+    NOTNULL(poses_dev); NOTNULL(attrs_dev);
+    CU(cudaSetDevice(h->map->device));
+    k_pf_init_gaussian<<<(n + 255) / 256, 256, 0, h->stream>>>(poses_dev, attrs_dev, first, n, g, seed);
+    LAUNCHED();
+    return B2_OK;
+}
+
 extern "C" int b2_pf_likelihood_stats(b2_pf* h, const b2_particle_attr* attrs_dev, uint32_t n, float* sum_out, float* max_out)
 {
     NOTNULL(h);

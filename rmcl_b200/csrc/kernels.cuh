@@ -1077,18 +1077,23 @@ B2_DEV void philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, ui
     out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
 }
 B2_DEV float u01_open(uint32_t r) { return mul(add((float)(r >> 8), 0.5f), 5.9604644775390625e-08f); }
+// three Box-Muller pairs on the words (r[0], r[1]), (r[2], r[3]), (r[4], r[5])
+B2_DEV void box_muller3(const uint32_t* r, float N[6])
+{
+    #pragma unroll
+    for (int p = 0; p < 3; p++) {
+        const float u1 = u01_open(r[2 * p]), u2 = u01_open(r[2 * p + 1]);
+        const float rad = sqrtf(mul(-2.0f, logf(u1))), ang = mul(6.283185307179586f, u2);
+        N[2 * p] = mul(rad, cosf(ang)); N[2 * p + 1] = mul(rad, sinf(ang));
+    }
+}
 B2_DEV void gladiator_draws(uint64_t seed, uint32_t step, uint32_t gidx, uint32_t& raw, float N[6])
 {
     uint32_t r[8];
     philox4x32_10(gidx, 0u, step, 0u, (uint32_t)seed, (uint32_t)(seed >> 32), r);
     philox4x32_10(gidx, 0u, step, 1u, (uint32_t)seed, (uint32_t)(seed >> 32), r + 4);
     raw = r[0];
-    #pragma unroll
-    for (int p = 0; p < 3; p++) {
-        const float u1 = u01_open(r[1 + 2 * p]), u2 = u01_open(r[2 + 2 * p]);
-        const float rad = sqrtf(mul(-2.0f, logf(u1))), ang = mul(6.283185307179586f, u2);
-        N[2 * p] = mul(rad, cosf(ang)); N[2 * p + 1] = mul(rad, sinf(ang));
-    }
+    box_muller3(r + 1, N);
 }
 // rm::EulerAngles <-> Quaternion [RM-recalled: standard ZYX conversions], op order as in oracle/oracle.c
 B2_DEV void quat_to_euler(Q4 q, float& roll, float& pitch, float& yaw)
@@ -1158,6 +1163,71 @@ __global__ void k_pf_gladiator_randoms(uint64_t seed, uint32_t step, uint32_t fi
     gladiator_draws(seed, step, first + i, raw, N);
     raw_out[i] = raw;
     for (int k = 0; k < 6; k++) normals_out[6 * (size_t)i + k] = N[k];
+}
+#endif
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Particle set initialisation: RmclNode::initSamplesUniform (rmcl_ros/src/nodes/rmcl_localization.cpp:277-342) and
+// RmclNode::initSamples(PoseWithCovarianceStamped) (:165-275).  Draws: Philox4x32-10 with counter (global particle index, domain tag,
+// 0, block) and key = seed.  The tags are non-zero and Gladiator's second counter word is always 0, so no two streams share a counter.
+// ---------------------------------------------------------------------------------------------------------------------
+#define B2_PF_INIT_TAG_UNIFORM 1u
+#define B2_PF_INIT_TAG_GAUSSIAN 2u
+struct PfInitBox { float lo[6], hi[6]; };                  // x, y, z, roll, pitch, yaw; lo <= hi, finite, hi - lo finite (checked on the host)
+struct PfInitGauss { float L[36]; b2_transform Tlm; };     // Cholesky factor of the covariance (row-major, lower), message pose
+B2_DEV float u01_closed_open(uint32_t r) { return mul((float)(r >> 8), 5.9604644775390625e-08f); }   // [0, 1), exact
+// the attributes both initialisers give a particle (:252-255, :322-325): Gaussian1D::Identity() with mean 1.0, state_sigma 0
+B2_DEV void pf_init_attr(b2_particle_attr* a)
+{
+    a->likelihood.mean = 1.0f; a->likelihood.sigma = 0.0f; a->likelihood.n_meas = 0u;
+    #pragma unroll
+    for (int k = 0; k < 6; k++) a->state_sigma[k] = 0.0f;
+}
+// uniform_real_distribution<float>(lo, hi) per dimension (:287-292, :318-319): lo + (hi - lo) u, u in [0, 1), never above hi
+B2_DEV void pf_init_uniform_one(uint64_t seed, uint32_t gidx, const PfInitBox& box, b2_transform* out_p, b2_particle_attr* out_a)
+{
+    uint32_t r[8];
+    philox4x32_10(gidx, B2_PF_INIT_TAG_UNIFORM, 0u, 0u, (uint32_t)seed, (uint32_t)(seed >> 32), r);
+    philox4x32_10(gidx, B2_PF_INIT_TAG_UNIFORM, 0u, 1u, (uint32_t)seed, (uint32_t)(seed >> 32), r + 4);
+    float v[6];
+    #pragma unroll
+    for (int k = 0; k < 6; k++) v[k] = fminf(add(box.lo[k], mul(sub(box.hi[k], box.lo[k]), u01_closed_open(r[k]))), box.hi[k]);
+    Tf T; T.t = mk3(v[0], v[1], v[2]); T.R = euler_to_quat(v[3], v[4], v[5]);
+    tf_store(out_p, T);
+    pf_init_attr(out_a);
+}
+// x = L N(0, I6) (rm::Matrix_ product, sums over k = 0..5 in order), pose = Tlm * Transform{EulerAngles{x3, x4, x5}, {x0, x1, x2}} (:231-251)
+B2_DEV void pf_init_gaussian_one(uint64_t seed, uint32_t gidx, const PfInitGauss& g, b2_transform* out_p, b2_particle_attr* out_a)
+{
+    uint32_t r[8];
+    philox4x32_10(gidx, B2_PF_INIT_TAG_GAUSSIAN, 0u, 0u, (uint32_t)seed, (uint32_t)(seed >> 32), r);
+    philox4x32_10(gidx, B2_PF_INIT_TAG_GAUSSIAN, 0u, 1u, (uint32_t)seed, (uint32_t)(seed >> 32), r + 4);
+    float N[6], x[6];
+    box_muller3(r, N);
+    #pragma unroll
+    for (int i = 0; i < 6; i++) {
+        float a = 0.0f;
+        #pragma unroll
+        for (int k = 0; k < 6; k++) a = add(a, mul(g.L[6 * i + k], N[k]));
+        x[i] = a;
+    }
+    Tf Pl; Pl.t = mk3(x[0], x[1], x[2]); Pl.R = euler_to_quat(x[3], x[4], x[5]);
+    tf_store(out_p, tf_mul(tf_from_pod(g.Tlm), Pl));
+    pf_init_attr(out_a);
+}
+#ifdef __CUDACC__
+// write-only: 32 B pose + 36 B attrs per particle, nothing read from HBM
+__global__ void __launch_bounds__(256) k_pf_init_uniform(b2_transform* __restrict__ poses, b2_particle_attr* __restrict__ attrs, uint32_t first, uint32_t n, PfInitBox box, uint64_t seed)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    pf_init_uniform_one(seed, first + i, box, poses + i, attrs + i);
+}
+__global__ void __launch_bounds__(256) k_pf_init_gaussian(b2_transform* __restrict__ poses, b2_particle_attr* __restrict__ attrs, uint32_t first, uint32_t n, PfInitGauss g, uint64_t seed)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    pf_init_gaussian_one(seed, first + i, g, poses + i, attrs + i);
 }
 #endif
 

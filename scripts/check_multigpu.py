@@ -5,7 +5,9 @@
 Checks, with particles sharded contiguously over the ranks and the map replicated:
   1. sensor update of the shards == the single-GPU update of the whole set (gathered on rank 0, compared byte for byte);
   2. Gladiator resampling: all-gather variant == peer-memory (CUDA IPC over NVLink) variant on every rank, and their concatenation ==
-     rank 0's single-GPU resampling of the gathered set; exchanged bytes of both variants.
+     rank 0's single-GPU resampling of the gathered set; exchanged bytes of both variants;
+  3. particle set initialisation (uniform and Gaussian): each rank's shard (first = rank * n) gathered == rank 0's initialisation of the
+     whole set, byte for byte.
 Prints one JSON line on rank 0; exit code 1 on any mismatch."""
 import json
 import os
@@ -80,20 +82,43 @@ def main():
     dist.all_gather_into_tensor(Pn_all, Pg); dist.all_gather_into_tensor(An_all, Ag)
     P_all = torch.empty((world * n_per, 8), dtype=torch.float32, device=dev)
     dist.all_gather_into_tensor(P_all, Pd)
+    # 3. initialisation: every rank initialises its shard (first = rank * n_per), the gathered set == one initialisation of the whole set
+    bb_min, bb_max = [1.0, 1.0, 0.5, 0.0, 0.0, -np.pi], [59.0, 39.0, 0.5, 0.0, 0.0, np.pi]
+    cov = np.diag([0.25, 0.25, 0.0, 0.0, 0.0, 0.0685])
+    Pi, Ai = torch.empty_like(Pd), torch.empty_like(Ad)
+    Pi_all, Ai_all = torch.empty_like(P_all), torch.empty_like(A_all)
+    gathered = {}
+    for kind in ("uniform", "gaussian"):
+        if kind == "uniform":
+            up.initSamplesUniform(Pi, Ai, bb_min, bb_max, seed=17, first=rank * n_per)
+        else:
+            up.initSamples(Pi, Ai, Tgt, cov, seed=17, first=rank * n_per)
+        dist.all_gather_into_tensor(Pi_all, Pi); dist.all_gather_into_tensor(Ai_all, Ai)
+        gathered[kind] = (Pi_all.clone(), Ai_all.clone())
     rc = 0
     if rank == 0:
+        ok_init = True
+        for kind, (Pg_i, Ag_i) in gathered.items():
+            Pw, Aw = torch.empty_like(P_all), torch.empty_like(A_all)
+            if kind == "uniform":
+                up.initSamplesUniform(Pw, Aw, bb_min, bb_max, seed=17)
+            else:
+                up.initSamples(Pw, Aw, Tgt, cov, seed=17)
+            torch.cuda.synchronize()
+            ok_init = ok_init and bool(torch.equal(Pw.view(torch.int32), Pg_i.view(torch.int32)) and torch.equal(Aw.view(torch.int32), Ag_i.view(torch.int32)))
         Pr, Ar = torch.empty_like(P_all), torch.empty_like(A_all)
         up.resample(P_all, A_all, Pr, Ar, cfg, seed=99, step=1)
         torch.cuda.synchronize()
         ok_resample = bool(torch.equal(Pr, Pn_all) and torch.equal(Ar, An_all))
         changed = float((Ar[:, 0] != A_all[:, 0]).float().mean())
         line = {"world": world, "particles_per_rank": n_per, "sensor_update_shards_equal_whole": ok_update, "resample_sharded_equals_single_gpu": ok_resample,
+                "init_shards_equal_whole": ok_init,
                 "p2p_equals_allgather_on_every_rank": [bool(int(f[0])) for f in allf] if p2p_err is None else None, "p2p_error": p2p_err,
                 "fraction_of_slots_replaced": changed, "checksum": hex(int(torch.from_numpy(Pn_all.cpu().numpy().view(np.uint32).astype(np.uint64)).sum().item()) & 0xffffffffffff),
                 "exchange_bytes": {"allgather_received_per_rank": (world - 1) * n_per * 68, "p2p_read_per_rank": [int(f[1]) for f in allf]},
                 "wall_ms": {"allgather_variant": t_allgather * 1e3, "p2p_variant": None if t_p2p is None else t_p2p * 1e3}}
         print(json.dumps(line))
-        if not (ok_update and ok_resample and (p2p_err is not None or all(int(f[0]) for f in allf))):
+        if not (ok_update and ok_resample and ok_init and (p2p_err is not None or all(int(f[0]) for f in allf))):
             rc = 1
     dist.barrier()
     dist.destroy_process_group()
