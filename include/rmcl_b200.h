@@ -315,6 +315,30 @@ B2_API int b2_pf_init_uniform(b2_pf* h, b2_transform* poses_dev, b2_particle_att
 B2_API int b2_pf_init_gaussian(b2_pf* h, b2_transform* poses_dev, b2_particle_attr* attrs_dev, uint32_t first, uint32_t n, const b2_transform* pose,
                                const double cov_rowmajor[36], uint64_t seed);
 
+/* rmcl_msgs/ParticleStats (rmcl_msgs/msg/ParticleStats.msg) with its LikelihoodStats and PoseWithCovariance flattened. */
+typedef struct { double min, max, mean, sigma; } b2_likelihood_stats;
+typedef struct {
+    double position[3];                        /* pose.pose.position: x y z */
+    double orientation[4];                     /* pose.pose.orientation: x y z w */
+    double covariance[36];                     /* pose.covariance, row-major: x y z roll pitch yaw */
+    double shift;
+    double trans_bb_min[3], trans_bb_max[3];
+    b2_likelihood_stats likelihood;
+    uint64_t nparticles;
+} b2_particle_stats;                           /* 440 B */
+typedef char b2_particle_stats_is_440_bytes[sizeof(b2_particle_stats) == 440 ? 1 : -1];      /* static assert, valid C and C++ */
+/* RmclNode::estimateStats (rmcl_ros/src/nodes/rmcl_localization.cpp:642-731) on the device: the statistics of the first n particles (the
+ * caller passes n = min(n_particles, max_induction_particles), as the node slices poses(0, k)); poses/attrs are DEVICE pointers, out_host a
+ * HOST record.  Two read passes on the handle's stream, then one copy of the record to the host and a synchronise.
+ *  - likelihood: sum, sum of squares, min (from DBL_MAX), max (from 0.0) of likelihood.mean in double; mean = sum / n, sigma = sqrt(sum_sq / n
+ *    - mean^2), 0 when rounding alone makes the variance negative; shift = min.  trans_bb_min/max: the float AABB of the translations.
+ *  - pose: the weighted Markley mean with w_i = L_i / sum: t = sum w_i t_i, R = the eigenvector of the largest eigenvalue of sum w_i q_i q_i^T
+ *    (sign: w >= 0), rounded to a float Transform Tbm.
+ *  - covariance: sum w_i v_i v_i^T with v_i = (d.t, roll, pitch, yaw of d.R), d = ~Tbm * pose_i, about Tbm (no re-centring).
+ * When the likelihood sum is not > 0 or not finite (every likelihood 0), the pose and covariance are NaN, as the reference's division by zero
+ * gives them, and the rest is filled in; the call still returns B2_OK.  n == 0 and null pointers are refused before any launch. */
+B2_API int b2_pf_estimate_stats(b2_pf* h, const b2_transform* poses_dev, const b2_particle_attr* attrs_dev, uint32_t n, b2_particle_stats* out_host);
+
 /* ---------------------------------------------------------------- introspection ------------------------------ */
 /* CUDA-event timing of the kernels inside b2_rcc_correct_once*(): when enabled, events are recorded on the handle's stream around the
  * find kernel and around the reduction/Umeyama kernels; b2_rcc_last_timing returns the two durations of the most recent call (ms). */

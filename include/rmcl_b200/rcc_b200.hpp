@@ -397,6 +397,17 @@ public:
         b2_check(b2_pf_init_gaussian(h_, reinterpret_cast<b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), first, (uint32_t)poses.size(),
                                      reinterpret_cast<const b2_transform*>(&pose), covariance.data(), seed), "initSamples");
     }
+    // RmclNode::estimateStats (rmcl_localization.cpp:642-731) on the device over the induction slice the caller passes, as the node passes
+    // poses(0, k) with k = min(n_particles, max_induction_particles).  The record's fields are those of rmcl_msgs/ParticleStats
+    // (rmcl::b200::fillParticleStats in rmcl_msgs_adapters.hpp copies them into the message).
+    b2_particle_stats estimateStats(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs)
+    {
+        if (poses.size() != attrs.size()) throw std::invalid_argument("estimateStats: poses and attrs differ in size");
+        b2_particle_stats s;
+        b2_check(b2_pf_estimate_stats(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<const b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(), &s),
+                 "estimateStats");
+        return s;
+    }
 private:
     B200MapPtr map_;
     b2_pf* h_ = nullptr;

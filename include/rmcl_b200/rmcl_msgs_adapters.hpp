@@ -10,6 +10,7 @@
 //                            RangeData.mask is ignored exactly like the reference ignores it: "TODOs: use input mask values", :189-191)
 //   unpackMessage(rcc, msg)  both, for a whole Scan / Depth / O1Dn / OnDn message (or its *Stamped payload)
 //   fillSensorStats(...)     rmcl_msgs/MICPSensorStats as published at rmcl_ros/src/nodes/micp_localization.cpp:1009-1015
+//   fillParticleStats(...)   rmcl_msgs/ParticleStats as RmclNode::estimateStats returns it (rmcl_ros/src/nodes/rmcl_localization.cpp:642-731)
 #pragma once
 #include <vector>
 
@@ -66,6 +67,21 @@ template <typename StatsMsgT> inline void fillSensorStats(StatsMsgT& stats, cons
 {
     stats.total_measurements = total_measurements; stats.valid_measurements = valid_measurements;
     stats.valid_matches = Cmerged_o.n_meas; stats.cov_trace = Cmerged_o.covariance.trace();
+}
+// rmcl_msgs/ParticleStats as RmclNode::estimateStats fills it (rmcl_ros/src/nodes/rmcl_localization.cpp:677-726), from
+// PCDSensorUpdaterB200::estimateStats; the message's pose goes to publishStats (:733-795) unchanged
+template <typename StatsMsgT> inline void fillParticleStats(StatsMsgT& msg, const b2_particle_stats& s)
+{
+    msg.nparticles = s.nparticles;
+    msg.pose.pose.position.x = s.position[0]; msg.pose.pose.position.y = s.position[1]; msg.pose.pose.position.z = s.position[2];
+    msg.pose.pose.orientation.x = s.orientation[0]; msg.pose.pose.orientation.y = s.orientation[1];
+    msg.pose.pose.orientation.z = s.orientation[2]; msg.pose.pose.orientation.w = s.orientation[3];
+    for (int i = 0; i < 36; i++) msg.pose.covariance[i] = s.covariance[i];
+    msg.shift = s.shift;
+    msg.trans_bb_min.x = s.trans_bb_min[0]; msg.trans_bb_min.y = s.trans_bb_min[1]; msg.trans_bb_min.z = s.trans_bb_min[2];
+    msg.trans_bb_max.x = s.trans_bb_max[0]; msg.trans_bb_max.y = s.trans_bb_max[1]; msg.trans_bb_max.z = s.trans_bb_max[2];
+    msg.likelihood.min = s.likelihood.min; msg.likelihood.max = s.likelihood.max;
+    msg.likelihood.mean = s.likelihood.mean; msg.likelihood.sigma = s.likelihood.sigma;
 }
 
 }  // namespace b200

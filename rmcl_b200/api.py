@@ -9,7 +9,7 @@ import os
 
 import numpy as np
 
-from .synth import CROSS_STATS_DTYPE, PARTICLE_ATTR_DTYPE, RANGE_MEAS_DTYPE, TRANSFORM_DTYPE
+from .synth import CROSS_STATS_DTYPE, PARTICLE_ATTR_DTYPE, PARTICLE_STATS_DTYPE, RANGE_MEAS_DTYPE, TRANSFORM_DTYPE
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.environ.get("B2_LIB_PATH") or os.path.join(_HERE, "lib", "librmcl_b200.so")     # B2_LIB_PATH: experiment builds (scripts/)
@@ -75,7 +75,7 @@ EXPORTS = [
     "b2_pf_set_stream", "b2_pf_sensor_update", "b2_pf_sensor_update_host", "b2_kernel_launch_count", "b2_rcc_enable_timing", "b2_rcc_last_timing", "b2_pf_motion_update", "b2_pf_likelihood_stats",
     "b2_rcc_set_correspondence_type", "b2_pf_resample_gladiator", "b2_pf_gladiator_randoms", "b2_rcc_segment", "b2_mesh_create_from_file", "b2_mesh_file_load", "b2_mesh_file_free", "b2_peek_cuda_error", "b2_mesh_blob_size", "b2_mesh_export_blob", "b2_mesh_create_from_blob", "b2_mesh_refit",
     "b2_rcc_correct_once_async", "b2_rcc_correct_once_wait", "b2_micp_correct_once", "b2_rcc_set_exec_mode", "b2_debug_read_bandwidth", "b2_rcc_set_sim_options", "b2_rcc_bind_dataset", "b2_rcc_bind_model_buffers", "b2_rcc_benchmark_batch", "b2_pf_p2p_init", "b2_pf_p2p_connect", "b2_pf_p2p_publish", "b2_pf_resample_gladiator_p2p", "b2_pf_p2p_connect_local", "b2_rcc_set_cpc_options", "b2_pf_set_mapping", "b2_pf_get_mapping",
-    "b2_micp_correct", "b2_pf_init_uniform", "b2_pf_init_gaussian",
+    "b2_micp_correct", "b2_pf_init_uniform", "b2_pf_init_gaussian", "b2_pf_estimate_stats",
 ]
 
 
@@ -676,6 +676,18 @@ class PCDSensorUpdaterB200:
         _chk(load_library().b2_pf_init_gaussian(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(first), C.c_uint32(n), _p(T), _p(c),
                                                 C.c_uint64(seed)))
         return particle_poses, particle_attrs
+
+    def estimateStats(self, particle_poses, particle_attrs, max_induction_particles=50000):
+        """RmclNode::estimateStats (rmcl_ros/src/nodes/rmcl_localization.cpp:642-731) on the device: the statistics of the first
+        min(n, max_induction_particles) particles of the (n, 8) / (n, 9) float32 CUDA tensors, as a synth.PARTICLE_STATS_DTYPE record (the
+        fields of rmcl_msgs/ParticleStats): likelihood statistics, translation bounds, the weighted Markley mean pose and its 6x6 covariance."""
+        n = particle_poses.numel() * particle_poses.element_size() // 32
+        if particle_attrs.numel() * particle_attrs.element_size() != 36 * n:
+            raise ValueError(f"estimateStats: {n} poses but {particle_attrs.numel() * particle_attrs.element_size() / 36:g} attrs")
+        k = max(0, min(n, int(max_induction_particles)))
+        out = np.zeros((), PARTICLE_STATS_DTYPE)
+        _chk(load_library().b2_pf_estimate_stats(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(k), _p(out)))
+        return out
 
     def gladiatorRandoms(self, seed, step, first, n, device=None):
         """The draws resample() uses for champions first..first+n-1 (raw u32 opponent word + 6 normals each), as torch CUDA tensors."""

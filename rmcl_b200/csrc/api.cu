@@ -1650,6 +1650,8 @@ struct b2_pf {
     // sharded resampling over NVLink peer memory (b2_pf_p2p_*): own exchange buffers (cudaMalloc: exportable through CUDA IPC) + the peers' mappings
     b2_transform* x_poses = nullptr; b2_particle_attr* x_attrs = nullptr; uint32_t x_cap = 0;
     PfPeers peers{}; bool peers_open = false; DevBuf<unsigned long long> d_traffic;
+    // pose estimate (b2_pf_estimate_stats), allocated at its first call: block partials of both passes, the record, Tbm and tickets
+    DevBuf<double> d_est_part; DevBuf<PfEstimateScratch> d_est; b2_particle_stats* h_est = nullptr;
 };
 
 extern "C" int b2_pf_destroy(b2_pf* h);
@@ -1707,6 +1709,8 @@ extern "C" int b2_pf_destroy(b2_pf* h)
     if (h->x_poses) cudaFree(h->x_poses);
     if (h->x_attrs) cudaFree(h->x_attrs);
     h->d_traffic.release();
+    h->d_est_part.release(); h->d_est.release();
+    if (h->h_est) cudaFreeHost(h->h_est);
     b2_mesh* map = h->map;
     delete h;
     (void)cudaGetLastError();
@@ -2126,5 +2130,27 @@ extern "C" int b2_pf_likelihood_stats(b2_pf* h, const b2_particle_attr* attrs_de
     }
     if (sum_out) *sum_out = s;
     if (max_out) *max_out = m;
+    return B2_OK;
+}
+
+// RmclNode::estimateStats (rmcl_localization.cpp:642-731): two read passes, Tbm handed from the first to the second in device memory
+extern "C" int b2_pf_estimate_stats(b2_pf* h, const b2_transform* poses_dev, const b2_particle_attr* attrs_dev, uint32_t n, b2_particle_stats* out_host)
+{
+    NOTNULL(h); NOTNULL(poses_dev); NOTNULL(attrs_dev); NOTNULL(out_host);
+    if (n == 0) return fail(B2_ERR_INVALID, "estimate stats: no particles (n = 0)");
+    CU(cudaSetDevice(h->map->device));
+    const uint32_t grid = std::min<uint32_t>((uint32_t)h->n_sm * 4u, (n + 255) / 256);
+    if (!h->d_est.p) {
+        RES(h->d_est_part.reserve((size_t)B2_EST_NV_MAX * 4 * (size_t)h->n_sm)); RES(h->d_est.reserve(1));
+        CU(cudaMemset(h->d_est.p, 0, sizeof(PfEstimateScratch)));
+        CU(cudaMallocHost((void**)&h->h_est, sizeof(b2_particle_stats)));
+    }
+    k_pf_estimate_moments<<<grid, 256, 0, h->stream>>>(poses_dev, attrs_dev, n, h->d_est_part.p, h->d_est.p);
+    LAUNCHED();
+    k_pf_estimate_cov<<<grid, 256, 0, h->stream>>>(poses_dev, attrs_dev, n, h->d_est_part.p, h->d_est.p);
+    LAUNCHED();
+    CU(cudaMemcpyAsync(h->h_est, &h->d_est.p->rec, sizeof(b2_particle_stats), cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    *out_host = *h->h_est;
     return B2_OK;
 }

@@ -1313,4 +1313,248 @@ __global__ void __launch_bounds__(256) k_pf_stats(const b2_particle_attr* __rest
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Pose estimate of the particle set: RmclNode::estimateStats (rmcl_ros/src/nodes/rmcl_localization.cpp:642-731) in two read passes.
+// Pass 1 (k_pf_estimate_moments): likelihood sums, min / max, translation AABB, sum L t and sum L q q^T; its last block forms the weighted
+// Markley mean Tbm (SURVEY decision E1).  Pass 2 (k_pf_estimate_cov): the 6x6 covariance of (~Tbm * pose) about Tbm (decision E2).  Weights
+// are w_i = L_i / L_sum; the sums are taken over L_i and divided by L_sum once, in FP64.
+// ---------------------------------------------------------------------------------------------------------------------
+#define B2_JACOBI_SWEEPS 16
+B2_DEV double f64_from_bits(unsigned long long u)
+{
+#if B2_ON_DEVICE
+    return __longlong_as_double((long long)u);
+#else
+    double d; memcpy(&d, &u, 8); return d;
+#endif
+}
+B2_DEV double f64_nan() { return f64_from_bits(0x7ff8000000000000ull); }
+B2_DEV double f64_inf() { return f64_from_bits(0x7ff0000000000000ull); }
+// eigenvector of the largest eigenvalue of a symmetric 4x4 matrix (row-major, FP64): cyclic Jacobi, at most B2_JACOBI_SWEEPS sweeps; a
+// non-finite entry gives a NaN vector.  Sign: w >= 0, and when w == 0 the first non-zero component is positive.
+B2_DEV void sym4_top_eigvec(const double* Ain, double v[4], double* lambda)
+{
+    // fully unrolled so that A and V stay in registers on the device
+    double A[4][4], V[4][4];
+    bool finite = true;
+    #pragma unroll
+    for (int i = 0; i < 4; i++)
+        #pragma unroll
+        for (int j = 0; j < 4; j++) { A[i][j] = Ain[4 * i + j]; V[i][j] = i == j ? 1.0 : 0.0; finite = finite && A[i][j] - A[i][j] == 0.0; }
+    if (!finite) {
+        v[0] = v[1] = v[2] = v[3] = *lambda = f64_nan();
+        return;
+    }
+    for (int sweep = 0; sweep < B2_JACOBI_SWEEPS; sweep++) {
+        double off = 0.0;
+        #pragma unroll
+        for (int p = 0; p < 3; p++)
+            #pragma unroll
+            for (int q = p + 1; q < 4; q++) off += A[p][q] * A[p][q];
+        if (!(off > 0.0)) break;
+        #pragma unroll
+        for (int p = 0; p < 3; p++)
+            #pragma unroll
+            for (int q = p + 1; q < 4; q++) {
+                const double apq = A[p][q];
+                if (apq == 0.0) continue;
+                // rotation J (J_pp = J_qq = c, J_pq = s, J_qp = -s) with (J^T A J)_pq = 0; t = tan of the smaller rotation angle
+                const double theta = (A[q][q] - A[p][p]) / (2.0 * apq);
+                const double t = fabs(theta) > 1e150 ? 0.5 / theta : (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
+                const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+                #pragma unroll
+                for (int k = 0; k < 4; k++) {
+                    const double akp = A[k][p], akq = A[k][q];
+                    A[k][p] = c * akp - s * akq; A[k][q] = s * akp + c * akq;
+                }
+                #pragma unroll
+                for (int k = 0; k < 4; k++) {
+                    const double apk = A[p][k], aqk = A[q][k];
+                    A[p][k] = c * apk - s * aqk; A[q][k] = s * apk + c * aqk;
+                }
+                A[p][q] = A[q][p] = 0.0;
+                #pragma unroll
+                for (int k = 0; k < 4; k++) {
+                    const double vkp = V[k][p], vkq = V[k][q];
+                    V[k][p] = c * vkp - s * vkq; V[k][q] = s * vkp + c * vkq;
+                }
+            }
+    }
+    double best = A[0][0], e[4] = {V[0][0], V[1][0], V[2][0], V[3][0]};
+    #pragma unroll
+    for (int i = 1; i < 4; i++)
+        if (A[i][i] > best) { best = A[i][i]; e[0] = V[0][i]; e[1] = V[1][i]; e[2] = V[2][i]; e[3] = V[3][i]; }
+    double sg = e[3] > 0.0 ? 1.0 : e[3] < 0.0 ? -1.0 : 0.0;
+    #pragma unroll
+    for (int i = 0; i < 3; i++) if (sg == 0.0) sg = e[i] > 0.0 ? 1.0 : e[i] < 0.0 ? -1.0 : 0.0;
+    if (sg == 0.0) sg = 1.0;
+    #pragma unroll
+    for (int i = 0; i < 4; i++) v[i] = sg * e[i];
+    *lambda = best;
+}
+// the 6-vector of one particle about the mean: d = ~Tbm * pose in rmagine's float Transform algebra, (d.t, roll, pitch, yaw of d.R)
+B2_DEV void pf_deviation(const Tf& Tbm_inv, const Tf& pose, float v[6])
+{
+    const Tf d = tf_mul(Tbm_inv, pose);
+    v[0] = d.t.x; v[1] = d.t.y; v[2] = d.t.z;
+    quat_to_euler(d.R, v[3], v[4], v[5]);
+}
+// pass-1 accumulator slots (FP64): the sums, then min / max of L, then the AABB
+#define B2_EST_SUM_L 0
+#define B2_EST_SUM_L2 1
+#define B2_EST_SUM_LT 2          /* 3 */
+#define B2_EST_SUM_LQQ 5         /* 10: xx xy xz xw yy yz yw zz zw ww */
+#define B2_EST_NSUM 15
+#define B2_EST_MIN_L 15
+#define B2_EST_MAX_L 16
+#define B2_EST_BB_MIN 17         /* 3 */
+#define B2_EST_BB_MAX 20         /* 3 */
+#define B2_EST_NV1 23
+#define B2_EST_NV2 21            /* pass 2: upper triangle of sum L v v^T, row by row */
+#define B2_EST_NV_MAX 23          /* partials per block: the larger of the two passes */
+struct PfEstimateScratch {
+    b2_particle_stats rec;       // the result, copied to the host after pass 2
+    b2_transform Tbm;            // float mean written by pass 1, read by pass 2
+    double L_sum;                // pass 1's sum of L (the weights' denominator)
+    unsigned int ticket[2];      // one last-block ticket per pass
+};
+// pass 1 slots below B2_EST_NSUM and every pass-2 slot are sums; min and max ignore NaN like std::min / std::max with the running value first
+template <bool SUMS> B2_DEV double est_combine(int slot, double a, double b)
+{
+    if (SUMS || slot < B2_EST_NSUM) return a + b;
+    if (slot == B2_EST_MIN_L || (slot >= B2_EST_BB_MIN && slot < B2_EST_BB_MAX)) return b < a ? b : a;
+    return a < b ? b : a;
+}
+template <bool SUMS> B2_DEV double est_identity(int slot)
+{
+    if (SUMS || slot < B2_EST_NSUM) return 0.0;
+    return (slot == B2_EST_MIN_L || (slot >= B2_EST_BB_MIN && slot < B2_EST_BB_MAX)) ? f64_inf() : -f64_inf();
+}
+#ifdef __CUDACC__
+template <bool SUMS> __device__ __forceinline__ double est_warp(int slot, double v)
+{
+    #pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = est_combine<SUMS>(slot, v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
+// block reduction of NV per-thread values to partials[blockIdx.x * NV + slot]; then the last block reduces the partials in a fixed order
+// (warp w handles slots w, w + 8, ...; lane l takes blocks l, l + 32, ...; then a warp butterfly) into tot[NV].  True in the last block only.
+template <int NV, bool SUMS>
+__device__ __forceinline__ bool est_grid_reduce(double (&acc)[NV], double* __restrict__ partials, unsigned int* __restrict__ ticket, double* s_w /* [8][NV] */, double* tot,
+                                                bool& is_last)
+{
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    #pragma unroll
+    for (int j = 0; j < NV; j++) acc[j] = est_warp<SUMS>(j, acc[j]);
+    if (lane == 0) for (int j = 0; j < NV; j++) s_w[warp * NV + j] = acc[j];
+    __syncthreads();
+    if (threadIdx.x < NV) {
+        double a = s_w[threadIdx.x];
+        for (int w = 1; w < 8; w++) a = est_combine<SUMS>(threadIdx.x, a, s_w[w * NV + threadIdx.x]);
+        partials[(size_t)blockIdx.x * NV + threadIdx.x] = a;
+        __threadfence();
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) is_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+    __syncthreads();
+    if (!is_last) return false;
+    __threadfence();
+    for (int j = warp; j < NV; j += 8) {
+        double a = est_identity<SUMS>(j);
+        for (uint32_t b = lane; b < gridDim.x; b += 32) a = est_combine<SUMS>(j, a, __ldcg(partials + (size_t)b * NV + j));
+        a = est_warp<SUMS>(j, a);
+        if (lane == 0) tot[j] = a;
+    }
+    __syncthreads();
+    return true;
+}
+// pass 1: 36 B read per particle (32 B pose, the 4 B likelihood.mean)
+__global__ void __launch_bounds__(256) k_pf_estimate_moments(const b2_transform* __restrict__ poses, const b2_particle_attr* __restrict__ attrs, uint32_t k,
+                                                             double* __restrict__ partials, PfEstimateScratch* __restrict__ sc)
+{
+    __shared__ double s_w[8 * B2_EST_NV1], tot[B2_EST_NV1];
+    __shared__ bool is_last;
+    double acc[B2_EST_NV1];
+    #pragma unroll
+    for (int j = 0; j < B2_EST_NSUM; j++) acc[j] = 0.0;
+    acc[B2_EST_MIN_L] = 1.7976931348623157e308; acc[B2_EST_MAX_L] = 0.0;                  // L_min = DBL_MAX, L_max = 0.0 (:664-665)
+    #pragma unroll
+    for (int c = 0; c < 3; c++) { acc[B2_EST_BB_MIN + c] = 3.402823466e38; acc[B2_EST_BB_MAX + c] = -3.402823466e38; }   // rm::AABB::init [RM-recalled]
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < k; i += gridDim.x * blockDim.x) {
+        const Tf P = tf_load(poses + i);
+        const double L = (double)attrs[i].likelihood.mean;
+        acc[B2_EST_SUM_L] += L; acc[B2_EST_SUM_L2] += L * L;
+        acc[B2_EST_MIN_L] = est_combine<false>(B2_EST_MIN_L, acc[B2_EST_MIN_L], L); acc[B2_EST_MAX_L] = est_combine<false>(B2_EST_MAX_L, acc[B2_EST_MAX_L], L);
+        const double t[3] = {(double)P.t.x, (double)P.t.y, (double)P.t.z}, q[4] = {(double)P.R.x, (double)P.R.y, (double)P.R.z, (double)P.R.w};
+        #pragma unroll
+        for (int c = 0; c < 3; c++) {
+            acc[B2_EST_SUM_LT + c] += L * t[c];
+            acc[B2_EST_BB_MIN + c] = est_combine<false>(B2_EST_BB_MIN, acc[B2_EST_BB_MIN + c], t[c]);
+            acc[B2_EST_BB_MAX + c] = est_combine<false>(B2_EST_BB_MAX, acc[B2_EST_BB_MAX + c], t[c]);
+        }
+        int s = B2_EST_SUM_LQQ;
+        #pragma unroll
+        for (int a = 0; a < 4; a++) {
+            const double La = L * q[a];
+            #pragma unroll
+            for (int b = a; b < 4; b++) acc[s++] += La * q[b];
+        }
+    }
+    if (!est_grid_reduce<B2_EST_NV1, false>(acc, partials, sc->ticket, s_w, tot, is_last)) return;
+    if (threadIdx.x != 0) return;
+    const double Ls = tot[B2_EST_SUM_L], n = (double)k, mean = Ls / n, var = tot[B2_EST_SUM_L2] / n - mean * mean;
+    const bool ok = Ls > 0.0 && Ls < f64_inf();                                             // else the reference divides by zero (decision E3)
+    const double nan = f64_nan();
+    double M[16];
+    int s = B2_EST_SUM_LQQ;
+    for (int a = 0; a < 4; a++) for (int b = a; b < 4; b++) { M[4 * a + b] = M[4 * b + a] = ok ? tot[s] / Ls : nan; s++; }
+    double qv[4], lambda;
+    sym4_top_eigvec(M, qv, &lambda);
+    b2_transform T; memset(&T, 0, sizeof(T));
+    T.R.x = (float)qv[0]; T.R.y = (float)qv[1]; T.R.z = (float)qv[2]; T.R.w = (float)qv[3];
+    T.t.x = (float)(ok ? tot[B2_EST_SUM_LT] / Ls : nan); T.t.y = (float)(ok ? tot[B2_EST_SUM_LT + 1] / Ls : nan); T.t.z = (float)(ok ? tot[B2_EST_SUM_LT + 2] / Ls : nan);
+    sc->Tbm = T; sc->L_sum = Ls;
+    b2_particle_stats& r = sc->rec;
+    r.position[0] = T.t.x; r.position[1] = T.t.y; r.position[2] = T.t.z;
+    r.orientation[0] = T.R.x; r.orientation[1] = T.R.y; r.orientation[2] = T.R.z; r.orientation[3] = T.R.w;
+    r.shift = tot[B2_EST_MIN_L];
+    for (int c = 0; c < 3; c++) { r.trans_bb_min[c] = (double)(float)tot[B2_EST_BB_MIN + c]; r.trans_bb_max[c] = (double)(float)tot[B2_EST_BB_MAX + c]; }
+    r.likelihood.min = tot[B2_EST_MIN_L]; r.likelihood.max = tot[B2_EST_MAX_L];
+    r.likelihood.mean = mean; r.likelihood.sigma = var < 0.0 ? 0.0 : sqrt(var);           // a rounding-only negative variance gives 0 (decision E4)
+    r.nparticles = k;
+    sc->ticket[0] = 0u;
+}
+// pass 2: the same 36 B per particle again, and Tbm from pass 1 (device memory)
+__global__ void __launch_bounds__(256) k_pf_estimate_cov(const b2_transform* __restrict__ poses, const b2_particle_attr* __restrict__ attrs, uint32_t k,
+                                                         double* __restrict__ partials, PfEstimateScratch* __restrict__ sc)
+{
+    __shared__ double s_w[8 * B2_EST_NV2], tot[B2_EST_NV2];
+    __shared__ bool is_last;
+    double acc[B2_EST_NV2];
+    #pragma unroll
+    for (int j = 0; j < B2_EST_NV2; j++) acc[j] = 0.0;
+    const Tf Tinv = tf_inv(tf_from_pod(sc->Tbm));
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < k; i += gridDim.x * blockDim.x) {
+        const double L = (double)attrs[i].likelihood.mean;
+        float v[6];
+        pf_deviation(Tinv, tf_load(poses + i), v);
+        int s = 0;
+        #pragma unroll
+        for (int a = 0; a < 6; a++) {
+            const double La = L * (double)v[a];
+            #pragma unroll
+            for (int b = a; b < 6; b++) acc[s++] += La * (double)v[b];
+        }
+    }
+    if (!est_grid_reduce<B2_EST_NV2, true>(acc, partials, sc->ticket + 1, s_w, tot, is_last)) return;
+    if (threadIdx.x != 0) return;
+    const double Ls = sc->L_sum;
+    const bool ok = Ls > 0.0 && Ls < f64_inf();
+    const double nan = f64_nan();
+    int s = 0;
+    for (int a = 0; a < 6; a++) for (int b = a; b < 6; b++) { sc->rec.covariance[6 * a + b] = sc->rec.covariance[6 * b + a] = ok ? tot[s] / Ls : nan; s++; }
+    sc->ticket[1] = 0u;
+}
+#endif
+
 #include "icp_loop.cuh"

@@ -291,6 +291,11 @@ PARTICLE_ATTR_DTYPE = np.dtype([("likelihood", GAUSSIAN1D_DTYPE), ("state_sigma"
 RANGE_MEAS_DTYPE = np.dtype([("orig", np.float32, 3), ("dir", np.float32, 3), ("range", np.float32), ("cov", np.float32, 9)])
 assert TRANSFORM_DTYPE.itemsize == 32 and CROSS_STATS_DTYPE.itemsize == 64
 assert PARTICLE_ATTR_DTYPE.itemsize == 36 and RANGE_MEAS_DTYPE.itemsize == 64
+# rmcl_msgs/ParticleStats as b2_particle_stats (include/rmcl_b200.h): what PCDSensorUpdaterB200.estimateStats returns
+LIKELIHOOD_STATS_DTYPE = np.dtype([("min", np.float64), ("max", np.float64), ("mean", np.float64), ("sigma", np.float64)])
+PARTICLE_STATS_DTYPE = np.dtype([("position", np.float64, 3), ("orientation", np.float64, 4), ("covariance", np.float64, 36), ("shift", np.float64),
+                                 ("trans_bb_min", np.float64, 3), ("trans_bb_max", np.float64, 3), ("likelihood", LIKELIHOOD_STATS_DTYPE), ("nparticles", np.uint64)])
+assert PARTICLE_STATS_DTYPE.itemsize == 440
 
 
 def quat_from_rpy(roll, pitch, yaw):
