@@ -507,14 +507,20 @@ O1DnCorrectorB200 = RCCB200O1Dn
 OnDnCorrectorB200 = RCCB200OnDn
 
 
-def micp_correct_once(sensors, Tbo, Tom, iterations=5, convergence_progress=0.0, merge_weights=None, ranges=None):
-    """MICPLocalizationNode::correctOnce over all sensors (micp_localization.cpp:899-984): `sensors` RCCB200 / CPCB200 handles on one device,
-    `Tbo` one Transform per sensor, `merge_weights` the sensors' merge_weight_multiplier (MICPSensor.hpp:103), `ranges` optional per-sensor
-    host scans (None entries keep the resident dataset).  -> (Tom_new, T_onew_oold, Cmerged_o)."""
+def _sensor_args(sensors, Tbo, merge_weights):
+    """-> (n, handle array, Tbo records, merge weights or None) of a multi-sensor call"""
     n = len(sensors)
     hs = (C.c_void_p * n)(*[s._h for s in sensors])
     Tb = np.ascontiguousarray(np.asarray(Tbo, TRANSFORM_DTYPE).reshape(n))
     w = None if merge_weights is None else np.ascontiguousarray(merge_weights, np.float64).reshape(n)
+    return n, hs, Tb, w
+
+
+def micp_correct_once(sensors, Tbo, Tom, iterations=5, convergence_progress=0.0, merge_weights=None, ranges=None):
+    """MICPLocalizationNode::correctOnce over all sensors (micp_localization.cpp:899-984): `sensors` RCCB200 / CPCB200 handles on one device,
+    `Tbo` one Transform per sensor, `merge_weights` the sensors' merge_weight_multiplier (MICPSensor.hpp:103), `ranges` optional per-sensor
+    host scans (None entries keep the resident dataset).  -> (Tom_new, T_onew_oold, Cmerged_o)."""
+    n, hs, Tb, w = _sensor_args(sensors, Tbo, merge_weights)
     keep, rp = [], None
     if ranges is not None:
         rp = (C.c_void_p * n)()
@@ -546,10 +552,7 @@ def micp_correct(sensors, Tbo, Tom, n_corrections=3, iterations=5, convergence_p
     each step traces at the pose the previous one produced and gates with the max_dist its convergence progress gives, without the host in
     between.  Runs on the sensors' resident datasets (setRanges / setDataset / bindDataset first).  -> (Tom, convergence_progress, steps) with
     `steps` a MICP_STEP_DTYPE record array, one per correction."""
-    n = len(sensors)
-    hs = (C.c_void_p * n)(*[s._h for s in sensors])
-    Tb = np.ascontiguousarray(np.asarray(Tbo, TRANSFORM_DTYPE).reshape(n))
-    w = None if merge_weights is None else np.ascontiguousarray(merge_weights, np.float64).reshape(n)
+    n, hs, Tb, w = _sensor_args(sensors, Tbo, merge_weights)
     T = np.array(_tf(Tom), copy=True)
     cp = C.c_double(float(convergence_progress))
     steps = np.zeros(int(n_corrections), MICP_STEP_DTYPE)

@@ -914,12 +914,73 @@ extern "C" int b2_rcc_download_dataset(b2_rcc* h, float* p, uint8_t* m)
 // ---------------------------------------------------------------------------------------------------------------------
 struct SensorCall { b2_rcc* h; b2_transform Tbo; double weight; const float* ranges_host; uint32_t n_ranges; };
 
-static void fill_sensor_frames(IcpSensor& S, const b2_transform& Tbo, const b2_transform& Tsb)
+// Tbm = Tom * Tbo (MICPSensor.hpp:148), same inline ops as the kernels
+static b2_transform body_in_map(const b2_transform& Tom, const b2_transform& Tbo)
 {
-    const Tf Tos = tf_mul(tf_from_pod(Tbo), tf_from_pod(Tsb));
-    memset(&S.Tos, 0, sizeof(S.Tos)); memset(&S.Tso, 0, sizeof(S.Tso));
-    tf_store(&S.Tos, Tos); tf_store(&S.Tso, tf_inv(Tos)); quat_to_mat(Tos.R, S.Ros);
+    b2_transform Tbm; memset(&Tbm, 0, sizeof(Tbm)); tf_store(&Tbm, tf_mul(tf_from_pod(Tom), tf_from_pod(Tbo))); return Tbm;
 }
+
+// Sensor list of b2_micp_correct_once / b2_micp_correct (`fn`, messages prefixed `what`): 1..B2_MAX_SENSORS distinct handles, nothing in flight
+// on the lead.  ranges_host NULL: every sensor keeps its dataset.
+static int sensor_list(const char* fn, const char* what, b2_rcc* const* sensors, const b2_transform* Tbo, const double* merge_weights,
+                       const float* const* ranges_host, uint32_t n_sensors, SensorCall* sc)
+{
+    if (n_sensors == 0 || n_sensors > B2_MAX_SENSORS) return fail(B2_ERR_INVALID, "%s: %u sensors (1..%d supported per call)", what, n_sensors, B2_MAX_SENSORS);
+    for (uint32_t k = 0; k < n_sensors; k++) {
+        if (!sensors[k]) return fail(B2_ERR_INVALID, "%s: null argument '%s'", fn, "sensors[k]");
+        for (uint32_t j = 0; j < k; j++) if (sensors[j] == sensors[k]) return fail(B2_ERR_INVALID, "%s: sensor %u given twice", what, k);
+        sc[k].h = sensors[k]; sc[k].Tbo = Tbo[k]; sc[k].weight = merge_weights ? merge_weights[k] : 1.0;
+        sc[k].ranges_host = ranges_host ? ranges_host[k] : nullptr; sc[k].n_ranges = sc[k].ranges_host ? sensors[k]->n : 0;
+    }
+    const b2_rcc* H = sc[0].h;
+    CU(cudaSetDevice(H->map->device));
+    if (!H->pending.empty()) return fail(B2_ERR_INVALID, "%s: asynchronous calls are still in flight on the lead handle, collect them first", what);
+    return B2_OK;
+}
+
+// Checks every sensor of a call and changes none, so that a refused call leaves all handles as they were.  *pairs = correspondences of all.
+static int check_sensors(const SensorCall* sc, uint32_t ns, const char* what, uint64_t* pairs)
+{
+    *pairs = 0;
+    for (uint32_t k = 0; k < ns; k++) {
+        const b2_rcc* h = sc[k].h;
+        if (h->map->device != sc[0].h->map->device) return fail(B2_ERR_INVALID, "%s: all sensors must live on the same device", what);
+        const bool cpc = h->corr_type == B2_CORR_CPC;
+        if (sc[k].ranges_host && cpc) return fail(B2_ERR_INVALID, "correctOnce(ranges) needs ray-casting correspondences (the handle is in closest-point mode)");
+        if (!cpc && !h->has_model) return fail(B2_ERR_INVALID, "%s before setModel", what);
+        if (sc[k].ranges_host && sc[k].n_ranges != h->n) return fail(B2_ERR_INVALID, "ranges size %u != model size %u", sc[k].n_ranges, h->n);
+        if (!sc[k].ranges_host && h->n_dataset != h->work_n()) return fail(B2_ERR_INVALID, "dataset size %u != model size %u", h->n_dataset, h->n);
+        *pairs += h->work_n();
+    }
+    return B2_OK;
+}
+
+// into_lead: the lead stream waits for the other sensors' streams (pending set_ranges / set_dataset copies); otherwise they wait for the lead
+// stream, so that later work on them sees the model buffers the call wrote
+static int join_streams(const SensorCall* sc, uint32_t ns, bool into_lead)
+{
+    for (uint32_t k = 1; k < ns; k++) {
+        b2_rcc* h = sc[k].h;
+        CU(cudaEventRecord(h->ev_join, into_lead ? h->stream : sc[0].h->stream));
+        CU(cudaStreamWaitEvent(into_lead ? sc[0].h->stream : h->stream, h->ev_join, 0));
+    }
+    return B2_OK;
+}
+
+// h's find on the lead H's stream, which carries all launches of a call.  arm_pdl: the loop follows this find and may start early behind it,
+// programmatically (B2_PDL, default 1; behind the last find only: event records / other kernels in between would serialise them anyway)
+static int find_on_lead(b2_rcc* H, b2_rcc* h, const b2_transform* Tbm_host, const IcpState* icp_dev, bool arm_pdl)
+{
+    static const int use_pdl = [] { const char* e = getenv("B2_PDL"); return e ? atoi(e) : 1; }();
+    const cudaStream_t own = h->stream;
+    h->stream = H->stream; h->pdl_next = arm_pdl && use_pdl && h->corr_type == B2_CORR_RCC;
+    const int rc = launch_find(h, Tbm_host, icp_dev);
+    h->pdl_next = false; h->stream = own;
+    return rc;
+}
+
+// sequence number of the next k_icp_loop launch; never 0, which the result chunks hold before the first launch
+static unsigned int next_seq(b2_rcc* H) { unsigned int seq = ++H->seq; if (seq == 0) seq = ++H->seq; return seq; }
 
 // slot < 0: no result chunks in mapped host memory (chain steps: their results stay on the device)
 static int launch_icp_loop(b2_rcc* H, const IcpLaunch& L, int grid, size_t smem, int mode, bool pdl, int slot)
@@ -959,18 +1020,15 @@ static int launch_icp_loop(b2_rcc* H, const IcpLaunch& L, int grid, size_t smem,
     return B2_OK;
 }
 
-// k_icp_loop launched programmatically behind the last find (B2_PDL, default 1)
-static bool pdl_enabled()
+// k_icp_loop's launch L for `total` pairs and its grid (returned).  Blocks per sensor: in proportion to the pairs, at least one for each sensor
+// with pairs.  A sensor without pairs gets none, so the other sensors' pairs are summed by exactly the blocks a call without it would use: its
+// presence cannot change a bit of the result.  Then per sensor the pairs per thread in shared memory, merge weight, range limits, frames and
+// dataset; the gate (max_dist) is the caller's.
+static int loop_layout(const b2_rcc* H, const SensorCall* sc, uint32_t ns, uint64_t total, const b2_transform& Tom, uint32_t iterations, IcpLaunch& L)
 {
-    static const int use_pdl = [] { const char* e = getenv("B2_PDL"); return e ? atoi(e) : 1; }();
-    return use_pdl != 0;
-}
-
-// Grid of k_icp_loop and blocks per sensor: in proportion to the pairs, at least one for each sensor with pairs.  A sensor without pairs gets
-// none, so the other sensors' pairs are summed by exactly the blocks a call without it would use: its presence cannot change a bit of the result.
-static int loop_blocks(const b2_rcc* H, const SensorCall* sc, uint32_t ns, uint64_t total, uint32_t* nblk)
-{
-    uint32_t ns_busy = 0;
+    memset(&L, 0, sizeof(L));
+    L.Tom = Tom; L.n_sensors = ns; L.iterations = iterations;
+    uint32_t ns_busy = 0, nblk[B2_MAX_SENSORS];
     for (uint32_t k = 0; k < ns; k++) if (sc[k].h->work_n() > 0) ns_busy++;
     const int grid = std::min<int>(H->fused_grid, (int)std::max<uint64_t>((total + B2_ICP_BLOCK - 1) / B2_ICP_BLOCK, ns_busy));
     int assigned = 0;
@@ -984,7 +1042,70 @@ static int loop_blocks(const b2_rcc* H, const SensorCall* sc, uint32_t ns, uint6
         for (uint32_t k = 0; k < ns; k++) { if (!nblk[k]) continue; const double l = (double)sc[k].h->work_n() / nblk[k]; if (l > load) { load = l; best = k; } }
         nblk[best]++; assigned++;
     }
+    uint32_t blk0 = 0;
+    for (uint32_t k = 0; k < ns; k++) {
+        const b2_rcc* h = sc[k].h;
+        IcpSensor& S = L.s[k];
+        S.n = h->work_n(); S.blk0 = blk0; S.nblk = nblk[k]; blk0 += nblk[k];
+        const uint32_t stride = S.nblk * B2_ICP_BLOCK, per_thread = stride ? (S.n + stride - 1) / stride : 0u;
+        S.smem_u = per_thread > B2_ICP_REG_PAIRS ? std::min<uint32_t>(per_thread - B2_ICP_REG_PAIRS, (uint32_t)H->smem_u_cap) : 0u;
+        L.smem_u_max = std::max(L.smem_u_max, S.smem_u);
+        S.merge_weight = sc[k].weight; S.range_min = h->range_min; S.range_max = h->range_max;
+        const Tf Tos = tf_mul(tf_from_pod(sc[k].Tbo), tf_from_pod(h->Tsb));
+        memset(&S.Tos, 0, sizeof(S.Tos)); memset(&S.Tso, 0, sizeof(S.Tso));
+        tf_store(&S.Tos, Tos); tf_store(&S.Tso, tf_inv(Tos)); quat_to_mat(Tos.R, S.Ros);
+        S.dpts = h->dpts(); S.dmask = h->dmask();
+    }
     return grid;
+}
+
+// k_icp_loop behind the finds of a call: their model buffers (a find may have grown them), tile-sort fields, dynamic shared memory (*smem_out),
+// sequence number; a programmatic launch if the last find armed it and pdl_ok.  Records the geometry for b2_rcc_debug_loop_geometry.
+static int launch_loop_after_finds(b2_rcc* H, const SensorCall* sc, uint32_t ns, IcpLaunch& L, int grid, int mode, bool pdl_ok, int slot, size_t* smem_out)
+{
+    uint32_t sort_tiles_max = 0;
+    for (uint32_t k = 0; k < ns; k++) {
+        const b2_rcc* h = sc[k].h;
+        IcpSensor& S = L.s[k];
+        S.mpts = h->mpts(); S.mnrm = h->mnrm(); S.mmask = h->mhits();
+        S.tile_cost = nullptr; S.tile_perm = nullptr; S.n_tiles = 0;
+        if (h->corr_type == B2_CORR_RCC && h->cost_tiles && L.iterations >= 3u) {
+            S.tile_cost = h->d_tile_cost.p; S.tile_perm = h->d_tile_perm.p; S.n_tiles = h->cost_tiles;
+            sort_tiles_max = std::max(sort_tiles_max, h->cost_tiles);
+        }
+    }
+    size_t smem = (size_t)L.smem_u_max * 9 * B2_ICP_BLOCK * sizeof(float);
+    if (sort_tiles_max) {
+        // the tile sort stages the durations behind the pair cache (2 bytes per tile); no room (very large scans): no sort, the order stays as it is
+        const size_t want = smem + 2 * (size_t)sort_tiles_max;
+        if (want <= (size_t)H->smem_u_cap * 9 * B2_ICP_BLOCK * sizeof(float)) smem = want;
+        else for (uint32_t k = 0; k < ns; k++) { L.s[k].tile_cost = nullptr; L.s[k].tile_perm = nullptr; L.s[k].n_tiles = 0; }
+    }
+    if (smem_out) *smem_out = smem;
+    L.seq = next_seq(H);
+    const bool pdl = mode == 2 && sc[ns - 1].h->pdl_armed && pdl_ok;
+    sc[ns - 1].h->pdl_armed = false;
+    RES(launch_icp_loop(H, L, grid, smem, mode, pdl, slot));
+    memset(H->loop_geom, 0, sizeof(H->loop_geom));
+    H->loop_geom[0] = ns; H->loop_geom[1] = (uint32_t)grid;
+    for (uint32_t k = 0; k < ns; k++) { uint32_t* g = H->loop_geom + 2 + 4 * k; g[0] = L.s[k].n; g[1] = L.s[k].blk0; g[2] = L.s[k].nblk; g[3] = L.s[k].smem_u; }
+    return B2_OK;
+}
+
+// Did the grid-wide exchange of a mode-2 loop give up (its blocks were not co-resident: SMs held by something that itself waits; or code 2: a
+// block's partial sum left the fixed-point range of the atomic exchange)?  That is a scheduling condition, not an error: the abort word and the
+// accumulator words the aborted rounds left inconsistent are reset, and the caller runs the work again through the cooperative launch, whose
+// co-residency the driver guarantees and which exchanges FP64.
+static int exchange_aborted(b2_rcc* H, bool* aborted)
+{
+    unsigned int bar_state[2] = {0u, 0u};
+    CU(cudaMemcpy(bar_state, H->d_bar.p, sizeof(bar_state), cudaMemcpyDeviceToHost));
+    *aborted = bar_state[1] != 0u;
+    if (*aborted) {
+        CU(cudaMemset(H->d_bar.p + 1, 0, sizeof(unsigned int)));
+        CU(cudaMemset(H->d_slots.p, 0, ((size_t)B2_ICP_ACC_WORDS + B2_ICP_BASE_WORDS) * sizeof(unsigned long long)));
+    }
+    return B2_OK;
 }
 
 static int micp_enqueue(SensorCall* sc, uint32_t ns, const b2_transform* Tom, uint32_t iterations, double cp)
@@ -993,28 +1114,19 @@ static int micp_enqueue(SensorCall* sc, uint32_t ns, const b2_transform* Tom, ui
     if (H->pending.size() >= B2_RING) return fail(B2_ERR_INVALID, "correctOnce: %d asynchronous calls are in flight already, collect one first (b2_rcc_correct_once_wait)", B2_RING);
     static const int use_zc = [] { const char* e = getenv("B2_ZEROCOPY"); return e ? atoi(e) : 1; }();
     static const int use_spin = [] { const char* e = getenv("B2_SPIN"); return e ? atoi(e) : 1; }();
-    const bool use_pdl = pdl_enabled();
     int mode = H->exec_mode;
     if (H->fused_grid <= 0) mode = 0;
     if (ns > 1 && mode == 0) mode = H->fused_grid > 0 ? 1 : 0;
     if (ns > 1 && mode == 0) return fail(B2_ERR_UNSUPPORTED, "multi-sensor correctOnce needs a device with cooperative launch");
     uint64_t total = 0;
-    for (uint32_t k = 0; k < ns; k++) {
-        b2_rcc* h = sc[k].h;
-        if (h->map->device != H->map->device) return fail(B2_ERR_INVALID, "correctOnce: all sensors must live on the same device");
-        const bool cpc = h->corr_type == B2_CORR_CPC;
-        if (sc[k].ranges_host && cpc) return fail(B2_ERR_INVALID, "correctOnce(ranges) needs ray-casting correspondences (the handle is in closest-point mode)");
-        if (!cpc && !h->has_model) return fail(B2_ERR_INVALID, "correctOnce before setModel");
-        if (sc[k].ranges_host) {
-            if (sc[k].n_ranges != h->n) return fail(B2_ERR_INVALID, "ranges size %u != model size %u", sc[k].n_ranges, h->n);
-            h->n_dataset = h->n; h->n_ranges_in = h->n; h->b_dpts = nullptr; h->b_dmask = nullptr;
-            if (h->n > 0) { RES(h->d_dpts.reserve(3 * (size_t)h->n)); RES(h->d_dmask.reserve(h->n)); RES(h->d_ranges_in.reserve(h->n)); }
-        }
-        if (h->n_dataset != h->work_n()) return fail(B2_ERR_INVALID, "dataset size %u != model size %u", h->n_dataset, h->n);
-        total += h->work_n();
-    }
+    RES(check_sensors(sc, ns, "correctOnce", &total));
     if (mode == 0 && !H->pending.empty()) return fail(B2_ERR_INVALID, "correctOnce: exec mode 0 keeps its state in one staging block: collect the pending call first");
     for (const PendingCall& q : H->pending) if (q.kind == 3) return fail(B2_ERR_INVALID, "correctOnce: an exec-mode-0 call is pending: collect it first");
+    for (uint32_t k = 0; k < ns; k++) if (sc[k].ranges_host) {          // accepted: the scans replace the datasets (uploaded below)
+        b2_rcc* h = sc[k].h;
+        h->n_dataset = h->n; h->n_ranges_in = h->n; h->b_dpts = nullptr; h->b_dmask = nullptr;
+        if (h->n > 0) { RES(h->d_dpts.reserve(3 * (size_t)h->n)); RES(h->d_dmask.reserve(h->n)); RES(h->d_ranges_in.reserve(h->n)); }
+    }
     H->pending.emplace_back();
     PendingCall& pc = H->pending.back();
     struct Guard { b2_rcc* H; bool ok = false; ~Guard() { if (!ok) H->pending.pop_back(); } } guard{H};
@@ -1023,7 +1135,7 @@ static int micp_enqueue(SensorCall* sc, uint32_t ns, const b2_transform* Tom, ui
         memset(&pc.res, 0, sizeof(pc.res));
         pc.res.Tom_new = *Tom; pc.res.T_onew_oold = tf_identity_pod();
         if (total > 0) for (uint32_t k = 0; k < ns; k++) {          // iterations == 0: the reference still runs findCorrespondences (:900-908)
-            b2_transform Tbm; memset(&Tbm, 0, sizeof(Tbm)); tf_store(&Tbm, tf_mul(tf_from_pod(*Tom), tf_from_pod(sc[k].Tbo)));
+            const b2_transform Tbm = body_in_map(*Tom, sc[k].Tbo);
             if (sc[k].ranges_host && sc[k].h->n) { RES(ranges_to_dataset(sc[k].h, sc[k].ranges_host, sc[k].n_ranges, 0)); CU(cudaStreamSynchronize(sc[k].h->stream)); }
             RES(launch_find(sc[k].h, &Tbm, nullptr));
         }
@@ -1036,7 +1148,7 @@ static int micp_enqueue(SensorCall* sc, uint32_t ns, const b2_transform* Tom, ui
         if (sc[0].ranges_host && h->n) RES(ranges_to_dataset(h, sc[0].ranges_host, sc[0].n_ranges, 0));
         IcpState& st = h->pin->icp;
         memset(&st, 0, sizeof(st));
-        st.Tom = *Tom; st.Tbo = sc[0].Tbo; st.Tsb = h->Tsb; st.max_dist = (float)(h->max_dist * (1.0 - cp) + h->adaptive_max_dist_min * cp);
+        st.Tom = *Tom; st.Tbo = sc[0].Tbo; st.Tsb = h->Tsb; st.max_dist = adaptive_max_dist(h, cp);
         st.T_onew_oold = tf_identity_pod(); st.Tom_new = *Tom;
         tf_store(&st.T_snew_sold, icp_pretransform(tf_from_pod(sc[0].Tbo), tf_from_pod(h->Tsb), tf_identity()));
         CU(cudaMemcpyAsync(h->d_icp.p, &st, sizeof(IcpState), cudaMemcpyHostToDevice, h->stream));
@@ -1051,31 +1163,21 @@ static int micp_enqueue(SensorCall* sc, uint32_t ns, const b2_transform* Tom, ui
     }
     // ---- fused path: find per sensor, then ALL inner iterations of ALL sensors in one k_icp_loop ----
     IcpLaunch& L = pc.launch;
-    memset(&L, 0, sizeof(L));
-    L.Tom = *Tom; L.n_sensors = ns; L.iterations = iterations;
-    uint32_t nblk[B2_MAX_SENSORS];
-    const int grid = loop_blocks(H, sc, ns, total, nblk);
+    const int grid = loop_layout(H, sc, ns, total, *Tom, iterations, L);
+    RES(join_streams(sc, ns, true));
     bool aux_any = false;
-    uint32_t blk0 = 0, smem_u_max = 0, sort_tiles_max = 0;
     if (H->timing) CU(cudaEventRecord(H->ev[0], H->stream));
     for (uint32_t k = 0; k < ns; k++) {
         b2_rcc* h = sc[k].h;
         IcpSensor& S = L.s[k];
-        const uint32_t nw = h->work_n();
-        S.n = nw; S.blk0 = blk0; S.nblk = nblk[k]; blk0 += nblk[k];
-        const uint32_t stride = S.nblk * B2_ICP_BLOCK;
-        const uint32_t per_thread = stride ? (nw + stride - 1) / stride : 0u;
-        S.smem_u = per_thread > B2_ICP_REG_PAIRS ? std::min<uint32_t>(per_thread - B2_ICP_REG_PAIRS, (uint32_t)H->smem_u_cap) : 0u;
-        smem_u_max = std::max(smem_u_max, S.smem_u);
-        S.max_dist = (float)(h->max_dist * (1.0 - cp) + h->adaptive_max_dist_min * cp);       // CorrespondencesCPU.cpp:21-23
-        S.merge_weight = sc[k].weight; S.range_min = h->range_min; S.range_max = h->range_max;
-        fill_sensor_frames(S, sc[k].Tbo, h->Tsb);
+        const uint32_t nw = S.n;
+        S.max_dist = adaptive_max_dist(h, cp);
         // Pinned scan (B2_ZEROCOPY, default 1): a copy engine moves it into the handle's buffer on the side stream WHILE find runs, a second small
         // copy behind it raises a flag, and the loop kernel -- launched programmatically behind find, no event in between -- checks the flag
         // before it unpacks the scan.  2: the loop kernel reads the caller's buffer itself over PCIe (latency-sensitive: 10-20 us slower on some
         // hosts).  Needs every pair of the sensor resident in registers / shared memory.  Pageable buffers take the staged upload below.
         const float* zc = nullptr; bool zc_dma = false;
-        if (sc[k].ranges_host && nw > 0 && use_zc && per_thread <= B2_ICP_REG_PAIRS + S.smem_u) {
+        if (sc[k].ranges_host && nw > 0 && use_zc && nw <= (uint64_t)(B2_ICP_REG_PAIRS + S.smem_u) * S.nblk * B2_ICP_BLOCK) {
             cudaPointerAttributes pa;      // asked on every call (about a microsecond): an address can change from pinned to pageable between calls
             if (cudaPointerGetAttributes(&pa, sc[k].ranges_host) == cudaSuccess && pa.type == cudaMemoryTypeHost && pa.devicePointer) {
                 if (use_zc == 2) zc = (const float*)pa.devicePointer; else { zc = h->d_ranges_in.p; zc_dma = true; }
@@ -1091,20 +1193,8 @@ static int micp_enqueue(SensorCall* sc, uint32_t ns, const b2_transform* Tom, ui
                 CU(cudaStreamWaitEvent(h->aux, h->ev_aux, 0));
             }
         }
-        if (h != H) {           // order the lead stream behind this sensor's own stream (pending set_ranges / set_dataset copies)
-            CU(cudaEventRecord(h->ev_join, h->stream));
-            CU(cudaStreamWaitEvent(H->stream, h->ev_join, 0));
-        }
-        b2_transform Tbm_host; memset(&Tbm_host, 0, sizeof(Tbm_host));
-        tf_store(&Tbm_host, tf_mul(tf_from_pod(*Tom), tf_from_pod(sc[k].Tbo)));          // MICPSensor.hpp:148, same inline ops as the kernels
-        pc.sensors[k] = h; pc.Tbm[k] = Tbm_host;
-        // the loop kernel may start early behind the LAST find only (event records / other kernels in between would serialise them anyway)
-        const cudaStream_t own = h->stream;
-        h->stream = H->stream;                                                        // all launches of this call ride the lead stream
-        h->pdl_next = (k + 1 == ns) && mode == 2 && use_pdl && !H->timing && h->corr_type == B2_CORR_RCC && !need_upload && !aux_any;
-        const int rc_find = launch_find(h, &Tbm_host, nullptr);
-        h->pdl_next = false; h->stream = own;
-        RES(rc_find);
+        pc.sensors[k] = h; pc.Tbm[k] = body_in_map(*Tom, sc[k].Tbo);
+        RES(find_on_lead(H, h, &pc.Tbm[k], nullptr, k + 1 == ns && mode == 2 && !H->timing && !need_upload && !aux_any));
         if (need_upload) {
             // the find kernel does not read the dataset: the scan is uploaded + unpacked on the side stream WHILE it runs
             CU(cudaMemcpyAsync(h->d_ranges_in.p, sc[k].ranges_host, sizeof(float) * h->n, cudaMemcpyHostToDevice, h->aux));
@@ -1122,40 +1212,15 @@ static int micp_enqueue(SensorCall* sc, uint32_t ns, const b2_transform* Tom, ui
             CU(cudaMemcpyAsync(h->d_bar.p, &h->pin->flag_src[fs], sizeof(unsigned int), cudaMemcpyHostToDevice, h->aux));
             S.zc_flag = h->d_bar.p; S.zc_seq = h->zc_seq;
         }
-        if (h->corr_type == B2_CORR_RCC && h->cost_tiles && iterations >= 3u) {
-            S.tile_cost = h->d_tile_cost.p; S.tile_perm = h->d_tile_perm.p; S.n_tiles = h->cost_tiles;
-            sort_tiles_max = std::max(sort_tiles_max, h->cost_tiles);
-        }
-        S.dpts = h->dpts(); S.dmask = h->dmask(); S.mpts = h->mpts(); S.mnrm = h->mnrm(); S.mmask = h->mhits();
         S.zc_ranges = zc; S.zc_dirs = h->d_dirs.p; S.zc_origs = h->d_origs.p; S.zc_n_origs = h->n_origs;
         S.dpts_out = h->d_dpts.p; S.dmask_out = h->d_dmask.p; S.ranges_out = h->d_ranges_in.p;
     }
     if (H->timing) CU(cudaEventRecord(H->ev[1], H->stream));
-    L.smem_u_max = smem_u_max;
-    unsigned int seq = ++H->seq; if (seq == 0) seq = ++H->seq;
-    L.seq = seq;
-    size_t smem = (size_t)smem_u_max * 9 * B2_ICP_BLOCK * sizeof(float);
-    if (sort_tiles_max) {
-        // the tile sort stages the durations behind the pair cache (2 bytes per tile); no room (very large scans): no sort, the order stays as it is
-        const size_t want = smem + 2 * (size_t)sort_tiles_max;
-        if (want <= (size_t)H->smem_u_cap * 9 * B2_ICP_BLOCK * sizeof(float)) smem = want;
-        else for (uint32_t k = 0; k < ns; k++) { L.s[k].tile_cost = nullptr; L.s[k].tile_perm = nullptr; L.s[k].n_tiles = 0; }
-    }
-    const bool pdl = mode == 2 && sc[ns - 1].h->pdl_armed && !aux_any;
-    sc[ns - 1].h->pdl_armed = false;
     pc.slot = (int)(H->slot_counter++ % B2_RING);
-    RES(launch_icp_loop(H, L, grid, smem, mode, pdl, pc.slot));
-    H->loop_geom[0] = ns; H->loop_geom[1] = (uint32_t)grid;
-    for (uint32_t k = 0; k < B2_MAX_SENSORS; k++) {
-        uint32_t* g = H->loop_geom + 2 + 4 * k;
-        if (k < ns) { g[0] = L.s[k].n; g[1] = L.s[k].blk0; g[2] = L.s[k].nblk; g[3] = L.s[k].smem_u; } else g[0] = g[1] = g[2] = g[3] = 0u;
-    }
+    RES(launch_loop_after_finds(H, sc, ns, L, grid, mode, !aux_any, pc.slot, &pc.smem));
     if (H->timing) { CU(cudaEventRecord(H->ev[2], H->stream)); H->timing_valid = true; }
-    for (uint32_t k = 1; k < ns; k++) {        // later work on the other sensors' own streams sees the model buffers this call wrote
-        CU(cudaEventRecord(sc[k].h->ev_join, H->stream));
-        CU(cudaStreamWaitEvent(sc[k].h->stream, sc[k].h->ev_join, 0));
-    }
-    pc.seq = seq; pc.grid = grid; pc.smem = smem; pc.barrier_used = mode == 2;
+    RES(join_streams(sc, ns, false));
+    pc.seq = L.seq; pc.grid = grid; pc.barrier_used = mode == 2;
     if (use_spin) pc.kind = 1;
     else { CU(cudaMemcpyAsync(&H->pin->res[pc.slot], H->d_res.p, sizeof(IcpResult), cudaMemcpyDeviceToHost, H->stream)); pc.kind = 2; }
     guard.ok = true;
@@ -1210,30 +1275,14 @@ static int micp_collect(b2_rcc* H, b2_transform* Tom_new, b2_transform* T_onew_o
             pc.res.Tom_new = st.Tom_new; pc.res.T_onew_oold = st.T_onew_oold; pc.res.Cmerged_o = st.Cmerged_o;
         } else {
             if (pc.barrier_used && !pc.rerun) {
-                unsigned int bar_state[2] = {0u, 0u};
-                CU(cudaMemcpy(bar_state, H->d_bar.p, sizeof(bar_state), cudaMemcpyDeviceToHost));
-                if (bar_state[1] != 0u) {
-                    // The loop's grid-wide exchange gave up (its blocks were not co-resident: SMs held by something that itself waits).  That is a
-                    // scheduling condition, not an error: reset the abort word; this call and every later call already in flight (their kernels
-                    // saw the abort word and left) run again through the cooperative launch, whose co-residency the driver guarantees.
-                    // (code 2: a block's partial sum left the fixed-point range of the atomic exchange; the cooperative variant exchanges FP64)
-                    CU(cudaMemset(H->d_bar.p + 1, 0, sizeof(unsigned int)));
-                    CU(cudaMemset(H->d_slots.p, 0, ((size_t)B2_ICP_ACC_WORDS + B2_ICP_BASE_WORDS) * sizeof(unsigned long long)));      // the aborted rounds left them inconsistent
-                    pc.rerun = true;
-                    for (PendingCall& q : H->pending) if (q.barrier_used) q.rerun = true;
-                }
+                // an abort: this call and every later call already in flight (their kernels saw the abort word and left) run again
+                RES(exchange_aborted(H, &pc.rerun));
+                if (pc.rerun) for (PendingCall& q : H->pending) if (q.barrier_used) q.rerun = true;
             }
             if (pc.rerun) {
                 H->n_reruns++;
-                for (uint32_t k = 0; k < pc.launch.n_sensors; k++) {
-                    b2_rcc* h = pc.sensors[k];
-                    const cudaStream_t own = h->stream; h->stream = H->stream; h->pdl_next = false;
-                    const int rc = launch_find(h, &pc.Tbm[k], nullptr);
-                    h->stream = own;
-                    RES(rc);
-                }
-                unsigned int seq = ++H->seq; if (seq == 0) seq = ++H->seq;
-                pc.launch.seq = seq; pc.seq = seq;
+                for (uint32_t k = 0; k < pc.launch.n_sensors; k++) RES(find_on_lead(H, pc.sensors[k], &pc.Tbm[k], nullptr, false));
+                pc.launch.seq = pc.seq = next_seq(H);
                 RES(launch_icp_loop(H, pc.launch, pc.grid, pc.smem, 1, false, pc.slot));
                 CU(cudaMemcpyAsync(&H->pin->res[pc.slot], H->d_res.p, sizeof(IcpResult), cudaMemcpyDeviceToHost, H->stream));
                 CU(cudaStreamSynchronize(H->stream));
@@ -1303,16 +1352,8 @@ extern "C" int b2_micp_correct_once(b2_rcc* const* sensors, const b2_transform* 
                                     const b2_transform* Tom, uint32_t iterations, double cp, b2_transform* Tom_new, b2_transform* T_onew_oold, b2_cross_stats* Cmerged)
 {
     NOTNULL(sensors); NOTNULL(Tbo); NOTNULL(Tom);
-    if (n_sensors == 0 || n_sensors > B2_MAX_SENSORS) return fail(B2_ERR_INVALID, "correctOnce: %u sensors (1..%d supported per call)", n_sensors, B2_MAX_SENSORS);
     SensorCall sc[B2_MAX_SENSORS];
-    for (uint32_t k = 0; k < n_sensors; k++) {
-        NOTNULL(sensors[k]);
-        for (uint32_t j = 0; j < k; j++) if (sensors[j] == sensors[k]) return fail(B2_ERR_INVALID, "correctOnce: sensor %u given twice", k);
-        sc[k].h = sensors[k]; sc[k].Tbo = Tbo[k]; sc[k].weight = merge_weights ? merge_weights[k] : 1.0;
-        sc[k].ranges_host = ranges_host ? ranges_host[k] : nullptr; sc[k].n_ranges = sc[k].ranges_host ? sensors[k]->n : 0;
-    }
-    CU(cudaSetDevice(sc[0].h->map->device));
-    if (!sc[0].h->pending.empty()) return fail(B2_ERR_INVALID, "correctOnce: asynchronous calls are still in flight on the lead handle, collect them first");
+    RES(sensor_list(__func__, "correctOnce", sensors, Tbo, merge_weights, ranges_host, n_sensors, sc));
     RES(micp_enqueue(sc, n_sensors, Tom, iterations, cp));
     return micp_collect(sc[0].h, Tom_new, T_onew_oold, Cmerged);
 }
@@ -1330,68 +1371,28 @@ static b2_micp_step* chain_records(const b2_rcc* H) { return reinterpret_cast<b2
 static int chain_step(SensorCall* sc, uint32_t ns, IcpLaunch& L, int grid, int mode, uint32_t step)
 {
     b2_rcc* H = sc[0].h;
-    uint32_t sort_tiles_max = 0;
-    for (uint32_t k = 0; k < ns; k++) {
-        b2_rcc* h = sc[k].h;
-        const cudaStream_t own = h->stream;
-        h->stream = H->stream;                                                        // all launches of the chain ride the lead stream
-        h->pdl_next = (k + 1 == ns) && mode == 2 && pdl_enabled() && h->corr_type == B2_CORR_RCC;
-        const int rc = launch_find(h, nullptr, &chain_state(H)->find[k]);
-        h->pdl_next = false; h->stream = own;
-        RES(rc);
-        IcpSensor& S = L.s[k];
-        S.mpts = h->mpts(); S.mnrm = h->mnrm(); S.mmask = h->mhits();                 // find may have grown the model buffers
-        S.tile_cost = nullptr; S.tile_perm = nullptr; S.n_tiles = 0;
-        if (h->corr_type == B2_CORR_RCC && h->cost_tiles && L.iterations >= 3u) {
-            S.tile_cost = h->d_tile_cost.p; S.tile_perm = h->d_tile_perm.p; S.n_tiles = h->cost_tiles;
-            sort_tiles_max = std::max(sort_tiles_max, h->cost_tiles);
-        }
-    }
-    size_t smem = (size_t)L.smem_u_max * 9 * B2_ICP_BLOCK * sizeof(float);
-    if (sort_tiles_max) {
-        const size_t want = smem + 2 * (size_t)sort_tiles_max;
-        if (want <= (size_t)H->smem_u_cap * 9 * B2_ICP_BLOCK * sizeof(float)) smem = want;
-        else for (uint32_t k = 0; k < ns; k++) { L.s[k].tile_cost = nullptr; L.s[k].tile_perm = nullptr; L.s[k].n_tiles = 0; }
-    }
-    const bool pdl = mode == 2 && sc[ns - 1].h->pdl_armed;
-    sc[ns - 1].h->pdl_armed = false;
-    unsigned int seq = ++H->seq; if (seq == 0) seq = ++H->seq;
-    L.seq = seq; L.step_out = chain_records(H) + step;
-    return launch_icp_loop(H, L, grid, smem, mode, pdl, -1);
+    for (uint32_t k = 0; k < ns; k++) RES(find_on_lead(H, sc[k].h, nullptr, &chain_state(H)->find[k], k + 1 == ns && mode == 2));
+    L.step_out = chain_records(H) + step;
+    return launch_loop_after_finds(H, sc, ns, L, grid, mode, true, -1, nullptr);
 }
 
 extern "C" int b2_micp_correct(b2_rcc* const* sensors, const b2_transform* Tbo, const double* merge_weights, uint32_t n_sensors,
                                b2_transform* Tom_inout, double* cp_inout, int adaptive_max_dist, uint32_t n_corrections, uint32_t iterations, b2_micp_step* steps_out)
 {
     NOTNULL(sensors); NOTNULL(Tbo); NOTNULL(Tom_inout); NOTNULL(cp_inout);
-    if (n_sensors == 0 || n_sensors > B2_MAX_SENSORS) return fail(B2_ERR_INVALID, "correct: %u sensors (1..%d supported per call)", n_sensors, B2_MAX_SENSORS);
     SensorCall sc[B2_MAX_SENSORS];
-    for (uint32_t k = 0; k < n_sensors; k++) {
-        NOTNULL(sensors[k]);
-        for (uint32_t j = 0; j < k; j++) if (sensors[j] == sensors[k]) return fail(B2_ERR_INVALID, "correct: sensor %u given twice", k);
-        sc[k].h = sensors[k]; sc[k].Tbo = Tbo[k]; sc[k].weight = merge_weights ? merge_weights[k] : 1.0; sc[k].ranges_host = nullptr; sc[k].n_ranges = 0;
-    }
+    RES(sensor_list(__func__, "correct", sensors, Tbo, merge_weights, nullptr, n_sensors, sc));
     b2_rcc* H = sc[0].h;
     const uint32_t ns = n_sensors;
-    CU(cudaSetDevice(H->map->device));
-    if (!H->pending.empty()) return fail(B2_ERR_INVALID, "correct: asynchronous calls are still in flight on the lead handle, collect them first");
     if (H->fused_grid <= 0) return fail(B2_ERR_UNSUPPORTED, "correct: a chain of corrections needs a device with cooperative launch");
     const int mode = H->exec_mode == 0 ? 1 : H->exec_mode;           // exec mode 0 keeps its state on the host between reductions: the chain runs the fused loop
-    uint64_t pairs = 0; uint32_t total_meas = 0;
-    for (uint32_t k = 0; k < ns; k++) {
-        const b2_rcc* h = sc[k].h;
-        if (h->map->device != H->map->device) return fail(B2_ERR_INVALID, "correct: all sensors must live on the same device");
-        if (h->corr_type != B2_CORR_CPC && !h->has_model) return fail(B2_ERR_INVALID, "correct before setModel");
-        if (h->n_dataset != h->work_n()) return fail(B2_ERR_INVALID, "dataset size %u != model size %u", h->n_dataset, h->n);
-        pairs += h->work_n(); total_meas += h->n_dataset;
-    }
+    uint64_t pairs = 0;
+    RES(check_sensors(sc, ns, "correct", &pairs));
+    const uint32_t total_meas = (uint32_t)pairs;                     // the dataset sizes: check_sensors saw n_dataset == work_n() for each
     if (n_corrections == 0) return B2_OK;
     const size_t bytes = sizeof(IcpChainState) + sizeof(b2_micp_step) * (size_t)n_corrections;
     RES(H->d_chain.reserve(bytes));
-    for (uint32_t k = 1; k < ns; k++) {        // order the lead stream behind the other sensors' own streams (pending set_ranges / set_dataset copies)
-        CU(cudaEventRecord(sc[k].h->ev_join, sc[k].h->stream));
-        CU(cudaStreamWaitEvent(H->stream, sc[k].h->ev_join, 0));
-    }
+    RES(join_streams(sc, ns, true));
     {
         IcpChainState st; memset(&st, 0, sizeof(st));
         for (uint32_t k = 0; k < ns; k++) { st.find[k].Tom = *Tom_inout; st.find[k].Tbo = sc[k].Tbo; }
@@ -1411,12 +1412,8 @@ extern "C" int b2_micp_correct(b2_rcc* const* sensors, const b2_transform* Tbo, 
     if (pairs == 0 || iterations == 0) {
         // Tom stays and the progress becomes 0 (micp_localization.cpp:974, :988-990); the finds still run (:900-908), at the same pose every step
         for (uint32_t k = 0; k < ns && pairs > 0; k++) {
-            b2_rcc* h = sc[k].h;
-            b2_transform Tbm; memset(&Tbm, 0, sizeof(Tbm)); tf_store(&Tbm, tf_mul(tf_from_pod(*Tom_inout), tf_from_pod(sc[k].Tbo)));
-            const cudaStream_t own = h->stream; h->stream = H->stream;
-            const int rc = launch_find(h, &Tbm, nullptr);
-            h->stream = own;
-            RES(rc);
+            const b2_transform Tbm = body_in_map(*Tom_inout, sc[k].Tbo);
+            RES(find_on_lead(H, sc[k].h, &Tbm, nullptr, false));
         }
         CU(cudaMemcpyAsync(out.data(), H->d_chain.p, sizeof(IcpChainState), cudaMemcpyDeviceToHost, H->stream));
         CU(cudaStreamSynchronize(H->stream));
@@ -1426,39 +1423,21 @@ extern "C" int b2_micp_correct(b2_rcc* const* sensors, const b2_transform* Tbo, 
         }
         got->find[0].Tom = *Tom_inout; got->cp = 0.0; got->done = n_corrections;
     } else {
-        IcpLaunch L; memset(&L, 0, sizeof(L));
-        L.Tom = *Tom_inout; L.n_sensors = ns; L.iterations = iterations; L.chain = chain_state(H); L.adaptive = adaptive_max_dist ? 1u : 0u;
-        uint32_t nblk[B2_MAX_SENSORS];
-        const int grid = loop_blocks(H, sc, ns, pairs, nblk);
-        uint32_t blk0 = 0;
-        for (uint32_t k = 0; k < ns; k++) {
-            const b2_rcc* h = sc[k].h;
-            IcpSensor& S = L.s[k];
-            S.n = h->work_n(); S.blk0 = blk0; S.nblk = nblk[k]; blk0 += nblk[k];
-            const uint32_t stride = S.nblk * B2_ICP_BLOCK, per_thread = stride ? (S.n + stride - 1) / stride : 0u;
-            S.smem_u = per_thread > B2_ICP_REG_PAIRS ? std::min<uint32_t>(per_thread - B2_ICP_REG_PAIRS, (uint32_t)H->smem_u_cap) : 0u;
-            L.smem_u_max = std::max(L.smem_u_max, S.smem_u);
-            S.max_dist = h->max_dist; S.max_dist_min = h->adaptive_max_dist_min;      // the loop interpolates with the progress (CorrespondencesCPU.cpp:21-23)
-            S.merge_weight = sc[k].weight; S.range_min = h->range_min; S.range_max = h->range_max;
-            fill_sensor_frames(S, sc[k].Tbo, h->Tsb);
-            S.dpts = h->dpts(); S.dmask = h->dmask();
+        IcpLaunch L;
+        const int grid = loop_layout(H, sc, ns, pairs, *Tom_inout, iterations, L);
+        L.chain = chain_state(H); L.adaptive = adaptive_max_dist ? 1u : 0u;
+        for (uint32_t k = 0; k < ns; k++) {          // the loop interpolates the gate with the progress (CorrespondencesCPU.cpp:21-23)
+            L.s[k].max_dist = sc[k].h->max_dist; L.s[k].max_dist_min = sc[k].h->adaptive_max_dist_min;
         }
         for (uint32_t s = 0; s < n_corrections; s++) RES(chain_step(sc, ns, L, grid, mode, s));
-        H->loop_geom[0] = ns; H->loop_geom[1] = (uint32_t)grid;
-        for (uint32_t k = 0; k < B2_MAX_SENSORS; k++) {
-            uint32_t* g = H->loop_geom + 2 + 4 * k;
-            if (k < ns) { g[0] = L.s[k].n; g[1] = L.s[k].blk0; g[2] = L.s[k].nblk; g[3] = L.s[k].smem_u; } else g[0] = g[1] = g[2] = g[3] = 0u;
-        }
         CU(cudaMemcpyAsync(out.data(), H->d_chain.p, bytes, cudaMemcpyDeviceToHost, H->stream));
         CU(cudaStreamSynchronize(H->stream));
         if (got->done < n_corrections) {
-            // A mode-2 exchange gave up (micp_collect: co-residency or fixed-point range); the steps behind it saw the abort word and left.  The
-            // device state is the last completed step's: reset the abort and accumulator words and run the rest of the chain cooperatively.
-            unsigned int bar_state[2] = {0u, 0u};
-            CU(cudaMemcpy(bar_state, H->d_bar.p, sizeof(bar_state), cudaMemcpyDeviceToHost));
-            if (mode != 2 || bar_state[1] == 0u) return fail(B2_ERR_CUDA, "correct: step %u of %u left no record", got->done + 1, n_corrections);
-            CU(cudaMemset(H->d_bar.p + 1, 0, sizeof(unsigned int)));
-            CU(cudaMemset(H->d_slots.p, 0, ((size_t)B2_ICP_ACC_WORDS + B2_ICP_BASE_WORDS) * sizeof(unsigned long long)));
+            // A mode-2 exchange gave up; the steps behind it saw the abort word and left.  The device state is the last completed step's: the
+            // rest of the chain runs cooperatively.
+            bool aborted = false;
+            if (mode == 2) RES(exchange_aborted(H, &aborted));
+            if (!aborted) return fail(B2_ERR_CUDA, "correct: step %u of %u left no record", got->done + 1, n_corrections);
             H->n_reruns++;
             for (uint32_t s = got->done; s < n_corrections; s++) RES(chain_step(sc, ns, L, grid, 1, s));
             CU(cudaMemcpyAsync(out.data(), H->d_chain.p, bytes, cudaMemcpyDeviceToHost, H->stream));
@@ -1466,10 +1445,7 @@ extern "C" int b2_micp_correct(b2_rcc* const* sensors, const b2_transform* Tbo, 
             if (got->done != n_corrections) return fail(B2_ERR_CUDA, "correct: the cooperative re-run left %u of %u records", got->done, n_corrections);
         }
     }
-    for (uint32_t k = 1; k < ns; k++) {        // later work on the other sensors' own streams sees the model buffers the chain wrote
-        CU(cudaEventRecord(sc[k].h->ev_join, H->stream));
-        CU(cudaStreamWaitEvent(sc[k].h->stream, sc[k].h->ev_join, 0));
-    }
+    RES(join_streams(sc, ns, false));
     *Tom_inout = got->find[0].Tom;
     *cp_inout = got->cp;
     if (steps_out) memcpy(steps_out, rec, sizeof(b2_micp_step) * (size_t)n_corrections);

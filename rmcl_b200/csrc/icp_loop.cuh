@@ -260,7 +260,7 @@ B2_DEV void icp_tail(const IcpLaunch& L, const double (*sums)[B2_NACC + 1], Tf& 
 // Between two corrections (host+device so that tests/emul runs the same code)
 // ---------------------------------------------------------------------------------------------------------------------
 // params.max_dist interpolated towards adaptive_max_dist_min by the progress (CorrespondencesCPU.cpp:21-23): float * double + float * double
-// in double, rounded to float -- the host's expression (api.cu: micp_enqueue), so that a chain step gates exactly like a host-fed call
+// in double, rounded to float -- the host's expression (api.cu: adaptive_max_dist), so that a chain step gates exactly like a host-fed call
 B2_DEV float icp_adaptive_max_dist(float max_dist, float max_dist_min, double cp)
 {
     return (float)((double)max_dist * (1.0 - cp) + (double)max_dist_min * cp);
@@ -494,7 +494,7 @@ __global__ void __launch_bounds__(B2_ICP_BLOCK) k_icp_loop(const __grid_constant
     }
     if (!COOP) asm volatile("griddepcontrol.wait;" ::: "memory");
     // ---- load this thread's pairs once: validity is folded into the dataset point (NaN fails the P2L gate like a masked pair) ----
-    // Slots beyond the sensor's pairs read pair 0 (and are then masked): every sensor that is given blocks has at least one pair (micp_enqueue).
+    // Slots beyond the sensor's pairs read pair 0 (and are then masked): every sensor that is given blocks has at least one pair (api.cu: loop_layout).
     for (uint32_t u = 0; u < n_cached; u++) {
         const uint32_t i = lid + u * stride;
         const bool in = i < n;

@@ -999,6 +999,39 @@ def test_multi_sensor_correct_once(po, synth):
         rmcl_b200.micp_correct_once([hs[0], hs[0]], Tbo, Tom, 5, 0.0)
 
 
+def test_multi_sensor_refusal_changes_no_handle(synth):
+    """A multi-sensor correctOnce refused because of its second sensor (a scan for a closest-point handle) leaves the first sensor's dataset
+    as it was: still none (a later correctOnce without a scan is refused for it), or still the bound tensors."""
+    import ctypes as C
+    import torch
+    import rmcl_b200
+    m = synth.c1_sensor()
+    h0 = _rcc(synth, "cube29", m)
+    h1 = rmcl_b200.CPCB200(gpu_map("cube29"))
+    I = synth.make_transform()
+    Tbo = np.stack([I, I])
+    r = np.full(m.size, 5.0, np.float32)
+
+    def refused():
+        with pytest.raises(rmcl_b200.B2Error, match="closest-point mode"):
+            rmcl_b200.micp_correct_once([h0, h1], Tbo, I, 5, 0.0, ranges=[r, r])
+
+    refused()
+    assert len(h0.datasetView()["mask"]) == 0
+    with pytest.raises(rmcl_b200.B2Error, match=f"dataset size 0 != model size {m.size}"):
+        h0.correctOnce(I, I)
+    nb = m.size // 2                                                          # a bound dataset of another size than the model's
+    p, mk = torch.zeros((nb, 3), dtype=torch.float32, device="cuda"), torch.ones(nb, dtype=torch.uint8, device="cuda")
+    h0.bindDataset(p, mk)
+    refused()
+    pp, pm, n = C.c_void_p(), C.c_void_p(), C.c_uint32()
+    assert rmcl_b200.load_library().b2_rcc_dataset_view(h0._h, C.byref(pp), C.byref(pm), C.byref(n)) == 0
+    assert (pp.value, pm.value, n.value) == (p.data_ptr(), mk.data_ptr(), nb)
+    with pytest.raises(rmcl_b200.B2Error, match=f"dataset size {nb} != model size {m.size}"):
+        h0.correctOnce(I, I)
+    torch.cuda.synchronize()
+
+
 def test_correct_once_async(po, synth):
     """b2_rcc_correct_once_async / _wait: enqueue, do something else, collect; one call pending per handle."""
     import torch
