@@ -143,6 +143,35 @@ B2_API int b2_rcc_bind_model_buffers(b2_rcc* h, float* points_xyz_dev, float* no
 /* MICP..Sensor..::unpackMessage (rmcl_ros/src/micpl/MICPSphericalSensorCPU.cpp:181-233) on the device: dataset = dir*range (+orig),
  * mask = range in [range.min, range.max].  Also the v1 setInputData(ranges) (lidar_corrector_embree_benchmark.cpp:118). */
 B2_API int b2_rcc_set_ranges(b2_rcc* h, const float* ranges, uint32_t n, int src_is_device);
+/* An organised sensor_msgs/PointCloud2 as the O1Dn sensor's scan.  b2_cloud_layout carries the message's geometry; the lookup of the fields
+ * named x, y and z stays with the caller (rmcl_msgs_adapters.hpp does it), B2_CLOUD_NO_FIELD marks one that is missing.  datatype is the
+ * PointField datatype of x, which decides how all three are read (7 FLOAT32, 8 FLOAT64 narrowed to float). */
+#define B2_CLOUD_NO_FIELD 0xffffffffu
+typedef struct {
+    uint32_t width, height, point_step, row_step;
+    uint32_t offset_x, offset_y, offset_z;
+    uint8_t  datatype, is_bigendian, pad[2];
+} b2_cloud_layout;                                                            /* 32 B */
+/* the parameters of pc2_to_o1dn (rmcl_ros/src/nodes/conversion/pc2_to_o1dn.cpp:48-77, FilterOptions2D, scan_operations.h:59-66) */
+typedef struct {
+    uint32_t height_skip_begin, height_skip_end, height_increment;
+    uint32_t width_skip_begin, width_skip_end, width_increment;
+    float    range_min, range_max;
+} b2_o1dn_cloud_filter;                                                       /* 32 B */
+/* Pc2ToO1DnNode::convert + MICPO1DnSensor*::unpackMessage + setModel on the device: estimateModelAndData (rmcl_ros/src/util/conversions.cpp:869-1073),
+ * filter (rmcl_ros/src/util/scan_operations.cpp:41-143), then the model and dataset of MICPO1DnSensorCUDA.cpp:142-148,171-230, in one kernel.
+ * Output ray (i, j), i < H = (height - h_skip_begin - h_skip_end) / h_increment, j < W likewise, reads the point at byte
+ * (i*h_inc + h_skip_begin) * row_step + (j*w_inc + w_skip_begin) * point_step.  A finite point p gives range = |p| and dir = p / range; any other
+ * gives dir 0 and range 0 (valid when range_min <= 0).  A finite (0,0,0) gives NaN directions, as in the reference.  The model becomes O1Dn
+ * W x H, orig 0, [range_min, range_max]; the dataset is point = dir*range, mask = range in [range_min, range_max], as b2_rcc_set_ranges.  A field
+ * named `mask` is not read (the reference would store it as the range).  src_is_device != 0: `data` is a device address, read in place (it
+ * must stay valid until the handle's stream has run the kernel); else the bytes up to the last point read are uploaded and the call
+ * synchronises.  When the handle's previous model came from this call with the same W x H, find's tile schedule is kept; any other model
+ * resets it.  Refused (B2_ERR_INVALID, no launch, handle unchanged): null pointers, a missing field, a datatype other than 7 / 8, is_bigendian,
+ * an increment of 0, skips larger than the dimension, a field that ends beyond point_step, `bytes` short of the last point read, more rays
+ * than any model may have.  On a closest-point handle the dataset is filled the same way (the ray table is not used there). */
+B2_API int b2_rcc_set_cloud_o1dn(b2_rcc* h, const void* data, uint64_t bytes, const b2_cloud_layout* layout, const b2_o1dn_cloud_filter* filter,
+                                 int src_is_device);
 /* RCC..::find(Tbm_est), rmcl/src/rmcl/registration/RCCEmbree.cpp:26-36,58-68,89-99,121-131 */
 B2_API int b2_rcc_find(b2_rcc* h, const b2_transform* Tbm_est);
 /* The three semantics of rm::*SimulatorEmbree::simulate that SURVEY.md Appendix A.3 cannot settle without rmagine's source, as switches (all 0 = the

@@ -230,6 +230,15 @@ public:
     explicit RCCB200O1Dn(B200MapPtr map) : CorrespondencesB200(std::move(map)) {}
     void setModel(const rm::O1DnModel& m) override                                                // RCCEmbree.cpp:84-87
     { b2_check(b2_rcc_set_model_o1dn(h_, m.width, m.height, &m.orig.x, reinterpret_cast<const float*>(b2_table_ptr(m.dirs)), m.range.min, m.range.max), "setModel"); note_model(m.width, m.height); }
+    // Pc2ToO1DnNode::convert + unpackMessage + setModel (conversions.cpp:869-1073, scan_operations.cpp:41-143, MICPO1DnSensorCUDA.cpp:142-148,171-230)
+    // on the device: an organised PointCloud2's bytes become this sensor's model and dataset (b2_rcc_set_cloud_o1dn)
+    void setPointCloud(const void* data, size_t bytes, const b2_cloud_layout& layout, const b2_o1dn_cloud_filter& filter, bool on_device = false)
+    {
+        b2_check(b2_rcc_set_cloud_o1dn(h_, data, bytes, &layout, &filter, on_device ? 1 : 0), "setPointCloud");
+        note_model((layout.width - filter.width_skip_begin - filter.width_skip_end) / filter.width_increment,
+                   (layout.height - filter.height_skip_begin - filter.height_skip_end) / filter.height_increment);
+        outdated = true; own_dataset_ = true;
+    }
 };
 class RCCB200OnDn : public CorrespondencesB200, public rm::ModelSetter<rm::OnDnModel> {
 public:

@@ -9,6 +9,8 @@
 //                            512 KiB upload + the unpack kernel on the device (dataset point = direction * range (+ origin), mask = range in [min, max];
 //                            RangeData.mask is ignored exactly like the reference ignores it: "TODOs: use input mask values", :189-191)
 //   unpackMessage(rcc, msg)  both, for a whole Scan / Depth / O1Dn / OnDn message (or its *Stamped payload)
+//   unpackPointCloud(rcc, cloud, filter)  pc2_to_o1dn (Pc2ToO1DnNode::convert: conversions.cpp:869-1073 + scan_operations.cpp:41-143) and the
+//                            O1Dn sensor's unpackMessage + setModel in one device call (RCCB200O1Dn::setPointCloud); fields x, y, z looked up by name
 //   fillSensorStats(...)     rmcl_msgs/MICPSensorStats as published at rmcl_ros/src/nodes/micp_localization.cpp:1009-1015
 //   fillParticleStats(...)   rmcl_msgs/ParticleStats as RmclNode::estimateStats returns it (rmcl_ros/src/nodes/rmcl_localization.cpp:642-731)
 #pragma once
@@ -61,6 +63,24 @@ template <typename RangeDataT> inline void setData(CorrespondencesB200& rcc, con
 
 // Scan / Depth / O1Dn / OnDn: { info, data }
 template <typename RCC, typename MsgT> inline void unpackMessage(RCC& rcc, const MsgT& msg) { setModel(rcc, msg.info); setData(rcc, msg.data); }
+
+// sensor_msgs/PointCloud2 (+ the node's FilterOptions2D-shaped parameters: range_min, range_max, width / height .skip_begin .skip_end .increment)
+template <typename PointCloud2T, typename FilterOptionsT> inline void unpackPointCloud(RCCB200O1Dn& rcc, const PointCloud2T& cloud, const FilterOptionsT& opt)
+{
+    b2_cloud_layout L{};
+    L.width = cloud.width; L.height = cloud.height; L.point_step = cloud.point_step; L.row_step = cloud.row_step;
+    L.offset_x = L.offset_y = L.offset_z = B2_CLOUD_NO_FIELD;
+    for (const auto& f : cloud.fields) {                                     // conversions.cpp:899-953
+        if (f.name == "x") { L.offset_x = f.offset; L.datatype = (uint8_t)f.datatype; }
+        else if (f.name == "y") L.offset_y = f.offset;
+        else if (f.name == "z") L.offset_z = f.offset;
+    }
+    L.is_bigendian = cloud.is_bigendian ? 1 : 0;
+    auto u32 = [](uint64_t v) { if (v > 0xffffffffu) throw std::runtime_error("unpackPointCloud: filter option out of range"); return (uint32_t)v; };
+    const b2_o1dn_cloud_filter F{u32(opt.height.skip_begin), u32(opt.height.skip_end), u32(opt.height.increment),
+                                 u32(opt.width.skip_begin), u32(opt.width.skip_end), u32(opt.width.increment), (float)opt.range_min, (float)opt.range_max};
+    rcc.setPointCloud(cloud.data.data(), cloud.data.size(), L, F);
+}
 
 // rmcl_msgs/MICPSensorStats (micp_localization.cpp:1009-1015): valid_matches = Cmerged_o.n_meas, cov_trace = trace(Cmerged_o.covariance)
 template <typename StatsMsgT> inline void fillSensorStats(StatsMsgT& stats, const rm::CrossStatistics& Cmerged_o, uint32_t total_measurements, uint32_t valid_measurements)

@@ -61,6 +61,36 @@ class GladiatorConfig(C.Structure):
         return GladiatorConfig(0.03, 0.03, 0.0, 0.0, 0.0, 0.01, 0.3, 0.2)
 
 
+class _CloudLayout(C.Structure):
+    _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("point_step", C.c_uint32), ("row_step", C.c_uint32), ("offset_x", C.c_uint32),
+                ("offset_y", C.c_uint32), ("offset_z", C.c_uint32), ("datatype", C.c_uint8), ("is_bigendian", C.c_uint8), ("pad", C.c_uint8 * 2)]
+
+
+B2_CLOUD_NO_FIELD = 0xFFFFFFFF
+
+
+class O1DnCloudFilter(C.Structure):
+    """The parameters of pc2_to_o1dn (rmcl_ros/src/nodes/conversion/pc2_to_o1dn.cpp:48-77): skips and increment of both axes, and the range
+    limits of the model.  defaults() are the node's declared defaults."""
+    _fields_ = [("height_skip_begin", C.c_uint32), ("height_skip_end", C.c_uint32), ("height_increment", C.c_uint32),
+                ("width_skip_begin", C.c_uint32), ("width_skip_end", C.c_uint32), ("width_increment", C.c_uint32),
+                ("range_min", C.c_float), ("range_max", C.c_float)]
+
+    @staticmethod
+    def defaults(range_min=0.3, range_max=50.0):
+        return O1DnCloudFilter(0, 0, 1, 0, 0, 1, range_min, range_max)
+
+
+def cloud_layout(cloud):
+    """b2_cloud_layout of a sensor_msgs/PointCloud2-shaped object (width, height, point_step, row_step, is_bigendian, fields with name / offset /
+    datatype): x, y and z are looked up by name, a missing one is marked B2_CLOUD_NO_FIELD; the datatype is that of x."""
+    off = {f.name: f for f in cloud.fields}
+    L = _CloudLayout(int(cloud.width), int(cloud.height), int(cloud.point_step), int(cloud.row_step),
+                     *[int(off[k].offset) if k in off else B2_CLOUD_NO_FIELD for k in ("x", "y", "z")],
+                     int(off["x"].datatype) if "x" in off else 0, int(bool(cloud.is_bigendian)))
+    return L
+
+
 class _MeshInfo(C.Structure):
     _fields_ = [("n_faces", C.c_uint32), ("n_vertices", C.c_uint32), ("n_nodes", C.c_uint32), ("n_leaf_tris", C.c_uint32), ("max_depth", C.c_uint32),
                 ("bvh_bytes", C.c_uint64), ("build_ms", C.c_float), ("device", C.c_int), ("build_mode", C.c_int), ("sah_cost", C.c_float)]
@@ -75,7 +105,7 @@ EXPORTS = [
     "b2_pf_set_stream", "b2_pf_sensor_update", "b2_pf_sensor_update_host", "b2_kernel_launch_count", "b2_rcc_enable_timing", "b2_rcc_last_timing", "b2_pf_motion_update", "b2_pf_likelihood_stats",
     "b2_rcc_set_correspondence_type", "b2_pf_resample_gladiator", "b2_pf_gladiator_randoms", "b2_rcc_segment", "b2_mesh_create_from_file", "b2_mesh_file_load", "b2_mesh_file_free", "b2_peek_cuda_error", "b2_mesh_blob_size", "b2_mesh_export_blob", "b2_mesh_create_from_blob", "b2_mesh_refit",
     "b2_rcc_correct_once_async", "b2_rcc_correct_once_wait", "b2_micp_correct_once", "b2_rcc_set_exec_mode", "b2_debug_read_bandwidth", "b2_rcc_set_sim_options", "b2_rcc_bind_dataset", "b2_rcc_bind_model_buffers", "b2_rcc_benchmark_batch", "b2_pf_p2p_init", "b2_pf_p2p_connect", "b2_pf_p2p_publish", "b2_pf_resample_gladiator_p2p", "b2_pf_p2p_connect_local", "b2_rcc_set_cpc_options", "b2_pf_set_mapping", "b2_pf_get_mapping",
-    "b2_micp_correct", "b2_pf_init_uniform", "b2_pf_init_gaussian", "b2_pf_estimate_stats",
+    "b2_micp_correct", "b2_pf_init_uniform", "b2_pf_init_gaussian", "b2_pf_estimate_stats", "b2_rcc_set_cloud_o1dn",
 ]
 
 
@@ -477,6 +507,26 @@ class RCCB200Pinhole(RCCB200):
 
 class RCCB200O1Dn(RCCB200):
     """rmcl::RCCEmbreeO1Dn twin (RCCEmbree.hpp:51-66)."""
+
+    def setPointCloud(self, cloud, filter=None):
+        """An organised sensor_msgs/PointCloud2 as this sensor's scan (b2_rcc_set_cloud_o1dn): pc2_to_o1dn's conversion and filter, the O1Dn
+        model and the dataset, in one kernel.  `cloud` is PointCloud2-shaped (synth.pointcloud2 or the ROS message); its `data` is a numpy /
+        bytes buffer or host tensor (uploaded, the call synchronises) or a CUDA uint8 tensor (read in place).  `filter`: O1DnCloudFilter, default defaults()."""
+        flt = filter if filter is not None else O1DnCloudFilter.defaults()
+        L = cloud_layout(cloud)
+        data = cloud.data
+        if hasattr(data, "data_ptr"):                  # torch tensor: CUDA (read in place) or host, pinned or pageable (uploaded)
+            if not data.is_contiguous():
+                raise TypeError("setPointCloud: cloud.data must be contiguous")
+            ptr, nbytes, dev = C.c_void_p(data.data_ptr()), data.numel() * data.element_size(), int(data.is_cuda)
+        else:
+            data = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.ascontiguousarray(data).view(np.uint8).reshape(-1)
+            ptr, nbytes, dev = C.c_void_p(data.ctypes.data) if data.size else None, data.size, 0
+        _chk(load_library().b2_rcc_set_cloud_o1dn(self._h, ptr, C.c_uint64(nbytes), C.byref(L), C.byref(flt), C.c_int(dev)))
+        w = (int(cloud.width) - flt.width_skip_begin - flt.width_skip_end) // flt.width_increment
+        hgt = (int(cloud.height) - flt.height_skip_begin - flt.height_skip_end) // flt.height_increment
+        self.model, self.n = None, w * hgt
+        self.outdated = True
 
 
 class RCCB200OnDn(RCCB200):

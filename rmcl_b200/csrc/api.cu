@@ -388,6 +388,7 @@ struct b2_rcc {
     int exec_mode = 2;                  // b2_rcc_set_exec_mode: 2 software grid barrier + programmatic launch (default), 1 cooperative launch, 0 one launch per reduction
     bool pdl_next = false, pdl_armed = false;   // the next find is followed by k_icp_loop launched with programmatic stream serialization / the find let it start early
     DevBuf<uint32_t> d_tile_cost; DevBuf<uint16_t> d_tile_perm; uint32_t perm_tiles = 0, cost_tiles = 0;    // tile schedule of k_rcc_find: warp durations of the last launch (cost_tiles of them if it recorded any), order for the next (always a permutation of perm_tiles tiles)
+    DevBuf<uint8_t> d_cloud; bool model_from_cloud = false;      // b2_rcc_set_cloud_o1dn: uploaded host cloud; the model came from that call (its tile schedule carries over)
     unsigned long long n_reruns = 0;                            // calls that were run again through the cooperative launch (exchange abort: co-residency or range)
     uint32_t loop_geom[2 + 4 * B2_MAX_SENSORS] = {};            // last fused call: sensors, grid, per sensor {n, blk0, nblk, smem_u} (b2_rcc_debug_loop_geometry)
     DevBuf<unsigned int> d_bar; unsigned int zc_seq = 0;        // [0] = "scan copy complete" flag (value: zc_seq of the call), [1] = abort word of the ICP loop
@@ -489,7 +490,7 @@ extern "C" int b2_rcc_destroy(b2_rcc* h)
     h->d_dirs.release(); h->d_origs.release(); h->d_dpts.release(); h->d_dmask.release(); h->d_ranges_in.release();
     h->d_mpts.release(); h->d_mnrm.release(); h->d_mranges.release(); h->d_mhits.release(); h->d_mfaces.release();
     h->d_partials.release(); h->d_ticket.release(); h->d_stats.release(); h->d_icp.release(); h->d_bar.release(); h->d_res.release(); h->d_dbg.release(); h->d_slots.release(); h->d_tile_cost.release(); h->d_tile_perm.release();
-    h->d_chain.release();
+    h->d_chain.release(); h->d_cloud.release();
     { DeviceCtx& dc = g_dev[h->map->device & 63]; std::lock_guard<std::mutex> lk(dc.m); dc.n_handles--; if (dc.last == h) { dc.last = nullptr; dc.recorded = false; } }
     h->d_poses.release(); h->d_tdelta.release(); h->d_ncorr.release(); h->d_bstats.release();
     if (h->pin) cudaFreeHost(h->pin);
@@ -561,6 +562,18 @@ extern "C" __attribute__((visibility("default"))) int b2_rcc_debug_tile_perm(b2_
     if (out && h->perm_tiles && capacity >= h->perm_tiles) CU(cudaMemcpy(out, h->d_tile_perm.p, h->perm_tiles * sizeof(uint16_t), cudaMemcpyDeviceToHost));
     return B2_OK;
 }
+// test aid (not part of the public header): host copies of the sensor model's ray directions (3 n floats) and the resident ranges (n floats);
+// either may be null.  *n receives the model's ray count.
+extern "C" __attribute__((visibility("default"))) int b2_rcc_debug_model_tables(b2_rcc* h, float* dirs, float* ranges, uint32_t* n)
+{
+    NOTNULL(h); NOTNULL(n);
+    CU(cudaSetDevice(h->map->device));
+    CU(cudaStreamSynchronize(h->stream));
+    *n = h->has_model ? h->n : 0;
+    if (dirs && *n) CU(cudaMemcpy(dirs, h->d_dirs.p, 3 * sizeof(float) * *n, cudaMemcpyDeviceToHost));
+    if (ranges && *n && h->n_ranges_in == *n) CU(cudaMemcpy(ranges, h->d_ranges_in.p, sizeof(float) * *n, cudaMemcpyDeviceToHost));
+    return B2_OK;
+}
 // make PROFILE=1 only: per block {ns at publish, ns at collect, cycles since the block reduce at publish, at collect} of iteration 1
 extern "C" __attribute__((visibility("default"))) int b2_rcc_debug_blocks(b2_rcc* h, unsigned long long* out /* 4 * B2_ICP_MAX_GRID */)
 {
@@ -593,7 +606,7 @@ static int set_model_tables(b2_rcc* h, uint32_t w, uint32_t hgt, const float* or
 {
     CU(cudaSetDevice(h->map->device));
     const size_t n = (size_t)w * hgt;
-    if (n == 0) { h->has_model = true; h->n = 0; h->width = w; h->height = hgt; return B2_OK; }   // zero-size model: find() silently returns (RCCOptix.cpp:30-34)
+    if (n == 0) { h->has_model = true; h->n = 0; h->width = w; h->height = hgt; h->model_from_cloud = false; return B2_OK; }   // zero-size model: find() silently returns (RCCOptix.cpp:30-34)
     if (n > 0xffffffffu / 4) return fail(B2_ERR_INVALID, "model too large");
     RES(h->d_dirs.reserve(3 * n)); RES(h->d_origs.reserve(3 * (size_t)n_origs));
     CU(cudaStreamSynchronize(h->stream));
@@ -601,6 +614,7 @@ static int set_model_tables(b2_rcc* h, uint32_t w, uint32_t hgt, const float* or
     CU(cudaMemcpy(h->d_origs.p, origs, sizeof(float) * 3 * (size_t)n_origs, cudaMemcpyHostToDevice));
     h->has_model = true; h->n = (uint32_t)n; h->width = w; h->height = hgt; h->n_origs = n_origs; h->range_min = rmin; h->range_max = rmax;
     h->perm_tiles = 0;                                             // the tile schedule belongs to the previous model
+    h->model_from_cloud = false;
     return B2_OK;
 }
 
@@ -692,6 +706,71 @@ extern "C" int b2_rcc_set_ranges(b2_rcc* h, const float* ranges, uint32_t n, int
     NOTNULL(h);
     CU(cudaSetDevice(h->map->device));
     RES(ranges_to_dataset(h, ranges, n, src_is_device));
+    if (!src_is_device) CU(cudaStreamSynchronize(h->stream));
+    return B2_OK;
+}
+
+// Pc2ToO1DnNode::convert + MICPO1DnSensorCUDA::unpackMessage + setModel (conversions.cpp:869-1073, scan_operations.cpp:41-143,
+// MICPO1DnSensorCUDA.cpp:142-148,171-230) as one kernel.  Every check runs before anything of the handle changes: where the reference
+// throws, divides by zero, underflows size_t or reads past the message, the call is refused.  A host cloud is uploaded whole up to the last
+// byte the filter reads (one copy; scripts/bench_pointcloud.py measures it against the host path).
+extern "C" int b2_rcc_set_cloud_o1dn(b2_rcc* h, const void* data, uint64_t bytes, const b2_cloud_layout* L, const b2_o1dn_cloud_filter* F, int src_is_device)
+{
+    NOTNULL(data); NOTNULL(L); NOTNULL(F);          // the arguments are checked before the handle: the checks need no device
+    const uint32_t off[3] = {L->offset_x, L->offset_y, L->offset_z};
+    if (off[0] == B2_CLOUD_NO_FIELD || off[1] == B2_CLOUD_NO_FIELD || off[2] == B2_CLOUD_NO_FIELD)
+        return fail(B2_ERR_INVALID, "set_cloud_o1dn: the cloud has no x, y or z field (\"NO POINT FIELD IN CLOUD!\", conversions.cpp:955-958)");
+    if (L->datatype != 7 && L->datatype != 8)
+        return fail(B2_ERR_INVALID, "set_cloud_o1dn: field x has datatype %u; FLOAT32 (7) and FLOAT64 (8) are read (conversions.cpp:977-990)", (unsigned)L->datatype);
+    if (L->is_bigendian) return fail(B2_ERR_INVALID, "set_cloud_o1dn: big-endian clouds are not read");
+    if (F->height_increment == 0 || F->width_increment == 0) return fail(B2_ERR_INVALID, "set_cloud_o1dn: increment 0 (height %u, width %u)", F->height_increment, F->width_increment);
+    if ((uint64_t)F->height_skip_begin + F->height_skip_end > L->height || (uint64_t)F->width_skip_begin + F->width_skip_end > L->width)
+        return fail(B2_ERR_INVALID, "set_cloud_o1dn: skips %u+%u of height %u / %u+%u of width %u", F->height_skip_begin, F->height_skip_end, L->height,
+                    F->width_skip_begin, F->width_skip_end, L->width);
+    const uint32_t fsz = L->datatype == 8 ? 8u : 4u;
+    for (int c = 0; c < 3; c++)
+        if ((uint64_t)off[c] + fsz > L->point_step) return fail(B2_ERR_INVALID, "set_cloud_o1dn: field %c at offset %u ends beyond point_step %u", "xyz"[c], off[c], L->point_step);
+    const uint64_t w_out = (L->width - F->width_skip_begin - F->width_skip_end) / F->width_increment;
+    const uint64_t h_out = (L->height - F->height_skip_begin - F->height_skip_end) / F->height_increment;
+    const uint64_t n = w_out * h_out;
+    if (n > 0xffffffffu / 4) return fail(B2_ERR_INVALID, "set_cloud_o1dn: model too large (%llu rays)", (unsigned long long)n);
+    uint64_t need = 0;
+    if (n) {
+        const unsigned __int128 last = (unsigned __int128)((h_out - 1) * F->height_increment + F->height_skip_begin) * L->row_step +
+                                       (unsigned __int128)((w_out - 1) * F->width_increment + F->width_skip_begin) * L->point_step +
+                                       std::max(off[0], std::max(off[1], off[2])) + fsz;
+        if (last > (unsigned __int128)bytes)
+            return fail(B2_ERR_INVALID, "set_cloud_o1dn: %llu bytes given, the last point read ends at byte %llu", (unsigned long long)bytes,
+                        last > (unsigned __int128)UINT64_MAX ? (unsigned long long)UINT64_MAX : (unsigned long long)last);
+        need = (uint64_t)last;
+    }
+    NOTNULL(h);
+    CU(cudaSetDevice(h->map->device));
+    const bool keep_schedule = h->model_from_cloud && h->has_model && h->width == (uint32_t)w_out && h->height == (uint32_t)h_out;
+    if (n) {
+        RES(h->d_dirs.reserve(3 * n)); RES(h->d_origs.reserve(3)); RES(h->d_dpts.reserve(3 * n)); RES(h->d_dmask.reserve(n)); RES(h->d_ranges_in.reserve(n));
+        const uint8_t* src = static_cast<const uint8_t*>(data);
+        if (!src_is_device) {
+            RES(h->d_cloud.reserve(need));
+            CU(cudaMemcpyAsync(h->d_cloud.p, data, need, cudaMemcpyHostToDevice, h->stream));
+            src = h->d_cloud.p;
+        }
+        CU(cudaMemsetAsync(h->d_origs.p, 0, 3 * sizeof(float), h->stream));
+        CloudO1Dn c;
+        c.w_out = (uint32_t)w_out; c.h_out = (uint32_t)h_out; c.row_step = L->row_step; c.point_step = L->point_step;
+        for (int k = 0; k < 3; k++) c.off[k] = off[k];
+        c.f64 = L->datatype == 8 ? 1u : 0u;
+        c.h_inc = F->height_increment; c.h_begin = F->height_skip_begin; c.w_inc = F->width_increment; c.w_begin = F->width_skip_begin;
+        c.range_min = F->range_min; c.range_max = F->range_max;
+        k_o1dn_from_cloud<<<(uint32_t)((n + 255) / 256), 256, 0, h->stream>>>(src, c, h->d_dirs.p, h->d_ranges_in.p, h->d_dpts.p, h->d_dmask.p);
+        LAUNCHED();
+    }
+    h->has_model = true; h->n = (uint32_t)n; h->width = (uint32_t)w_out; h->height = (uint32_t)h_out; h->n_origs = 1;
+    h->range_min = F->range_min; h->range_max = F->range_max;
+    if (!keep_schedule) h->perm_tiles = 0;
+    h->model_from_cloud = true;
+    h->b_dpts = nullptr; h->b_dmask = nullptr;
+    h->n_dataset = (uint32_t)n; h->n_ranges_in = (uint32_t)n;
     if (!src_is_device) CU(cudaStreamSynchronize(h->stream));
     return B2_OK;
 }

@@ -422,6 +422,16 @@ __global__ void __launch_bounds__(128) k_intersect(BvhView bvh, const float* __r
 // ---------------------------------------------------------------------------------------------------------------------
 // MICP*Sensor*::unpackMessage on the device (MICPSphericalSensorCPU.cpp:181-233)
 // ---------------------------------------------------------------------------------------------------------------------
+// one dataset entry: point = dir * range + orig, mask = range in [range_min, range_max] (MICPO1DnSensorCUDA.cpp:201-215)
+// (dir[di ..], orig[oi ..]: 32-bit element indices, as the tables are indexed everywhere else)
+B2_DEV void dataset_entry(uint32_t i, float r, const float* dir, uint32_t di, const float* orig, uint32_t oi, float range_min, float range_max, float* pts, uint8_t* mask)
+{
+    pts[3 * i + 0] = add(mul(dir[di + 0], r), orig[oi + 0]);
+    pts[3 * i + 1] = add(mul(dir[di + 1], r), orig[oi + 1]);
+    pts[3 * i + 2] = add(mul(dir[di + 2], r), orig[oi + 2]);
+    mask[i] = (r < range_min || r > range_max) ? 0 : 1;
+}
+
 __global__ void k_dataset_from_ranges(const float* __restrict__ ranges, const float* __restrict__ dirs, const float* __restrict__ origs, uint32_t n_origs,
                                       uint32_t n, float range_min, float range_max, float* __restrict__ pts, uint8_t* __restrict__ mask)
 {
@@ -429,10 +439,75 @@ __global__ void k_dataset_from_ranges(const float* __restrict__ ranges, const fl
     if (i >= n) return;
     const float r = ranges[i];
     const uint32_t oi = n_origs == 1 ? 0 : i;
-    pts[3 * i + 0] = add(mul(dirs[3 * i + 0], r), origs[3 * oi + 0]);
-    pts[3 * i + 1] = add(mul(dirs[3 * i + 1], r), origs[3 * oi + 1]);
-    pts[3 * i + 2] = add(mul(dirs[3 * i + 2], r), origs[3 * oi + 2]);
-    mask[i] = (r < range_min || r > range_max) ? 0 : 1;
+    dataset_entry(i, r, dirs, 3 * i, origs, 3 * oi, range_min, range_max, pts, mask);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Pc2ToO1DnNode::convert on the device: estimateModelAndData (conversions.cpp:869-1073) + filter (scan_operations.cpp:41-143)
+// ---------------------------------------------------------------------------------------------------------------------
+struct CloudO1Dn {
+    uint32_t w_out, h_out;                  // output raster (filtered)
+    uint64_t row_step; uint32_t point_step;
+    uint32_t off[3];                        // byte offsets of x, y, z inside a point
+    uint32_t f64;                           // 1: FLOAT64 fields (narrowed to float), 0: FLOAT32
+    uint32_t h_inc, h_begin, w_inc, w_begin;
+    float range_min, range_max;
+};
+
+// little-endian loads at any byte address (PointField offsets need not be aligned)
+B2_DEV uint32_t cloud_u32(const uint8_t* p)
+{
+    if (!((uintptr_t)p & 3u)) return *reinterpret_cast<const uint32_t*>(p);
+    return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24);
+}
+B2_DEV float cloud_coord(const uint8_t* p, bool f64)
+{
+    if (!f64) return u2f(cloud_u32(p));
+    const unsigned long long u = (unsigned long long)cloud_u32(p) | ((unsigned long long)cloud_u32(p + 4) << 32);
+    double d;
+#if B2_ON_DEVICE
+    d = __longlong_as_double((long long)u);
+#else
+    memcpy(&d, &u, 8);
+#endif
+    return (float)d;                        // round to nearest, as the reference's implicit double -> float
+}
+B2_DEV bool finite_f32(float a) { return (f2u(a) & 0x7f800000u) != 0x7f800000u; }
+
+// one point of the cloud -> ray direction and range (conversions.cpp:992-1011; rm::Vector::l2norm and operator/=)
+B2_DEV void o1dn_from_point(float x, float y, float z, float* dir, float& range)
+{
+    if (finite_f32(x) && finite_f32(y) && finite_f32(z)) {
+        range = v_l2norm(mk3(x, y, z));
+        dir[0] = dvd(x, range); dir[1] = dvd(y, range); dir[2] = dvd(z, range);
+    } else {
+        dir[0] = 0.f; dir[1] = 0.f; dir[2] = 0.f; range = 0.f;
+    }
+}
+
+// output ray k of the filtered raster (scan_operations.cpp:100-111): reads its source point, converts it, writes the ray table entry, the
+// range and the dataset entry (the model's origin is 0)
+B2_DEV void o1dn_cloud_entry(const uint8_t* cloud, const CloudO1Dn& c, uint32_t k, float* dirs, float* ranges, float* pts, uint8_t* mask)
+{
+    const uint32_t i = k / c.w_out, j = k - i * c.w_out;
+    const uint64_t src_i = (uint64_t)i * c.h_inc + c.h_begin, src_j = (uint64_t)j * c.w_inc + c.w_begin;
+    const uint8_t* p = cloud + src_i * c.row_step + src_j * c.point_step;
+    const bool f64 = c.f64 != 0;
+    float d[3], r;
+    o1dn_from_point(cloud_coord(p + c.off[0], f64), cloud_coord(p + c.off[1], f64), cloud_coord(p + c.off[2], f64), d, r);
+    dirs[3 * k + 0] = d[0]; dirs[3 * k + 1] = d[1]; dirs[3 * k + 2] = d[2];
+    ranges[k] = r;
+    const float orig[3] = {0.f, 0.f, 0.f};
+    dataset_entry(k, r, d, 0, orig, 0, c.range_min, c.range_max, pts, mask);
+}
+
+// one thread per output ray
+__global__ void k_o1dn_from_cloud(const uint8_t* __restrict__ cloud, CloudO1Dn c, float* __restrict__ dirs, float* __restrict__ ranges,
+                                  float* __restrict__ pts, uint8_t* __restrict__ mask)
+{
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= c.w_out * c.h_out) return;
+    o1dn_cloud_entry(cloud, c, k, dirs, ranges, pts, mask);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

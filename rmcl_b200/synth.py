@@ -422,3 +422,55 @@ def pf_beams(points, k, seed=42):
     B["range"] = rngs
     B["cov"][:, [0, 4, 8]] = 0.1
     return B
+
+
+# --------------------------------------------------------------------------------------------------
+# sensor_msgs/PointCloud2 (field names of the ROS message; PointField datatypes: 2 UINT8, 7 FLOAT32, 8 FLOAT64)
+# --------------------------------------------------------------------------------------------------
+
+@dataclass
+class PointField:
+    name: str
+    offset: int
+    datatype: int
+    count: int = 1
+
+
+@dataclass
+class PointCloud2:
+    width: int
+    height: int
+    fields: list
+    is_bigendian: bool
+    point_step: int
+    row_step: int
+    data: np.ndarray            # uint8 (or a CUDA uint8 tensor)
+    is_dense: bool = False
+
+
+def pointcloud2(points, width, height, *, dtype=np.float32, point_step=16, offsets=(0, 4, 8), extra=None, row_pad=0, seed=0):
+    """An organised cloud of `points` ((height*width, 3) in the sensor frame, row-major; NaN marks a miss, e.g. the points of a spherical
+    scan's find with misses left as NaN): x, y, z as `dtype` (float32 or float64) at `offsets` inside `point_step` bytes, `row_pad` bytes
+    after each row.  `extra` maps further field names to offsets: a field named "mask" is one UINT8 (random 0/1, as a filter node would
+    write it), any other a FLOAT32 of random values.  Bytes no field covers are random as well, so nothing reads them unnoticed."""
+    rng = np.random.default_rng(seed)
+    P = np.asarray(points, np.float64).reshape(height, width, 3)
+    dt = np.dtype(dtype).newbyteorder("<")
+    fields = [PointField(n, int(o), 8 if dt.itemsize == 8 else 7) for n, o in zip("xyz", offsets)]
+    for name, o in (extra or {}).items():
+        fields.append(PointField(name, int(o), 2 if name == "mask" else 7))
+    for f in fields:
+        if f.offset + (1 if f.datatype == 2 else 4 if f.datatype == 7 else 8) > point_step:
+            raise ValueError(f"field {f.name} does not fit into point_step {point_step}")
+    row_step = width * point_step + row_pad
+    buf = rng.integers(0, 256, height * row_step, dtype=np.uint8)
+    rows = buf.reshape(height, row_step)[:, :width * point_step].reshape(height, width, point_step)
+    with np.errstate(over="ignore"):                # a double beyond float range stays inf in a FLOAT32 cloud
+        for k, f in enumerate(fields[:3]):
+            rows[:, :, f.offset:f.offset + dt.itemsize] = P[:, :, k].astype(dt)[..., None].view(np.uint8)
+    for f in fields[3:]:
+        if f.datatype == 2:
+            rows[:, :, f.offset] = rng.integers(0, 2, (height, width), dtype=np.uint8)
+        else:
+            rows[:, :, f.offset:f.offset + 4] = rng.uniform(0, 100, (height, width)).astype("<f4")[..., None].view(np.uint8)
+    return PointCloud2(width, height, fields, False, point_step, row_step, buf)
