@@ -172,6 +172,22 @@ typedef struct {
  * than any model may have.  On a closest-point handle the dataset is filled the same way (the ray table is not used there). */
 B2_API int b2_rcc_set_cloud_o1dn(b2_rcc* h, const void* data, uint64_t bytes, const b2_cloud_layout* layout, const b2_o1dn_cloud_filter* filter,
                                  int src_is_device);
+/* Pc2ToScanNode::convert + fillEmpty + MICPSphericalSensor*::unpackMessage on the device (rmcl_ros/src/nodes/conversion/pc2_to_scan.cpp:105-213,
+ * rmcl_ros/src/util/scan_operations.cpp:25-39, MICPSphericalSensorCUDA.cpp:176-235): a sensor_msgs/PointCloud2 binned into the spherical model
+ * the handle holds (b2_rcc_set_model_spherical) as its scan.  Point (row, col) is read at row * row_step + col * point_step.  A point with a
+ * non-finite x, y or z is skipped; else p = T_sensor_cloud * (x, y, z), range = |p| (float), theta = atan2(p.y, p.x) and
+ * phi = atan2(p.z, sqrt(p.x^2 + p.y^2)), both in FP64 rounded to float (the reference takes phi against the 3-D norm: SURVEY D21);
+ * id = int((angle - min) / inc + 0.5) with the float division and the double + 0.5 of the reference (no wrap-around, D23); a dimension of
+ * size 1 with increment 0 puts every point at 0 (D24).  A point inside the model with range in [range_min, range_max] writes its cell; the
+ * last such point in index order wins.  Every other cell gets range_max + 1.  The dataset is point = dir * range, mask = range in
+ * [range_min, range_max], as b2_rcc_set_ranges.  The model, its direction table and find's tile schedule stay as they are.
+ * src_is_device != 0: `data` is a device address, read in place (valid until the handle's stream has run the kernels); else the bytes up to
+ * the last point read are uploaded and the call synchronises.  `data` may be null for a cloud of no points.  Refused (B2_ERR_INVALID, no
+ * launch, handle unchanged): null pointers, a missing field, a datatype other than 7 / 8, is_bigendian, a field that ends beyond point_step,
+ * `bytes` short of the last point read, more than 2^32 - 2 points, a non-finite T_sensor_cloud, a handle whose current model is not
+ * spherical, a model increment of 0 with a size above 1, a non-finite model parameter.  Works on a closest-point handle holding a spherical model. */
+B2_API int b2_rcc_set_cloud_spherical(b2_rcc* h, const void* data, uint64_t bytes, const b2_cloud_layout* layout, const b2_transform* T_sensor_cloud,
+                                      int src_is_device);
 /* RCC..::find(Tbm_est), rmcl/src/rmcl/registration/RCCEmbree.cpp:26-36,58-68,89-99,121-131 */
 B2_API int b2_rcc_find(b2_rcc* h, const b2_transform* Tbm_est);
 /* The three semantics of rm::*SimulatorEmbree::simulate that SURVEY.md Appendix A.3 cannot settle without rmagine's source, as switches (all 0 = the

@@ -215,6 +215,13 @@ public:
         b2_spherical_model s{m.phi.min, m.phi.inc, m.phi.size, m.theta.min, m.theta.inc, m.theta.size, m.range.min, m.range.max};
         b2_check(b2_rcc_set_model_spherical(h_, &s), "setModel"); note_model(m.theta.size, m.phi.size);
     }
+    // Pc2ToScanNode::convert + fillEmpty + unpackMessage (pc2_to_scan.cpp:105-213, scan_operations.cpp:25-39, MICPSphericalSensorCUDA.cpp:176-235)
+    // on the device: a PointCloud2's bytes binned into the model of the last setModel as this sensor's dataset (b2_rcc_set_cloud_spherical)
+    void setPointCloud(const void* data, size_t bytes, const b2_cloud_layout& layout, const rm::Transform& T_sensor_cloud, bool on_device = false)
+    {
+        b2_check(b2_rcc_set_cloud_spherical(h_, data, bytes, &layout, tf(&T_sensor_cloud), on_device ? 1 : 0), "setPointCloud");
+        outdated = true; own_dataset_ = true;
+    }
 };
 class RCCB200Pinhole : public CorrespondencesB200, public rm::ModelSetter<rm::PinholeModel> {
 public:

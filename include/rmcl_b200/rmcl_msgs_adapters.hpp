@@ -11,6 +11,8 @@
 //   unpackMessage(rcc, msg)  both, for a whole Scan / Depth / O1Dn / OnDn message (or its *Stamped payload)
 //   unpackPointCloud(rcc, cloud, filter)  pc2_to_o1dn (Pc2ToO1DnNode::convert: conversions.cpp:869-1073 + scan_operations.cpp:41-143) and the
 //                            O1Dn sensor's unpackMessage + setModel in one device call (RCCB200O1Dn::setPointCloud); fields x, y, z looked up by name
+//   unpackPointCloud(rcc, cloud, T)  pc2_to_scan (Pc2ToScanNode::convert + fillEmpty: pc2_to_scan.cpp:105-213, scan_operations.cpp:25-39) and the
+//                            spherical sensor's unpackMessage in one device call (RCCB200Spherical::setPointCloud), into the model of its setModel
 //   fillSensorStats(...)     rmcl_msgs/MICPSensorStats as published at rmcl_ros/src/nodes/micp_localization.cpp:1009-1015
 //   fillParticleStats(...)   rmcl_msgs/ParticleStats as RmclNode::estimateStats returns it (rmcl_ros/src/nodes/rmcl_localization.cpp:642-731)
 #pragma once
@@ -64,22 +66,38 @@ template <typename RangeDataT> inline void setData(CorrespondencesB200& rcc, con
 // Scan / Depth / O1Dn / OnDn: { info, data }
 template <typename RCC, typename MsgT> inline void unpackMessage(RCC& rcc, const MsgT& msg) { setModel(rcc, msg.info); setData(rcc, msg.data); }
 
-// sensor_msgs/PointCloud2 (+ the node's FilterOptions2D-shaped parameters: range_min, range_max, width / height .skip_begin .skip_end .increment)
-template <typename PointCloud2T, typename FilterOptionsT> inline void unpackPointCloud(RCCB200O1Dn& rcc, const PointCloud2T& cloud, const FilterOptionsT& opt)
+// sensor_msgs/PointCloud2 -> b2_cloud_layout: fields x, y, z looked up by name (conversions.cpp:899-953, pc2_to_scan.cpp:141-155), a missing
+// one marked B2_CLOUD_NO_FIELD (the device call refuses it)
+template <typename PointCloud2T> inline b2_cloud_layout cloudLayout(const PointCloud2T& cloud)
 {
     b2_cloud_layout L{};
     L.width = cloud.width; L.height = cloud.height; L.point_step = cloud.point_step; L.row_step = cloud.row_step;
     L.offset_x = L.offset_y = L.offset_z = B2_CLOUD_NO_FIELD;
-    for (const auto& f : cloud.fields) {                                     // conversions.cpp:899-953
+    for (const auto& f : cloud.fields) {
         if (f.name == "x") { L.offset_x = f.offset; L.datatype = (uint8_t)f.datatype; }
         else if (f.name == "y") L.offset_y = f.offset;
         else if (f.name == "z") L.offset_z = f.offset;
     }
     L.is_bigendian = cloud.is_bigendian ? 1 : 0;
+    return L;
+}
+
+// sensor_msgs/PointCloud2 (+ the node's FilterOptions2D-shaped parameters: range_min, range_max, width / height .skip_begin .skip_end .increment)
+template <typename PointCloud2T, typename FilterOptionsT> inline void unpackPointCloud(RCCB200O1Dn& rcc, const PointCloud2T& cloud, const FilterOptionsT& opt)
+{
+    const b2_cloud_layout L = cloudLayout(cloud);
     auto u32 = [](uint64_t v) { if (v > 0xffffffffu) throw std::runtime_error("unpackPointCloud: filter option out of range"); return (uint32_t)v; };
     const b2_o1dn_cloud_filter F{u32(opt.height.skip_begin), u32(opt.height.skip_end), u32(opt.height.increment),
                                  u32(opt.width.skip_begin), u32(opt.width.skip_end), u32(opt.width.increment), (float)opt.range_min, (float)opt.range_max};
     rcc.setPointCloud(cloud.data.data(), cloud.data.size(), L, F);
+}
+
+// sensor_msgs/PointCloud2 into the spherical model the sensor holds (pc2_to_scan's convert + the spherical unpackMessage); T_sensor_cloud is
+// the transform the node looks up from the cloud's frame to the sensor frame (pc2_to_scan.cpp:111-133), identity when they are the same
+template <typename PointCloud2T> inline void unpackPointCloud(RCCB200Spherical& rcc, const PointCloud2T& cloud,
+                                                              const rm::Transform& T_sensor_cloud = rm::Transform::Identity())
+{
+    rcc.setPointCloud(cloud.data.data(), cloud.data.size(), cloudLayout(cloud), T_sensor_cloud);
 }
 
 // rmcl_msgs/MICPSensorStats (micp_localization.cpp:1009-1015): valid_matches = Cmerged_o.n_meas, cov_trace = trace(Cmerged_o.covariance)

@@ -91,6 +91,24 @@ def cloud_layout(cloud):
     return L
 
 
+def _identity_tf():
+    T = np.zeros((), TRANSFORM_DTYPE)
+    T["R"][3] = 1.0
+    return T
+
+
+def _cloud_buffer(cloud):
+    """(address, bytes, on device) of a PointCloud2-shaped object's data: a torch tensor, CUDA (read in place) or host, pinned or pageable
+    (uploaded), or a numpy / bytes buffer (uploaded)"""
+    data = cloud.data
+    if hasattr(data, "data_ptr"):
+        if not data.is_contiguous():
+            raise TypeError("setPointCloud: cloud.data must be contiguous")
+        return C.c_void_p(data.data_ptr()), data.numel() * data.element_size(), int(data.is_cuda)
+    data = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.ascontiguousarray(data).view(np.uint8).reshape(-1)
+    return C.c_void_p(data.ctypes.data) if data.size else None, data.size, 0
+
+
 class _MeshInfo(C.Structure):
     _fields_ = [("n_faces", C.c_uint32), ("n_vertices", C.c_uint32), ("n_nodes", C.c_uint32), ("n_leaf_tris", C.c_uint32), ("max_depth", C.c_uint32),
                 ("bvh_bytes", C.c_uint64), ("build_ms", C.c_float), ("device", C.c_int), ("build_mode", C.c_int), ("sah_cost", C.c_float)]
@@ -106,6 +124,7 @@ EXPORTS = [
     "b2_rcc_set_correspondence_type", "b2_pf_resample_gladiator", "b2_pf_gladiator_randoms", "b2_rcc_segment", "b2_mesh_create_from_file", "b2_mesh_file_load", "b2_mesh_file_free", "b2_peek_cuda_error", "b2_mesh_blob_size", "b2_mesh_export_blob", "b2_mesh_create_from_blob", "b2_mesh_refit",
     "b2_rcc_correct_once_async", "b2_rcc_correct_once_wait", "b2_micp_correct_once", "b2_rcc_set_exec_mode", "b2_debug_read_bandwidth", "b2_rcc_set_sim_options", "b2_rcc_bind_dataset", "b2_rcc_bind_model_buffers", "b2_rcc_benchmark_batch", "b2_pf_p2p_init", "b2_pf_p2p_connect", "b2_pf_p2p_publish", "b2_pf_resample_gladiator_p2p", "b2_pf_p2p_connect_local", "b2_rcc_set_cpc_options", "b2_pf_set_mapping", "b2_pf_get_mapping",
     "b2_micp_correct", "b2_pf_init_uniform", "b2_pf_init_gaussian", "b2_pf_estimate_stats", "b2_rcc_set_cloud_o1dn",
+    "b2_rcc_set_cloud_spherical",
 ]
 
 
@@ -500,6 +519,18 @@ class RCCB200:
 class RCCB200Spherical(RCCB200):
     """rmcl::RCCEmbreeSpherical / RCCOptixSpherical twin (rmcl/include/rmcl/registration/RCCEmbree.hpp:18-33)."""
 
+    def setPointCloud(self, cloud, T_sensor_cloud=None):
+        """A sensor_msgs/PointCloud2 binned into the spherical model of the last setModel as this sensor's scan (b2_rcc_set_cloud_spherical):
+        pc2_to_scan's conversion, fillEmpty and the dataset, in two kernels; the model and find's tile schedule stay.  `cloud` is
+        PointCloud2-shaped (synth.pointcloud2 or the ROS message); its `data` is a numpy / bytes buffer or host tensor (uploaded, the call
+        synchronises) or a CUDA uint8 tensor (read in place).  `T_sensor_cloud`: the cloud frame in the sensor frame (TRANSFORM_DTYPE),
+        None = identity."""
+        T = _tf(_identity_tf() if T_sensor_cloud is None else T_sensor_cloud)
+        L = cloud_layout(cloud)
+        ptr, nbytes, dev = _cloud_buffer(cloud)
+        _chk(load_library().b2_rcc_set_cloud_spherical(self._h, ptr, C.c_uint64(nbytes), C.byref(L), _p(T), C.c_int(dev)))
+        self.outdated = True
+
 
 class RCCB200Pinhole(RCCB200):
     """rmcl::RCCEmbreePinhole twin (RCCEmbree.hpp:35-49)."""
@@ -514,14 +545,7 @@ class RCCB200O1Dn(RCCB200):
         bytes buffer or host tensor (uploaded, the call synchronises) or a CUDA uint8 tensor (read in place).  `filter`: O1DnCloudFilter, default defaults()."""
         flt = filter if filter is not None else O1DnCloudFilter.defaults()
         L = cloud_layout(cloud)
-        data = cloud.data
-        if hasattr(data, "data_ptr"):                  # torch tensor: CUDA (read in place) or host, pinned or pageable (uploaded)
-            if not data.is_contiguous():
-                raise TypeError("setPointCloud: cloud.data must be contiguous")
-            ptr, nbytes, dev = C.c_void_p(data.data_ptr()), data.numel() * data.element_size(), int(data.is_cuda)
-        else:
-            data = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.ascontiguousarray(data).view(np.uint8).reshape(-1)
-            ptr, nbytes, dev = C.c_void_p(data.ctypes.data) if data.size else None, data.size, 0
+        ptr, nbytes, dev = _cloud_buffer(cloud)
         _chk(load_library().b2_rcc_set_cloud_o1dn(self._h, ptr, C.c_uint64(nbytes), C.byref(L), C.byref(flt), C.c_int(dev)))
         w = (int(cloud.width) - flt.width_skip_begin - flt.width_skip_end) // flt.width_increment
         hgt = (int(cloud.height) - flt.height_skip_begin - flt.height_skip_end) // flt.height_increment

@@ -389,6 +389,8 @@ struct b2_rcc {
     bool pdl_next = false, pdl_armed = false;   // the next find is followed by k_icp_loop launched with programmatic stream serialization / the find let it start early
     DevBuf<uint32_t> d_tile_cost; DevBuf<uint16_t> d_tile_perm; uint32_t perm_tiles = 0, cost_tiles = 0;    // tile schedule of k_rcc_find: warp durations of the last launch (cost_tiles of them if it recorded any), order for the next (always a permutation of perm_tiles tiles)
     DevBuf<uint8_t> d_cloud; bool model_from_cloud = false;      // b2_rcc_set_cloud_o1dn: uploaded host cloud; the model came from that call (its tile schedule carries over)
+    b2_spherical_model sph{}; bool model_spherical = false;    // the model b2_rcc_set_model_spherical set, while it is the current one (b2_rcc_set_cloud_spherical bins into it)
+    DevBuf<unsigned long long> d_scan_keys;                     // b2_rcc_set_cloud_spherical: one key per cell, all 0 between calls
     unsigned long long n_reruns = 0;                            // calls that were run again through the cooperative launch (exchange abort: co-residency or range)
     uint32_t loop_geom[2 + 4 * B2_MAX_SENSORS] = {};            // last fused call: sensors, grid, per sensor {n, blk0, nblk, smem_u} (b2_rcc_debug_loop_geometry)
     DevBuf<unsigned int> d_bar; unsigned int zc_seq = 0;        // [0] = "scan copy complete" flag (value: zc_seq of the call), [1] = abort word of the ICP loop
@@ -490,7 +492,7 @@ extern "C" int b2_rcc_destroy(b2_rcc* h)
     h->d_dirs.release(); h->d_origs.release(); h->d_dpts.release(); h->d_dmask.release(); h->d_ranges_in.release();
     h->d_mpts.release(); h->d_mnrm.release(); h->d_mranges.release(); h->d_mhits.release(); h->d_mfaces.release();
     h->d_partials.release(); h->d_ticket.release(); h->d_stats.release(); h->d_icp.release(); h->d_bar.release(); h->d_res.release(); h->d_dbg.release(); h->d_slots.release(); h->d_tile_cost.release(); h->d_tile_perm.release();
-    h->d_chain.release(); h->d_cloud.release();
+    h->d_chain.release(); h->d_cloud.release(); h->d_scan_keys.release();
     { DeviceCtx& dc = g_dev[h->map->device & 63]; std::lock_guard<std::mutex> lk(dc.m); dc.n_handles--; if (dc.last == h) { dc.last = nullptr; dc.recorded = false; } }
     h->d_poses.release(); h->d_tdelta.release(); h->d_ncorr.release(); h->d_bstats.release();
     if (h->pin) cudaFreeHost(h->pin);
@@ -606,7 +608,7 @@ static int set_model_tables(b2_rcc* h, uint32_t w, uint32_t hgt, const float* or
 {
     CU(cudaSetDevice(h->map->device));
     const size_t n = (size_t)w * hgt;
-    if (n == 0) { h->has_model = true; h->n = 0; h->width = w; h->height = hgt; h->model_from_cloud = false; return B2_OK; }   // zero-size model: find() silently returns (RCCOptix.cpp:30-34)
+    if (n == 0) { h->has_model = true; h->n = 0; h->width = w; h->height = hgt; h->model_from_cloud = false; h->model_spherical = false; return B2_OK; }   // zero-size model: find() silently returns (RCCOptix.cpp:30-34)
     if (n > 0xffffffffu / 4) return fail(B2_ERR_INVALID, "model too large");
     RES(h->d_dirs.reserve(3 * n)); RES(h->d_origs.reserve(3 * (size_t)n_origs));
     CU(cudaStreamSynchronize(h->stream));
@@ -614,7 +616,7 @@ static int set_model_tables(b2_rcc* h, uint32_t w, uint32_t hgt, const float* or
     CU(cudaMemcpy(h->d_origs.p, origs, sizeof(float) * 3 * (size_t)n_origs, cudaMemcpyHostToDevice));
     h->has_model = true; h->n = (uint32_t)n; h->width = w; h->height = hgt; h->n_origs = n_origs; h->range_min = rmin; h->range_max = rmax;
     h->perm_tiles = 0;                                             // the tile schedule belongs to the previous model
-    h->model_from_cloud = false;
+    h->model_from_cloud = false; h->model_spherical = false;
     return B2_OK;
 }
 
@@ -635,7 +637,9 @@ extern "C" int b2_rcc_set_model_spherical(b2_rcc* h, const b2_spherical_model* m
         }
     }
     const float o[3] = {0.f, 0.f, 0.f};
-    return set_model_tables(h, m->theta_size, m->phi_size, o, 1, dirs.data(), m->range_min, m->range_max);
+    RES(set_model_tables(h, m->theta_size, m->phi_size, o, 1, dirs.data(), m->range_min, m->range_max));
+    h->sph = *m; h->model_spherical = true;
+    return B2_OK;
 }
 
 extern "C" int b2_rcc_set_model_pinhole(b2_rcc* h, const b2_pinhole_model* m)
@@ -768,9 +772,86 @@ extern "C" int b2_rcc_set_cloud_o1dn(b2_rcc* h, const void* data, uint64_t bytes
     h->has_model = true; h->n = (uint32_t)n; h->width = (uint32_t)w_out; h->height = (uint32_t)h_out; h->n_origs = 1;
     h->range_min = F->range_min; h->range_max = F->range_max;
     if (!keep_schedule) h->perm_tiles = 0;
-    h->model_from_cloud = true;
+    h->model_from_cloud = true; h->model_spherical = false;
     h->b_dpts = nullptr; h->b_dmask = nullptr;
     h->n_dataset = (uint32_t)n; h->n_ranges_in = (uint32_t)n;
+    if (!src_is_device) CU(cudaStreamSynchronize(h->stream));
+    return B2_OK;
+}
+
+static bool all_finite(const float* v, int n)
+{
+    for (int k = 0; k < n; k++) if (!std::isfinite(v[k])) return false;
+    return true;
+}
+
+// Pc2ToScanNode::convert + fillEmpty + MICPSphericalSensorCUDA::unpackMessage (pc2_to_scan.cpp:105-213, scan_operations.cpp:25-39,
+// MICPSphericalSensorCUDA.cpp:176-235) as two kernels on the handle's stream with no host round trip between them.  The model stays the
+// one b2_rcc_set_model_spherical set: its direction table and find's tile schedule are kept.  Every check runs before anything of the
+// handle changes.  A host cloud is uploaded whole up to the last byte read (scripts/bench_pointcloud_scan.py measures the call).
+extern "C" int b2_rcc_set_cloud_spherical(b2_rcc* h, const void* data, uint64_t bytes, const b2_cloud_layout* L, const b2_transform* T, int src_is_device)
+{
+    NOTNULL(L); NOTNULL(T);                         // the arguments are checked before the handle: the checks need no device
+    const uint64_t n_points = (uint64_t)L->width * L->height;
+    if (n_points) NOTNULL(data);
+    const uint32_t off[3] = {L->offset_x, L->offset_y, L->offset_z};
+    if (off[0] == B2_CLOUD_NO_FIELD || off[1] == B2_CLOUD_NO_FIELD || off[2] == B2_CLOUD_NO_FIELD)
+        return fail(B2_ERR_INVALID, "set_cloud_spherical: the cloud has no x, y or z field");
+    if (L->datatype != 7 && L->datatype != 8)
+        return fail(B2_ERR_INVALID, "set_cloud_spherical: field x has datatype %u; FLOAT32 (7) and FLOAT64 (8) are read (pc2_to_scan.cpp:167-184)", (unsigned)L->datatype);
+    if (L->is_bigendian) return fail(B2_ERR_INVALID, "set_cloud_spherical: big-endian clouds are not read");
+    const uint32_t fsz = L->datatype == 8 ? 8u : 4u;
+    for (int c = 0; c < 3; c++)
+        if ((uint64_t)off[c] + fsz > L->point_step) return fail(B2_ERR_INVALID, "set_cloud_spherical: field %c at offset %u ends beyond point_step %u", "xyz"[c], off[c], L->point_step);
+    if (n_points > 0xfffffffeull) return fail(B2_ERR_INVALID, "set_cloud_spherical: %llu points, at most 2^32 - 2 are read", (unsigned long long)n_points);
+    uint64_t need = 0;
+    if (n_points) {
+        const unsigned __int128 last = (unsigned __int128)(L->height - 1) * L->row_step + (unsigned __int128)(L->width - 1) * L->point_step +
+                                       std::max(off[0], std::max(off[1], off[2])) + fsz;
+        if (last > (unsigned __int128)bytes)
+            return fail(B2_ERR_INVALID, "set_cloud_spherical: %llu bytes given, the last point read ends at byte %llu", (unsigned long long)bytes,
+                        last > (unsigned __int128)UINT64_MAX ? (unsigned long long)UINT64_MAX : (unsigned long long)last);
+        need = (uint64_t)last;
+    }
+    const float Tv[7] = {T->R.x, T->R.y, T->R.z, T->R.w, T->t.x, T->t.y, T->t.z};
+    if (!all_finite(Tv, 7)) return fail(B2_ERR_INVALID, "set_cloud_spherical: T_sensor_cloud is not finite");
+    NOTNULL(h);
+    if (!h->model_spherical) return fail(B2_ERR_INVALID, "set_cloud_spherical: the handle's current model is not spherical (b2_rcc_set_model_spherical first)");
+    const b2_spherical_model& m = h->sph;
+    const float mv[6] = {m.phi_min, m.phi_inc, m.theta_min, m.theta_inc, m.range_min, m.range_max};
+    if (!all_finite(mv, 6)) return fail(B2_ERR_INVALID, "set_cloud_spherical: the spherical model has a non-finite parameter");
+    if ((m.phi_inc == 0.f && m.phi_size > 1) || (m.theta_inc == 0.f && m.theta_size > 1))
+        return fail(B2_ERR_INVALID, "set_cloud_spherical: model increment 0 with more than one bin (phi %u, theta %u)", m.phi_size, m.theta_size);
+    CU(cudaSetDevice(h->map->device));
+    const uint32_t n = h->n;
+    if (n == 0) { h->n_dataset = 0; return B2_OK; }                             // as b2_rcc_set_ranges on a zero-size model
+    RES(h->d_dpts.reserve(3 * (size_t)n)); RES(h->d_dmask.reserve(n)); RES(h->d_ranges_in.reserve(n));
+    if (h->d_scan_keys.cap < n) {
+        RES(h->d_scan_keys.reserve(n));
+        CU(cudaMemsetAsync(h->d_scan_keys.p, 0, sizeof(unsigned long long) * h->d_scan_keys.cap, h->stream));   // k_scan_cells keeps them 0 from here on
+    }
+    CloudScan c;
+    c.width = L->width; c.n_points = (uint32_t)n_points; c.row_step = L->row_step; c.point_step = L->point_step;
+    for (int k = 0; k < 3; k++) c.off[k] = off[k];
+    c.f64 = L->datatype == 8 ? 1u : 0u;
+    c.T = tf_from_pod(*T);
+    c.phi_min = m.phi_min; c.phi_inc = m.phi_inc; c.theta_min = m.theta_min; c.theta_inc = m.theta_inc; c.phi_n = m.phi_size; c.theta_n = m.theta_size;
+    c.range_min = m.range_min; c.range_max = m.range_max;
+    c.fill = (float)((double)m.range_max + 1.0);                                  // scan.info.range_max + 1.0 stored as float
+    if (n_points) {
+        const uint8_t* src = static_cast<const uint8_t*>(data);
+        if (!src_is_device) {
+            RES(h->d_cloud.reserve(need));
+            CU(cudaMemcpyAsync(h->d_cloud.p, data, need, cudaMemcpyHostToDevice, h->stream));
+            src = h->d_cloud.p;
+        }
+        k_scan_bin_cloud<<<(uint32_t)((n_points + 255) / 256), 256, 0, h->stream>>>(src, c, h->d_scan_keys.p);
+        LAUNCHED();
+    }
+    k_scan_cells<<<(n + 255) / 256, 256, 0, h->stream>>>(c, h->d_scan_keys.p, h->d_dirs.p, h->d_origs.p, h->d_ranges_in.p, h->d_dpts.p, h->d_dmask.p);
+    LAUNCHED();
+    h->b_dpts = nullptr; h->b_dmask = nullptr;
+    h->n_dataset = n; h->n_ranges_in = n;
     if (!src_is_device) CU(cudaStreamSynchronize(h->stream));
     return B2_OK;
 }

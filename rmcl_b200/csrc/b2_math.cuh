@@ -69,6 +69,19 @@ B2_DEV uint32_t byte_perm(uint32_t x, uint32_t y, uint32_t s)
 template <int SEL> inline uint32_t prmt_imm(uint32_t x, uint32_t y) { return byte_perm(x, y, (uint32_t)SEL); }
 #endif
 
+// FP64, individually rounded on both sides (atan2: CUDA's double atan2 on the device, libm's on the host)
+#if B2_ON_DEVICE
+B2_DEV double mul_d(double a, double b) { return __dmul_rn(a, b); }
+B2_DEV double add_d(double a, double b) { return __dadd_rn(a, b); }
+B2_DEV double sqrt_d(double a) { return __dsqrt_rn(a); }
+B2_DEV double atan2_d(double y, double x) { return ::atan2(y, x); }
+#else
+B2_DEV double mul_d(double a, double b) { return a * b; }
+B2_DEV double add_d(double a, double b) { return a + b; }
+B2_DEV double sqrt_d(double a) { return std::sqrt(a); }
+B2_DEV double atan2_d(double y, double x) { return std::atan2(y, x); }
+#endif
+
 B2_DEV V3 mk3(float x, float y, float z) { V3 r; r.x = x; r.y = y; r.z = z; return r; }
 B2_DEV V3 v_add(V3 a, V3 b) { return mk3(add(a.x, b.x), add(a.y, b.y), add(a.z, b.z)); }
 B2_DEV V3 v_sub(V3 a, V3 b) { return mk3(sub(a.x, b.x), sub(a.y, b.y), sub(a.z, b.z)); }

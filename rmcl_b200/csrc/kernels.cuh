@@ -511,6 +511,88 @@ __global__ void k_o1dn_from_cloud(const uint8_t* __restrict__ cloud, CloudO1Dn c
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
+// Pc2ToScanNode::convert (pc2_to_scan.cpp:105-213) + fillEmpty (scan_operations.cpp:25-39) + MICPSphericalSensor*::unpackMessage
+// (MICPSphericalSensorCUDA.cpp:176-235) on the device, as a scatter in two passes: every point proposes a key to its cell, every cell
+// turns its key into a range and a dataset entry.  A key is ((point index + 1) << 32) | range bits, so the atomicMax of a cell keeps the
+// point of the highest index -- the reference's last writer in index order, whatever order the atomics arrive in.  0 = no point.
+// ---------------------------------------------------------------------------------------------------------------------
+struct CloudScan {
+    uint32_t width, n_points;               // points of the cloud (width * height, at most 2^32 - 2)
+    uint64_t row_step; uint32_t point_step;
+    uint32_t off[3];                        // byte offsets of x, y, z inside a point
+    uint32_t f64;                           // 1: FLOAT64 fields (narrowed to float), 0: FLOAT32
+    Tf T;                                   // T_sensor_cloud
+    float phi_min, phi_inc, theta_min, theta_inc;
+    uint32_t phi_n, theta_n;
+    float range_min, range_max, fill;       // fill: fillEmpty's range_max + 1
+};
+
+// bin of one angle (pc2_to_scan.cpp:195-196): (a - min) / inc in float, + 0.5 in double, truncated toward zero, so (-1.5, -0.5] goes to 0
+// and nothing wraps around (SURVEY D23); -1 outside [0, n).  A dimension of size 1 with increment 0 takes every angle (D24: the reference
+// divides 0 by 0 there); an increment of 0 with more than one bin is refused before any launch.
+B2_DEV int scan_bin(float a, float mn, float inc, uint32_t n)
+{
+    if (inc == 0.f) return n == 1 ? 0 : -1;
+    const double b = add_d((double)dvd(sub(a, mn), inc), 0.5);
+    return (b > -1.0 && b < (double)n) ? (int)b : -1;
+}
+
+// point i of the cloud (pc2_to_scan.cpp:186-209) -> its key, or 0 when it writes no cell; *cell receives the cell.  The angles are FP64
+// atan2 rounded to float; the elevation is taken against the horizontal distance sqrt(x^2 + y^2), not the reference's 3-D norm (D21).
+B2_DEV unsigned long long scan_point_key(float x, float y, float z, uint32_t i, const CloudScan& c, uint32_t& cell)
+{
+    if (!(finite_f32(x) && finite_f32(y) && finite_f32(z))) return 0ull;
+    const V3 p = tf_apply(c.T, mk3(x, y, z));                               // rm::Transform * Vector
+    const float r = v_l2norm(p);
+    const double px = p.x, py = p.y, pz = p.z;
+    const float theta = (float)atan2_d(py, px);
+    const float phi = (float)atan2_d(pz, sqrt_d(add_d(mul_d(px, px), mul_d(py, py))));
+    const int pid = scan_bin(phi, c.phi_min, c.phi_inc, c.phi_n), tid = scan_bin(theta, c.theta_min, c.theta_inc, c.theta_n);
+    if (pid < 0 || tid < 0 || !(r >= c.range_min && r <= c.range_max)) return 0ull;     // model.range.inside
+    cell = (uint32_t)pid * c.theta_n + (uint32_t)tid;
+    return ((unsigned long long)(i + 1u) << 32) | f2u(r);
+}
+
+// point i read at row * row_step + col * point_step (D22: the reference ignores row_step)
+B2_DEV unsigned long long scan_cloud_key(const uint8_t* cloud, const CloudScan& c, uint32_t i, uint32_t& cell)
+{
+    const uint32_t row = i / c.width, col = i - row * c.width;
+    const uint8_t* p = cloud + (uint64_t)row * c.row_step + (uint64_t)col * c.point_step;
+    const bool f64 = c.f64 != 0;
+    return scan_point_key(cloud_coord(p + c.off[0], f64), cloud_coord(p + c.off[1], f64), cloud_coord(p + c.off[2], f64), i, c, cell);
+}
+
+// cell k: its range (fill when no point won it), the dataset entry through the model's direction table, and the key reset for the next call
+B2_DEV void scan_cell_entry(uint32_t k, unsigned long long* keys, const CloudScan& c, const float* dirs, const float* origs, float* ranges,
+                            float* pts, uint8_t* mask)
+{
+    const unsigned long long key = keys[k];
+    keys[k] = 0ull;
+    const float r = key ? u2f((uint32_t)key) : c.fill;
+    ranges[k] = r;
+    dataset_entry(k, r, dirs, 3 * k, origs, 0, c.range_min, c.range_max, pts, mask);
+}
+
+// one thread per point of the cloud
+__global__ void k_scan_bin_cloud(const uint8_t* __restrict__ cloud, CloudScan c, unsigned long long* __restrict__ keys)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= c.n_points) return;
+    uint32_t cell = 0;
+    const unsigned long long key = scan_cloud_key(cloud, c, i, cell);
+    if (key) atomicMax(keys + cell, key);
+}
+
+// one thread per cell of the model
+__global__ void k_scan_cells(CloudScan c, unsigned long long* __restrict__ keys, const float* __restrict__ dirs, const float* __restrict__ origs,
+                             float* __restrict__ ranges, float* __restrict__ pts, uint8_t* __restrict__ mask)
+{
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= c.phi_n * c.theta_n) return;
+    scan_cell_entry(k, keys, c, dirs, origs, ranges, pts, mask);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
 // RCC*::find (RCCEmbree.cpp:26-36 ...): one thread per (pose, ray); writes the model buffers in the SENSOR frame
 // ---------------------------------------------------------------------------------------------------------------------
 struct RayModel {
