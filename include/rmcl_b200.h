@@ -306,6 +306,26 @@ B2_API int b2_pf_sensor_update(b2_pf* h, const b2_transform* poses_dev, b2_parti
  * kernel).  attrs_host is updated in place. */
 B2_API int b2_pf_sensor_update_host(b2_pf* h, const b2_transform* poses_host, b2_particle_attr* attrs_host, uint32_t n_particles,
                                     const b2_transform* Tsb, const b2_range_meas* beams_host, uint32_t n_beams, const b2_pf_params* params);
+/* PCDSensorUpdaterOptix::update's beam sampling (rmcl_ros/src/rmcl/PCDSensorUpdaterOptix.cpp:227-311): the beams of one sensor update drawn
+ * from a sensor_msgs/PointCloud2, for b2_pf_sensor_update / b2_pf_sensor_update_host as they are.
+ *  - Points are i = row * width + col, n_points = width * height; point i is read at row * row_step + col * point_step through the x, y and z
+ *    fields of `layout` (FLOAT32 as is, FLOAT64 narrowed to float), as b2_rcc_set_cloud_o1dn reads them.
+ *  - Sample k < n_samples makes up to 100 tries.  Try t takes raw = word t % 4 of Philox4x32-10 with counter (k, 3, step, t / 4) and key
+ *    `seed`, and reads point raw % n_points.  The draws depend on (seed, step, k) only: every rank of a sharded particle set that passes the
+ *    same seed and step gets the same beams.  Advance `step` per update.
+ *  - A try is valid iff x == x && y == y && z == z (NaN fails, an infinite coordinate passes).  A valid sample is orig = 0, range = |p|,
+ *    dir = p / range (float, individually rounded), cov = 0.1 I.  A finite (0,0,0) gives range 0 and NaN directions; an infinite coordinate
+ *    gives range inf.  A NaN component is stored as 0x7fffffff.
+ *  - Sampling stops at the 10th sample whose 100 tries all failed.  beams_host receives the valid samples before that point in sample order
+ *    (their likelihood merge order), *n_beams their count.  n_points == 0 or n_samples == 0: no beams, B2_OK.
+ * src_is_device != 0: `data` is a device address, read in place by one kernel on the handle's stream (one thread per sample); 68 B per
+ * sample come back and the call synchronises the stream.  Else `data` is host memory and the same function runs on the host over the
+ * points it draws; nothing is uploaded and nothing is launched.  Both give the same bytes.  Refused (B2_ERR_INVALID, no launch, nothing
+ * written): null pointers, a missing x, y or z field, a datatype other than 7 / 8, is_bigendian, a field that ends beyond point_step,
+ * `bytes` short of the end of the last point (any point may be drawn), more than 2^32 - 1 points.  The arguments are checked before the
+ * handle. */
+B2_API int b2_pf_sample_cloud(b2_pf* h, const void* data, uint64_t bytes, const b2_cloud_layout* layout, int src_is_device, uint32_t n_samples,
+                              uint64_t seed, uint32_t step, b2_range_meas* beams_host, uint32_t* n_beams);
 
 /* rest of the particle-filter cycle on the device (SURVEY.md 8f2), so that particles never leave HBM between stages:
  * TFMotionUpdaterGPU / particle_move_and_forget (rmcl_ros/src/rmcl/particle_motion.cu:11-46): pose = pose * T_bnew_bold, n_meas -= forget_rate * n_meas.

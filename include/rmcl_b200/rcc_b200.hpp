@@ -341,10 +341,15 @@ class PCDSensorUpdaterB200
 {
 public:
     // SensorUpdaterBase::init / reset (SensorUpdater.hpp:18-25).  The Embree updater loads its map in init() (PCDSensorUpdaterEmbree.cpp:136-189);
-    // here the map arrives through the constructor, so init() only checks it and reset() drops the beams of the last cloud.
+    // here the map arrives through the constructor, so init() only checks it and reset() drops the input cloud and the beams.
     void init() B2_PF_OVERRIDE { if (!map_) throw std::runtime_error("NO MAP"); }
-    void reset() B2_PF_OVERRIDE { beams_.clear(); }
+    void reset() B2_PF_OVERRIDE { beams_.clear(); input_ = CloudInput{}; }
     b2_pf_params config{2.0f, 100.0f, 100.0f, 0.0f, 0.05f, 80.0f, 0, 0};                         // PCDSensorUpdaterEmbree.cpp:122-134
+    // beam sampling from the input cloud (b2_pf_sample_cloud): `samples` per update (PCDSensorUpdaterEmbree.cpp:124), drawn with (seed, step);
+    // every update that samples advances step.  Set seed once (e.g. from the clock); every rank of a sharded set must use the same seed and step.
+    uint32_t samples = 100;
+    uint64_t seed = 0;
+    uint32_t step = 0;
     explicit PCDSensorUpdaterB200(B200MapPtr map) : map_(std::move(map))
     {
         if (!map_) throw std::runtime_error("NO MAP");
@@ -352,13 +357,22 @@ public:
     }
     ~PCDSensorUpdaterB200() { b2_pf_destroy(h_); }
     void setTsb(const rm::Transform& Tsb) { Tsb_ = Tsb; }
-    // beams replace the random_device sampling of :276-327 (quirk D5): the caller samples the cloud and passes RangeMeasurements
-    void setBeams(const std::vector<RangeMeasurement>& beams) { beams_ = beams; }
+    // Input<PointCloud2::ConstSharedPtr>::setInput (rmcl_localization.cpp:512-530): the PointCloud2 bytes both update()s sample their beams
+    // from (PCDSensorUpdaterOptix.cpp:227-311).  The bytes are read when update() runs: keep_alive holds their owner until the next
+    // setInput / setBeams / reset.  on_device: `data` is a device address, read in place by a kernel.  Replaces beams set by setBeams.
+    void setInput(const void* data, uint64_t bytes, const b2_cloud_layout& layout, bool on_device, std::shared_ptr<const void> keep_alive = {})
+    {
+        input_ = CloudInput{true, data, bytes, layout, on_device, std::move(keep_alive)};
+        beams_.clear();
+    }
+    // beams passed as they are (quirk D5: the caller samples the cloud into RangeMeasurements); replaces the input cloud
+    void setBeams(const std::vector<RangeMeasurement>& beams) { beams_ = beams; input_ = CloudInput{}; }
     // how rays are mapped to lanes (a schedule, results identical): 0 beams of one particle, 1 particles, 2 particles sorted by pose, 3 (default) by timing
     void setMapping(int mode) { b2_check(b2_pf_set_mapping(h_, mode), "setMapping"); }
     // ParticleUpdater<RAM>::update
     ParticleUpdateResults update(rm::MemoryView<rm::Transform, rm::RAM> poses, rm::MemoryView<ParticleAttributes, rm::RAM> attrs, const ParticleUpdateConfig& = {})
     {
+        sample_input();
         b2_check(b2_pf_sensor_update_host(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(),
                                           reinterpret_cast<const b2_transform*>(&Tsb_), reinterpret_cast<const b2_range_meas*>(beams_.data()), (uint32_t)beams_.size(), &config), "update");
         return {};
@@ -366,6 +380,7 @@ public:
     // ParticleUpdater<VRAM_CUDA>::update (ParticleUpdater.hpp:39-43)
     ParticleUpdateResults update(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs, const ParticleUpdateConfig& = {}) B2_PF_OVERRIDE
     {
+        sample_input();
         b2_check(b2_pf_sensor_update(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(),
                                      reinterpret_cast<const b2_transform*>(&Tsb_), reinterpret_cast<const b2_range_meas*>(beams_.data()), (uint32_t)beams_.size(), &config), "update");
         return {};
@@ -425,10 +440,23 @@ public:
         return s;
     }
 private:
+    struct CloudInput { bool set = false; const void* data = nullptr; uint64_t bytes = 0; b2_cloud_layout layout{}; bool on_device = false; std::shared_ptr<const void> keep_alive; };
+    // with an input cloud: this update's beams, `samples` drawn with (seed, step), then step advances
+    void sample_input()
+    {
+        if (!input_.set) return;
+        beams_.resize(samples);
+        uint32_t n = 0;
+        b2_check(b2_pf_sample_cloud(h_, input_.data, input_.bytes, &input_.layout, input_.on_device ? 1 : 0, samples, seed, step,
+                                    reinterpret_cast<b2_range_meas*>(beams_.data()), &n), "update");
+        beams_.resize(n);
+        step++;
+    }
     B200MapPtr map_;
     b2_pf* h_ = nullptr;
     rm::Transform Tsb_ = rm::Transform::Identity();
     std::vector<RangeMeasurement> beams_;
+    CloudInput input_;
 };
 
 }  // namespace rmcl

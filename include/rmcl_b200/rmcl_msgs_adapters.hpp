@@ -13,6 +13,8 @@
 //                            O1Dn sensor's unpackMessage + setModel in one device call (RCCB200O1Dn::setPointCloud); fields x, y, z looked up by name
 //   unpackPointCloud(rcc, cloud, T)  pc2_to_scan (Pc2ToScanNode::convert + fillEmpty: pc2_to_scan.cpp:105-213, scan_operations.cpp:25-39) and the
 //                            spherical sensor's unpackMessage in one device call (RCCB200Spherical::setPointCloud), into the model of its setModel
+//   setInput(updater, msg)   Input<PointCloud2::ConstSharedPtr>::setInput of the PF sensor updater (rmcl_localization.cpp:512-530): its
+//                            updates sample their beams from the message (PCDSensorUpdaterB200::setInput), which it holds meanwhile
 //   fillSensorStats(...)     rmcl_msgs/MICPSensorStats as published at rmcl_ros/src/nodes/micp_localization.cpp:1009-1015
 //   fillParticleStats(...)   rmcl_msgs/ParticleStats as RmclNode::estimateStats returns it (rmcl_ros/src/nodes/rmcl_localization.cpp:642-731)
 #pragma once
@@ -98,6 +100,14 @@ template <typename PointCloud2T> inline void unpackPointCloud(RCCB200Spherical& 
                                                               const rm::Transform& T_sensor_cloud = rm::Transform::Identity())
 {
     rcc.setPointCloud(cloud.data.data(), cloud.data.size(), cloudLayout(cloud), T_sensor_cloud);
+}
+
+// RmclNode::sensorUpdate hands each cloud to the updater (rmcl_localization.cpp:512-530); the updater holds the message as Input<> holds
+// input_, and its next update() samples the beams from it on the host
+template <typename PointCloud2T> inline void setInput(PCDSensorUpdaterB200& updater, const std::shared_ptr<const PointCloud2T>& msg)
+{
+    if (!msg) throw std::invalid_argument("setInput: null message");
+    updater.setInput(msg->data.data(), msg->data.size(), cloudLayout(*msg), false, msg);
 }
 
 // rmcl_msgs/MICPSensorStats (micp_localization.cpp:1009-1015): valid_matches = Cmerged_o.n_meas, cov_trace = trace(Cmerged_o.covariance)

@@ -124,7 +124,7 @@ EXPORTS = [
     "b2_rcc_set_correspondence_type", "b2_pf_resample_gladiator", "b2_pf_gladiator_randoms", "b2_rcc_segment", "b2_mesh_create_from_file", "b2_mesh_file_load", "b2_mesh_file_free", "b2_peek_cuda_error", "b2_mesh_blob_size", "b2_mesh_export_blob", "b2_mesh_create_from_blob", "b2_mesh_refit",
     "b2_rcc_correct_once_async", "b2_rcc_correct_once_wait", "b2_micp_correct_once", "b2_rcc_set_exec_mode", "b2_debug_read_bandwidth", "b2_rcc_set_sim_options", "b2_rcc_bind_dataset", "b2_rcc_bind_model_buffers", "b2_rcc_benchmark_batch", "b2_pf_p2p_init", "b2_pf_p2p_connect", "b2_pf_p2p_publish", "b2_pf_resample_gladiator_p2p", "b2_pf_p2p_connect_local", "b2_rcc_set_cpc_options", "b2_pf_set_mapping", "b2_pf_get_mapping",
     "b2_micp_correct", "b2_pf_init_uniform", "b2_pf_init_gaussian", "b2_pf_estimate_stats", "b2_rcc_set_cloud_o1dn",
-    "b2_rcc_set_cloud_spherical",
+    "b2_rcc_set_cloud_spherical", "b2_pf_sample_cloud",
 ]
 
 
@@ -647,7 +647,8 @@ def umeyama_transform(stats, device=0):
 
 class PCDSensorUpdaterB200:
     """Particle-filter sensor update: ParticleUpdater<MemT>::update (rmcl_ros/include/rmcl_ros/rmcl/ParticleUpdater.hpp:39-43) with the
-    hot loop of PCDSensorUpdaterEmbree::update (PCDSensorUpdaterEmbree.cpp:290-342).  Beams are an input (quirk D5)."""
+    hot loop of PCDSensorUpdaterEmbree::update (PCDSensorUpdaterEmbree.cpp:290-342).  Its beams are drawn from the cloud of setInput
+    (`samples` of them, keyed by `seed` and `step`; quirk D5) or passed to update()."""
 
     def __init__(self, map_: Map):
         self.map = map_
@@ -655,6 +656,10 @@ class PCDSensorUpdaterB200:
         _chk(load_library().b2_pf_create(map_._h, C.byref(h)))
         self._h = h
         self.config = PFParams.defaults()
+        self.samples = 100              # PCDSensorUpdaterEmbree.cpp:124
+        self.seed = 0                   # the same on every rank of a sharded particle set
+        self.step = 0                   # advanced by every update() that samples the input
+        self._input = None
 
     def close(self):
         if getattr(self, "_h", None):
@@ -679,11 +684,36 @@ class PCDSensorUpdaterB200:
         _chk(load_library().b2_pf_get_mapping(self._h, C.byref(mode), C.byref(cur)))
         return mode.value, cur.value
 
-    def update(self, particle_poses, particle_attrs, Tsb, beams, params: PFParams | None = None, inplace=False):
+    def sampleBeams(self, cloud, n_samples=None, seed=None, step=None):
+        """PCDSensorUpdaterOptix::update's beam sampling (PCDSensorUpdaterOptix.cpp:227-311, b2_pf_sample_cloud): up to `n_samples` (default
+        self.samples) beams drawn from the finite points of a PointCloud2-shaped `cloud`, keyed by (seed, step) (default self.seed / self.step),
+        as a RANGE_MEAS_DTYPE array in merge order.  A CUDA uint8 tensor as cloud.data is read in place by a kernel; host data is read on the
+        host where the draws land."""
+        n = self.samples if n_samples is None else int(n_samples)
+        L = cloud_layout(cloud)
+        ptr, nbytes, dev = _cloud_buffer(cloud)
+        out = np.zeros(n, RANGE_MEAS_DTYPE)
+        got = C.c_uint32()
+        _chk(load_library().b2_pf_sample_cloud(self._h, ptr, C.c_uint64(nbytes), C.byref(L), C.c_int(dev), C.c_uint32(n),
+                                               C.c_uint64(self.seed if seed is None else int(seed)), C.c_uint32(self.step if step is None else int(step)),
+                                               _p(out) if n else None, C.byref(got)))
+        return out[: got.value]
+
+    def setInput(self, cloud):
+        """Input<PointCloud2::ConstSharedPtr>::setInput (rmcl_localization.cpp:512-530): the cloud the next update() samples its beams from.
+        The reference is kept; the data is read when update() runs."""
+        self._input = cloud
+
+    def update(self, particle_poses, particle_attrs, Tsb, beams=None, params: PFParams | None = None, inplace=False):
         """RAM variant: numpy arrays in, updated attrs array out (inplace=True: the caller's attrs array is updated itself, as the reference's
         update(MemoryView) does -- no staging copy; pin the arrays and the transfers overlap the kernel).  VRAM variant: torch CUDA tensors, attrs
-        updated in place."""
+        updated in place.  beams=None: `samples` beams are drawn from the setInput cloud with (seed, step), then step advances by one."""
         prm = params or self.config
+        if beams is None:
+            if self._input is None:
+                raise B2Error(-1, "update: no beams and no input cloud (setInput first)")
+            beams = self.sampleBeams(self._input)
+            self.step += 1
         beams = np.ascontiguousarray(beams)
         assert beams.dtype.itemsize == 64
         Tsb = _tf(Tsb)

@@ -714,6 +714,33 @@ extern "C" int b2_rcc_set_ranges(b2_rcc* h, const float* ranges, uint32_t n, int
     return B2_OK;
 }
 
+// The layout checks every cloud entry point makes before it reads a byte: x, y and z present, FLOAT32 or FLOAT64, little-endian, each
+// field inside point_step, and -- when the call reads any point -- `bytes` reaching the end of the last point it reads (row last_row,
+// column last_col).  *need receives that end (0 when nothing is read).  `who` prefixes every message; the two refs follow the messages
+// on a missing field and on the datatype.
+static int check_cloud_layout(const b2_cloud_layout* L, uint64_t bytes, bool reads, uint64_t last_row, uint64_t last_col, const char* who,
+                              const char* no_field_ref, const char* datatype_ref, uint64_t* need)
+{
+    const uint32_t off[3] = {L->offset_x, L->offset_y, L->offset_z};
+    if (off[0] == B2_CLOUD_NO_FIELD || off[1] == B2_CLOUD_NO_FIELD || off[2] == B2_CLOUD_NO_FIELD)
+        return fail(B2_ERR_INVALID, "%s: the cloud has no x, y or z field%s", who, no_field_ref);
+    if (L->datatype != 7 && L->datatype != 8)
+        return fail(B2_ERR_INVALID, "%s: field x has datatype %u; FLOAT32 (7) and FLOAT64 (8) are read%s", who, (unsigned)L->datatype, datatype_ref);
+    if (L->is_bigendian) return fail(B2_ERR_INVALID, "%s: big-endian clouds are not read", who);
+    const uint32_t fsz = L->datatype == 8 ? 8u : 4u;
+    for (int c = 0; c < 3; c++)
+        if ((uint64_t)off[c] + fsz > L->point_step) return fail(B2_ERR_INVALID, "%s: field %c at offset %u ends beyond point_step %u", who, "xyz"[c], off[c], L->point_step);
+    *need = 0;
+    if (!reads) return B2_OK;
+    const unsigned __int128 last = (unsigned __int128)last_row * L->row_step + (unsigned __int128)last_col * L->point_step +
+                                   std::max(off[0], std::max(off[1], off[2])) + fsz;
+    if (last > (unsigned __int128)bytes)
+        return fail(B2_ERR_INVALID, "%s: %llu bytes given, the last point read ends at byte %llu", who, (unsigned long long)bytes,
+                    last > (unsigned __int128)UINT64_MAX ? (unsigned long long)UINT64_MAX : (unsigned long long)last);
+    *need = (uint64_t)last;
+    return B2_OK;
+}
+
 // Pc2ToO1DnNode::convert + MICPO1DnSensorCUDA::unpackMessage + setModel (conversions.cpp:869-1073, scan_operations.cpp:41-143,
 // MICPO1DnSensorCUDA.cpp:142-148,171-230) as one kernel.  Every check runs before anything of the handle changes: where the reference
 // throws, divides by zero, underflows size_t or reads past the message, the call is refused.  A host cloud is uploaded whole up to the last
@@ -721,33 +748,18 @@ extern "C" int b2_rcc_set_ranges(b2_rcc* h, const float* ranges, uint32_t n, int
 extern "C" int b2_rcc_set_cloud_o1dn(b2_rcc* h, const void* data, uint64_t bytes, const b2_cloud_layout* L, const b2_o1dn_cloud_filter* F, int src_is_device)
 {
     NOTNULL(data); NOTNULL(L); NOTNULL(F);          // the arguments are checked before the handle: the checks need no device
-    const uint32_t off[3] = {L->offset_x, L->offset_y, L->offset_z};
-    if (off[0] == B2_CLOUD_NO_FIELD || off[1] == B2_CLOUD_NO_FIELD || off[2] == B2_CLOUD_NO_FIELD)
-        return fail(B2_ERR_INVALID, "set_cloud_o1dn: the cloud has no x, y or z field (\"NO POINT FIELD IN CLOUD!\", conversions.cpp:955-958)");
-    if (L->datatype != 7 && L->datatype != 8)
-        return fail(B2_ERR_INVALID, "set_cloud_o1dn: field x has datatype %u; FLOAT32 (7) and FLOAT64 (8) are read (conversions.cpp:977-990)", (unsigned)L->datatype);
-    if (L->is_bigendian) return fail(B2_ERR_INVALID, "set_cloud_o1dn: big-endian clouds are not read");
     if (F->height_increment == 0 || F->width_increment == 0) return fail(B2_ERR_INVALID, "set_cloud_o1dn: increment 0 (height %u, width %u)", F->height_increment, F->width_increment);
     if ((uint64_t)F->height_skip_begin + F->height_skip_end > L->height || (uint64_t)F->width_skip_begin + F->width_skip_end > L->width)
         return fail(B2_ERR_INVALID, "set_cloud_o1dn: skips %u+%u of height %u / %u+%u of width %u", F->height_skip_begin, F->height_skip_end, L->height,
                     F->width_skip_begin, F->width_skip_end, L->width);
-    const uint32_t fsz = L->datatype == 8 ? 8u : 4u;
-    for (int c = 0; c < 3; c++)
-        if ((uint64_t)off[c] + fsz > L->point_step) return fail(B2_ERR_INVALID, "set_cloud_o1dn: field %c at offset %u ends beyond point_step %u", "xyz"[c], off[c], L->point_step);
     const uint64_t w_out = (L->width - F->width_skip_begin - F->width_skip_end) / F->width_increment;
     const uint64_t h_out = (L->height - F->height_skip_begin - F->height_skip_end) / F->height_increment;
     const uint64_t n = w_out * h_out;
     if (n > 0xffffffffu / 4) return fail(B2_ERR_INVALID, "set_cloud_o1dn: model too large (%llu rays)", (unsigned long long)n);
     uint64_t need = 0;
-    if (n) {
-        const unsigned __int128 last = (unsigned __int128)((h_out - 1) * F->height_increment + F->height_skip_begin) * L->row_step +
-                                       (unsigned __int128)((w_out - 1) * F->width_increment + F->width_skip_begin) * L->point_step +
-                                       std::max(off[0], std::max(off[1], off[2])) + fsz;
-        if (last > (unsigned __int128)bytes)
-            return fail(B2_ERR_INVALID, "set_cloud_o1dn: %llu bytes given, the last point read ends at byte %llu", (unsigned long long)bytes,
-                        last > (unsigned __int128)UINT64_MAX ? (unsigned long long)UINT64_MAX : (unsigned long long)last);
-        need = (uint64_t)last;
-    }
+    RES(check_cloud_layout(L, bytes, n != 0, n ? (h_out - 1) * F->height_increment + F->height_skip_begin : 0, n ? (w_out - 1) * F->width_increment + F->width_skip_begin : 0,
+                           "set_cloud_o1dn", " (\"NO POINT FIELD IN CLOUD!\", conversions.cpp:955-958)", " (conversions.cpp:977-990)", &need));
+    const uint32_t off[3] = {L->offset_x, L->offset_y, L->offset_z};
     NOTNULL(h);
     CU(cudaSetDevice(h->map->device));
     const bool keep_schedule = h->model_from_cloud && h->has_model && h->width == (uint32_t)w_out && h->height == (uint32_t)h_out;
@@ -794,25 +806,11 @@ extern "C" int b2_rcc_set_cloud_spherical(b2_rcc* h, const void* data, uint64_t 
     NOTNULL(L); NOTNULL(T);                         // the arguments are checked before the handle: the checks need no device
     const uint64_t n_points = (uint64_t)L->width * L->height;
     if (n_points) NOTNULL(data);
-    const uint32_t off[3] = {L->offset_x, L->offset_y, L->offset_z};
-    if (off[0] == B2_CLOUD_NO_FIELD || off[1] == B2_CLOUD_NO_FIELD || off[2] == B2_CLOUD_NO_FIELD)
-        return fail(B2_ERR_INVALID, "set_cloud_spherical: the cloud has no x, y or z field");
-    if (L->datatype != 7 && L->datatype != 8)
-        return fail(B2_ERR_INVALID, "set_cloud_spherical: field x has datatype %u; FLOAT32 (7) and FLOAT64 (8) are read (pc2_to_scan.cpp:167-184)", (unsigned)L->datatype);
-    if (L->is_bigendian) return fail(B2_ERR_INVALID, "set_cloud_spherical: big-endian clouds are not read");
-    const uint32_t fsz = L->datatype == 8 ? 8u : 4u;
-    for (int c = 0; c < 3; c++)
-        if ((uint64_t)off[c] + fsz > L->point_step) return fail(B2_ERR_INVALID, "set_cloud_spherical: field %c at offset %u ends beyond point_step %u", "xyz"[c], off[c], L->point_step);
     if (n_points > 0xfffffffeull) return fail(B2_ERR_INVALID, "set_cloud_spherical: %llu points, at most 2^32 - 2 are read", (unsigned long long)n_points);
     uint64_t need = 0;
-    if (n_points) {
-        const unsigned __int128 last = (unsigned __int128)(L->height - 1) * L->row_step + (unsigned __int128)(L->width - 1) * L->point_step +
-                                       std::max(off[0], std::max(off[1], off[2])) + fsz;
-        if (last > (unsigned __int128)bytes)
-            return fail(B2_ERR_INVALID, "set_cloud_spherical: %llu bytes given, the last point read ends at byte %llu", (unsigned long long)bytes,
-                        last > (unsigned __int128)UINT64_MAX ? (unsigned long long)UINT64_MAX : (unsigned long long)last);
-        need = (uint64_t)last;
-    }
+    RES(check_cloud_layout(L, bytes, n_points != 0, n_points ? L->height - 1 : 0, n_points ? L->width - 1 : 0, "set_cloud_spherical", "",
+                           " (pc2_to_scan.cpp:167-184)", &need));
+    const uint32_t off[3] = {L->offset_x, L->offset_y, L->offset_z};
     const float Tv[7] = {T->R.x, T->R.y, T->R.z, T->R.w, T->t.x, T->t.y, T->t.z};
     if (!all_finite(Tv, 7)) return fail(B2_ERR_INVALID, "set_cloud_spherical: T_sensor_cloud is not finite");
     NOTNULL(h);
@@ -1788,6 +1786,8 @@ struct b2_pf {
     PfPeers peers{}; bool peers_open = false; DevBuf<unsigned long long> d_traffic;
     // pose estimate (b2_pf_estimate_stats), allocated at its first call: block partials of both passes, the record, Tbm and tickets
     DevBuf<double> d_est_part; DevBuf<PfEstimateScratch> d_est; b2_particle_stats* h_est = nullptr;
+    // beam sampling from a device cloud (b2_pf_sample_cloud): one record per sample, and its pinned host copy
+    DevBuf<PfBeamSample> d_samples; PfBeamSample* h_samples = nullptr; uint32_t h_samples_cap = 0;
 };
 
 extern "C" int b2_pf_destroy(b2_pf* h);
@@ -1847,6 +1847,8 @@ extern "C" int b2_pf_destroy(b2_pf* h)
     h->d_traffic.release();
     h->d_est_part.release(); h->d_est.release();
     if (h->h_est) cudaFreeHost(h->h_est);
+    h->d_samples.release();
+    if (h->h_samples) cudaFreeHost(h->h_samples);
     b2_mesh* map = h->map;
     delete h;
     (void)cudaGetLastError();
@@ -2039,6 +2041,54 @@ extern "C" int b2_pf_sensor_update_host(b2_pf* h, const b2_transform* poses, b2_
     }
     if (n_chunks > 1) { CU(cudaEventRecord(h->ev_side, h->side)); CU(cudaStreamWaitEvent(h->stream, h->ev_side, 0)); }
     CU(cudaStreamSynchronize(h->stream));
+    return B2_OK;
+}
+
+// PCDSensorUpdaterOptix::update's beam sampling (PCDSensorUpdaterOptix.cpp:227-311).  pf_sample_beam (kernels.cuh) runs where the cloud
+// lives: a device cloud by k_pf_sample_cloud on the handle's stream, after which 68 B per sample come back; a host cloud by the same
+// function in a host loop that reads only the points it draws, so the cloud is never uploaded (scripts/bench_pf_cloud.py measures both).
+// The give-up rule then runs over the samples in order.
+extern "C" int b2_pf_sample_cloud(b2_pf* h, const void* data, uint64_t bytes, const b2_cloud_layout* L, int src_is_device, uint32_t n_samples,
+                                  uint64_t seed, uint32_t step, b2_range_meas* beams, uint32_t* n_beams)
+{
+    NOTNULL(L); NOTNULL(n_beams);                   // the arguments are checked before the handle: the checks need no device
+    const uint64_t n_points = (uint64_t)L->width * L->height;
+    if (n_points) NOTNULL(data);
+    if (n_samples) NOTNULL(beams);
+    if (n_points > 0xffffffffull) return fail(B2_ERR_INVALID, "pf_sample_cloud: %llu points, at most 2^32 - 1 are read", (unsigned long long)n_points);
+    uint64_t need = 0;
+    RES(check_cloud_layout(L, bytes, n_points != 0, n_points ? L->height - 1 : 0, n_points ? L->width - 1 : 0, "pf_sample_cloud", "", "", &need));
+    NOTNULL(h);
+    *n_beams = 0;
+    if (n_points == 0 || n_samples == 0) return B2_OK;
+    CloudBeams c;
+    c.width = L->width; c.n_points = (uint32_t)n_points; c.row_step = L->row_step; c.point_step = L->point_step;
+    c.off[0] = L->offset_x; c.off[1] = L->offset_y; c.off[2] = L->offset_z;
+    c.f64 = L->datatype == 8 ? 1u : 0u;
+    c.seed = seed; c.step = step;
+    const uint8_t* src = static_cast<const uint8_t*>(data);
+    if (src_is_device) {
+        CU(cudaSetDevice(h->map->device));
+        RES(h->d_samples.reserve(n_samples));
+        if (h->h_samples_cap < n_samples) {
+            if (h->h_samples) cudaFreeHost(h->h_samples);
+            h->h_samples = nullptr; h->h_samples_cap = 0;
+            CU(cudaMallocHost((void**)&h->h_samples, sizeof(PfBeamSample) * (size_t)n_samples));
+            h->h_samples_cap = n_samples;
+        }
+        k_pf_sample_cloud<<<(n_samples + 127) / 128, 128, 0, h->stream>>>(src, c, n_samples, h->d_samples.p);
+        LAUNCHED();
+        CU(cudaMemcpyAsync(h->h_samples, h->d_samples.p, sizeof(PfBeamSample) * (size_t)n_samples, cudaMemcpyDeviceToHost, h->stream));
+        CU(cudaStreamSynchronize(h->stream));
+    }
+    uint32_t n_out = 0, invalids = 0;
+    for (uint32_t k = 0; k < n_samples && invalids < B2_PF_BEAM_MAX_INVALIDS; k++) {       // :264-287: stop at the 10th sample that found no point
+        b2_range_meas m;
+        const bool valid = src_is_device ? (m = h->h_samples[k].m, h->h_samples[k].valid != 0u) : pf_sample_beam(src, c, k, &m);
+        if (valid) beams[n_out++] = m;
+        else invalids++;
+    }
+    *n_beams = n_out;
     return B2_OK;
 }
 

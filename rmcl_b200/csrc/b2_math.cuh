@@ -10,7 +10,8 @@
 #include "../../include/rmcl_b200.h"
 
 // B2_DEV functions are host+device so that tests/emul can run the SAME traversal/math code on the CPU (test harness only;
-// the product library instantiates them in __global__ kernels exclusively).
+// the product library instantiates them in __global__ kernels, and on the host only in b2_pf_sample_cloud's loop over a host cloud,
+// which api.cu compiles with -ffp-contract=off like the harness).
 #define B2_DEV __host__ __device__ __forceinline__
 #if defined(__CUDA_ARCH__)
 #define B2_ON_DEVICE 1

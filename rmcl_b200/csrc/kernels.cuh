@@ -1327,9 +1327,11 @@ __global__ void k_pf_gladiator_randoms(uint64_t seed, uint32_t step, uint32_t fi
 // Particle set initialisation: RmclNode::initSamplesUniform (rmcl_ros/src/nodes/rmcl_localization.cpp:277-342) and
 // RmclNode::initSamples(PoseWithCovarianceStamped) (:165-275).  Draws: Philox4x32-10 with counter (global particle index, domain tag,
 // 0, block) and key = seed.  The tags are non-zero and Gladiator's second counter word is always 0, so no two streams share a counter.
+// The beam sampling of the sensor update (b2_pf_sample_cloud, below) draws with tag 3.
 // ---------------------------------------------------------------------------------------------------------------------
 #define B2_PF_INIT_TAG_UNIFORM 1u
 #define B2_PF_INIT_TAG_GAUSSIAN 2u
+#define B2_PF_BEAM_TAG 3u
 struct PfInitBox { float lo[6], hi[6]; };                  // x, y, z, roll, pitch, yaw; lo <= hi, finite, hi - lo finite (checked on the host)
 struct PfInitGauss { float L[36]; b2_transform Tlm; };     // Cholesky factor of the covariance (row-major, lower), message pose
 B2_DEV float u01_closed_open(uint32_t r) { return mul((float)(r >> 8), 5.9604644775390625e-08f); }   // [0, 1), exact
@@ -1385,6 +1387,65 @@ __global__ void __launch_bounds__(256) k_pf_init_gaussian(b2_transform* __restri
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     pf_init_gaussian_one(seed, first + i, g, poses + i, attrs + i);
+}
+#endif
+
+// ---------------------------------------------------------------------------------------------------------------------
+// The sensor update's beam sampling: PCDSensorUpdaterOptix::update (rmcl_ros/src/rmcl/PCDSensorUpdaterOptix.cpp:227-311).  Sample k makes
+// up to B2_PF_BEAM_TRIES tries; try t reads point raw % n_points, raw = word t % 4 of Philox4x32-10 with counter (k, B2_PF_BEAM_TAG, step,
+// t / 4) and key = seed.  The draws depend on (seed, step, k) only, so every rank of a sharded particle set samples the same beams.  The
+// give-up rule over the samples (B2_PF_BEAM_MAX_INVALIDS) runs on the host (b2_pf_sample_cloud).
+// ---------------------------------------------------------------------------------------------------------------------
+#define B2_PF_BEAM_TRIES 100u                  // max_tries (:267)
+#define B2_PF_BEAM_MAX_INVALIDS 10u            // max_invalids (:264)
+struct CloudBeams {
+    uint32_t width, n_points;               // points of the cloud (width * height, 1 .. 2^32 - 1)
+    uint64_t row_step; uint32_t point_step;
+    uint32_t off[3];                        // byte offsets of x, y, z inside a point
+    uint32_t f64;                           // 1: FLOAT64 fields (narrowed to float), 0: FLOAT32
+    uint64_t seed; uint32_t step;
+};
+struct PfBeamSample { b2_range_meas m; uint32_t valid; };         // one sample as the kernel hands it to the host (68 B)
+
+// word w (0..3) of a Philox block, without indexing the array at run time (it stays in registers)
+B2_DEV uint32_t philox_word(const uint32_t r[4], uint32_t w) { return w == 0u ? r[0] : w == 1u ? r[1] : w == 2u ? r[2] : r[3]; }
+// NaN components are stored as 0x7fffffff whatever produced them, so that the host and the device write the same bytes
+B2_DEV float canon_nan(float v) { return v == v ? v : u2f(0x7fffffffu); }
+
+// sample k (:265-306): true and *m filled from the first try whose x, y and z are not NaN (an infinite coordinate passes, :278); false when
+// every try failed.  orig = 0, range = |p|, dir = p / range (:291-293) -- a finite (0,0,0) gives range 0 and NaN directions -- cov = 0.1 I
+// (:296-301).  Point i is read at row * row_step + col * point_step through the fields (the reference reads float32 at i * point_step, D26).
+B2_DEV bool pf_sample_beam(const uint8_t* cloud, const CloudBeams& c, uint32_t k, b2_range_meas* m)
+{
+    const bool f64 = c.f64 != 0;
+    uint32_t r[4] = {0u, 0u, 0u, 0u};
+    for (uint32_t t = 0; t < B2_PF_BEAM_TRIES; t++) {
+        if ((t & 3u) == 0u) philox4x32_10(k, B2_PF_BEAM_TAG, c.step, t >> 2, (uint32_t)c.seed, (uint32_t)(c.seed >> 32), r);
+        const uint32_t i = philox_word(r, t & 3u) % c.n_points;
+        const uint32_t row = i / c.width, col = i - row * c.width;
+        const uint8_t* p = cloud + (uint64_t)row * c.row_step + (uint64_t)col * c.point_step;
+        const float x = cloud_coord(p + c.off[0], f64), y = cloud_coord(p + c.off[1], f64), z = cloud_coord(p + c.off[2], f64);
+        if (!(x == x && y == y && z == z)) continue;
+        const float range = v_l2norm(mk3(x, y, z));
+        m->orig.x = 0.f; m->orig.y = 0.f; m->orig.z = 0.f;
+        m->dir.x = canon_nan(dvd(x, range)); m->dir.y = canon_nan(dvd(y, range)); m->dir.z = canon_nan(dvd(z, range));
+        m->range = range;
+        #pragma unroll
+        for (int e = 0; e < 9; e++) m->cov.m[e] = (e % 4 == 0) ? 0.1f : 0.f;
+        return true;
+    }
+    return false;
+}
+
+#ifdef __CUDACC__
+// one thread per sample; reads at most B2_PF_BEAM_TRIES points, writes 68 B
+__global__ void __launch_bounds__(128) k_pf_sample_cloud(const uint8_t* __restrict__ cloud, CloudBeams c, uint32_t n_samples, PfBeamSample* __restrict__ out)
+{
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n_samples) return;
+    PfBeamSample s = {};
+    s.valid = pf_sample_beam(cloud, c, k, &s.m) ? 1u : 0u;
+    out[k] = s;
 }
 #endif
 
