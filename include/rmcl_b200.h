@@ -404,6 +404,29 @@ typedef char b2_particle_stats_is_440_bytes[sizeof(b2_particle_stats) == 440 ? 1
  * gives them, and the rest is filled in; the call still returns B2_OK.  n == 0 and null pointers are refused before any launch. */
 B2_API int b2_pf_estimate_stats(b2_pf* h, const b2_transform* poses_dev, const b2_particle_attr* attrs_dev, uint32_t n, b2_particle_stats* out_host);
 
+/* ResidualResamplerCPU::update (rmcl_ros/src/rmcl/ResidualResamplerCPU.cpp:55-202; config and defaults :35-47, the fields of Gladiator's) on
+ * the device.  Resamples the n particles poses_dev / attrs_dev into an output set of M = n_new slots; the set may grow (the node passes its
+ * whole max_particles buffer).
+ *  - S = weight_sum and weight_max = max(0, L_i) of likelihood.mean in double, in the order of b2_pf_estimate_stats: S / n and weight_max
+ *    equal its likelihood.mean and .max bit for bit for the same n.
+ *  - Draw j = 0, 1, ... picks parent word j % 4 of Philox4x32-10 with counter (lo(j / 4), 4, step, hi(j / 4)) and key `seed`, modulo n, and
+ *    inserts min((uint64)(L / S * M), slots left) copies.  Draws that insert nothing are consumed.  The draws stop when all M slots are
+ *    filled, or after D_max = 16 * max(n, M) draws (the reference's loop need not end); the slots filled by then are the result.
+ *  - The copy in slot k takes its six normals from Box-Muller on words 0-5 of the counters (k, 5, step, 0) and (k, 5, step, 1): t += N *
+ *    (float)(min_noise / (L / weight_max)) for x, y, z, then roll, pitch, yaw of R likewise; n_meas *= (float)(pow(forget_per_meter,
+ *    |d.t|^2) * pow(forget_per_radian, |d.R|)) with d = ~pose * pose_new, truncated; the rest, the stamp included, is the parent's.
+ *  - S not finite, S <= 0 or a likelihood below 0: 0 slots, nothing written, B2_OK (the node skips resampling below 10 particles).
+ * poses_new_dev / attrs_new_dev hold n_local entries: entry i is slot first + i.  The call writes the entries whose slot is below
+ * n_particles and leaves the others untouched, so ranks of a sharded set that pass the same (all-gathered) input and disjoint slices
+ * [first, first + n_local) together write the one global result.  Runs on the handle's stream and synchronises it: one read-back after the
+ * statistics and one per chunk of draws (chunks double from max(2n, 2^16) up to 2 max(n, M)).  Refused (B2_ERR_INVALID, no launch, nothing
+ * written): null pointers, n == 0, n_new == 0, first + n_local > n_new, an output range overlapping an input range or the other output. */
+typedef b2_gladiator_config b2_residual_config;
+typedef struct { uint64_t n_particles, draws; double weight_sum, weight_max; } b2_residual_result;
+B2_API int b2_pf_resample_residual(b2_pf* h, const b2_transform* poses_dev, const b2_particle_attr* attrs_dev, uint32_t n, uint32_t n_new,
+                                   uint32_t first, uint32_t n_local, b2_transform* poses_new_dev, b2_particle_attr* attrs_new_dev,
+                                   const b2_gladiator_config* cfg, uint64_t seed, uint32_t step, b2_residual_result* out_host);
+
 /* ---------------------------------------------------------------- introspection ------------------------------ */
 /* CUDA-event timing of the kernels inside b2_rcc_correct_once*(): when enabled, events are recorded on the handle's stream around the
  * find kernel and around the reduction/Umeyama kernels; b2_rcc_last_timing returns the two durations of the most recent call (ms). */

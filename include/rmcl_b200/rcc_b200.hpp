@@ -72,6 +72,7 @@ struct ParticleAttributes { rm::Gaussian1D likelihood; float state_sigma[6]; }; 
 struct RangeMeasurement { rm::Vector3f orig, dir; float range; rm::Matrix3x3 cov; };            // RangeMeasurement.hpp:10-21
 struct ParticleUpdateResults {};
 struct ParticleUpdateConfig {};
+struct ParticleUpdateDynamicResults { uint32_t n_particles; };                                    // ParticleUpdater.hpp:49-52
 #endif
 static_assert(sizeof(ParticleAttributes) == 36 && sizeof(RangeMeasurement) == 64, "rmcl layouts");
 
@@ -409,6 +410,24 @@ public:
         b2_check(b2_pf_resample_gladiator(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<const b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(),
                                           first, (uint32_t)poses_new.size(), reinterpret_cast<b2_transform*>(poses_new.raw()), reinterpret_cast<b2_particle_attr*>(attrs_new.raw()),
                                           &resampler_config, seed, step, nullptr, nullptr), "resample");
+    }
+    // ResidualResamplerCPU::update (ResidualResamplerCPU.cpp:55-202; config and defaults :35-47) on the device: all of `poses/attrs` resampled
+    // into an output set of n_new slots (0: first + poses_new.size(), the node's whole max_particles buffer); the outputs receive slots
+    // first .. first+poses_new.size()-1, and only those below the returned n_particles are written.  `last_residual` keeps the whole record.
+    b2_residual_config residual_config{0.03f, 0.03f, 0.0f, 0.0f, 0.0f, 0.01f, 0.3f, 0.2f};
+    b2_residual_result last_residual{};
+    ParticleUpdateDynamicResults resampleResidual(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs,
+                                                  rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses_new, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs_new,
+                                                  uint64_t seed = 1234, uint32_t step = 0, uint32_t first = 0, uint32_t n_new = 0)
+    {
+        if (poses.size() != attrs.size() || poses_new.size() != attrs_new.size()) throw std::invalid_argument("resampleResidual: poses and attrs differ in size");
+        if (n_new == 0) n_new = first + (uint32_t)poses_new.size();
+        b2_check(b2_pf_resample_residual(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<const b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(),
+                                         n_new, first, (uint32_t)poses_new.size(), reinterpret_cast<b2_transform*>(poses_new.raw()),
+                                         reinterpret_cast<b2_particle_attr*>(attrs_new.raw()), &residual_config, seed, step, &last_residual), "resampleResidual");
+        ParticleUpdateDynamicResults res;
+        res.n_particles = (uint32_t)last_residual.n_particles;
+        return res;
     }
     // RmclNode::initSamplesUniform (rmcl_localization.cpp:277-342) on the device: particles first .. first+poses.size()-1 of a set drawn
     // uniformly from [bb_min, bb_max] (x, y, z, roll, pitch, yaw).  Draws keyed by (seed, global index): shards concatenate to the whole set.

@@ -9,7 +9,7 @@ import os
 
 import numpy as np
 
-from .synth import CROSS_STATS_DTYPE, PARTICLE_ATTR_DTYPE, PARTICLE_STATS_DTYPE, RANGE_MEAS_DTYPE, TRANSFORM_DTYPE
+from .synth import CROSS_STATS_DTYPE, PARTICLE_ATTR_DTYPE, PARTICLE_STATS_DTYPE, RANGE_MEAS_DTYPE, RESIDUAL_RESULT_DTYPE, TRANSFORM_DTYPE
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.environ.get("B2_LIB_PATH") or os.path.join(_HERE, "lib", "librmcl_b200.so")     # B2_LIB_PATH: experiment builds (scripts/)
@@ -124,7 +124,7 @@ EXPORTS = [
     "b2_rcc_set_correspondence_type", "b2_pf_resample_gladiator", "b2_pf_gladiator_randoms", "b2_rcc_segment", "b2_mesh_create_from_file", "b2_mesh_file_load", "b2_mesh_file_free", "b2_peek_cuda_error", "b2_mesh_blob_size", "b2_mesh_export_blob", "b2_mesh_create_from_blob", "b2_mesh_refit",
     "b2_rcc_correct_once_async", "b2_rcc_correct_once_wait", "b2_micp_correct_once", "b2_rcc_set_exec_mode", "b2_debug_read_bandwidth", "b2_rcc_set_sim_options", "b2_rcc_bind_dataset", "b2_rcc_bind_model_buffers", "b2_rcc_benchmark_batch", "b2_pf_p2p_init", "b2_pf_p2p_connect", "b2_pf_p2p_publish", "b2_pf_resample_gladiator_p2p", "b2_pf_p2p_connect_local", "b2_rcc_set_cpc_options", "b2_pf_set_mapping", "b2_pf_get_mapping",
     "b2_micp_correct", "b2_pf_init_uniform", "b2_pf_init_gaussian", "b2_pf_estimate_stats", "b2_rcc_set_cloud_o1dn",
-    "b2_rcc_set_cloud_spherical", "b2_pf_sample_cloud",
+    "b2_rcc_set_cloud_spherical", "b2_pf_sample_cloud", "b2_pf_resample_residual",
 ]
 
 
@@ -815,6 +815,23 @@ class PCDSensorUpdaterB200:
                                                      _devptr(particle_poses_new), _devptr(particle_attrs_new), C.byref(cfg), C.c_uint64(seed), C.c_uint32(step),
                                                      _devptr(raw) if raw is not None else None, _devptr(normals) if normals is not None else None))
         return particle_poses_new, particle_attrs_new
+
+    def resampleResidual(self, particle_poses, particle_attrs, particle_poses_new, particle_attrs_new, config=None, seed=1234, step=0, first=0, n_new=None):
+        """ResidualResamplerCPU::update (rmcl_ros/src/rmcl/ResidualResamplerCPU.cpp:55-202) on torch CUDA tensors (b2_pf_resample_residual).
+        Resamples all particles of `particle_poses/attrs` into an output set of n_new slots (default: the length of the outputs); the outputs
+        receive slots first .. first+len(out)-1, and entries at or beyond the result's n_particles are left untouched.  `config` is a
+        GladiatorConfig (the same fields and defaults).  -> a synth.RESIDUAL_RESULT_DTYPE record: n_particles, draws, weight_sum, weight_max."""
+        cfg = config or GladiatorConfig.defaults()
+        n = particle_poses.numel() * particle_poses.element_size() // 32
+        n_local = particle_poses_new.numel() * particle_poses_new.element_size() // 32
+        if particle_attrs.numel() * particle_attrs.element_size() != 36 * n or particle_attrs_new.numel() * particle_attrs_new.element_size() != 36 * n_local:
+            raise ValueError("resampleResidual: poses and attrs differ in length")
+        n_new = first + n_local if n_new is None else int(n_new)
+        out = np.zeros((), RESIDUAL_RESULT_DTYPE)
+        _chk(load_library().b2_pf_resample_residual(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(n), C.c_uint32(n_new), C.c_uint32(first),
+                                                    C.c_uint32(n_local), _devptr(particle_poses_new), _devptr(particle_attrs_new), C.byref(cfg), C.c_uint64(seed),
+                                                    C.c_uint32(step), _p(out)))
+        return out
 
     def p2pConnect(self, dist, n_per_rank):
         """Map the other ranks' particle exchange buffers over NVLink (CUDA IPC): once per particle-set size.  Raises B2Error if the GPUs have no

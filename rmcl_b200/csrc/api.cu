@@ -2,6 +2,7 @@
 // the CUDA path or fails with B2_ERR_CUDA.
 #include "kernels.cuh"
 #include "lbvh.cuh"
+#include <cub/device/device_scan.cuh>
 
 #include <algorithm>
 #include <atomic>
@@ -1788,6 +1789,10 @@ struct b2_pf {
     DevBuf<double> d_est_part; DevBuf<PfEstimateScratch> d_est; b2_particle_stats* h_est = nullptr;
     // beam sampling from a device cloud (b2_pf_sample_cloud): one record per sample, and its pinned host copy
     DevBuf<PfBeamSample> d_samples; PfBeamSample* h_samples = nullptr; uint32_t h_samples_cap = 0;
+    // residual resampling (b2_pf_resample_residual), grown at its calls: statistics partials, per-draw parents, counts and their prefix for
+    // the largest chunk, the scan's temporary storage, and the state record with its pinned host copy
+    DevBuf<double> d_res_part; DevBuf<uint32_t> d_res_parents; DevBuf<unsigned long long> d_res_counts, d_res_prefix; DevBuf<unsigned char> d_res_tmp;
+    DevBuf<PfResidualState> d_res; PfResidualState* h_res = nullptr;
 };
 
 extern "C" int b2_pf_destroy(b2_pf* h);
@@ -1849,6 +1854,8 @@ extern "C" int b2_pf_destroy(b2_pf* h)
     if (h->h_est) cudaFreeHost(h->h_est);
     h->d_samples.release();
     if (h->h_samples) cudaFreeHost(h->h_samples);
+    h->d_res_part.release(); h->d_res_parents.release(); h->d_res_counts.release(); h->d_res_prefix.release(); h->d_res_tmp.release(); h->d_res.release();
+    if (h->h_res) cudaFreeHost(h->h_res);
     b2_mesh* map = h->map;
     delete h;
     (void)cudaGetLastError();
@@ -2338,5 +2345,76 @@ extern "C" int b2_pf_estimate_stats(b2_pf* h, const b2_transform* poses_dev, con
     CU(cudaMemcpyAsync(h->h_est, &h->d_est.p->rec, sizeof(b2_particle_stats), cudaMemcpyDeviceToHost, h->stream));
     CU(cudaStreamSynchronize(h->stream));
     *out_host = *h->h_est;
+    return B2_OK;
+}
+
+// ResidualResamplerCPU::update (ResidualResamplerCPU.cpp:55-202): a statistics pass, then the draws in chunks of doubling size, each counted,
+// scanned and searched for the draw that fills the last slot, with one read-back per chunk; the slots a chunk filled are built right after it
+static bool ranges_overlap(const void* a, size_t a_bytes, const void* b, size_t b_bytes)
+{
+    const uintptr_t pa = (uintptr_t)a, pb = (uintptr_t)b;
+    return a_bytes && b_bytes && pa < pb + b_bytes && pb < pa + a_bytes;
+}
+extern "C" int b2_pf_resample_residual(b2_pf* h, const b2_transform* poses_dev, const b2_particle_attr* attrs_dev, uint32_t n, uint32_t n_new,
+                                       uint32_t first, uint32_t n_local, b2_transform* poses_new_dev, b2_particle_attr* attrs_new_dev,
+                                       const b2_gladiator_config* cfg, uint64_t seed, uint32_t step, b2_residual_result* out_host)
+{
+    NOTNULL(h); NOTNULL(poses_dev); NOTNULL(attrs_dev); NOTNULL(poses_new_dev); NOTNULL(attrs_new_dev); NOTNULL(cfg); NOTNULL(out_host);
+    if (n == 0 || n_new == 0) return fail(B2_ERR_INVALID, "resample residual: %u particles into %u slots (both must be > 0)", n, n_new);
+    if ((uint64_t)first + n_local > n_new) return fail(B2_ERR_INVALID, "resample residual: slots %u+%u exceed the %u output slots", first, n_local, n_new);
+    const size_t in_p = sizeof(b2_transform) * (size_t)n, in_a = sizeof(b2_particle_attr) * (size_t)n;
+    const size_t out_p = sizeof(b2_transform) * (size_t)n_local, out_a = sizeof(b2_particle_attr) * (size_t)n_local;
+    if (ranges_overlap(poses_new_dev, out_p, poses_dev, in_p) || ranges_overlap(poses_new_dev, out_p, attrs_dev, in_a) ||
+        ranges_overlap(attrs_new_dev, out_a, poses_dev, in_p) || ranges_overlap(attrs_new_dev, out_a, attrs_dev, in_a) ||
+        ranges_overlap(poses_new_dev, out_p, attrs_new_dev, out_a))
+        return fail(B2_ERR_INVALID, "resample residual: an output range overlaps an input range or the other output (the node double-buffers)");
+    CU(cudaSetDevice(h->map->device));
+    const uint64_t M = n_new, nm = std::max<uint64_t>(n, M), d_max = 16 * nm;
+    // draws are keyed by their index: the chunk size changes no result.  2^30 keeps a chunk within the scan's int item count.
+    const uint64_t cap = std::min<uint64_t>(2 * nm, 1ull << 30);
+    uint64_t chunk = std::min<uint64_t>(std::max<uint64_t>(2 * (uint64_t)n, 1ull << 16), cap);
+    const uint32_t grid = std::min<uint32_t>((uint32_t)h->n_sm * 4u, (n + 255) / 256);
+    if (!h->d_res.p) {
+        RES(h->d_res_part.reserve((size_t)B2_RES_NV * 4 * (size_t)h->n_sm)); RES(h->d_res.reserve(1));
+        CU(cudaMemset(h->d_res.p, 0, sizeof(PfResidualState)));
+        CU(cudaMallocHost((void**)&h->h_res, sizeof(PfResidualState)));
+    }
+    k_pf_residual_stats<<<grid, 256, 0, h->stream>>>(attrs_dev, n, h->d_res_part.p, h->d_res.p);
+    LAUNCHED();
+    CU(cudaMemcpyAsync(h->h_res, h->d_res.p, sizeof(PfResidualState), cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    const double S = h->h_res->S, L_min = h->h_res->L_min, L_max = h->h_res->L_max;
+    b2_residual_result res = {0, 0, S, L_max};
+    // a NaN or infinite likelihood makes S non-finite; all zero gives 0 / 0 in the reference (SURVEY D31)
+    if (!(std::isfinite(S) && S > 0.0 && L_min >= 0.0)) { *out_host = res; return B2_OK; }
+    size_t tmp_bytes = 0;
+    CU(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, h->d_res_counts.p, h->d_res_prefix.p, (int)cap, h->stream));
+    RES(h->d_res_parents.reserve(cap)); RES(h->d_res_counts.reserve(cap)); RES(h->d_res_prefix.reserve(cap)); RES(h->d_res_tmp.reserve(std::max<size_t>(tmp_bytes, 16)));
+    uint64_t fill = 0, draws = 0;
+    while (fill < M && draws < d_max) {
+        const uint32_t len = (uint32_t)std::min<uint64_t>(chunk, d_max - draws);
+        k_pf_residual_counts<<<(len + 255) / 256, 256, 0, h->stream>>>(attrs_dev, n, M, S, seed, step, draws, len, h->d_res_parents.p, h->d_res_counts.p);
+        LAUNCHED();
+        size_t bytes = h->d_res_tmp.cap;
+        CU(cub::DeviceScan::InclusiveSum(h->d_res_tmp.p, bytes, h->d_res_counts.p, h->d_res_prefix.p, (int)len, h->stream));
+        LAUNCHED();
+        k_pf_residual_find<<<1, 1, 0, h->stream>>>(h->d_res_prefix.p, len, M - fill, h->d_res.p);
+        LAUNCHED();
+        CU(cudaMemcpyAsync(h->h_res, h->d_res.p, sizeof(PfResidualState), cudaMemcpyDeviceToHost, h->stream));
+        CU(cudaStreamSynchronize(h->stream));
+        const uint64_t filled = h->h_res->filled, used = h->h_res->used;
+        const uint64_t lo = std::max<uint64_t>(fill, first), hi = std::min<uint64_t>(fill + filled, (uint64_t)first + n_local);
+        if (lo < hi) {
+            const uint32_t n_k = (uint32_t)(hi - lo);
+            k_pf_residual_expand<<<(n_k + 255) / 256, 256, 0, h->stream>>>(poses_dev, attrs_dev, h->d_res_parents.p, h->d_res_prefix.p, len, fill, (uint32_t)lo, n_k, first,
+                                                                          L_max, *cfg, seed, step, poses_new_dev, attrs_new_dev);
+            LAUNCHED();
+        }
+        fill += filled; draws += used;
+        chunk = std::min(2 * chunk, cap);
+    }
+    CU(cudaStreamSynchronize(h->stream));
+    res.n_particles = fill; res.draws = draws;
+    *out_host = res;
     return B2_OK;
 }

@@ -1270,17 +1270,27 @@ B2_DEV Q4 euler_to_quat(float roll, float pitch, float yaw)
     q.z = sub(mul(mul(cr, cp), sy), mul(mul(sr, sp), cy));
     return q;
 }
+// the perturbed copy of a pose, shared by both resamplers (resampling.cu:166-175, ResidualResamplerCPU.cpp:150-162): t += N[0..2] * s[0..2],
+// the Euler angles of R += N[3..5] * s[3..5]; diff = ~pose * pose_new.  The forget rule applied to diff is each resampler's own.
+B2_DEV Tf pf_perturb(const Tf& pose, const float N[6], const float s[6], Tf& diff)
+{
+    Tf pnew = pose;
+    pnew.t = mk3(add(pose.t.x, mul(N[0], s[0])), add(pose.t.y, mul(N[1], s[1])), add(pose.t.z, mul(N[2], s[2])));
+    float roll, pitch, yaw; quat_to_euler(pose.R, roll, pitch, yaw);
+    pnew.R = euler_to_quat(add(roll, mul(N[3], s[3])), add(pitch, mul(N[4], s[4])), add(yaw, mul(N[5], s[5])));
+    diff = tf_mul(tf_inv(pose), pnew);
+    return pnew;
+}
+// Quaternion::l2norm, the "rotation distance" of both resamplers: the 4-norm of diff.R, ~1 for any rotation (SURVEY D32)
+B2_DEV float quat_l2norm(Q4 q) { return sqrtf(add(add(add(mul(q.x, q.x), mul(q.y, q.y)), mul(q.z, q.z)), mul(q.w, q.w))); }
 // the opponent won (resampling.cu:150-192): the champion's slot receives a perturbed copy of the opponent whose n_meas is reduced by the forget rate
 B2_DEV void gladiator_take(b2_transform pn, b2_particle_attr an, const float N[6], const b2_gladiator_config& cfg, b2_transform* out_p, b2_particle_attr* out_a)
 {
-    const Tf pose = tf_from_pod(pn);
-    Tf pnew = pose;
-    pnew.t = mk3(add(pose.t.x, mul(N[0], cfg.min_noise_tx)), add(pose.t.y, mul(N[1], cfg.min_noise_ty)), add(pose.t.z, mul(N[2], cfg.min_noise_tz)));   // :166-168
-    float roll, pitch, yaw; quat_to_euler(pose.R, roll, pitch, yaw);
-    pnew.R = euler_to_quat(add(roll, mul(N[3], cfg.min_noise_roll)), add(pitch, mul(N[4], cfg.min_noise_pitch)), add(yaw, mul(N[5], cfg.min_noise_yaw)));   // :169-173
-    const Tf diff = tf_mul(tf_inv(pose), pnew);                                            // :175
+    const float s[6] = {cfg.min_noise_tx, cfg.min_noise_ty, cfg.min_noise_tz, cfg.min_noise_roll, cfg.min_noise_pitch, cfg.min_noise_yaw};
+    Tf diff;
+    const Tf pnew = pf_perturb(tf_from_pod(pn), N, s, diff);                               // :166-175
     const float trans_dist = v_l2norm(diff.t);                                             // :178
-    const float rot_dist = sqrtf(add(add(add(mul(diff.R.x, diff.R.x), mul(diff.R.y, diff.R.y)), mul(diff.R.z, diff.R.z)), mul(diff.R.w, diff.R.w)));   // :179
+    const float rot_dist = quat_l2norm(diff.R);                                            // :179
     const float frs = (float)(1.0 - pow(1.0 - (double)cfg.likelihood_forget_per_meter, (double)trans_dist));    // :182
     const float frr = (float)(1.0 - pow(1.0 - (double)cfg.likelihood_forget_per_radian, (double)rot_dist));     // :183
     const float forget = frs > frr ? frs : frr;
@@ -1636,39 +1646,48 @@ struct PfEstimateScratch {
     double L_sum;                // pass 1's sum of L (the weights' denominator)
     unsigned int ticket[2];      // one last-block ticket per pass
 };
-// pass 1 slots below B2_EST_NSUM and every pass-2 slot are sums; min and max ignore NaN like std::min / std::max with the running value first
-template <bool SUMS> B2_DEV double est_combine(int slot, double a, double b)
+// Which accumulator slots of a grid reduction are sums, minima and maxima (every other slot is a maximum).  Pass 1: the slots below
+// B2_EST_NSUM are sums; every pass-2 slot is a sum.  Min and max ignore NaN like std::min / std::max with the running value first.
+struct EstSlots1 {
+    static B2_DEV bool is_sum(int slot) { return slot < B2_EST_NSUM; }
+    static B2_DEV bool is_min(int slot) { return slot == B2_EST_MIN_L || (slot >= B2_EST_BB_MIN && slot < B2_EST_BB_MAX); }
+};
+struct EstSlots2 {
+    static B2_DEV bool is_sum(int) { return true; }
+    static B2_DEV bool is_min(int) { return false; }
+};
+template <class SLOTS> B2_DEV double est_combine(int slot, double a, double b)
 {
-    if (SUMS || slot < B2_EST_NSUM) return a + b;
-    if (slot == B2_EST_MIN_L || (slot >= B2_EST_BB_MIN && slot < B2_EST_BB_MAX)) return b < a ? b : a;
+    if (SLOTS::is_sum(slot)) return a + b;
+    if (SLOTS::is_min(slot)) return b < a ? b : a;
     return a < b ? b : a;
 }
-template <bool SUMS> B2_DEV double est_identity(int slot)
+template <class SLOTS> B2_DEV double est_identity(int slot)
 {
-    if (SUMS || slot < B2_EST_NSUM) return 0.0;
-    return (slot == B2_EST_MIN_L || (slot >= B2_EST_BB_MIN && slot < B2_EST_BB_MAX)) ? f64_inf() : -f64_inf();
+    if (SLOTS::is_sum(slot)) return 0.0;
+    return SLOTS::is_min(slot) ? f64_inf() : -f64_inf();
 }
 #ifdef __CUDACC__
-template <bool SUMS> __device__ __forceinline__ double est_warp(int slot, double v)
+template <class SLOTS> __device__ __forceinline__ double est_warp(int slot, double v)
 {
     #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = est_combine<SUMS>(slot, v, __shfl_xor_sync(0xffffffffu, v, o));
+    for (int o = 16; o > 0; o >>= 1) v = est_combine<SLOTS>(slot, v, __shfl_xor_sync(0xffffffffu, v, o));
     return v;
 }
 // block reduction of NV per-thread values to partials[blockIdx.x * NV + slot]; then the last block reduces the partials in a fixed order
 // (warp w handles slots w, w + 8, ...; lane l takes blocks l, l + 32, ...; then a warp butterfly) into tot[NV].  True in the last block only.
-template <int NV, bool SUMS>
+template <int NV, class SLOTS>
 __device__ __forceinline__ bool est_grid_reduce(double (&acc)[NV], double* __restrict__ partials, unsigned int* __restrict__ ticket, double* s_w /* [8][NV] */, double* tot,
                                                 bool& is_last)
 {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     #pragma unroll
-    for (int j = 0; j < NV; j++) acc[j] = est_warp<SUMS>(j, acc[j]);
+    for (int j = 0; j < NV; j++) acc[j] = est_warp<SLOTS>(j, acc[j]);
     if (lane == 0) for (int j = 0; j < NV; j++) s_w[warp * NV + j] = acc[j];
     __syncthreads();
     if (threadIdx.x < NV) {
         double a = s_w[threadIdx.x];
-        for (int w = 1; w < 8; w++) a = est_combine<SUMS>(threadIdx.x, a, s_w[w * NV + threadIdx.x]);
+        for (int w = 1; w < 8; w++) a = est_combine<SLOTS>(threadIdx.x, a, s_w[w * NV + threadIdx.x]);
         partials[(size_t)blockIdx.x * NV + threadIdx.x] = a;
         __threadfence();
     }
@@ -1678,9 +1697,9 @@ __device__ __forceinline__ bool est_grid_reduce(double (&acc)[NV], double* __res
     if (!is_last) return false;
     __threadfence();
     for (int j = warp; j < NV; j += 8) {
-        double a = est_identity<SUMS>(j);
-        for (uint32_t b = lane; b < gridDim.x; b += 32) a = est_combine<SUMS>(j, a, __ldcg(partials + (size_t)b * NV + j));
-        a = est_warp<SUMS>(j, a);
+        double a = est_identity<SLOTS>(j);
+        for (uint32_t b = lane; b < gridDim.x; b += 32) a = est_combine<SLOTS>(j, a, __ldcg(partials + (size_t)b * NV + j));
+        a = est_warp<SLOTS>(j, a);
         if (lane == 0) tot[j] = a;
     }
     __syncthreads();
@@ -1702,13 +1721,13 @@ __global__ void __launch_bounds__(256) k_pf_estimate_moments(const b2_transform*
         const Tf P = tf_load(poses + i);
         const double L = (double)attrs[i].likelihood.mean;
         acc[B2_EST_SUM_L] += L; acc[B2_EST_SUM_L2] += L * L;
-        acc[B2_EST_MIN_L] = est_combine<false>(B2_EST_MIN_L, acc[B2_EST_MIN_L], L); acc[B2_EST_MAX_L] = est_combine<false>(B2_EST_MAX_L, acc[B2_EST_MAX_L], L);
+        acc[B2_EST_MIN_L] = est_combine<EstSlots1>(B2_EST_MIN_L, acc[B2_EST_MIN_L], L); acc[B2_EST_MAX_L] = est_combine<EstSlots1>(B2_EST_MAX_L, acc[B2_EST_MAX_L], L);
         const double t[3] = {(double)P.t.x, (double)P.t.y, (double)P.t.z}, q[4] = {(double)P.R.x, (double)P.R.y, (double)P.R.z, (double)P.R.w};
         #pragma unroll
         for (int c = 0; c < 3; c++) {
             acc[B2_EST_SUM_LT + c] += L * t[c];
-            acc[B2_EST_BB_MIN + c] = est_combine<false>(B2_EST_BB_MIN, acc[B2_EST_BB_MIN + c], t[c]);
-            acc[B2_EST_BB_MAX + c] = est_combine<false>(B2_EST_BB_MAX, acc[B2_EST_BB_MAX + c], t[c]);
+            acc[B2_EST_BB_MIN + c] = est_combine<EstSlots1>(B2_EST_BB_MIN, acc[B2_EST_BB_MIN + c], t[c]);
+            acc[B2_EST_BB_MAX + c] = est_combine<EstSlots1>(B2_EST_BB_MAX, acc[B2_EST_BB_MAX + c], t[c]);
         }
         int s = B2_EST_SUM_LQQ;
         #pragma unroll
@@ -1718,7 +1737,7 @@ __global__ void __launch_bounds__(256) k_pf_estimate_moments(const b2_transform*
             for (int b = a; b < 4; b++) acc[s++] += La * q[b];
         }
     }
-    if (!est_grid_reduce<B2_EST_NV1, false>(acc, partials, sc->ticket, s_w, tot, is_last)) return;
+    if (!est_grid_reduce<B2_EST_NV1, EstSlots1>(acc, partials, sc->ticket, s_w, tot, is_last)) return;
     if (threadIdx.x != 0) return;
     const double Ls = tot[B2_EST_SUM_L], n = (double)k, mean = Ls / n, var = tot[B2_EST_SUM_L2] / n - mean * mean;
     const bool ok = Ls > 0.0 && Ls < f64_inf();                                             // else the reference divides by zero (decision E3)
@@ -1764,7 +1783,7 @@ __global__ void __launch_bounds__(256) k_pf_estimate_cov(const b2_transform* __r
             for (int b = a; b < 6; b++) acc[s++] += La * (double)v[b];
         }
     }
-    if (!est_grid_reduce<B2_EST_NV2, true>(acc, partials, sc->ticket + 1, s_w, tot, is_last)) return;
+    if (!est_grid_reduce<B2_EST_NV2, EstSlots2>(acc, partials, sc->ticket + 1, s_w, tot, is_last)) return;
     if (threadIdx.x != 0) return;
     const double Ls = sc->L_sum;
     const bool ok = Ls > 0.0 && Ls < f64_inf();
@@ -1772,6 +1791,128 @@ __global__ void __launch_bounds__(256) k_pf_estimate_cov(const b2_transform* __r
     int s = 0;
     for (int a = 0; a < 6; a++) for (int b = a; b < 6; b++) { sc->rec.covariance[6 * a + b] = sc->rec.covariance[6 * b + a] = ok ? tot[s] / Ls : nan; s++; }
     sc->ticket[1] = 0u;
+}
+#endif
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Residual resampling: ResidualResamplerCPU::update (rmcl_ros/src/rmcl/ResidualResamplerCPU.cpp:55-202).  Draw j (64-bit) picks parent
+// word j % 4 of Philox4x32-10 with counter (lo(j / 4), B2_PF_RESIDUAL_DRAW_TAG, step, hi(j / 4)) and key = seed, modulo n; it inserts
+// min(floor(L / S * M), slots left) copies.  The copy in output slot k draws its six normals from words 0-5 of the counters
+// (k, B2_PF_RESIDUAL_NOISE_TAG, step, 0 and 1).  Draws are keyed by their index and copies by their slot, so neither the chunking of the
+// draws nor the slice of slots one call writes can change a byte.  The draws run in chunks: k_pf_residual_counts, an inclusive scan of the
+// counts, k_pf_residual_find, then k_pf_residual_expand over the slots the chunk filled (b2_pf_resample_residual).  SURVEY D31-D34.
+// ---------------------------------------------------------------------------------------------------------------------
+#define B2_PF_RESIDUAL_DRAW_TAG 4u
+#define B2_PF_RESIDUAL_NOISE_TAG 5u
+// the parent of draw j among n particles (:104, std::uniform_int_distribution(0, n - 1) replaced, SURVEY D33)
+B2_DEV uint32_t residual_parent(uint64_t seed, uint32_t step, uint64_t j, uint32_t n)
+{
+    uint32_t r[4];
+    const uint64_t b = j >> 2;
+    philox4x32_10((uint32_t)b, B2_PF_RESIDUAL_DRAW_TAG, step, (uint32_t)(b >> 32), (uint32_t)seed, (uint32_t)(seed >> 32), r);
+    return philox_word(r, (uint32_t)(j & 3u)) % n;
+}
+// n_expected_insertions = (size_t)(L / weight_sum * (double)M) (:110-120); 0 <= L <= S (checked on the host) keeps it in [0, M]
+B2_DEV uint64_t residual_count(float L, double S, uint64_t M)
+{
+    const double c = (double)L / S * (double)M;
+    return c >= (double)M ? M : (uint64_t)c;
+}
+// the six N(0, 1) draws of output slot k, in the reference's order tx, ty, tz, roll, pitch, yaw (:151-157)
+B2_DEV void residual_normals(uint64_t seed, uint32_t step, uint32_t k, float N[6])
+{
+    uint32_t r[8];
+    philox4x32_10(k, B2_PF_RESIDUAL_NOISE_TAG, step, 0u, (uint32_t)seed, (uint32_t)(seed >> 32), r);
+    philox4x32_10(k, B2_PF_RESIDUAL_NOISE_TAG, step, 1u, (uint32_t)seed, (uint32_t)(seed >> 32), r + 4);
+    box_muller3(r, N);
+}
+// one copy of the parent (pn, an) (:129-177): noise scales (float)(min_noise / (L / L_max)), so less likely parents spread wider; n_meas
+// *= (float)(pow(forget_per_meter, |d.t|^2) * pow(forget_per_radian, |d.R|)) with d = ~pose * pose_new, the squared translation and the
+// quaternion norm as the reference takes them (SURVEY D32), double pow of the float arguments (SURVEY E5); the stamp is the parent's.
+B2_DEV void residual_copy(b2_transform pn, b2_particle_attr an, double L_max, const float N[6], const b2_gladiator_config& cfg, b2_transform* out_p,
+                          b2_particle_attr* out_a)
+{
+    const double Lmn = (double)an.likelihood.mean / L_max;                                  // L_max_normed (:112)
+    const float s[6] = {(float)((double)cfg.min_noise_tx / Lmn), (float)((double)cfg.min_noise_ty / Lmn), (float)((double)cfg.min_noise_tz / Lmn),
+                        (float)((double)cfg.min_noise_roll / Lmn), (float)((double)cfg.min_noise_pitch / Lmn), (float)((double)cfg.min_noise_yaw / Lmn)};   // :143-149
+    Tf diff;
+    const Tf pnew = pf_perturb(tf_from_pod(pn), N, s, diff);                               // :151-160
+    const float trans_dist = add(add(mul(diff.t.x, diff.t.x), mul(diff.t.y, diff.t.y)), mul(diff.t.z, diff.t.z));   // :163 l2normSquared
+    const float rot_dist = quat_l2norm(diff.R);                                            // :164
+    const float f = (float)(pow((double)cfg.likelihood_forget_per_meter, (double)trans_dist) * pow((double)cfg.likelihood_forget_per_radian, (double)rot_dist));   // :165-166
+    an.likelihood.n_meas = (uint32_t)mul((float)an.likelihood.n_meas, f);                 // :167 uint *= float
+    pn.R.x = pnew.R.x; pn.R.y = pnew.R.y; pn.R.z = pnew.R.z; pn.R.w = pnew.R.w; pn.t.x = pnew.t.x; pn.t.y = pnew.t.y; pn.t.z = pnew.t.z;
+    *out_p = pn; *out_a = an;
+}
+// slots of the statistics pass: the sum of L, its minimum (from DBL_MAX) and its maximum (from 0.0), as pass 1 of the estimate takes them
+#define B2_RES_SUM 0
+#define B2_RES_MIN 1
+#define B2_RES_MAX 2
+#define B2_RES_NV 3
+struct ResidualSlots {
+    static B2_DEV bool is_sum(int slot) { return slot == B2_RES_SUM; }
+    static B2_DEV bool is_min(int slot) { return slot == B2_RES_MIN; }
+};
+// the device record the host reads back after the statistics pass and after every chunk
+struct PfResidualState {
+    double S, L_min, L_max;             // statistics pass
+    unsigned long long filled, used;    // k_pf_residual_find: slots the chunk filled, draws it consumed
+    unsigned int ticket, pad;
+};
+#ifdef __CUDACC__
+// 4 B read per particle; grid, block and grid-stride order of k_pf_estimate_moments, so S is bit-equal to its L_sum for the same n
+__global__ void __launch_bounds__(256) k_pf_residual_stats(const b2_particle_attr* __restrict__ attrs, uint32_t n, double* __restrict__ partials, PfResidualState* __restrict__ st)
+{
+    __shared__ double s_w[8 * B2_RES_NV], tot[B2_RES_NV];
+    __shared__ bool is_last;
+    double acc[B2_RES_NV];
+    acc[B2_RES_SUM] = 0.0; acc[B2_RES_MIN] = 1.7976931348623157e308; acc[B2_RES_MAX] = 0.0;     // :73-83
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const double L = (double)attrs[i].likelihood.mean;
+        acc[B2_RES_SUM] += L;
+        acc[B2_RES_MIN] = est_combine<ResidualSlots>(B2_RES_MIN, acc[B2_RES_MIN], L); acc[B2_RES_MAX] = est_combine<ResidualSlots>(B2_RES_MAX, acc[B2_RES_MAX], L);
+    }
+    if (!est_grid_reduce<B2_RES_NV, ResidualSlots>(acc, partials, &st->ticket, s_w, tot, is_last)) return;
+    if (threadIdx.x != 0) return;
+    st->S = tot[B2_RES_SUM]; st->L_min = tot[B2_RES_MIN]; st->L_max = tot[B2_RES_MAX];
+    st->ticket = 0u;
+}
+// one thread per draw d0 + i of the chunk: its parent and its count (4 B gathered per draw)
+__global__ void __launch_bounds__(256) k_pf_residual_counts(const b2_particle_attr* __restrict__ attrs, uint32_t n, uint64_t M, double S, uint64_t seed, uint32_t step,
+                                                            uint64_t d0, uint32_t len, uint32_t* __restrict__ parents, unsigned long long* __restrict__ counts)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= len) return;
+    const uint32_t p = residual_parent(seed, step, d0 + i, n);
+    parents[i] = p;
+    counts[i] = residual_count(attrs[p].likelihood.mean, S, M);
+}
+// one thread: over the chunk's inclusive prefix of the counts, the first draw whose running fill reaches the `left` slots still empty
+// (that draw ends the reference's loop, :102) -- or the whole chunk when the fill stays short of it
+__global__ void k_pf_residual_find(const unsigned long long* __restrict__ prefix, uint32_t len, uint64_t left, PfResidualState* __restrict__ st)
+{
+    if (prefix[len - 1] < left) { st->filled = prefix[len - 1]; st->used = len; return; }
+    uint32_t lo = 0, hi = len - 1;
+    while (lo < hi) { const uint32_t mid = lo + (hi - lo) / 2; if (prefix[mid] < left) lo = mid + 1; else hi = mid; }
+    st->filled = left; st->used = lo + 1u;
+}
+// one thread per output slot k = k0 + i that this chunk filled (k - fill0 < the chunk's fill): its draw is the first whose prefix exceeds
+// k - fill0; writes entry k - first of the caller's slice.  68 B gathered from the parent and 68 B written per slot.
+__global__ void __launch_bounds__(256) k_pf_residual_expand(const b2_transform* __restrict__ poses, const b2_particle_attr* __restrict__ attrs, const uint32_t* __restrict__ parents,
+                                                            const unsigned long long* __restrict__ prefix, uint32_t len, uint64_t fill0, uint32_t k0, uint32_t n_k, uint32_t first,
+                                                            double L_max, b2_gladiator_config cfg, uint64_t seed, uint32_t step, b2_transform* __restrict__ poses_new,
+                                                            b2_particle_attr* __restrict__ attrs_new)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_k) return;
+    const uint32_t k = k0 + i;
+    const uint64_t local = (uint64_t)k - fill0;
+    uint32_t lo = 0, hi = len - 1;
+    while (lo < hi) { const uint32_t mid = lo + (hi - lo) / 2; if (prefix[mid] <= local) lo = mid + 1; else hi = mid; }
+    const uint32_t p = parents[lo];
+    float N[6];
+    residual_normals(seed, step, k, N);
+    residual_copy(poses[p], attrs[p], L_max, N, cfg, poses_new + (k - first), attrs_new + (k - first));
 }
 #endif
 

@@ -296,6 +296,9 @@ LIKELIHOOD_STATS_DTYPE = np.dtype([("min", np.float64), ("max", np.float64), ("m
 PARTICLE_STATS_DTYPE = np.dtype([("position", np.float64, 3), ("orientation", np.float64, 4), ("covariance", np.float64, 36), ("shift", np.float64),
                                  ("trans_bb_min", np.float64, 3), ("trans_bb_max", np.float64, 3), ("likelihood", LIKELIHOOD_STATS_DTYPE), ("nparticles", np.uint64)])
 assert PARTICLE_STATS_DTYPE.itemsize == 440
+# b2_residual_result: what PCDSensorUpdaterB200.resampleResidual returns
+RESIDUAL_RESULT_DTYPE = np.dtype([("n_particles", np.uint64), ("draws", np.uint64), ("weight_sum", np.float64), ("weight_max", np.float64)])
+assert RESIDUAL_RESULT_DTYPE.itemsize == 32
 
 
 def quat_from_rpy(roll, pitch, yaw):
