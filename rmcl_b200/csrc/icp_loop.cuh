@@ -86,19 +86,27 @@ B2_DEV float icp_finalize_elem(double vi, double vm /* S_m[r] */, double vd /* S
     if (i < 6) return (float)(vi * inv);
     return (float)(vi * inv - (vm * inv) * (vd * inv));
 }
-// Tos * stats in rotation-matrix form (means as points, C -> R C R^T), explicit FMAs; s = {dm, mm, C} as 15 floats, same element numbering
-B2_DEV float icp_to_odom_elem(const float* R, const float* t, const float* s, int i)
+// Tos * stats in rotation-matrix form (means as points, C -> R C R^T), explicit FMAs, one element from what it reads: rows r and j of R
+// (icp_odom_rows), t[r], the point p (dm or mm) and C.  Element i < 6: (R p + t)[r];  i >= 6: o.C[j*3 + r] = sum_l (R C)[r][l] * R[j][l]
+B2_DEV void icp_odom_rows(int i, int& r, int& j)
 {
-    if (i < 6) {
-        const float* p = s + (i < 3 ? 0 : 3); const int r = i < 3 ? i : i - 3;
-        return fma_rn(R[r * 3 + 2], p[2], fma_rn(R[r * 3 + 1], p[1], fma_rn(R[r * 3 + 0], p[0], t[r])));
-    }
-    const int j = (i - 6) / 3, r = (i - 6) - 3 * j;                 // o.C[j*3 + r] = sum_l (R C)[r][l] * R[j][l]
-    const float* C = s + 6;
+    if (i < 6) { r = i < 3 ? i : i - 3; j = 0; }
+    else { j = (i - 6) / 3; r = (i - 6) - 3 * j; }
+}
+B2_DEV float icp_to_odom_rows(const float* Rr, const float* Rj, float tr, const float* p, const float* C, int i)
+{
+    if (i < 6) return fma_rn(Rr[2], p[2], fma_rn(Rr[1], p[1], fma_rn(Rr[0], p[0], tr)));
     float RC[3];
     #pragma unroll
-    for (int l = 0; l < 3; l++) RC[l] = fma_rn(R[r * 3 + 2], C[l * 3 + 2], fma_rn(R[r * 3 + 1], C[l * 3 + 1], mul(R[r * 3 + 0], C[l * 3 + 0])));
-    return fma_rn(RC[2], R[j * 3 + 2], fma_rn(RC[1], R[j * 3 + 1], mul(RC[0], R[j * 3 + 0])));
+    for (int l = 0; l < 3; l++) RC[l] = fma_rn(Rr[2], C[l * 3 + 2], fma_rn(Rr[1], C[l * 3 + 1], mul(Rr[0], C[l * 3 + 0])));
+    return fma_rn(RC[2], Rj[2], fma_rn(RC[1], Rj[1], mul(RC[0], Rj[0])));
+}
+// the same over a whole statistics record s = {dm, mm, C} as 15 floats, same element numbering
+B2_DEV float icp_to_odom_elem(const float* R, const float* t, const float* s, int i)
+{
+    int r, j;
+    icp_odom_rows(i, r, j);
+    return icp_to_odom_rows(R + r * 3, R + j * 3, t[r], s + (i < 3 ? 0 : 3), s + 6, i);
 }
 // per-sensor statistics in the odom frame from the reduced sums: serial form (host emulation; k_icp_loop spreads the elements over lanes)
 B2_DEV uint32_t icp_sensor_stats(const IcpSensor& S, const double* v, float* o /* 16 */)
@@ -113,9 +121,42 @@ B2_DEV uint32_t icp_sensor_stats(const IcpSensor& S, const double* v, float* o /
     return n;
 }
 
+// One Newton step of the polar iteration, X <- a X + b X^-T with X^-T = Cf / det; Frobenius-scaled in the first three steps.  Returns
+// |X_k+1 - X_k|^2; `ok` drops when det <= 1e-12 (reflection, singular, NaN).
+B2_DEV float icp_polar_step(float* X, bool scaled, bool& ok)
+{
+    float Cf[9];
+    Cf[0] = fma_rn(X[4], X[8], -mul(X[5], X[7])); Cf[1] = fma_rn(X[5], X[6], -mul(X[3], X[8])); Cf[2] = fma_rn(X[3], X[7], -mul(X[4], X[6]));
+    Cf[3] = fma_rn(X[2], X[7], -mul(X[1], X[8])); Cf[4] = fma_rn(X[0], X[8], -mul(X[2], X[6])); Cf[5] = fma_rn(X[1], X[6], -mul(X[0], X[7]));
+    Cf[6] = fma_rn(X[1], X[5], -mul(X[2], X[4])); Cf[7] = fma_rn(X[2], X[3], -mul(X[0], X[5])); Cf[8] = fma_rn(X[0], X[4], -mul(X[1], X[3]));
+    const float det = fma_rn(X[2], Cf[2], fma_rn(X[1], Cf[1], mul(X[0], Cf[0])));
+    ok = ok && det > 1e-12f;
+    float a, b;
+    if (scaled) {
+        // g = (|X^-1|_F / |X|_F)^(1/2) with X^-1 = Cf^T / det:  a = g / 2,  b = 1 / (2 g det).  Three short FMA chains per norm; the
+        // reciprocal roots of det and |X|^2 do not wait for the cofactor norm, so only two special-function results are chained.
+        const float nx = add(add(fma_rn(X[2], X[2], fma_rn(X[1], X[1], mul(X[0], X[0]))), fma_rn(X[5], X[5], fma_rn(X[4], X[4], mul(X[3], X[3])))),
+                             fma_rn(X[8], X[8], fma_rn(X[7], X[7], mul(X[6], X[6]))));
+        const float nc = add(add(fma_rn(Cf[2], Cf[2], fma_rn(Cf[1], Cf[1], mul(Cf[0], Cf[0]))), fma_rn(Cf[5], Cf[5], fma_rn(Cf[4], Cf[4], mul(Cf[3], Cf[3])))),
+                             fma_rn(Cf[8], Cf[8], fma_rn(Cf[7], Cf[7], mul(Cf[6], Cf[6]))));
+        const float rd = b2_rsqrt_approx(det), rx = b2_rsqrt_approx(nx);          // det^-1/2, |X|_F^-1
+        const float ratio = mul(mul(nc, b2_rsqrt_approx(nc)), rx);                 // |Cf|_F / |X|_F
+        const float rr = b2_rsqrt_approx(ratio);
+        b = mul(mul(0.5f, rr), rd);                                                // 1 / (2 g det),  g = ratio^1/2 det^-1/2
+        a = mul(mul(ratio, rr), mul(0.5f, rd));
+    } else { a = 0.5f; b = mul(0.5f, b2_rcp_approx(det)); }
+    float d2[3] = {0.f, 0.f, 0.f};
+    #pragma unroll
+    for (int i = 0; i < 9; i++) { const float y = fma_rn(b, Cf[i], mul(a, X[i])); const float d = sub(y, X[i]); d2[i / 3] = fma_rn(d, d, d2[i / 3]); X[i] = y; }
+    return add(add(d2[0], d2[1]), d2[2]);
+}
+
 // Orthogonal polar factor of C (det > 0) by the Frobenius-scaled Newton iteration, everything in registers: FP32 iterations, one FP64
 // polishing step whose 1/det is a Newton reciprocal around 1.  Returns false for reflections / singular / non-converged input (the caller
 // then takes the Jacobi SVD).  Same mathematics as polar_newton3, minus the call, the stack frame and the software divisions.
+// Converged after step k (k >= 2): |X_k+1 - X_k| < 3e-4 -- the step after it is at FP32 rounding level, and the FP64 step squares what is
+// left.  The cross-covariance of an ICP scan converges after three or four steps, so those four run as one straight chain: the fourth is
+// computed before the test of the third (and dropped if the third converged), the rest of the 40 only if the fourth has not.
 B2_DEV bool icp_polar(const float* C /* column-major, like CStats::C */, float* Rf /* row-major */, long long* st = nullptr)
 {
     float X[9];
@@ -130,35 +171,28 @@ B2_DEV bool icp_polar(const float* C /* column-major, like CStats::C */, float* 
     const float inv_n = b2_rsqrt_approx(fro);
     #pragma unroll
     for (int i = 0; i < 9; i++) X[i] = mul(X[i], inv_n);
-    bool conv = false;
-    for (int it = 0; it < 40 && !conv; it++) {
-        float Cf[9];
-        Cf[0] = fma_rn(X[4], X[8], -mul(X[5], X[7])); Cf[1] = fma_rn(X[5], X[6], -mul(X[3], X[8])); Cf[2] = fma_rn(X[3], X[7], -mul(X[4], X[6]));
-        Cf[3] = fma_rn(X[2], X[7], -mul(X[1], X[8])); Cf[4] = fma_rn(X[0], X[8], -mul(X[2], X[6])); Cf[5] = fma_rn(X[1], X[6], -mul(X[0], X[7]));
-        Cf[6] = fma_rn(X[1], X[5], -mul(X[2], X[4])); Cf[7] = fma_rn(X[2], X[3], -mul(X[0], X[5])); Cf[8] = fma_rn(X[0], X[4], -mul(X[1], X[3]));
-        const float det = fma_rn(X[2], Cf[2], fma_rn(X[1], Cf[1], mul(X[0], Cf[0])));
-        if (!(det > 1e-12f)) return false;
-        float a, b;
-        if (it < 3) {
-            // g = (|X^-1|_F / |X|_F)^(1/2) with X^-1 = Cf^T / det:  a = g / 2,  b = 1 / (2 g det).  Three short FMA chains per norm; the
-            // reciprocal roots of det and |X|^2 do not wait for the cofactor norm, so only two special-function results are chained.
-            const float nx = add(add(fma_rn(X[2], X[2], fma_rn(X[1], X[1], mul(X[0], X[0]))), fma_rn(X[5], X[5], fma_rn(X[4], X[4], mul(X[3], X[3])))),
-                                 fma_rn(X[8], X[8], fma_rn(X[7], X[7], mul(X[6], X[6]))));
-            const float nc = add(add(fma_rn(Cf[2], Cf[2], fma_rn(Cf[1], Cf[1], mul(Cf[0], Cf[0]))), fma_rn(Cf[5], Cf[5], fma_rn(Cf[4], Cf[4], mul(Cf[3], Cf[3])))),
-                                 fma_rn(Cf[8], Cf[8], fma_rn(Cf[7], Cf[7], mul(Cf[6], Cf[6]))));
-            const float rd = b2_rsqrt_approx(det), rx = b2_rsqrt_approx(nx);          // det^-1/2, |X|_F^-1
-            const float ratio = mul(mul(nc, b2_rsqrt_approx(nc)), rx);                 // |Cf|_F / |X|_F
-            const float rr = b2_rsqrt_approx(ratio);
-            b = mul(mul(0.5f, rr), rd);                                                // 1 / (2 g det),  g = ratio^1/2 det^-1/2
-            a = mul(mul(ratio, rr), mul(0.5f, rd));
-        } else { a = 0.5f; b = mul(0.5f, b2_rcp_approx(det)); }
-        float d2[3] = {0.f, 0.f, 0.f};
+    bool ok = true, ok3 = true;
+    icp_polar_step(X, true, ok);
+    icp_polar_step(X, true, ok);
+    const float s2 = icp_polar_step(X, true, ok);
+    float X3[9];
+    #pragma unroll
+    for (int i = 0; i < 9; i++) X3[i] = X[i];
+    const float s3 = icp_polar_step(X3, false, ok3);
+    if (!ok) return false;
+    bool conv = s2 < 1e-7f;
+    if (!conv) {
+        if (!ok3) return false;
         #pragma unroll
-        for (int i = 0; i < 9; i++) { const float y = fma_rn(b, Cf[i], mul(a, X[i])); const float d = sub(y, X[i]); d2[i / 3] = fma_rn(d, d, d2[i / 3]); X[i] = y; }
-        // |X_k+1 - X_k| < 3e-4: the step after it is at FP32 rounding level, and the FP64 step below squares what is left
-        conv = (it >= 2) && add(add(d2[0], d2[1]), d2[2]) < 1e-7f;
+        for (int i = 0; i < 9; i++) X[i] = X3[i];
+        conv = s3 < 1e-7f;
+        for (int it = 4; it < 40 && !conv; it++) {
+            const float s = icp_polar_step(X, false, ok);
+            if (!ok) return false;
+            conv = s < 1e-7f;
+        }
+        if (!conv) return false;
     }
-    if (!conv) return false;
     B2_TAIL_STAMP(st, 3);
     double Y[9];
     #pragma unroll
@@ -218,23 +252,22 @@ B2_DEV Tf icp_umeyama(const CStats& s, long long* st = nullptr)
     return out;
 }
 
-// One inner iteration after the per-sensor statistics are known in the odom frame (o[k] = Tbo * (Tsb * stats_s), :931).  T_onew_oold is updated in
-// place, Tpre_out[s] receives the pre-transform of sensor s for the NEXT pass (T_snew_sold = Tso * T_onew_oold * Tos: MICPSensor.hpp:178 with
-// the constant frame chain pre-composed) for the sensors [k0, k1) -- on the device lane k of the warp computes sensor k --, `res` is filled
-// after the last iteration (micp_localization.cpp:972-984).
-B2_DEV void icp_tail_rest(const IcpLaunch& L, const b2_transform& Tom_pod, const float (*odo)[16], const uint32_t* cnt, Tf& T_onew_oold, Tf* Tpre_out, uint32_t k0, uint32_t k1,
+// Sensor k's statistics in the odom frame (o = Tbo * (Tsb * stats_s), :931) into the merged statistics, in sensor order; merged / merged_w
+// start as cs_identity().  One sensor: merging with the empty identity is an exact no-op, so the sensor's statistics are taken as they are.
+B2_DEV void icp_merge_sensor(const IcpLaunch& L, uint32_t k, const CStats& o, CStats& merged, CStats& merged_w)
+{
+    CStats w = o;
+    if (L.s[k].merge_weight != 1.0) w.n = (uint32_t)((double)o.n * L.s[k].merge_weight);              // :933-934 (u32 *= double; exact no-op for weight 1)
+    if (L.n_sensors == 1) { merged = o; merged_w = w; }
+    else { merged = cs_merge(merged, o); merged_w = cs_merge(merged_w, w); }                          // :936-937
+}
+
+// One inner iteration after the merged statistics are known.  T_onew_oold is updated in place, Tpre_out[s] receives the pre-transform of sensor s
+// for the NEXT pass (T_snew_sold = Tso * T_onew_oold * Tos: MICPSensor.hpp:178 with the constant frame chain pre-composed) for the sensors
+// [k0, k1) -- on the device lane k of the warp computes sensor k --, `res` is filled after the last iteration (micp_localization.cpp:972-984).
+B2_DEV void icp_tail_rest(const IcpLaunch& L, const b2_transform& Tom_pod, const CStats& merged, const CStats& merged_w, Tf& T_onew_oold, Tf* Tpre_out, uint32_t k0, uint32_t k1,
                           bool last, IcpResult* res, long long* st = nullptr)
 {
-    CStats merged = cs_identity(), merged_w = cs_identity();
-    for (uint32_t k = 0; k < L.n_sensors; k++) {
-        CStats o; o.n = cnt[k]; o.dm = mk3(odo[k][0], odo[k][1], odo[k][2]); o.mm = mk3(odo[k][3], odo[k][4], odo[k][5]);
-        #pragma unroll
-        for (int q = 0; q < 9; q++) o.C[q] = odo[k][6 + q];
-        CStats w = o;
-        if (L.s[k].merge_weight != 1.0) w.n = (uint32_t)((double)o.n * L.s[k].merge_weight);          // :933-934 (u32 *= double; exact no-op for weight 1)
-        if (L.n_sensors == 1) { merged = o; merged_w = w; }                                           // merging with the empty identity is an exact no-op
-        else { merged = cs_merge(merged, o); merged_w = cs_merge(merged_w, w); }                      // :936-937
-    }
     B2_TAIL_STAMP(st, 2);
     const Tf T_inner = icp_umeyama(merged_w, st);                                                     // :952-953
     T_onew_oold = tf_mul(T_onew_oold, T_inner);                                                       // :963
@@ -251,9 +284,15 @@ B2_DEV void icp_tail_rest(const IcpLaunch& L, const b2_transform& Tom_pod, const
 // the whole serial tail from the reduced sums (host emulation: tests/emul)
 B2_DEV void icp_tail(const IcpLaunch& L, const double (*sums)[B2_NACC + 1], Tf& T_onew_oold, Tf* Tpre_out, bool last, IcpResult* res)
 {
-    float odo[B2_MAX_SENSORS][16]; uint32_t cnt[B2_MAX_SENSORS];
-    for (uint32_t k = 0; k < L.n_sensors; k++) cnt[k] = icp_sensor_stats(L.s[k], sums[k], odo[k]);
-    icp_tail_rest(L, L.Tom, odo, cnt, T_onew_oold, Tpre_out, 0, L.n_sensors, last, res);
+    CStats merged = cs_identity(), merged_w = cs_identity();
+    for (uint32_t k = 0; k < L.n_sensors; k++) {
+        float odo[16];
+        CStats o; o.n = icp_sensor_stats(L.s[k], sums[k], odo);
+        o.dm = mk3(odo[0], odo[1], odo[2]); o.mm = mk3(odo[3], odo[4], odo[5]);
+        for (int q = 0; q < 9; q++) o.C[q] = odo[6 + q];
+        icp_merge_sensor(L, k, o, merged, merged_w);
+    }
+    icp_tail_rest(L, L.Tom, merged, merged_w, T_onew_oold, Tpre_out, 0, L.n_sensors, last, res);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -430,13 +469,10 @@ __global__ void __launch_bounds__(B2_ICP_BLOCK) k_icp_loop(const __grid_constant
     extern __shared__ float s_pairs[];                             // [smem_u][9][B2_ICP_BLOCK]
     __shared__ double smem[16 * (B2_ICP_BLOCK / 32)];
     __shared__ double s_part[B2_MAX_SENSORS][B2_ICP_BLOCK / 32][B2_NACC + 1];
-    __shared__ float s_fin[B2_MAX_SENSORS][16], s_odo[B2_MAX_SENSORS][16];   // per-sensor statistics: sensor frame, odom frame
     __shared__ float s_Rt[B2_MAX_SENSORS][12];                     // Ros (9) + translation of Tos (3): lane-indexed reads in the tail
-    __shared__ uint32_t s_n[B2_MAX_SENSORS];
     __shared__ unsigned long long s_prev[2][B2_MAX_SENSORS][32];   // accumulator words before the current round, per parity
     __shared__ uint32_t s_bin[1 + 16 * 15];                        // tile schedule of the next find (first block of each sensor)
     __shared__ Tf s_Tpre[B2_MAX_SENSORS];
-    __shared__ Tf s_T;                                             // T_onew_oold
     __shared__ b2_transform s_Tom;                                 // Tom of this correctOnce (micp_localization.cpp:860)
     __shared__ IcpResult s_res;
     const long long k0 = clock64();
@@ -452,7 +488,7 @@ __global__ void __launch_bounds__(B2_ICP_BLOCK) k_icp_loop(const __grid_constant
     if (tid < L.n_sensors) {
         // pre-transform of the first pass: T_onew_oold = I  ->  Tso * I * Tos with the same individually rounded ops as later iterations
         s_Tpre[tid] = tf_mul(tf_mul(tf_from_pod(L.s[tid].Tso), tf_identity()), tf_from_pod(L.s[tid].Tos));
-        if (tid == 0) { s_T = tf_identity(); s_Tom = L.chain ? L.chain->find[0].Tom : L.Tom; }
+        if (tid == 0) s_Tom = L.chain ? L.chain->find[0].Tom : L.Tom;
     }
     if (tid >= 32u && tid < 32u + 12u * L.n_sensors) {
         const uint32_t k = (tid - 32u) / 12u, e = (tid - 32u) - 12u * k;
@@ -524,6 +560,7 @@ __global__ void __launch_bounds__(B2_ICP_BLOCK) k_icp_loop(const __grid_constant
     __syncthreads();
     // a chain step gates with the progress the previous step left (written before this grid's find was launched)
     const float max_dist = L.chain ? icp_adaptive_max_dist(S.max_dist, S.max_dist_min, L.chain->cp) : S.max_dist;
+    Tf T = tf_identity();                                          // T_onew_oold: the same value on every lane of warp 0
     const long long k1 = clock64();
     for (uint32_t it = 0; it < L.iterations; it++) {
         const long long c0 = clock64();
@@ -603,8 +640,16 @@ __global__ void __launch_bounds__(B2_ICP_BLOCK) k_icp_loop(const __grid_constant
                 if (it == 1 && dbg && lane == 0) { dbg[16 + 4 * blockIdx.x] = globaltimer_ns(); dbg[16 + 4 * blockIdx.x + 2] = (unsigned long long)(clock64() - c1); }
 #endif
             }
-            // ---- per sensor: the grid-wide sums on lanes 0..15, then the 15 elements of the statistics on 15 lanes ----
+            // ---- per sensor: the grid-wide sums on lanes 0..15, then the 15 elements of the statistics on 15 lanes, moved between the lanes
+            //      by shuffles: finalised (sensor frame) -> odom frame -> every lane's copy of the sensor's statistics -> merged ----
+            int orow, ocol;                                         // the rows of Ros that this lane's odom-frame element reads
+            icp_odom_rows(lane < 15u ? e : 0, orow, ocol);
+            CStats merged = cs_identity(), merged_w = cs_identity();
             for (uint32_t k = 0; k < L.n_sensors; k++) {
+                float Rr[3], Rj[3];
+                #pragma unroll
+                for (int q = 0; q < 3; q++) { Rr[q] = s_Rt[k][orow * 3 + q]; Rj[q] = s_Rt[k][ocol * 3 + q]; }
+                const float tr = s_Rt[k][9 + orow];
                 double x = 0.0;
                 if (COOP) {
                     if (lane < 16u) {
@@ -633,23 +678,30 @@ __global__ void __launch_bounds__(B2_ICP_BLOCK) k_icp_loop(const __grid_constant
                     const double lo = __shfl_down_sync(0xffffffffu, part, 16);
                     x = part + lo * 9.094947017729282379150390625e-13;                                // 2^-40
                 }
-                const double cnt = __shfl_sync(0xffffffffu, x, 15), vm = __shfl_sync(0xffffffffu, x, 3 + rr), vd = __shfl_sync(0xffffffffu, x, cc);
+                // the count first: its reciprocal is the longest chain here and does not wait for the value shuffles
+                const double cnt = __shfl_sync(0xffffffffu, x, 15);
                 const uint32_t nk = (uint32_t)(cnt + 0.5);
                 const double inv = nk ? b2_rcp_u32(nk) : 0.0;
-                if (lane < 15u) s_fin[k][lane] = icp_finalize_elem(x, vm, vd, inv, e);
-                if (lane == 15u) s_n[k] = nk;
+                const double vm = __shfl_sync(0xffffffffu, x, 3 + rr), vd = __shfl_sync(0xffffffffu, x, cc);
+                const float fin = icp_finalize_elem(x, vm, vd, inv, e);                              // lanes 0..14 (the rest is not read)
+                float p[3], Cs[9];
+                #pragma unroll
+                for (int q = 0; q < 3; q++) p[q] = __shfl_sync(0xffffffffu, fin, (lane < 3u ? 0 : 3) + q);
+                #pragma unroll
+                for (int q = 0; q < 9; q++) Cs[q] = __shfl_sync(0xffffffffu, fin, 6 + q);
+                const float od = icp_to_odom_rows(Rr, Rj, tr, p, Cs, e);
+                CStats o; o.n = nk;
+                o.dm = mk3(__shfl_sync(0xffffffffu, od, 0), __shfl_sync(0xffffffffu, od, 1), __shfl_sync(0xffffffffu, od, 2));
+                o.mm = mk3(__shfl_sync(0xffffffffu, od, 3), __shfl_sync(0xffffffffu, od, 4), __shfl_sync(0xffffffffu, od, 5));
+                #pragma unroll
+                for (int q = 0; q < 9; q++) o.C[q] = __shfl_sync(0xffffffffu, od, 6 + q);
+                icp_merge_sensor(L, k, o, merged, merged_w);
             }
-            __syncwarp();
-            for (uint32_t k = 0; k < L.n_sensors; k++) if (lane < 15u) s_odo[k][lane] = icp_to_odom_elem(s_Rt[k], s_Rt[k] + 9, s_fin[k], e);
-            __syncwarp();
             const long long c3 = clock64();
-            Tf T = s_T;
             long long st[8] = {0, 0, 0, 0, 0, 0, 0, 0};
             const bool prof = it == 1 && blockIdx.x == 0 && dbg && lane == 0;
             const bool mine = lane < L.n_sensors;                                                    // lane k prepares sensor k's next pre-transform
-            if (ok) icp_tail_rest(L, s_Tom, s_odo, s_n, T, s_Tpre, mine ? lane : 0u, mine ? lane + 1u : 0u, it + 1 == L.iterations, lane == 0 ? &s_res : nullptr, prof ? st : nullptr);
-            __syncwarp();                                           // every lane has read s_T (and the statistics) before lane 0 replaces it
-            if (lane == 0) s_T = T;
+            if (ok) icp_tail_rest(L, s_Tom, merged, merged_w, T, s_Tpre, mine ? lane : 0u, mine ? lane + 1u : 0u, it + 1 == L.iterations, lane == 0 ? &s_res : nullptr, prof ? st : nullptr);
             if (prof) {
                 const long long c4 = clock64();
                 dbg[0] = (unsigned long long)(c1 - c0); dbg[1] = (unsigned long long)(c2 - c1); dbg[2] = (unsigned long long)(c3 - c2); dbg[3] = (unsigned long long)(c4 - c3);
