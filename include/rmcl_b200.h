@@ -427,6 +427,28 @@ B2_API int b2_pf_resample_residual(b2_pf* h, const b2_transform* poses_dev, cons
                                    uint32_t first, uint32_t n_local, b2_transform* poses_new_dev, b2_particle_attr* attrs_new_dev,
                                    const b2_gladiator_config* cfg, uint64_t seed, uint32_t step, b2_residual_result* out_host);
 
+/* The motion stage's surface constraint, "a MotionUpdater constrained to the mesh surface" (rmcl/docs/RMCL.md:72, listed as missing; no
+ * reference implementation, SURVEY appendix F): keeps the particle set on the walkable surface of a mesh map (ramps, stairs, floors) after any
+ * stage that moves it (init, motion, resampling).  Up is map +z (REP-103).  Per particle, with t, R its pose, in float arithmetic rounded in
+ * the order written, cos_max = (float)cos((double)max_slope) and tfar = probe_above + probe_below:
+ *  1. probe: the closest hit of the ray from (t.x, t.y, t.z + probe_above) along (0, 0, -1) with t_hit in (0, tfar], ties to the smaller face
+ *     id (the rule of b2_mesh_intersect);
+ *  2. ground iff n.z >= cos_max, n = normalize(Ng) of the hit triangle, negated if n.z < 0 (it faces the ray origin); a NaN normal is not ground;
+ *  3. on ground: g = (t.x, t.y, (t.z + probe_above) - t_hit).  align 0: R' = R, t' = (g.x, g.y, g.z + base_height).  align 1: a = R e_z (the
+ *     quaternion rotation), c = a . n, q = (R e_x, 0) if 1 + c < 1e-6 else (a x n, 1 + c), R' = normalize(normalize(q) * R) and
+ *     t' = g + base_height * n: the smallest rotation that takes the body z-axis onto n, so the heading changes as little as possible.
+ *     The stamp and the attributes are unchanged;
+ *  4. off surface (no hit, a hit that is not ground, a non-finite t or R; a non-finite position hits nothing): the pose is unchanged and the likelihood
+ *     becomes {0, 0, MAX_N_MEAS}, the wall check's mark (b2_pf_motion_update); state_sigma is unchanged.  The next resampling replaces it.
+ * Limits: a probe_above larger than the clearance under a table or an upper floor lands the particle on top of it; with base_height 0 the wall
+ * check's old -> new ray runs along the ground and can graze it on curved terrain (use base_height > 0 with check_collision).
+ * In place on poses_dev / attrs_dev (DEVICE pointers), one thread per particle on the handle's stream, no synchronisation; n == 0 launches
+ * nothing.  Refused (B2_ERR_INVALID, no launch, both buffers untouched): null h or cfg, null buffers with n > 0, a non-finite field,
+ * probe_above < 0, probe_below < 0, tfar <= 0, base_height < 0, max_slope outside [0, pi/2], align other than 0 or 1.
+ * Suggested values: probe_above 0.5, probe_below 1.0, base_height 0.0, max_slope 0.6 rad, align 1. */
+typedef struct { float probe_above, probe_below, base_height, max_slope; int32_t align; } b2_surface_config;      /* 20 B */
+B2_API int b2_pf_project_to_surface(b2_pf* h, b2_transform* poses_dev, b2_particle_attr* attrs_dev, uint32_t n_particles, const b2_surface_config* cfg);
+
 /* ---------------------------------------------------------------- introspection ------------------------------ */
 /* CUDA-event timing of the kernels inside b2_rcc_correct_once*(): when enabled, events are recorded on the handle's stream around the
  * find kernel and around the reduction/Umeyama kernels; b2_rcc_last_timing returns the two durations of the most recent call (ms). */

@@ -393,6 +393,17 @@ public:
         b2_check(b2_pf_motion_update(h_, reinterpret_cast<b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(),
                                      reinterpret_cast<const b2_transform*>(&T_bnew_bold), forget_rate, check_collision ? 1 : 0), "motionUpdate");
     }
+    // The surface-constrained motion update of docs/RMCL.md:72 (b2_pf_project_to_surface): each particle is put on the walkable surface
+    // under it, in place; one with no such surface in the probe window gets the likelihood {0, 0, MAX_N_MEAS}.  Call it after motionUpdate,
+    // after initSamplesUniform and after resampling.  surface_config() gives the suggested values.
+    static b2_surface_config surface_config() { return b2_surface_config{0.5f, 1.0f, 0.0f, 0.6f, 1}; }
+    void projectToSurface(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs,
+                          const b2_surface_config& cfg = surface_config())
+    {
+        if (poses.size() != attrs.size()) throw std::invalid_argument("projectToSurface: poses and attrs differ in size");
+        b2_check(b2_pf_project_to_surface(h_, reinterpret_cast<b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(), &cfg),
+                 "projectToSurface");
+    }
     struct SimpleLikelihoodStats { float sum = 0.0f; float max = -1.0f; };                       // resampling.cuh:26-30
     SimpleLikelihoodStats computeStats(rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs)
     {

@@ -61,6 +61,16 @@ class GladiatorConfig(C.Structure):
         return GladiatorConfig(0.03, 0.03, 0.0, 0.0, 0.0, 0.01, 0.3, 0.2)
 
 
+class SurfaceConfig(C.Structure):
+    """b2_surface_config: the surface constraint of projectToSurface (m, rad; align 0 keeps the orientation, 1 tilts the body z-axis onto
+    the ground normal).  defaults() are the suggested values."""
+    _fields_ = [("probe_above", C.c_float), ("probe_below", C.c_float), ("base_height", C.c_float), ("max_slope", C.c_float), ("align", C.c_int32)]
+
+    @staticmethod
+    def defaults():
+        return SurfaceConfig(0.5, 1.0, 0.0, 0.6, 1)
+
+
 class _CloudLayout(C.Structure):
     _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("point_step", C.c_uint32), ("row_step", C.c_uint32), ("offset_x", C.c_uint32),
                 ("offset_y", C.c_uint32), ("offset_z", C.c_uint32), ("datatype", C.c_uint8), ("is_bigendian", C.c_uint8), ("pad", C.c_uint8 * 2)]
@@ -124,7 +134,7 @@ EXPORTS = [
     "b2_rcc_set_correspondence_type", "b2_pf_resample_gladiator", "b2_pf_gladiator_randoms", "b2_rcc_segment", "b2_mesh_create_from_file", "b2_mesh_file_load", "b2_mesh_file_free", "b2_peek_cuda_error", "b2_mesh_blob_size", "b2_mesh_export_blob", "b2_mesh_create_from_blob", "b2_mesh_refit",
     "b2_rcc_correct_once_async", "b2_rcc_correct_once_wait", "b2_micp_correct_once", "b2_rcc_set_exec_mode", "b2_debug_read_bandwidth", "b2_rcc_set_sim_options", "b2_rcc_bind_dataset", "b2_rcc_bind_model_buffers", "b2_rcc_benchmark_batch", "b2_pf_p2p_init", "b2_pf_p2p_connect", "b2_pf_p2p_publish", "b2_pf_resample_gladiator_p2p", "b2_pf_p2p_connect_local", "b2_rcc_set_cpc_options", "b2_pf_set_mapping", "b2_pf_get_mapping",
     "b2_micp_correct", "b2_pf_init_uniform", "b2_pf_init_gaussian", "b2_pf_estimate_stats", "b2_rcc_set_cloud_o1dn",
-    "b2_rcc_set_cloud_spherical", "b2_pf_sample_cloud", "b2_pf_resample_residual",
+    "b2_rcc_set_cloud_spherical", "b2_pf_sample_cloud", "b2_pf_resample_residual", "b2_pf_project_to_surface",
 ]
 
 
@@ -739,6 +749,17 @@ class PCDSensorUpdaterB200:
         n = particle_poses.numel() * particle_poses.element_size() // 32
         _chk(load_library().b2_pf_motion_update(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(n), _p(_tf(T_bnew_bold)), C.c_double(forget_rate),
                                                 C.c_int(int(check_collision))))
+
+    def projectToSurface(self, particle_poses, particle_attrs, config=None):
+        """Keep the particles on the map's walkable surface (b2_pf_project_to_surface; the surface-constrained motion update of
+        rmcl/docs/RMCL.md:72): in place on torch CUDA tensors, on the handle's stream.  Each particle is put on the first surface under it
+        within `config`'s probe window whose slope is at most max_slope (and tilted onto it with align 1); one found no such surface keeps
+        its pose and gets the likelihood {0, 0, 10000}, so the next resampling replaces it.  `config`: a SurfaceConfig (default: defaults())."""
+        cfg = config or SurfaceConfig.defaults()
+        n = particle_poses.numel() * particle_poses.element_size() // 32
+        if particle_attrs.numel() * particle_attrs.element_size() != 36 * n:
+            raise ValueError("projectToSurface: poses and attrs differ in length")
+        _chk(load_library().b2_pf_project_to_surface(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(n), C.byref(cfg)))
 
     def likelihoodStats(self, particle_attrs, dist=None):
         """compute_stats (rmcl_ros/src/rmcl/resampling.cu:41-92) of the local particles; with `dist` (torch.distributed, particles sharded

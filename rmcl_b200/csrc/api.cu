@@ -2111,6 +2111,29 @@ extern "C" int b2_pf_motion_update(b2_pf* h, b2_transform* poses_dev, b2_particl
     return B2_OK;
 }
 
+// the motion stage's surface constraint (docs/RMCL.md:72; SURVEY appendix F): one downward ray per particle, in place
+extern "C" int b2_pf_project_to_surface(b2_pf* h, b2_transform* poses_dev, b2_particle_attr* attrs_dev, uint32_t n, const b2_surface_config* cfg)
+{
+    NOTNULL(h); NOTNULL(cfg);
+    if (n > 0) { NOTNULL(poses_dev); NOTNULL(attrs_dev); }
+    const b2_surface_config c = *cfg;
+    const float f[4] = {c.probe_above, c.probe_below, c.base_height, c.max_slope};
+    if (!all_finite(f, 4)) return fail(B2_ERR_INVALID, "project to surface: a config field is not finite (%g, %g, %g, %g)", f[0], f[1], f[2], f[3]);
+    const float tfar = c.probe_above + c.probe_below;
+    if (c.probe_above < 0.0f || c.probe_below < 0.0f || !(tfar > 0.0f))
+        return fail(B2_ERR_INVALID, "project to surface: probe_above %g and probe_below %g must be >= 0 with a positive sum", f[0], f[1]);
+    if (c.base_height < 0.0f) return fail(B2_ERR_INVALID, "project to surface: base_height %g < 0", f[2]);
+    if (!(c.max_slope >= 0.0f && c.max_slope <= (float)1.5707963267948966))           // pi/2 rounded to float, as a caller passes it
+        return fail(B2_ERR_INVALID, "project to surface: max_slope %g outside [0, pi/2]", f[3]);
+    if (c.align != 0 && c.align != 1) return fail(B2_ERR_INVALID, "project to surface: align is 0 or 1, not %d", (int)c.align);
+    if (n == 0) return B2_OK;
+    const float cos_max = (float)std::cos((double)c.max_slope);
+    CU(cudaSetDevice(h->map->device));
+    k_pf_surface<<<(n + 127) / 128, 128, 0, h->stream>>>(h->map->view(), poses_dev, attrs_dev, n, c, cos_max, tfar);
+    LAUNCHED();
+    return B2_OK;
+}
+
 extern "C" int b2_pf_resample_gladiator(b2_pf* h, const b2_transform* poses_dev, const b2_particle_attr* attrs_dev, uint32_t n_all, uint32_t first, uint32_t n_local,
                                         b2_transform* poses_new_dev, b2_particle_attr* attrs_new_dev, const b2_gladiator_config* cfg, uint64_t seed, uint32_t step,
                                         const uint32_t* raw_dev, const float* normals_dev)

@@ -1216,6 +1216,68 @@ __global__ void __launch_bounds__(128) k_pf_motion(BvhView bvh, b2_transform* __
 }
 #endif
 
+// The surface constraint of the motion stage (docs/RMCL.md:72 lists it as missing; no reference implementation, SURVEY appendix F).  One
+// ray straight down (map -z) from probe_above over the particle, closest hit in (0, tfar]; the hit is ground iff the unit normal, turned
+// to face the ray origin, has n.z >= cos_max.  On ground the particle is put base_height over it (along +z, or along n with align, where
+// the smallest rotation also takes the body z-axis onto n); else it keeps its pose and gets the wall check's mark {0, 0, MAX_N_MEAS}.
+// The stamp and the rest of the attributes are left as they are.  cos_max = (float)cos((double)max_slope), tfar = probe_above + probe_below.
+B2_DEV void pf_surface_one(const BvhView& bvh, b2_transform* pose_io, b2_particle_attr* attr_io, const b2_surface_config& cfg, float cos_max, float tfar)
+{
+    const Tf T = tf_load(pose_io);
+    const float oz = add(T.t.z, cfg.probe_above);
+    HitRec h = trace_init(tfar);
+    // A non-finite pose is off surface.  A non-finite origin hits no triangle anyway, but its box tests pass everywhere (fmaxf / fminf drop
+    // NaN): do not walk the whole tree for it.
+    const float inf = u2f(0x7f800000u);
+    if (fabsf(T.t.x) < inf && fabsf(T.t.y) < inf && fabsf(oz) < inf &&
+        fabsf(T.R.x) < inf && fabsf(T.R.y) < inf && fabsf(T.R.z) < inf && fabsf(T.R.w) < inf) {
+        const RaySetup r = ray_setup(mk3(T.t.x, T.t.y, oz), mk3(0.0f, 0.0f, -1.0f), bvh);
+        uint32_t nn = 0, nt = 0;
+        trace_closest<false>(bvh, r, h, nn, nt);
+    }
+    V3 n = mk3(0.0f, 0.0f, 0.0f);
+    if (h.face != B2_NOFACE) {
+        n = v_normalize(tri_ng(bvh, h.tri));
+        if (n.z < 0.0f) n = v_neg(n);
+    }
+    if (!(h.face != B2_NOFACE && n.z >= cos_max)) {                                   // no hit, too steep, or a NaN normal
+        b2_gaussian1d lk = attr_io->likelihood;
+        lk.mean = 0.0f; lk.sigma = 0.0f; lk.n_meas = 10000u;
+        attr_io->likelihood = lk;
+        return;
+    }
+    const V3 g = mk3(T.t.x, T.t.y, sub(oz, h.t));
+    Tf out;
+    if (cfg.align) {
+        const V3 a = q_rot(T.R, mk3(0.0f, 0.0f, 1.0f));
+        const float w = add(1.0f, v_dot(a, n));
+        Q4 q;
+        if (w < 1e-6f) {                                                               // body z-axis opposite to n: half turn about body x
+            const V3 ex = q_rot(T.R, mk3(1.0f, 0.0f, 0.0f));
+            q.x = ex.x; q.y = ex.y; q.z = ex.z; q.w = 0.0f;
+        } else {                                                                       // a x n, rm::Vector3::cross
+            q.x = sub(mul(a.y, n.z), mul(a.z, n.y)); q.y = sub(mul(a.z, n.x), mul(a.x, n.z)); q.z = sub(mul(a.x, n.y), mul(a.y, n.x)); q.w = w;
+        }
+        out.R = q_normalize(q_mul(q_normalize(q), T.R));
+        out.t = v_add(g, v_scale(n, cfg.base_height));
+    } else {
+        out.R = T.R;
+        out.t = mk3(g.x, g.y, add(g.z, cfg.base_height));
+    }
+    // R and t only: the stamp stays
+    pose_io->R.x = out.R.x; pose_io->R.y = out.R.y; pose_io->R.z = out.R.z; pose_io->R.w = out.R.w;
+    pose_io->t.x = out.t.x; pose_io->t.y = out.t.y; pose_io->t.z = out.t.z;
+}
+#ifdef __CUDACC__
+__global__ void __launch_bounds__(128) k_pf_surface(BvhView bvh, b2_transform* __restrict__ poses, b2_particle_attr* __restrict__ attrs, uint32_t n,
+                                                    b2_surface_config cfg, float cos_max, float tfar)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    pf_surface_one(bvh, poses + i, attrs + i, cfg, cos_max, tfar);
+}
+#endif
+
 // ---------------------------------------------------------------------------------------------------------------------
 // Gladiator resampling (rmcl_ros/src/rmcl/resampling.cu:108-199).  Draws: Philox4x32-10 (Salmon et al., SC'11), counter =
 // (global particle index, 0, step, block), key = seed -- one raw u32 (opponent) + three Box-Muller pairs per particle; a function

@@ -187,6 +187,75 @@ def indoor(n_faces: int = 500_000):
     return _rects_to_mesh(rects, n_faces)
 
 
+# terrain(): the geometry its users need to know (m).  The ramp rises TERRAIN_RAMP["rise"] over TERRAIN_RAMP["run"] along +x, 10.008 deg.
+TERRAIN_FLOOR = ((0.0, 0.0, 48.0, 32.0), (48.0, 16.0, 64.0, 32.0))                   # z = 0: (x0, y0, x1, y1) rectangles
+TERRAIN_RAMP = {"x0": 4.0, "y0": 0.0, "y1": 4.0, "run": 17.0, "rise": 3.0}           # from z = 0 at x0 to the mezzanine at x0 + run
+TERRAIN_MEZZANINE = {"x0": 21.0, "y0": 0.0, "x1": 37.0, "y1": 16.0, "top": 3.0, "bottom": 2.75}
+TERRAIN_STAIRS = {"x0": 40.0, "y0": 20.0, "y1": 24.0, "steps": 8, "tread": 0.5, "riser": 0.25}   # up along +x, a wall behind the top
+TERRAIN_BUMPS = {"x0": 48.0, "y0": 0.0, "size": 16.0, "height": 0.4, "period": 8.0}
+
+
+def terrain_bump_z(x, y):
+    """height of the bump field: height * (sin(2 pi u / period) sin(2 pi v / period))^2 over its square, 0 on its border (steepest 17.4 deg)"""
+    b = TERRAIN_BUMPS
+    k = 2.0 * math.pi / b["period"]
+    return b["height"] * (np.sin(k * (np.asarray(x) - b["x0"])) * np.sin(k * (np.asarray(y) - b["y0"]))) ** 2
+
+
+def _terrain_lattice(s):
+    """the parts of terrain() on the dyadic lattice, with cell size s = 2^-k"""
+    def n(length):
+        return max(1, int(round(length / s)))
+    parts = []
+    for x0, y0, x1, y1 in TERRAIN_FLOOR:
+        parts.append(_grid_rect([x0, y0, 0.0], [x1 - x0, 0, 0], [0, y1 - y0, 0], n(x1 - x0), n(y1 - y0)))
+    r = TERRAIN_RAMP
+    # ramp cells: run / 2^j along the slope (vertices x0 + run i / 2^j, rise i / 2^j stay dyadic)
+    parts.append(_grid_rect([r["x0"], r["y0"], 0.0], [r["run"], 0, r["rise"]], [0, r["y1"] - r["y0"], 0], n(16.0), n(r["y1"] - r["y0"])))
+    m = TERRAIN_MEZZANINE
+    dx, dy, dz = m["x1"] - m["x0"], m["y1"] - m["y0"], m["top"] - m["bottom"]
+    parts.append(_grid_rect([m["x0"], m["y0"], m["top"]], [dx, 0, 0], [0, dy, 0], n(dx), n(dy)))          # top (+z)
+    parts.append(_grid_rect([m["x0"], m["y0"], m["bottom"]], [0, dy, 0], [dx, 0, 0], n(dy), n(dx)))       # underside (-z)
+    parts.append(_grid_rect([m["x0"], m["y0"], m["bottom"]], [dx, 0, 0], [0, 0, dz], n(dx), 1))           # y = y0
+    parts.append(_grid_rect([m["x0"], m["y1"], m["bottom"]], [0, 0, dz], [dx, 0, 0], 1, n(dx)))           # y = y1
+    parts.append(_grid_rect([m["x0"], m["y0"], m["bottom"]], [0, 0, dz], [0, dy, 0], 1, n(dy)))           # x = x0
+    parts.append(_grid_rect([m["x1"], m["y0"], m["bottom"]], [0, dy, 0], [0, 0, dz], n(dy), 1))           # x = x1
+    st = TERRAIN_STAIRS
+    w = st["y1"] - st["y0"]
+    for k in range(st["steps"]):
+        x = st["x0"] + k * st["tread"]
+        parts.append(_grid_rect([x, st["y0"], k * st["riser"]], [0, w, 0], [0, 0, st["riser"]], n(w), n(st["riser"])))      # riser (vertical)
+        parts.append(_grid_rect([x, st["y0"], (k + 1) * st["riser"]], [st["tread"], 0, 0], [0, w, 0], n(st["tread"]), n(w)))  # tread
+    top = st["steps"] * st["riser"]
+    parts.append(_grid_rect([st["x0"] + st["steps"] * st["tread"], st["y0"], 0.0], [0, 0, top], [0, w, 0], n(top), n(w)))  # back wall
+    return parts
+
+
+def terrain(n_tris: int = 1_000_000):
+    """A mesh map for the surface constraint (PCDSensorUpdaterB200.projectToSurface): a flat floor at z = 0 (TERRAIN_FLOOR), a ramp
+    (TERRAIN_RAMP, 3 m over 17 m) up to a mezzanine slab whose top is at 3 m over part of the floor (TERRAIN_MEZZANINE, 0.25 m thick),
+    stairs with vertical risers (TERRAIN_STAIRS) and a field of smooth bumps (TERRAIN_BUMPS, terrain_bump_z) in the floor's missing corner.
+    Every vertex except the bumps' is on a dyadic lattice (cell 2^-k, exact in float32), so points on its edges and vertices are exact.
+    About n_tris triangles, at most n_tris: the finest lattice with at most n_tris / 2 triangles, the rest an nb x nb bump grid."""
+    def count(parts):
+        return sum(F.shape[0] for _, F in parts)
+    s = 1.0
+    parts = _terrain_lattice(s)
+    if count(parts) + 2 * 4 * 4 > n_tris:
+        raise ValueError(f"terrain needs at least {count(parts) + 32} triangles")
+    while True:
+        finer = _terrain_lattice(s / 2)
+        if count(finer) > n_tris // 2:
+            break
+        s, parts = s / 2, finer
+    b = TERRAIN_BUMPS
+    nb = int(math.isqrt((n_tris - count(parts)) // 2))
+    V, F = _grid_rect([b["x0"], b["y0"], 0.0], [b["size"], 0, 0], [0, b["size"], 0], nb, nb)
+    V[:, 2] = terrain_bump_z(V[:, 0], V[:, 1])
+    V[np.isin(V[:, 0], (b["x0"], b["x0"] + b["size"])) | np.isin(V[:, 1], (b["y0"], b["y0"] + b["size"])), 2] = 0.0     # the border meets the floor
+    return _merge(parts + [(V, F)])
+
+
 # --------------------------------------------------------------------------------------------------
 # sensor models (field names follow rmagine / rmcl_msgs ScanInfo, DepthInfo: rmcl_ros/src/util/conversions.cpp:22-60)
 # --------------------------------------------------------------------------------------------------
