@@ -427,6 +427,38 @@ B2_API int b2_pf_resample_residual(b2_pf* h, const b2_transform* poses_dev, cons
                                    uint32_t first, uint32_t n_local, b2_transform* poses_new_dev, b2_particle_attr* attrs_new_dev,
                                    const b2_gladiator_config* cfg, uint64_t seed, uint32_t step, b2_residual_result* out_host);
 
+/* KLD-sampling (Fox, "Adapting the sample size in particle filters through KLD-sampling", IJRR 2003; "reduce the number of particles more
+ * intelligently", rmcl/docs/RMCL.md:80-83, listed as missing; SURVEY appendix G): resamples the n particles poses_dev / attrs_dev into an
+ * output set of at most n_max slots (the node passes its whole max_particles buffer), as many as the spread of the drawn set calls for.
+ *  - S = weight_sum, L_min and weight_max = L_max of likelihood.mean as b2_pf_resample_residual takes them.  S not finite, S <= 0 or L_min < 0:
+ *    0 particles, nothing written, B2_OK.
+ *  - Weights w_i = (uint64)((double)L_i / L_max * 2^32), inclusive prefix W (exact in 64 bits).  Draw j takes u = words 2(j % 2) (low) and
+ *    2(j % 2) + 1 (high) of Philox4x32-10 with counter (lo(j / 2), 6, step, hi(j / 2)) and key `seed`; its parent is the smallest i with
+ *    W[i] > mulhi64(u, W[n-1]).  A zero weight is never drawn.
+ *  - The bin of a draw is its parent's ix = floor(t.x / res_xy), iy likewise, iz with res_z (res_z = 0: z not binned), clamped to [-2^19, 2^19)
+ *    and [-2^7, 2^7), and the yaw sector of the heading h = (1 - 2(y^2 + z^2), 2(xy + wz)) among K = ceil(2 pi / res_yaw (1 - 2^-20)) sectors with
+ *    boundaries -pi + 2 pi k / K; roll and pitch are not binned.  A non-finite pose is its own bin.
+ *  - Stop at the first draw j with j + 1 >= max(n_min, bound(k_j)) or j + 1 = n_max, k_j the number of bins among draws 0 .. j and
+ *    bound(k) = ceil((k - 1) / (2 epsilon) x^3), x = 1 - 2 / (9(k - 1)) + sqrt(2 / (9(k - 1))) z, bound(k <= 1) = n_min.  z is the upper
+ *    standard normal quantile of the bound's confidence, used as given.  n_particles = j + 1, bins = k_j.
+ *  - Slot j is a copy of draw j's parent as b2_pf_resample_residual copies it (normals keyed by the slot with tag 5, noise scaled by
+ *    L_max / L, forget factors, the parent's stamp), with the Gladiator config `cfg`.
+ * poses_new_dev / attrs_new_dev hold n_local entries: entry i is slot first + i.  Only slots below n_particles are written, so ranks that pass
+ * the same (all-gathered) input and disjoint slices together write the one global result.  Runs on the handle's stream and synchronises it:
+ * one read-back after the statistics and one per chunk of draws (chunks double from max(n_min, 2^16) up to n_max; at most n_max draws).
+ * The handle keeps a hash set of at least 2 n_max slots (12 B each) and 24 B per draw of the largest chunk.  Refused (B2_ERR_INVALID, no
+ * launch, nothing written): null pointers, n == 0, n_max == 0, n_min == 0, n_min > n_max, first + n_local > n_max, an output range overlapping
+ * an input range or the other output, res_xy or epsilon not finite and > 0, res_z not finite and >= 0, z not finite, K outside [1, 32768].
+ * Suggested values (AMCL's defaults but res_z; AMCL passes its kld_z of 0.99 as the quantile itself): res_xy 0.5 m, res_z 0, res_yaw 10 deg
+ * (K = 36), epsilon 0.01, z 0.99, n_min 100. */
+typedef struct { float res_xy, res_z, res_yaw; uint32_t n_min; double epsilon, z; } b2_kld_config;            /* 32 B */
+typedef char b2_kld_config_is_32_bytes[sizeof(b2_kld_config) == 32 ? 1 : -1];
+typedef struct { uint64_t n_particles, bins; double weight_sum, weight_max; } b2_kld_result;                  /* 32 B */
+typedef char b2_kld_result_is_32_bytes[sizeof(b2_kld_result) == 32 ? 1 : -1];
+B2_API int b2_pf_resample_kld(b2_pf* h, const b2_transform* poses_dev, const b2_particle_attr* attrs_dev, uint32_t n, uint32_t n_max, uint32_t first,
+                              uint32_t n_local, b2_transform* poses_new_dev, b2_particle_attr* attrs_new_dev, const b2_gladiator_config* cfg,
+                              const b2_kld_config* kld, uint64_t seed, uint32_t step, b2_kld_result* out_host);
+
 /* The motion stage's surface constraint, "a MotionUpdater constrained to the mesh surface" (rmcl/docs/RMCL.md:72, listed as missing; no
  * reference implementation, SURVEY appendix F): keeps the particle set on the walkable surface of a mesh map (ramps, stairs, floors) after any
  * stage that moves it (init, motion, resampling).  Up is map +z (REP-103).  Per particle, with t, R its pose, in float arithmetic rounded in

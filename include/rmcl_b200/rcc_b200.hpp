@@ -440,6 +440,25 @@ public:
         res.n_particles = (uint32_t)last_residual.n_particles;
         return res;
     }
+    // KLD-sampling (Fox 2003; the open TODO of docs/RMCL.md:80-83) on the device (b2_pf_resample_kld): all of `poses/attrs` resampled into at
+    // most n_max slots (0: first + poses_new.size(), the node's whole max_particles buffer), as many as the bins of the drawn set call for;
+    // the outputs receive slots first .. first+poses_new.size()-1, and only those below the returned n_particles are written.  The copies
+    // use resampler_config; kld_config holds the suggested bins and bound.  `last_kld` keeps the whole record.
+    b2_kld_config kld_config{0.5f, 0.0f, 0.17453292f, 100u, 0.01, 0.99};       // res_xy, res_z, res_yaw (10 deg), n_min, epsilon, z
+    b2_kld_result last_kld{};
+    ParticleUpdateDynamicResults resampleKLD(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs,
+                                             rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses_new, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs_new,
+                                             uint64_t seed = 1234, uint32_t step = 0, uint32_t first = 0, uint32_t n_max = 0)
+    {
+        if (poses.size() != attrs.size() || poses_new.size() != attrs_new.size()) throw std::invalid_argument("resampleKLD: poses and attrs differ in size");
+        if (n_max == 0) n_max = first + (uint32_t)poses_new.size();
+        b2_check(b2_pf_resample_kld(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<const b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(),
+                                    n_max, first, (uint32_t)poses_new.size(), reinterpret_cast<b2_transform*>(poses_new.raw()),
+                                    reinterpret_cast<b2_particle_attr*>(attrs_new.raw()), &resampler_config, &kld_config, seed, step, &last_kld), "resampleKLD");
+        ParticleUpdateDynamicResults res;
+        res.n_particles = (uint32_t)last_kld.n_particles;
+        return res;
+    }
     // RmclNode::initSamplesUniform (rmcl_localization.cpp:277-342) on the device: particles first .. first+poses.size()-1 of a set drawn
     // uniformly from [bb_min, bb_max] (x, y, z, roll, pitch, yaw).  Draws keyed by (seed, global index): shards concatenate to the whole set.
     void initSamplesUniform(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs,

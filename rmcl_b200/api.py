@@ -5,11 +5,12 @@ Class / method names follow the reference (file:line cited per method); all arit
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 
 import numpy as np
 
-from .synth import CROSS_STATS_DTYPE, PARTICLE_ATTR_DTYPE, PARTICLE_STATS_DTYPE, RANGE_MEAS_DTYPE, RESIDUAL_RESULT_DTYPE, TRANSFORM_DTYPE
+from .synth import CROSS_STATS_DTYPE, KLD_RESULT_DTYPE, PARTICLE_ATTR_DTYPE, PARTICLE_STATS_DTYPE, RANGE_MEAS_DTYPE, RESIDUAL_RESULT_DTYPE, TRANSFORM_DTYPE
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.environ.get("B2_LIB_PATH") or os.path.join(_HERE, "lib", "librmcl_b200.so")     # B2_LIB_PATH: experiment builds (scripts/)
@@ -69,6 +70,17 @@ class SurfaceConfig(C.Structure):
     @staticmethod
     def defaults():
         return SurfaceConfig(0.5, 1.0, 0.0, 0.6, 1)
+
+
+class KLDConfig(C.Structure):
+    """b2_kld_config: the bins and the bound of KLD-sampling (resampleKLD): res_xy and res_z in m (res_z = 0 leaves z unbinned), res_yaw in
+    rad, the least particle count n_min, the bound's error epsilon and its upper normal quantile z.  defaults() are the suggested values:
+    AMCL's defaults, whose kld_z of 0.99 AMCL passes as the quantile itself."""
+    _fields_ = [("res_xy", C.c_float), ("res_z", C.c_float), ("res_yaw", C.c_float), ("n_min", C.c_uint32), ("epsilon", C.c_double), ("z", C.c_double)]
+
+    @staticmethod
+    def defaults():
+        return KLDConfig(0.5, 0.0, math.radians(10.0), 100, 0.01, 0.99)
 
 
 class _CloudLayout(C.Structure):
@@ -135,6 +147,7 @@ EXPORTS = [
     "b2_rcc_correct_once_async", "b2_rcc_correct_once_wait", "b2_micp_correct_once", "b2_rcc_set_exec_mode", "b2_debug_read_bandwidth", "b2_rcc_set_sim_options", "b2_rcc_bind_dataset", "b2_rcc_bind_model_buffers", "b2_rcc_benchmark_batch", "b2_pf_p2p_init", "b2_pf_p2p_connect", "b2_pf_p2p_publish", "b2_pf_resample_gladiator_p2p", "b2_pf_p2p_connect_local", "b2_rcc_set_cpc_options", "b2_pf_set_mapping", "b2_pf_get_mapping",
     "b2_micp_correct", "b2_pf_init_uniform", "b2_pf_init_gaussian", "b2_pf_estimate_stats", "b2_rcc_set_cloud_o1dn",
     "b2_rcc_set_cloud_spherical", "b2_pf_sample_cloud", "b2_pf_resample_residual", "b2_pf_project_to_surface",
+    "b2_pf_resample_kld",
 ]
 
 
@@ -852,6 +865,25 @@ class PCDSensorUpdaterB200:
         _chk(load_library().b2_pf_resample_residual(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(n), C.c_uint32(n_new), C.c_uint32(first),
                                                     C.c_uint32(n_local), _devptr(particle_poses_new), _devptr(particle_attrs_new), C.byref(cfg), C.c_uint64(seed),
                                                     C.c_uint32(step), _p(out)))
+        return out
+
+    def resampleKLD(self, particle_poses, particle_attrs, particle_poses_new, particle_attrs_new, kld=None, config=None, seed=1234, step=0, first=0, n_max=None):
+        """KLD-sampling (Fox 2003; b2_pf_resample_kld) on torch CUDA tensors: all particles of `particle_poses/attrs` are resampled into an
+        output set of at most n_max slots (default: the length of the outputs), as many as the bins the drawn set occupies call for; the
+        outputs receive slots first .. first+len(out)-1, and entries at or beyond the result's n_particles are left untouched.  `kld` is a
+        KLDConfig, `config` a GladiatorConfig (the copies' noise and forget factors).  -> a synth.KLD_RESULT_DTYPE record: n_particles, bins,
+        weight_sum, weight_max."""
+        kcfg = kld or KLDConfig.defaults()
+        cfg = config or GladiatorConfig.defaults()
+        n = particle_poses.numel() * particle_poses.element_size() // 32
+        n_local = particle_poses_new.numel() * particle_poses_new.element_size() // 32
+        if particle_attrs.numel() * particle_attrs.element_size() != 36 * n or particle_attrs_new.numel() * particle_attrs_new.element_size() != 36 * n_local:
+            raise ValueError("resampleKLD: poses and attrs differ in length")
+        n_max = first + n_local if n_max is None else int(n_max)
+        out = np.zeros((), KLD_RESULT_DTYPE)
+        _chk(load_library().b2_pf_resample_kld(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(n), C.c_uint32(n_max), C.c_uint32(first),
+                                               C.c_uint32(n_local), _devptr(particle_poses_new), _devptr(particle_attrs_new), C.byref(cfg), C.byref(kcfg),
+                                               C.c_uint64(seed), C.c_uint32(step), _p(out)))
         return out
 
     def p2pConnect(self, dist, n_per_rank):

@@ -1793,6 +1793,12 @@ struct b2_pf {
     // the largest chunk, the scan's temporary storage, and the state record with its pinned host copy
     DevBuf<double> d_res_part; DevBuf<uint32_t> d_res_parents; DevBuf<unsigned long long> d_res_counts, d_res_prefix; DevBuf<unsigned char> d_res_tmp;
     DevBuf<PfResidualState> d_res; PfResidualState* h_res = nullptr;
+    // KLD-sampling (b2_pf_resample_kld), grown at its calls (its statistics pass uses the residual's buffers above): integer weights and their
+    // prefix, the hash set (keys, first draws), per-draw parents, hash slots, flags and their prefix for the largest chunk, the scan's
+    // temporary storage, the yaw-sector table of kld_K sectors with its host copy, and the state record with its pinned host copy
+    DevBuf<unsigned long long> d_kld_w, d_kld_W, d_kld_keys, d_kld_slots; DevBuf<unsigned int> d_kld_first; DevBuf<uint32_t> d_kld_parents, d_kld_flags, d_kld_cum;
+    DevBuf<unsigned char> d_kld_tmp; DevBuf<float> d_kld_tab; std::vector<float> h_kld_tab; uint32_t kld_K = 0;
+    DevBuf<PfKldState> d_kld; PfKldState* h_kld = nullptr;
 };
 
 extern "C" int b2_pf_destroy(b2_pf* h);
@@ -1856,6 +1862,9 @@ extern "C" int b2_pf_destroy(b2_pf* h)
     if (h->h_samples) cudaFreeHost(h->h_samples);
     h->d_res_part.release(); h->d_res_parents.release(); h->d_res_counts.release(); h->d_res_prefix.release(); h->d_res_tmp.release(); h->d_res.release();
     if (h->h_res) cudaFreeHost(h->h_res);
+    h->d_kld_w.release(); h->d_kld_W.release(); h->d_kld_keys.release(); h->d_kld_slots.release(); h->d_kld_first.release(); h->d_kld_parents.release();
+    h->d_kld_flags.release(); h->d_kld_cum.release(); h->d_kld_tmp.release(); h->d_kld_tab.release(); h->d_kld.release();
+    if (h->h_kld) cudaFreeHost(h->h_kld);
     b2_mesh* map = h->map;
     delete h;
     (void)cudaGetLastError();
@@ -2438,6 +2447,122 @@ extern "C" int b2_pf_resample_residual(b2_pf* h, const b2_transform* poses_dev, 
     }
     CU(cudaStreamSynchronize(h->stream));
     res.n_particles = fill; res.draws = draws;
+    *out_host = res;
+    return B2_OK;
+}
+
+// KLD-sampling (Fox 2003; rmcl/docs/RMCL.md:80-83): the residual's statistics pass, the integer weights and their scan, then the draws in
+// chunks of doubling size, each drawn into the hash set, flagged, scanned and searched for the first draw that meets the stop rule, with one
+// read-back per chunk; the slots a chunk filled are built right after it
+static int kld_stats(b2_pf* h, const b2_particle_attr* attrs_dev, uint32_t n)
+{
+    const uint32_t grid = std::min<uint32_t>((uint32_t)h->n_sm * 4u, (n + 255) / 256);
+    if (!h->d_res.p) {
+        RES(h->d_res_part.reserve((size_t)B2_RES_NV * 4 * (size_t)h->n_sm)); RES(h->d_res.reserve(1));
+        CU(cudaMemset(h->d_res.p, 0, sizeof(PfResidualState)));
+        CU(cudaMallocHost((void**)&h->h_res, sizeof(PfResidualState)));
+    }
+    k_pf_residual_stats<<<grid, 256, 0, h->stream>>>(attrs_dev, n, h->d_res_part.p, h->d_res.p);
+    LAUNCHED();
+    CU(cudaMemcpyAsync(h->h_res, h->d_res.p, sizeof(PfResidualState), cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    return B2_OK;
+}
+extern "C" int b2_pf_resample_kld(b2_pf* h, const b2_transform* poses_dev, const b2_particle_attr* attrs_dev, uint32_t n, uint32_t n_max, uint32_t first,
+                                  uint32_t n_local, b2_transform* poses_new_dev, b2_particle_attr* attrs_new_dev, const b2_gladiator_config* cfg,
+                                  const b2_kld_config* kld, uint64_t seed, uint32_t step, b2_kld_result* out_host)
+{
+    NOTNULL(h); NOTNULL(poses_dev); NOTNULL(attrs_dev); NOTNULL(poses_new_dev); NOTNULL(attrs_new_dev); NOTNULL(cfg); NOTNULL(kld); NOTNULL(out_host);
+    if (n == 0 || n_max == 0) return fail(B2_ERR_INVALID, "resample kld: %u particles into %u slots (both must be > 0)", n, n_max);
+    if (kld->n_min == 0 || kld->n_min > n_max) return fail(B2_ERR_INVALID, "resample kld: n_min = %u must lie in [1, n_max = %u]", kld->n_min, n_max);
+    if ((uint64_t)first + n_local > n_max) return fail(B2_ERR_INVALID, "resample kld: slots %u+%u exceed the %u output slots", first, n_local, n_max);
+    const size_t in_p = sizeof(b2_transform) * (size_t)n, in_a = sizeof(b2_particle_attr) * (size_t)n;
+    const size_t out_p = sizeof(b2_transform) * (size_t)n_local, out_a = sizeof(b2_particle_attr) * (size_t)n_local;
+    if (ranges_overlap(poses_new_dev, out_p, poses_dev, in_p) || ranges_overlap(poses_new_dev, out_p, attrs_dev, in_a) ||
+        ranges_overlap(attrs_new_dev, out_a, poses_dev, in_p) || ranges_overlap(attrs_new_dev, out_a, attrs_dev, in_a) ||
+        ranges_overlap(poses_new_dev, out_p, attrs_new_dev, out_a))
+        return fail(B2_ERR_INVALID, "resample kld: an output range overlaps an input range or the other output (the node double-buffers)");
+    if (!(std::isfinite(kld->res_xy) && kld->res_xy > 0.0f) || !(std::isfinite(kld->epsilon) && kld->epsilon > 0.0))
+        return fail(B2_ERR_INVALID, "resample kld: res_xy = %g and epsilon = %g must be finite and > 0", (double)kld->res_xy, kld->epsilon);
+    if (!(std::isfinite(kld->res_z) && kld->res_z >= 0.0f)) return fail(B2_ERR_INVALID, "resample kld: res_z = %g must be finite and >= 0", (double)kld->res_z);
+    if (!std::isfinite(kld->z)) return fail(B2_ERR_INVALID, "resample kld: z = %g must be finite", kld->z);
+    const double kPi = 3.14159265358979323846;
+    // K = ceil(2 pi / res_yaw) of the ratio shrunk by 2^-20: a float res_yaw is 2 pi / K rounded (10 deg in float is a hair under 10 deg), and
+    // a plain ceil would then give K + 1 sectors; with the shrink every float within 2^-21 of 2 pi / K gives K (SURVEY G3)
+    const double Kd = std::ceil(2.0 * kPi / (double)kld->res_yaw * (1.0 - 0x1p-20));
+    if (!(Kd >= 1.0 && Kd <= (double)B2_KLD_MAX_SECTORS))
+        return fail(B2_ERR_INVALID, "resample kld: res_yaw = %g gives %g yaw sectors (1 .. %u)", (double)kld->res_yaw, Kd, B2_KLD_MAX_SECTORS);
+    const uint32_t K = (uint32_t)Kd;
+    CU(cudaSetDevice(h->map->device));
+    RES(kld_stats(h, attrs_dev, n));
+    const double S = h->h_res->S, L_min = h->h_res->L_min, L_max = h->h_res->L_max;
+    b2_kld_result res = {0, 0, S, L_max};
+    if (!(std::isfinite(S) && S > 0.0 && L_min >= 0.0)) { *out_host = res; return B2_OK; }       // as residual (SURVEY D31)
+    // the chunk schedule: sizes double from max(n_min, 2^16) up to n_max draws in all; 2^30 keeps a chunk within the scan's int item count
+    const uint64_t c0 = std::min<uint64_t>(std::max<uint64_t>(kld->n_min, 1ull << 16), n_max);
+    uint64_t max_len = 0;
+    for (uint64_t c = c0, d = 0; d < n_max; d += std::min<uint64_t>(c, n_max - d), c = std::min<uint64_t>(2 * c, 1ull << 30))
+        max_len = std::max<uint64_t>(max_len, std::min<uint64_t>(c, n_max - d));
+    uint64_t T = 1;                                      // the hash set: a power of two >= 2 n_max slots (load <= 1/2)
+    while (T < 2 * (uint64_t)n_max) T <<= 1;
+    size_t scan_w = 0, scan_f = 0;
+    CU(cub::DeviceScan::InclusiveSum(nullptr, scan_w, h->d_kld_w.p, h->d_kld_W.p, (int)n, h->stream));
+    CU(cub::DeviceScan::InclusiveSum(nullptr, scan_f, h->d_kld_flags.p, h->d_kld_cum.p, (int)max_len, h->stream));
+    RES(h->d_kld_w.reserve(n)); RES(h->d_kld_W.reserve(n)); RES(h->d_kld_keys.reserve(T)); RES(h->d_kld_first.reserve(T));
+    RES(h->d_kld_parents.reserve(max_len)); RES(h->d_kld_slots.reserve(max_len)); RES(h->d_kld_flags.reserve(max_len)); RES(h->d_kld_cum.reserve(max_len));
+    RES(h->d_kld_tmp.reserve(std::max<size_t>(std::max(scan_w, scan_f), 16)));
+    if (!h->d_kld.p) { RES(h->d_kld.reserve(1)); CU(cudaMallocHost((void**)&h->h_kld, sizeof(PfKldState))); }
+    if (h->kld_K != K) {                                 // boundaries theta_k = -pi + 2 pi k / K, as (float)cos, (float)sin of the double angle
+        h->h_kld_tab.resize(2 * (size_t)K);
+        for (uint32_t k = 0; k < K; k++) {
+            const double th = -kPi + 2.0 * kPi * (double)k / (double)K;
+            h->h_kld_tab[2 * k] = (float)std::cos(th); h->h_kld_tab[2 * k + 1] = (float)std::sin(th);
+        }
+        RES(h->d_kld_tab.reserve(2 * (size_t)K));
+        CU(cudaMemcpyAsync(h->d_kld_tab.p, h->h_kld_tab.data(), sizeof(float) * 2 * K, cudaMemcpyHostToDevice, h->stream));
+        h->kld_K = K;
+    }
+    // the hash set is cleared by memset on the stream: at 12 B per slot it costs less than one chunk's draws, and unlike epoch tags it keeps
+    // every stored key a plain 64-bit word that one atomicCAS claims
+    CU(cudaMemsetAsync(h->d_kld_keys.p, 0, sizeof(unsigned long long) * T, h->stream));
+    CU(cudaMemsetAsync(h->d_kld_first.p, 0xff, sizeof(unsigned int) * T, h->stream));
+    k_pf_kld_weights<<<(n + 255) / 256, 256, 0, h->stream>>>(attrs_dev, n, L_max, h->d_kld_w.p);
+    LAUNCHED();
+    size_t bytes = h->d_kld_tmp.cap;
+    CU(cub::DeviceScan::InclusiveSum(h->d_kld_tmp.p, bytes, h->d_kld_w.p, h->d_kld_W.p, (int)n, h->stream));
+    LAUNCHED();
+    const KldBins bins{kld->res_xy, kld->res_z, K, h->d_kld_tab.p};
+    uint64_t d0 = 0, n_bins = 0, chunk = c0;
+    bool done = false;
+    while (!done && d0 < n_max) {
+        const uint32_t len = (uint32_t)std::min<uint64_t>(chunk, n_max - d0), grid = (len + 255) / 256;
+        k_pf_kld_draw<<<grid, 256, 0, h->stream>>>(h->d_kld_W.p, n, poses_dev, bins, seed, step, d0, len, h->d_kld_keys.p, h->d_kld_first.p, T - 1,
+                                                   h->d_kld_parents.p, h->d_kld_slots.p, h->d_kld.p);
+        LAUNCHED();
+        k_pf_kld_flags<<<grid, 256, 0, h->stream>>>(h->d_kld_first.p, h->d_kld_slots.p, d0, len, h->d_kld_flags.p);
+        LAUNCHED();
+        bytes = h->d_kld_tmp.cap;
+        CU(cub::DeviceScan::InclusiveSum(h->d_kld_tmp.p, bytes, h->d_kld_flags.p, h->d_kld_cum.p, (int)len, h->stream));
+        LAUNCHED();
+        k_pf_kld_stop<<<grid, 256, 0, h->stream>>>(h->d_kld_cum.p, d0, len, n_bins, kld->n_min, n_max, kld->epsilon, kld->z, h->d_kld.p);
+        LAUNCHED();
+        CU(cudaMemcpyAsync(h->h_kld, h->d_kld.p, sizeof(PfKldState), cudaMemcpyDeviceToHost, h->stream));
+        CU(cudaStreamSynchronize(h->stream));
+        const unsigned long long stop = h->h_kld->stop;
+        done = stop != ~0ull;
+        const uint64_t used = done ? (stop >> 32) + 1 : len, chunk_bins = done ? (stop & 0xffffffffull) : h->h_kld->bins;
+        const uint64_t lo = std::max<uint64_t>(d0, first), hi = std::min<uint64_t>(d0 + used, (uint64_t)first + n_local);
+        if (lo < hi) {
+            const uint32_t n_k = (uint32_t)(hi - lo);
+            k_pf_kld_expand<<<(n_k + 255) / 256, 256, 0, h->stream>>>(poses_dev, attrs_dev, h->d_kld_parents.p, d0, (uint32_t)lo, n_k, first, L_max, *cfg, seed, step,
+                                                                      poses_new_dev, attrs_new_dev);
+            LAUNCHED();
+        }
+        d0 += used; n_bins += chunk_bins;
+        chunk = std::min<uint64_t>(2 * chunk, 1ull << 30);
+    }
+    CU(cudaStreamSynchronize(h->stream));
+    res.n_particles = d0; res.bins = n_bins;
     *out_host = res;
     return B2_OK;
 }

@@ -1978,4 +1978,176 @@ __global__ void __launch_bounds__(256) k_pf_residual_expand(const b2_transform* 
 }
 #endif
 
+// ---------------------------------------------------------------------------------------------------------------------
+// KLD-sampling (Fox, "Adapting the sample size in particle filters through KLD-sampling", IJRR 2003; the open TODO of rmcl/docs/RMCL.md:80-83,
+// no reference implementation): draws parents one at a time and stops once the number drawn reaches the chi-square bound on the number of
+// histogram bins they occupy (b2_pf_resample_kld).  Weights are integers w_i = (uint64)(L_i / L_max * 2^32) with the 64-bit inclusive prefix
+// W; draw j takes u = words 2(j % 2) (low) and 2(j % 2) + 1 (high) of Philox4x32-10 with counter (lo(j / 2), 6, step, hi(j / 2)) and key =
+// seed, and its parent is the smallest i with W[i] > mulhi64(u, W[n-1]).  A bin is the parent's (x, y, z, yaw sector) cell, computed without
+// transcendental functions, so host and device agree bit for bit.  Slot j is draw j's parent copied as residual_copy copies (normals of
+// residual_normals keyed by the slot).  The draws run in chunks: k_pf_kld_draw inserts the keys into a hash set that keeps each key's first
+// draw, k_pf_kld_flags marks the first draws, a scan counts the bins, k_pf_kld_stop finds the first draw that meets the stop rule, one
+// read-back, then k_pf_kld_expand over the slots the chunk filled.  SURVEY appendix G.
+// ---------------------------------------------------------------------------------------------------------------------
+#define B2_PF_KLD_DRAW_TAG 6u
+#define B2_KLD_NONFINITE_KEY 0xFFFFFFFFFFFFFFFFull     // bit 15 is never set in a real key
+#define B2_KLD_XY_HALF 524288.0f                        // 2^19: ix, iy in [-2^19, 2^19)
+#define B2_KLD_Z_HALF 128.0f                            // 2^7:  iz in [-2^7, 2^7)
+#define B2_KLD_MAX_SECTORS 32768u
+#if B2_ON_DEVICE
+B2_DEV uint64_t kld_mulhi64(uint64_t a, uint64_t b) { return __umul64hi(a, b); }
+B2_DEV double kld_sub_d(double a, double b) { return __dadd_rn(a, -b); }
+B2_DEV double kld_div_d(double a, double b) { return __ddiv_rn(a, b); }
+#else
+B2_DEV uint64_t kld_mulhi64(uint64_t a, uint64_t b) { return (uint64_t)(((unsigned __int128)a * b) >> 64); }
+B2_DEV double kld_sub_d(double a, double b) { return a - b; }
+B2_DEV double kld_div_d(double a, double b) { return a / b; }
+#endif
+// the integer weight of likelihood L: at most 2^32, exact sums in 64 bits for any n < 2^32
+B2_DEV uint64_t kld_weight(float L, double L_max) { return (uint64_t)mul_d(kld_div_d((double)L, L_max), 4294967296.0); }
+// the parent of draw j among the n particles of the inclusive weight prefix W (W[n-1] > 0): bias at most W[n-1] / 2^64 per particle
+B2_DEV uint32_t kld_parent(uint64_t seed, uint32_t step, uint64_t j, const unsigned long long* W, uint32_t n)
+{
+    uint32_t r[4];
+    const uint64_t b = j >> 1;
+    philox4x32_10((uint32_t)b, B2_PF_KLD_DRAW_TAG, step, (uint32_t)(b >> 32), (uint32_t)seed, (uint32_t)(seed >> 32), r);
+    const uint64_t u = (j & 1u) ? ((uint64_t)r[3] << 32 | r[2]) : ((uint64_t)r[1] << 32 | r[0]);
+    const uint64_t x = kld_mulhi64(u, W[n - 1]);
+    uint32_t lo = 0, hi = n - 1;                         // W[n-1] > x: the answer lies in [0, n-1]
+    while (lo < hi) { const uint32_t mid = lo + (hi - lo) / 2; if ((uint64_t)W[mid] > x) hi = mid; else lo = mid + 1; }
+    return lo;
+}
+// the bin resolution: res_z = 0 leaves z unbinned; cs = the K boundary vectors (cos, sin) of theta_k = -pi + 2 pi k / K as floats
+struct KldBins { float res_xy, res_z; uint32_t K; const float* cs; };
+// boundary k lies in the lower half (theta_k < 0) iff 2k < K; within one half, theta_k <= phi(h) iff c_k h.y - s_k h.x >= 0 (each product of
+// two floats is exact in double, so the sign is exact)
+B2_DEV bool kld_at_or_before(const float* cs, uint32_t k, float hx, float hy)
+{
+    return kld_sub_d(mul_d((double)cs[2 * k], (double)hy), mul_d((double)cs[2 * k + 1], (double)hx)) >= 0.0;
+}
+// the number of boundaries k in [1, K) with theta_k <= phi(h), phi in [-pi, pi); the predicate is monotone in k within a half
+B2_DEV uint32_t kld_sector(float hx, float hy, const float* cs, uint32_t K)
+{
+    if (hx == 0.0f && hy == 0.0f) return 0u;
+    const bool lower = hy < 0.0f || (hy == 0.0f && hx < 0.0f);
+    const uint32_t n_low = (K - 1u) / 2u;               // boundaries 1 .. n_low are in the lower half
+    uint32_t lo = lower ? 1u : n_low + 1u, hi = lower ? n_low + 1u : K;     // count the true prefix of [lo, hi)
+    const uint32_t base = lo;
+    while (lo < hi) { const uint32_t mid = lo + (hi - lo) / 2; if (kld_at_or_before(cs, mid, hx, hy)) lo = mid + 1; else hi = mid; }
+    return (lower ? 0u : n_low) + (lo - base);
+}
+B2_DEV float kld_cell(float v, float res, float half)
+{
+    float c = floorf(dvd(v, res));
+    c = c < -half ? -half : c;
+    c = c > half - 1.0f ? half - 1.0f : c;
+    return c;
+}
+// the bin key of pose p: (ix + 2^19) << 44 | (iy + 2^19) << 24 | (iz + 2^7) << 16 | yaw sector; roll and pitch are not binned
+B2_DEV uint64_t kld_key(const b2_transform& p, const KldBins& b)
+{
+    if (!(finite_f32(p.t.x) && finite_f32(p.t.y) && finite_f32(p.t.z) && finite_f32(p.R.x) && finite_f32(p.R.y) && finite_f32(p.R.z) && finite_f32(p.R.w)))
+        return B2_KLD_NONFINITE_KEY;
+    const float ix = kld_cell(p.t.x, b.res_xy, B2_KLD_XY_HALF), iy = kld_cell(p.t.y, b.res_xy, B2_KLD_XY_HALF);
+    const float iz = b.res_z > 0.0f ? kld_cell(p.t.z, b.res_z, B2_KLD_Z_HALF) : 0.0f;
+    const float x = p.R.x, y = p.R.y, z = p.R.z, w = p.R.w;
+    const float hx = sub(1.0f, mul(2.0f, add(mul(y, y), mul(z, z))));     // R e_x: 1 - 2(y^2 + z^2), 2(xy + wz)
+    const float hy = mul(2.0f, add(mul(x, y), mul(w, z)));
+    const uint64_t sector = kld_sector(hx, hy, b.cs, b.K);
+    return (uint64_t)((int64_t)ix + 524288) << 44 | (uint64_t)((int64_t)iy + 524288) << 24 | (uint64_t)((int64_t)iz + 128) << 16 | sector;
+}
+// Fox's bound on the sample count for k occupied bins: ceil((k-1) / (2 eps) * x^3), x = 1 - 2 / (9(k-1)) + sqrt(2 / (9(k-1))) z, in double
+// rounded in the order written (pf_resample_limit's arithmetic); k <= 1 (a converged set) gives n_min
+B2_DEV uint64_t kld_bound(uint64_t k, double epsilon, double z, uint32_t n_min)
+{
+    if (k <= 1u) return n_min;
+    const double km1 = (double)(k - 1u);
+    const double a = kld_div_d(2.0, mul_d(9.0, km1));
+    const double x = add_d(kld_sub_d(1.0, a), mul_d(sqrt_d(a), z));
+    const double v = mul_d(kld_div_d(km1, mul_d(2.0, epsilon)), mul_d(mul_d(x, x), x));
+    if (!(v > 0.0)) return 0u;
+    const double c = ceil(v);
+    return c >= 18446744073709551616.0 ? ~0ull : (uint64_t)c;
+}
+// the stop rule after draw j with k bins among draws 0 .. j
+B2_DEV bool kld_stop(uint64_t j, uint64_t k, double epsilon, double z, uint32_t n_min, uint64_t n_max)
+{
+    const uint64_t b = kld_bound(k, epsilon, z, n_min);
+    return j + 1u >= (b > n_min ? b : (uint64_t)n_min) || j + 1u == n_max;
+}
+// the device record the host reads back after every chunk
+struct PfKldState {
+    unsigned long long stop;     // min over the chunk's draws i that meet the stop rule of i << 32 | bins among the chunk's draws 0 .. i
+    unsigned int bins, pad;      // bins among the chunk's draws
+};
+#ifdef __CUDACC__
+B2_DEV uint64_t kld_hash(uint64_t v)                    // splitmix64's finaliser
+{
+    v ^= v >> 30; v *= 0xbf58476d1ce4e5b9ull; v ^= v >> 27; v *= 0x94d049bb133111ebull; v ^= v >> 31;
+    return v;
+}
+__global__ void __launch_bounds__(256) k_pf_kld_weights(const b2_particle_attr* __restrict__ attrs, uint32_t n, double L_max, unsigned long long* __restrict__ w)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) w[i] = kld_weight(attrs[i].likelihood.mean, L_max);
+}
+// one thread per draw d0 + i: its parent, and its key into the hash set (stored as key ^ 0x8000, so the memset 0 marks empty slots and no
+// key stores 0); each slot keeps the smallest draw index of its key, so membership and first draws do not depend on the insertion order
+__global__ void __launch_bounds__(256) k_pf_kld_draw(const unsigned long long* __restrict__ W, uint32_t n, const b2_transform* __restrict__ poses, KldBins bins,
+                                                     uint64_t seed, uint32_t step, uint64_t d0, uint32_t len, unsigned long long* __restrict__ keys,
+                                                     unsigned int* __restrict__ first, uint64_t mask, uint32_t* __restrict__ parents, unsigned long long* __restrict__ slots,
+                                                     PfKldState* __restrict__ st)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i == 0) { st->stop = ~0ull; st->bins = 0u; }
+    if (i >= len) return;
+    const uint64_t j = d0 + i;
+    const uint32_t p = kld_parent(seed, step, j, W, n);
+    parents[i] = p;
+    const unsigned long long v = kld_key(poses[p], bins) ^ 0x8000ull;
+    uint64_t s = kld_hash(v) & mask;
+    for (;;) {
+        const unsigned long long old = atomicCAS(keys + s, 0ull, v);
+        if (old == 0ull || old == v) break;
+        s = (s + 1u) & mask;
+    }
+    atomicMin(first + s, (unsigned int)j);
+    slots[i] = s;
+}
+// a draw opens a bin iff it is the first draw of its key
+__global__ void __launch_bounds__(256) k_pf_kld_flags(const unsigned int* __restrict__ first, const unsigned long long* __restrict__ slots, uint64_t d0, uint32_t len,
+                                                      uint32_t* __restrict__ flags)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < len) flags[i] = first[slots[i]] == (unsigned int)(d0 + i) ? 1u : 0u;
+}
+// the first draw of the chunk that meets the stop rule: every draw is tested (the rule is not monotone in j), the lowest lane of each warp
+// that meets it takes part in one atomicMin
+__global__ void __launch_bounds__(256) k_pf_kld_stop(const uint32_t* __restrict__ cum, uint64_t d0, uint32_t len, uint64_t bins0, uint32_t n_min, uint64_t n_max,
+                                                     double epsilon, double z, PfKldState* __restrict__ st)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    const bool in = i < len;
+    const uint32_t c = in ? cum[i] : 0u;
+    const bool hit = in && kld_stop(d0 + i, bins0 + c, epsilon, z, n_min, n_max);
+    const unsigned m = __ballot_sync(0xffffffffu, hit);
+    if (hit && (threadIdx.x & 31u) == (unsigned)(__ffs(m) - 1)) atomicMin(&st->stop, (unsigned long long)i << 32 | c);
+    if (i + 1u == len) st->bins = c;
+}
+// one thread per output slot k = k0 + i that this chunk filled: slot k is draw k's parent, copied with the normals of slot k; writes entry
+// k - first of the caller's slice.  68 B gathered from the parent and 68 B written per slot.
+__global__ void __launch_bounds__(256) k_pf_kld_expand(const b2_transform* __restrict__ poses, const b2_particle_attr* __restrict__ attrs, const uint32_t* __restrict__ parents,
+                                                       uint64_t d0, uint32_t k0, uint32_t n_k, uint32_t first, double L_max, b2_gladiator_config cfg, uint64_t seed,
+                                                       uint32_t step, b2_transform* __restrict__ poses_new, b2_particle_attr* __restrict__ attrs_new)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_k) return;
+    const uint32_t k = k0 + i;
+    const uint32_t p = parents[k - d0];
+    float N[6];
+    residual_normals(seed, step, k, N);
+    residual_copy(poses[p], attrs[p], L_max, N, cfg, poses_new + (k - first), attrs_new + (k - first));
+}
+#endif
+
 #include "icp_loop.cuh"

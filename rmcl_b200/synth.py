@@ -368,6 +368,9 @@ assert PARTICLE_STATS_DTYPE.itemsize == 440
 # b2_residual_result: what PCDSensorUpdaterB200.resampleResidual returns
 RESIDUAL_RESULT_DTYPE = np.dtype([("n_particles", np.uint64), ("draws", np.uint64), ("weight_sum", np.float64), ("weight_max", np.float64)])
 assert RESIDUAL_RESULT_DTYPE.itemsize == 32
+# b2_kld_result: what PCDSensorUpdaterB200.resampleKLD returns
+KLD_RESULT_DTYPE = np.dtype([("n_particles", np.uint64), ("bins", np.uint64), ("weight_sum", np.float64), ("weight_max", np.float64)])
+assert KLD_RESULT_DTYPE.itemsize == 32
 
 
 def quat_from_rpy(roll, pitch, yaw):
