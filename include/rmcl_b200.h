@@ -459,6 +459,43 @@ B2_API int b2_pf_resample_kld(b2_pf* h, const b2_transform* poses_dev, const b2_
                               uint32_t n_local, b2_transform* poses_new_dev, b2_particle_attr* attrs_new_dev, const b2_gladiator_config* cfg,
                               const b2_kld_config* kld, uint64_t seed, uint32_t step, b2_kld_result* out_host);
 
+/* The filter's pose hypotheses: the clusters of the particle set, heaviest first, each with the estimate b2_pf_estimate_stats would give of
+ * it alone.  What AMCL publishes is the mean of its heaviest cluster (pf_cluster_stats); the reference reports one mean over the whole set,
+ * which during global localisation lies between the modes (no reference implementation; SURVEY appendix H).  poses_dev / attrs_dev are DEVICE
+ * pointers to n particles, records_host a HOST array of cfg->max_records records, labels_dev a DEVICE array of n labels or null.
+ *  - S = weight_sum, L_min and weight_max = L_max of likelihood.mean as b2_pf_resample_kld takes them.  S not finite, S <= 0 or L_min < 0:
+ *    0 clusters, nothing written but out_host, B2_OK.
+ *  - Particle i is a member iff w_i = (uint64)((double)L_i / L_max * 2^32) > 0 and its pose is finite.  n_clustered counts the members,
+ *    weight_total = sum w_i over them (exact in 64 bits).  A particle the wall check or the surface projection marked (L = 0) is in no
+ *    cluster and joins none.
+ *  - A member's bin is b2_pf_resample_kld's: the x, y, z cell (res_z = 0: z not binned) and the yaw sector among K = ceil(2 pi / res_yaw
+ *    (1 - 2^-20)) sectors.  bins counts the occupied bins.
+ *  - Two occupied bins touch iff their x, y and z cells each differ by at most 1 and their sectors by at most 1 modulo K: yaw wraps, while a
+ *    cell clamped at +-2^19 (z: +-2^7) has no neighbour beyond the clamp.  With K <= 2 some of the 80 neighbours (26 when z is not binned)
+ *    coincide; joining a pair twice changes nothing.  A cluster is a connected component of that graph.  Its key is its smallest bin key
+ *    ((ix + 2^19) << 44 | (iy + 2^19) << 24 | (iz + 2^7) << 16 | sector), its weight_int the sum of its members' w_i, weight = weight_int /
+ *    weight_total, bins its occupied bins.
+ *  - Clusters are ranked by weight_int descending, ties by the smaller key; rank 0 is the best hypothesis.  records_host[r], r < n_records =
+ *    min(n_clusters, max_records), describes rank r: `stats` is byte for byte what b2_pf_estimate_stats returns for the cluster's members
+ *    alone, in ascending particle index.  labels_dev[i] is the rank of particle i's cluster (any rank, recorded or not), 0xFFFFFFFF for a
+ *    particle in none.
+ *  - rounds: the labelling rounds run.  A round joins every touching pair with lock-free union-find hooks and ends in the fixed point, so
+ *    this is 1; the call gives up with an error after 64.
+ * Every sum that decides a result is an integer, so nothing depends on the order in which threads run.  Runs on the handle's stream and
+ * synchronises it: one read-back after the statistics, one per round, one for the ranking, one for the records.  The handle shares
+ * b2_pf_resample_kld's hash set (at least 2 n slots of 12 B) and adds 16 B per slot (weight, members, bins / rank), 20 B per particle (slot,
+ * sort keys and indices) and 68 B per member of a recorded cluster.  Refused (B2_ERR_INVALID, no launch, nothing written): null h, poses_dev,
+ * attrs_dev, cfg, records_host or out_host, n == 0 or n > 2^30, res_xy not finite and > 0, res_z not finite and >= 0, K outside [1, 32768],
+ * max_records outside [1, 16].  Suggested values (AMCL's bin sizes): res_xy 0.5 m, res_z 0, res_yaw 10 deg, max_records 8. */
+typedef struct { float res_xy, res_z, res_yaw; uint32_t max_records; } b2_cluster_config;                     /* 16 B */
+typedef char b2_cluster_config_is_16_bytes[sizeof(b2_cluster_config) == 16 ? 1 : -1];
+typedef struct { b2_particle_stats stats; double weight; uint64_t weight_int, bins, key; } b2_cluster_record; /* 472 B */
+typedef char b2_cluster_record_is_472_bytes[sizeof(b2_cluster_record) == 472 ? 1 : -1];
+typedef struct { uint64_t n_clusters, n_records, bins, n_clustered, weight_total, rounds; double weight_sum, weight_max; } b2_cluster_result;   /* 64 B */
+typedef char b2_cluster_result_is_64_bytes[sizeof(b2_cluster_result) == 64 ? 1 : -1];
+B2_API int b2_pf_cluster_stats(b2_pf* h, const b2_transform* poses_dev, const b2_particle_attr* attrs_dev, uint32_t n, const b2_cluster_config* cfg,
+                               b2_cluster_record* records_host, uint32_t* labels_dev /* nullable */, b2_cluster_result* out_host);
+
 /* The motion stage's surface constraint, "a MotionUpdater constrained to the mesh surface" (rmcl/docs/RMCL.md:72, listed as missing; no
  * reference implementation, SURVEY appendix F): keeps the particle set on the walkable surface of a mesh map (ramps, stairs, floors) after any
  * stage that moves it (init, motion, resampling).  Up is map +z (REP-103).  Per particle, with t, R its pose, in float arithmetic rounded in

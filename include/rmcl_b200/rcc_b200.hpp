@@ -488,6 +488,21 @@ public:
                  "estimateStats");
         return s;
     }
+    // The filter's pose hypotheses (b2_pf_cluster_stats; AMCL's cluster statistics): the clusters of the set, heaviest first, at most
+    // cluster_config.max_records of them, each with the estimateStats of its members alone in `stats` and its share of the set in `weight`.
+    // `labels`, if given, receives every particle's rank (0xFFFFFFFF: in no cluster).  `last_clusters` keeps the counts of the whole set.
+    b2_cluster_config cluster_config{0.5f, 0.0f, 0.17453292f, 8u};             // res_xy, res_z, res_yaw (10 deg), max_records
+    b2_cluster_result last_clusters{};
+    std::vector<b2_cluster_record> estimateClusters(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs,
+                                                    uint32_t* labels = nullptr)
+    {
+        if (poses.size() != attrs.size()) throw std::invalid_argument("estimateClusters: poses and attrs differ in size");
+        std::vector<b2_cluster_record> recs(16);                                // max_records is at most 16
+        b2_check(b2_pf_cluster_stats(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<const b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(),
+                                     &cluster_config, recs.data(), labels, &last_clusters), "estimateClusters");
+        recs.resize(last_clusters.n_records);
+        return recs;
+    }
 private:
     struct CloudInput { bool set = false; const void* data = nullptr; uint64_t bytes = 0; b2_cloud_layout layout{}; bool on_device = false; std::shared_ptr<const void> keep_alive; };
     // with an input cloud: this update's beams, `samples` drawn with (seed, step), then step advances

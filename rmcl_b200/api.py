@@ -10,7 +10,7 @@ import os
 
 import numpy as np
 
-from .synth import CROSS_STATS_DTYPE, KLD_RESULT_DTYPE, PARTICLE_ATTR_DTYPE, PARTICLE_STATS_DTYPE, RANGE_MEAS_DTYPE, RESIDUAL_RESULT_DTYPE, TRANSFORM_DTYPE
+from .synth import CLUSTER_RECORD_DTYPE, CLUSTER_RESULT_DTYPE, CROSS_STATS_DTYPE, KLD_RESULT_DTYPE, PARTICLE_ATTR_DTYPE, PARTICLE_STATS_DTYPE, RANGE_MEAS_DTYPE, RESIDUAL_RESULT_DTYPE, TRANSFORM_DTYPE
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.environ.get("B2_LIB_PATH") or os.path.join(_HERE, "lib", "librmcl_b200.so")     # B2_LIB_PATH: experiment builds (scripts/)
@@ -83,6 +83,16 @@ class KLDConfig(C.Structure):
         return KLDConfig(0.5, 0.0, math.radians(10.0), 100, 0.01, 0.99)
 
 
+class ClusterConfig(C.Structure):
+    """b2_cluster_config: the bins of estimateClusters (res_xy and res_z in m, res_z = 0 leaves z unbinned, res_yaw in rad: KLDConfig's) and
+    the number of clusters to record, heaviest first (1 .. 16).  defaults() are AMCL's bin sizes and 8 records."""
+    _fields_ = [("res_xy", C.c_float), ("res_z", C.c_float), ("res_yaw", C.c_float), ("max_records", C.c_uint32)]
+
+    @staticmethod
+    def defaults():
+        return ClusterConfig(0.5, 0.0, math.radians(10.0), 8)
+
+
 class _CloudLayout(C.Structure):
     _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("point_step", C.c_uint32), ("row_step", C.c_uint32), ("offset_x", C.c_uint32),
                 ("offset_y", C.c_uint32), ("offset_z", C.c_uint32), ("datatype", C.c_uint8), ("is_bigendian", C.c_uint8), ("pad", C.c_uint8 * 2)]
@@ -147,7 +157,7 @@ EXPORTS = [
     "b2_rcc_correct_once_async", "b2_rcc_correct_once_wait", "b2_micp_correct_once", "b2_rcc_set_exec_mode", "b2_debug_read_bandwidth", "b2_rcc_set_sim_options", "b2_rcc_bind_dataset", "b2_rcc_bind_model_buffers", "b2_rcc_benchmark_batch", "b2_pf_p2p_init", "b2_pf_p2p_connect", "b2_pf_p2p_publish", "b2_pf_resample_gladiator_p2p", "b2_pf_p2p_connect_local", "b2_rcc_set_cpc_options", "b2_pf_set_mapping", "b2_pf_get_mapping",
     "b2_micp_correct", "b2_pf_init_uniform", "b2_pf_init_gaussian", "b2_pf_estimate_stats", "b2_rcc_set_cloud_o1dn",
     "b2_rcc_set_cloud_spherical", "b2_pf_sample_cloud", "b2_pf_resample_residual", "b2_pf_project_to_surface",
-    "b2_pf_resample_kld",
+    "b2_pf_resample_kld", "b2_pf_cluster_stats",
 ]
 
 
@@ -829,6 +839,25 @@ class PCDSensorUpdaterB200:
         out = np.zeros((), PARTICLE_STATS_DTYPE)
         _chk(load_library().b2_pf_estimate_stats(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(k), _p(out)))
         return out
+
+    def estimateClusters(self, particle_poses, particle_attrs, config=None, labels=None):
+        """The filter's pose hypotheses (b2_pf_cluster_stats; AMCL's cluster statistics) of the (n, 8) / (n, 9) float32 CUDA tensors: the
+        particles of likelihood > 0 are binned as resampleKLD bins them, touching bins are joined, and the clusters are ranked by weight.
+        `config` is a ClusterConfig; `labels`, if given, is an n-element int32 / uint32 CUDA tensor that receives every particle's rank
+        (0xFFFFFFFF: in no cluster).  -> (result, records): a synth.CLUSTER_RESULT_DTYPE record (n_clusters, n_records, bins, n_clustered,
+        weight_total, rounds, weight_sum, weight_max) and the n_records heaviest clusters as synth.CLUSTER_RECORD_DTYPE, records[0] the
+        best hypothesis: its share `weight` of the set, and in `stats` what estimateStats gives of its members alone."""
+        cfg = config or ClusterConfig.defaults()
+        n = particle_poses.numel() * particle_poses.element_size() // 32
+        if particle_attrs.numel() * particle_attrs.element_size() != 36 * n:
+            raise ValueError(f"estimateClusters: {n} poses but {particle_attrs.numel() * particle_attrs.element_size() / 36:g} attrs")
+        if labels is not None and labels.numel() * labels.element_size() != 4 * n:
+            raise ValueError(f"estimateClusters: {n} particles but {labels.numel() * labels.element_size() / 4:g} labels")
+        out = np.zeros((), CLUSTER_RESULT_DTYPE)
+        recs = np.zeros(max(1, min(int(cfg.max_records), 16)), CLUSTER_RECORD_DTYPE)
+        _chk(load_library().b2_pf_cluster_stats(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(n), C.byref(cfg), _p(recs),
+                                                None if labels is None else _devptr(labels), _p(out)))
+        return out, recs[:int(out["n_records"])]
 
     def gladiatorRandoms(self, seed, step, first, n, device=None):
         """The draws resample() uses for champions first..first+n-1 (raw u32 opponent word + 6 normals each), as torch CUDA tensors."""

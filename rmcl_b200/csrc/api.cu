@@ -1799,6 +1799,14 @@ struct b2_pf {
     DevBuf<unsigned long long> d_kld_w, d_kld_W, d_kld_keys, d_kld_slots; DevBuf<unsigned int> d_kld_first; DevBuf<uint32_t> d_kld_parents, d_kld_flags, d_kld_cum;
     DevBuf<unsigned char> d_kld_tmp; DevBuf<float> d_kld_tab; std::vector<float> h_kld_tab; uint32_t kld_K = 0;
     DevBuf<PfKldState> d_kld; PfKldState* h_kld = nullptr;
+    // pose hypotheses (b2_pf_cluster_stats), grown at its calls.  It shares KLD's hash set (d_kld_keys; d_kld_first holds each slot's link
+    // to its root), sector table, temporary storage and, for the cluster sort's keys, d_kld_w / d_kld_W.  Its own: per slot the weight, the
+    // member count and the bin count / rank; per particle the slot, the sort key and the index, each of the latter two before and after the
+    // sort (the index buffers also list the roots); the gathered members; the heads and records of the recorded clusters; the state record;
+    // and one pinned host block for the state, the heads and the records
+    DevBuf<unsigned long long> d_cl_w; DevBuf<unsigned int> d_cl_cnt, d_cl_aux; DevBuf<uint32_t> d_cl_slot, d_cl_key, d_cl_key2, d_cl_idx, d_cl_idx2;
+    DevBuf<b2_transform> d_cl_poses; DevBuf<b2_particle_attr> d_cl_attrs; DevBuf<PfClusterHead> d_cl_heads; DevBuf<b2_particle_stats> d_cl_recs;
+    DevBuf<PfClusterState> d_cl; unsigned char* h_cl = nullptr;
 };
 
 extern "C" int b2_pf_destroy(b2_pf* h);
@@ -1865,6 +1873,9 @@ extern "C" int b2_pf_destroy(b2_pf* h)
     h->d_kld_w.release(); h->d_kld_W.release(); h->d_kld_keys.release(); h->d_kld_slots.release(); h->d_kld_first.release(); h->d_kld_parents.release();
     h->d_kld_flags.release(); h->d_kld_cum.release(); h->d_kld_tmp.release(); h->d_kld_tab.release(); h->d_kld.release();
     if (h->h_kld) cudaFreeHost(h->h_kld);
+    h->d_cl_w.release(); h->d_cl_cnt.release(); h->d_cl_aux.release(); h->d_cl_slot.release(); h->d_cl_key.release(); h->d_cl_key2.release(); h->d_cl_idx.release();
+    h->d_cl_idx2.release(); h->d_cl_poses.release(); h->d_cl_attrs.release(); h->d_cl_heads.release(); h->d_cl_recs.release(); h->d_cl.release();
+    if (h->h_cl) cudaFreeHost(h->h_cl);
     b2_mesh* map = h->map;
     delete h;
     (void)cudaGetLastError();
@@ -2359,11 +2370,9 @@ extern "C" int b2_pf_likelihood_stats(b2_pf* h, const b2_particle_attr* attrs_de
 }
 
 // RmclNode::estimateStats (rmcl_localization.cpp:642-731): two read passes, Tbm handed from the first to the second in device memory
-extern "C" int b2_pf_estimate_stats(b2_pf* h, const b2_transform* poses_dev, const b2_particle_attr* attrs_dev, uint32_t n, b2_particle_stats* out_host)
+// both passes over n > 0 particles; the record is left in h->d_est.p->rec
+static int estimate_launch(b2_pf* h, const b2_transform* poses_dev, const b2_particle_attr* attrs_dev, uint32_t n)
 {
-    NOTNULL(h); NOTNULL(poses_dev); NOTNULL(attrs_dev); NOTNULL(out_host);
-    if (n == 0) return fail(B2_ERR_INVALID, "estimate stats: no particles (n = 0)");
-    CU(cudaSetDevice(h->map->device));
     const uint32_t grid = std::min<uint32_t>((uint32_t)h->n_sm * 4u, (n + 255) / 256);
     if (!h->d_est.p) {
         RES(h->d_est_part.reserve((size_t)B2_EST_NV_MAX * 4 * (size_t)h->n_sm)); RES(h->d_est.reserve(1));
@@ -2374,6 +2383,14 @@ extern "C" int b2_pf_estimate_stats(b2_pf* h, const b2_transform* poses_dev, con
     LAUNCHED();
     k_pf_estimate_cov<<<grid, 256, 0, h->stream>>>(poses_dev, attrs_dev, n, h->d_est_part.p, h->d_est.p);
     LAUNCHED();
+    return B2_OK;
+}
+extern "C" int b2_pf_estimate_stats(b2_pf* h, const b2_transform* poses_dev, const b2_particle_attr* attrs_dev, uint32_t n, b2_particle_stats* out_host)
+{
+    NOTNULL(h); NOTNULL(poses_dev); NOTNULL(attrs_dev); NOTNULL(out_host);
+    if (n == 0) return fail(B2_ERR_INVALID, "estimate stats: no particles (n = 0)");
+    CU(cudaSetDevice(h->map->device));
+    RES(estimate_launch(h, poses_dev, attrs_dev, n));
     CU(cudaMemcpyAsync(h->h_est, &h->d_est.p->rec, sizeof(b2_particle_stats), cudaMemcpyDeviceToHost, h->stream));
     CU(cudaStreamSynchronize(h->stream));
     *out_host = *h->h_est;
@@ -2468,6 +2485,24 @@ static int kld_stats(b2_pf* h, const b2_particle_attr* attrs_dev, uint32_t n)
     CU(cudaStreamSynchronize(h->stream));
     return B2_OK;
 }
+// K = ceil(2 pi / res_yaw) of the ratio shrunk by 2^-20: a float res_yaw is 2 pi / K rounded (10 deg in float is a hair under 10 deg), and
+// a plain ceil would then give K + 1 sectors; with the shrink every float within 2^-21 of 2 pi / K gives K (SURVEY G3)
+static const double kKldPi = 3.14159265358979323846;
+static double kld_sector_count(float res_yaw) { return std::ceil(2.0 * kKldPi / (double)res_yaw * (1.0 - 0x1p-20)); }
+// the handle's table of the K sector boundaries theta_k = -pi + 2 pi k / K, as (float)cos, (float)sin of the double angle
+static int kld_sector_table(b2_pf* h, uint32_t K)
+{
+    if (h->kld_K == K) return B2_OK;
+    h->h_kld_tab.resize(2 * (size_t)K);
+    for (uint32_t k = 0; k < K; k++) {
+        const double th = -kKldPi + 2.0 * kKldPi * (double)k / (double)K;
+        h->h_kld_tab[2 * k] = (float)std::cos(th); h->h_kld_tab[2 * k + 1] = (float)std::sin(th);
+    }
+    RES(h->d_kld_tab.reserve(2 * (size_t)K));
+    CU(cudaMemcpyAsync(h->d_kld_tab.p, h->h_kld_tab.data(), sizeof(float) * 2 * K, cudaMemcpyHostToDevice, h->stream));
+    h->kld_K = K;
+    return B2_OK;
+}
 extern "C" int b2_pf_resample_kld(b2_pf* h, const b2_transform* poses_dev, const b2_particle_attr* attrs_dev, uint32_t n, uint32_t n_max, uint32_t first,
                                   uint32_t n_local, b2_transform* poses_new_dev, b2_particle_attr* attrs_new_dev, const b2_gladiator_config* cfg,
                                   const b2_kld_config* kld, uint64_t seed, uint32_t step, b2_kld_result* out_host)
@@ -2486,10 +2521,7 @@ extern "C" int b2_pf_resample_kld(b2_pf* h, const b2_transform* poses_dev, const
         return fail(B2_ERR_INVALID, "resample kld: res_xy = %g and epsilon = %g must be finite and > 0", (double)kld->res_xy, kld->epsilon);
     if (!(std::isfinite(kld->res_z) && kld->res_z >= 0.0f)) return fail(B2_ERR_INVALID, "resample kld: res_z = %g must be finite and >= 0", (double)kld->res_z);
     if (!std::isfinite(kld->z)) return fail(B2_ERR_INVALID, "resample kld: z = %g must be finite", kld->z);
-    const double kPi = 3.14159265358979323846;
-    // K = ceil(2 pi / res_yaw) of the ratio shrunk by 2^-20: a float res_yaw is 2 pi / K rounded (10 deg in float is a hair under 10 deg), and
-    // a plain ceil would then give K + 1 sectors; with the shrink every float within 2^-21 of 2 pi / K gives K (SURVEY G3)
-    const double Kd = std::ceil(2.0 * kPi / (double)kld->res_yaw * (1.0 - 0x1p-20));
+    const double Kd = kld_sector_count(kld->res_yaw);
     if (!(Kd >= 1.0 && Kd <= (double)B2_KLD_MAX_SECTORS))
         return fail(B2_ERR_INVALID, "resample kld: res_yaw = %g gives %g yaw sectors (1 .. %u)", (double)kld->res_yaw, Kd, B2_KLD_MAX_SECTORS);
     const uint32_t K = (uint32_t)Kd;
@@ -2512,16 +2544,7 @@ extern "C" int b2_pf_resample_kld(b2_pf* h, const b2_transform* poses_dev, const
     RES(h->d_kld_parents.reserve(max_len)); RES(h->d_kld_slots.reserve(max_len)); RES(h->d_kld_flags.reserve(max_len)); RES(h->d_kld_cum.reserve(max_len));
     RES(h->d_kld_tmp.reserve(std::max<size_t>(std::max(scan_w, scan_f), 16)));
     if (!h->d_kld.p) { RES(h->d_kld.reserve(1)); CU(cudaMallocHost((void**)&h->h_kld, sizeof(PfKldState))); }
-    if (h->kld_K != K) {                                 // boundaries theta_k = -pi + 2 pi k / K, as (float)cos, (float)sin of the double angle
-        h->h_kld_tab.resize(2 * (size_t)K);
-        for (uint32_t k = 0; k < K; k++) {
-            const double th = -kPi + 2.0 * kPi * (double)k / (double)K;
-            h->h_kld_tab[2 * k] = (float)std::cos(th); h->h_kld_tab[2 * k + 1] = (float)std::sin(th);
-        }
-        RES(h->d_kld_tab.reserve(2 * (size_t)K));
-        CU(cudaMemcpyAsync(h->d_kld_tab.p, h->h_kld_tab.data(), sizeof(float) * 2 * K, cudaMemcpyHostToDevice, h->stream));
-        h->kld_K = K;
-    }
+    RES(kld_sector_table(h, K));
     // the hash set is cleared by memset on the stream: at 12 B per slot it costs less than one chunk's draws, and unlike epoch tags it keeps
     // every stored key a plain 64-bit word that one atomicCAS claims
     CU(cudaMemsetAsync(h->d_kld_keys.p, 0, sizeof(unsigned long long) * T, h->stream));
@@ -2563,6 +2586,124 @@ extern "C" int b2_pf_resample_kld(b2_pf* h, const b2_transform* poses_dev, const
     }
     CU(cudaStreamSynchronize(h->stream));
     res.n_particles = d0; res.bins = n_bins;
+    *out_host = res;
+    return B2_OK;
+}
+
+// The filter's pose hypotheses (SURVEY appendix H): the statistics pass, the members' bins into the hash set, the union-find labelling, the
+// ranking of the clusters, every particle's label, a stable sort that lines the recorded clusters' members up, and the two estimate passes
+// on each of them
+extern "C" int b2_pf_cluster_stats(b2_pf* h, const b2_transform* poses_dev, const b2_particle_attr* attrs_dev, uint32_t n, const b2_cluster_config* cfg,
+                                   b2_cluster_record* records_host, uint32_t* labels_dev, b2_cluster_result* out_host)
+{
+    NOTNULL(h); NOTNULL(poses_dev); NOTNULL(attrs_dev); NOTNULL(cfg); NOTNULL(records_host); NOTNULL(out_host);
+    if (n == 0 || n > (1u << 30)) return fail(B2_ERR_INVALID, "cluster stats: %u particles (1 .. 2^30)", n);
+    if (!(std::isfinite(cfg->res_xy) && cfg->res_xy > 0.0f)) return fail(B2_ERR_INVALID, "cluster stats: res_xy = %g must be finite and > 0", (double)cfg->res_xy);
+    if (!(std::isfinite(cfg->res_z) && cfg->res_z >= 0.0f)) return fail(B2_ERR_INVALID, "cluster stats: res_z = %g must be finite and >= 0", (double)cfg->res_z);
+    const double Kd = kld_sector_count(cfg->res_yaw);
+    if (!(Kd >= 1.0 && Kd <= (double)B2_KLD_MAX_SECTORS))
+        return fail(B2_ERR_INVALID, "cluster stats: res_yaw = %g gives %g yaw sectors (1 .. %u)", (double)cfg->res_yaw, Kd, B2_KLD_MAX_SECTORS);
+    if (cfg->max_records < 1 || cfg->max_records > B2_CLUSTER_MAX_RECORDS)
+        return fail(B2_ERR_INVALID, "cluster stats: max_records = %u must lie in [1, %u]", cfg->max_records, B2_CLUSTER_MAX_RECORDS);
+    const uint32_t K = (uint32_t)Kd;
+    CU(cudaSetDevice(h->map->device));
+    RES(kld_stats(h, attrs_dev, n));
+    const double S = h->h_res->S, L_min = h->h_res->L_min, L_max = h->h_res->L_max;
+    b2_cluster_result res = {0, 0, 0, 0, 0, 0, S, L_max};
+    if (!(std::isfinite(S) && S > 0.0 && L_min >= 0.0)) { *out_host = res; return B2_OK; }       // as KLD (SURVEY G1)
+    uint64_t T = 1;                                      // the hash set: a power of two >= 2 n slots (load <= 1/2)
+    while (T < 2 * (uint64_t)n) T <<= 1;
+    size_t sort_c = 0, sort_p = 0;
+    CU(cub::DeviceRadixSort::SortPairs(nullptr, sort_c, h->d_kld_w.p, h->d_kld_W.p, h->d_cl_idx.p, h->d_cl_idx2.p, (int)n, 0, 64, h->stream));
+    CU(cub::DeviceRadixSort::SortPairs(nullptr, sort_p, h->d_cl_key.p, h->d_cl_key2.p, h->d_cl_idx.p, h->d_cl_idx2.p, (int)n, 0, 5, h->stream));
+    RES(h->d_kld_keys.reserve(T)); RES(h->d_kld_first.reserve(T)); RES(h->d_cl_w.reserve(T)); RES(h->d_cl_cnt.reserve(T)); RES(h->d_cl_aux.reserve(T));
+    RES(h->d_kld_w.reserve(n)); RES(h->d_kld_W.reserve(n)); RES(h->d_cl_slot.reserve(n)); RES(h->d_cl_key.reserve(n)); RES(h->d_cl_key2.reserve(n));
+    RES(h->d_cl_idx.reserve(n)); RES(h->d_cl_idx2.reserve(n)); RES(h->d_kld_tmp.reserve(std::max<size_t>(std::max(sort_c, sort_p), 16)));
+    const size_t off_heads = sizeof(PfClusterState), off_recs = off_heads + sizeof(PfClusterHead) * B2_CLUSTER_MAX_RECORDS;
+    if (!h->d_cl.p) {
+        RES(h->d_cl.reserve(1)); RES(h->d_cl_heads.reserve(B2_CLUSTER_MAX_RECORDS)); RES(h->d_cl_recs.reserve(B2_CLUSTER_MAX_RECORDS));
+        CU(cudaMallocHost((void**)&h->h_cl, off_recs + sizeof(b2_particle_stats) * B2_CLUSTER_MAX_RECORDS));
+    }
+    const PfClusterState* st = reinterpret_cast<const PfClusterState*>(h->h_cl);
+    const PfClusterHead* heads = reinterpret_cast<const PfClusterHead*>(h->h_cl + off_heads);
+    const b2_particle_stats* recs = reinterpret_cast<const b2_particle_stats*>(h->h_cl + off_recs);
+    RES(kld_sector_table(h, K));
+    CU(cudaMemsetAsync(h->d_kld_keys.p, 0, sizeof(unsigned long long) * T, h->stream));
+    CU(cudaMemsetAsync(h->d_cl_w.p, 0, sizeof(unsigned long long) * T, h->stream));
+    CU(cudaMemsetAsync(h->d_cl_cnt.p, 0, sizeof(unsigned int) * T, h->stream));
+    CU(cudaMemsetAsync(h->d_cl.p, 0, sizeof(PfClusterState), h->stream));
+    const KldBins bins{cfg->res_xy, cfg->res_z, K, h->d_kld_tab.p};
+    const uint32_t grid_n = (n + 255) / 256, grid_T = (uint32_t)((T + 255) / 256);
+    k_pf_cluster_insert<<<grid_n, 256, 0, h->stream>>>(poses_dev, attrs_dev, n, L_max, bins, h->d_kld_keys.p, T - 1, h->d_kld_first.p, h->d_cl_w.p, h->d_cl_cnt.p,
+                                                       h->d_cl_slot.p, h->d_cl.p);
+    LAUNCHED();
+    // A round joins every pair of touching bins and ends in the fixed point unless one of its bounded loops ran out, which the bounds (the
+    // table's size, above any path or retry count) do not allow; the cap keeps the call finite even so.
+    uint32_t rounds = 0;
+    for (;;) {
+        if (rounds == B2_CLUSTER_MAX_ROUNDS) return fail(B2_ERR_CUDA, "cluster stats: the labelling did not settle within %u rounds", B2_CLUSTER_MAX_ROUNDS);
+        rounds++;
+        CU(cudaMemsetAsync(&h->d_cl.p->retry, 0, sizeof(unsigned int), h->stream));
+        k_pf_cluster_hook<<<grid_T, 256, 0, h->stream>>>(h->d_kld_keys.p, T - 1, K, cfg->res_z > 0.0f ? 1 : 0, h->d_kld_first.p, h->d_cl_aux.p, h->d_cl.p);
+        LAUNCHED();
+        k_pf_cluster_flatten<<<grid_T, 256, 0, h->stream>>>(h->d_kld_keys.p, T - 1, h->d_kld_first.p, h->d_cl_w.p, h->d_cl_cnt.p, h->d_cl_aux.p, h->d_cl_idx.p,
+                                                            h->d_kld_w.p, h->d_cl.p);
+        LAUNCHED();
+        CU(cudaMemcpyAsync(h->h_cl, h->d_cl.p, sizeof(PfClusterState), cudaMemcpyDeviceToHost, h->stream));
+        CU(cudaStreamSynchronize(h->stream));
+        if (st->fault) return fail(B2_ERR_CUDA, "cluster stats: the hash set of %llu slots had no room for %u particles", (unsigned long long)T, n);
+        if (!st->retry) break;
+    }
+    const uint32_t m = st->n_clusters, n_records = std::min<uint32_t>(m, cfg->max_records);
+    res.n_clusters = m; res.n_records = n_records; res.bins = st->bins; res.n_clustered = st->n_clustered; res.weight_total = st->weight_total; res.rounds = rounds;
+    if (m == 0) {                                        // weights > 0, but no finite pose among them
+        if (labels_dev) CU(cudaMemsetAsync(labels_dev, 0xff, sizeof(uint32_t) * (size_t)n, h->stream));
+        CU(cudaStreamSynchronize(h->stream));
+        *out_host = res;
+        return B2_OK;
+    }
+    // rank: by key, then stably by the weight's complement; d_cl_idx lists the roots in rank order afterwards
+    size_t bytes = h->d_kld_tmp.cap;
+    if (m > 1) {
+        CU(cub::DeviceRadixSort::SortPairs(h->d_kld_tmp.p, bytes, h->d_kld_w.p, h->d_kld_W.p, h->d_cl_idx.p, h->d_cl_idx2.p, (int)m, 0, 64, h->stream));
+        LAUNCHED();
+        k_pf_cluster_weight_keys<<<(m + 255) / 256, 256, 0, h->stream>>>(h->d_cl_idx2.p, h->d_cl_w.p, m, h->d_kld_w.p);
+        LAUNCHED();
+        bytes = h->d_kld_tmp.cap;
+        CU(cub::DeviceRadixSort::SortPairs(h->d_kld_tmp.p, bytes, h->d_kld_w.p, h->d_kld_W.p, h->d_cl_idx2.p, h->d_cl_idx.p, (int)m, 0, 64, h->stream));
+        LAUNCHED();
+    }
+    k_pf_cluster_rank<<<(m + 255) / 256, 256, 0, h->stream>>>(h->d_cl_idx.p, m, n_records, h->d_kld_keys.p, h->d_cl_w.p, h->d_cl_cnt.p, h->d_cl_aux.p, h->d_cl_heads.p);
+    LAUNCHED();
+    CU(cudaMemcpyAsync(h->h_cl + off_heads, h->d_cl_heads.p, sizeof(PfClusterHead) * n_records, cudaMemcpyDeviceToHost, h->stream));
+    k_pf_cluster_labels<<<grid_n, 256, 0, h->stream>>>(h->d_cl_slot.p, n, h->d_kld_first.p, h->d_cl_aux.p, n_records, labels_dev, h->d_cl_key.p, h->d_cl_idx.p);
+    LAUNCHED();
+    int bits = 1;                                        // sort keys 0 .. n_records
+    while ((1u << bits) <= n_records) bits++;
+    bytes = h->d_kld_tmp.cap;
+    CU(cub::DeviceRadixSort::SortPairs(h->d_kld_tmp.p, bytes, h->d_cl_key.p, h->d_cl_key2.p, h->d_cl_idx.p, h->d_cl_idx2.p, (int)n, 0, bits, h->stream));
+    LAUNCHED();
+    CU(cudaStreamSynchronize(h->stream));
+    uint64_t total = 0;
+    for (uint32_t r = 0; r < n_records; r++) total += heads[r].members;
+    RES(h->d_cl_poses.reserve(total)); RES(h->d_cl_attrs.reserve(total));
+    k_pf_cluster_gather<<<(uint32_t)((total + 255) / 256), 256, 0, h->stream>>>(h->d_cl_idx2.p, (uint32_t)total, poses_dev, attrs_dev, h->d_cl_poses.p, h->d_cl_attrs.p);
+    LAUNCHED();
+    uint64_t at = 0;
+    for (uint32_t r = 0; r < n_records; r++) {
+        RES(estimate_launch(h, h->d_cl_poses.p + at, h->d_cl_attrs.p + at, heads[r].members));
+        CU(cudaMemcpyAsync(h->d_cl_recs.p + r, &h->d_est.p->rec, sizeof(b2_particle_stats), cudaMemcpyDeviceToDevice, h->stream));
+        at += heads[r].members;
+    }
+    CU(cudaMemcpyAsync(h->h_cl + off_recs, h->d_cl_recs.p, sizeof(b2_particle_stats) * n_records, cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    for (uint32_t r = 0; r < n_records; r++) {
+        b2_cluster_record& o = records_host[r];
+        memset(&o, 0, sizeof(o));
+        o.stats = recs[r];
+        o.weight = (double)heads[r].weight_int / (double)res.weight_total;
+        o.weight_int = heads[r].weight_int; o.bins = heads[r].bins; o.key = heads[r].key;
+    }
     *out_host = res;
     return B2_OK;
 }

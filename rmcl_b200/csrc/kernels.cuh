@@ -2150,4 +2150,214 @@ __global__ void __launch_bounds__(256) k_pf_kld_expand(const b2_transform* __res
 }
 #endif
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Pose hypotheses of the particle set (b2_pf_cluster_stats; what AMCL reports as pf_cluster_stats; no reference implementation, SURVEY
+// appendix H): the members (integer weight > 0, finite pose) are binned with kld_key, occupied bins that touch (each of x, y, z within one
+// cell, the yaw sector within one modulo K) are joined, and every connected component is a cluster with the exact integer sum of its
+// members' weights.  k_pf_cluster_insert puts the keys into KLD's hash set and sums weight and member count per slot; k_pf_cluster_hook
+// joins every slot with its occupied neighbours of smaller key in a union-find forest over slot indices whose links only ever lead to a
+// smaller key, so a component's root is its smallest key whatever the order of the threads (lock-free hooking of roots with path halving,
+// after Jaiganesh and Burtscher's ECL-CC); k_pf_cluster_flatten points every slot at its root and sums weight, members and bins there.  The
+// roots are then sorted by (weight descending, key ascending), every particle takes its root's rank as its label, a stable sort of the
+// particle indices by min(label, n_records) lines the recorded clusters' members up in index order, and k_pf_estimate_moments /
+// k_pf_estimate_cov run on each gathered segment.  Every sum is an integer, so no result depends on the order in which threads ran.
+// ---------------------------------------------------------------------------------------------------------------------
+#define B2_CLUSTER_NONE 0xFFFFFFFFu                     // the label of a particle in no cluster, and the slot of one in no bin
+#define B2_CLUSTER_MAX_RECORDS 16u
+#define B2_CLUSTER_MAX_ROUNDS 64u
+// the key of the bin at offset (dx, dy, dz, ds), each in {-1, 0, 1}, from the bin `key` (kld_key's layout), or B2_KLD_NONFINITE_KEY where
+// there is none: x, y and z end at their clamps, z has no neighbours when it is not binned, the yaw sector wraps modulo K.  With K <= 2
+// several offsets name the same bin (or the bin itself); joining a pair twice changes nothing.
+B2_DEV uint64_t kld_key_neighbour(uint64_t key, int dx, int dy, int dz, int ds, uint32_t K, bool has_z)
+{
+    const int64_t ix = (int64_t)(key >> 44) + dx, iy = (int64_t)((key >> 24) & 0xFFFFFu) + dy, iz = (int64_t)((key >> 16) & 0xFFu) + dz;
+    if (ix < 0 || ix > 0xFFFFF || iy < 0 || iy > 0xFFFFF || iz < 0 || iz > 0xFF || (!has_z && dz != 0)) return B2_KLD_NONFINITE_KEY;
+    const uint64_t s = (uint64_t)(((int64_t)(key & 0xFFFFu) + ds + (int64_t)K) % (int64_t)K);
+    return (uint64_t)ix << 44 | (uint64_t)iy << 24 | (uint64_t)iz << 16 | s;
+}
+// offset o of the 81 (27 when z is not binned) around a bin, the bin itself included
+B2_DEV uint64_t kld_key_offset(uint64_t key, uint32_t o, uint32_t K, bool has_z)
+{
+    return kld_key_neighbour(key, (int)(o / 3u % 3u) - 1, (int)(o / 9u % 3u) - 1, has_z ? (int)(o / 27u) - 1 : 0, (int)(o % 3u) - 1, K, has_z);
+}
+// the device record the host reads back after the labelling
+struct PfClusterState {
+    unsigned long long weight_total;   // the sum of the members' integer weights
+    unsigned int n_clustered, bins, n_clusters;
+    unsigned int retry;                // a bounded loop of k_pf_cluster_hook ran out: the round has to be repeated
+    unsigned int fault, pad;           // the hash set had no free slot (it holds 2 n and more: cannot happen)
+};
+// what the host needs of each recorded cluster before the estimate runs on it
+struct PfClusterHead { unsigned long long weight_int, key; unsigned int bins, members; };
+#ifdef __CUDACC__
+// The lanes of a warp that name the same slot add to it once: the lowest of them adds the sum of their values.  All 32 lanes call it; a lane
+// with slot B2_CLUSTER_NONE adds nothing.
+__device__ __forceinline__ void cluster_warp_add(uint32_t s, unsigned long long wv, uint32_t cv, uint32_t bv, unsigned long long* __restrict__ w,
+                                                 unsigned int* __restrict__ cnt, unsigned int* __restrict__ aux)
+{
+    const uint32_t lane = threadIdx.x & 31u;
+    unsigned long long ws = 0ull;
+    uint32_t cs = 0u, bs = 0u;
+    bool lowest = true;
+    for (uint32_t l = 0; l < 32u; l++) {
+        const uint32_t sl = __shfl_sync(0xffffffffu, s, l), cl = __shfl_sync(0xffffffffu, cv, l), bl = __shfl_sync(0xffffffffu, bv, l);
+        const unsigned long long wl = __shfl_sync(0xffffffffu, wv, l);
+        if (sl == s) { ws += wl; cs += cl; bs += bl; lowest = lowest && l >= lane; }
+    }
+    if (s == B2_CLUSTER_NONE || !lowest) return;
+    if (ws) atomicAdd(w + s, ws);
+    if (cs) atomicAdd(cnt + s, cs);
+    if (bs) atomicAdd(aux + s, bs);
+}
+// one thread per particle: a member's key goes into the hash set (as k_pf_kld_draw stores it: key ^ 0x8000, 0 an empty slot); the thread
+// that claims a slot makes it its own root.  36 B read per particle (the likelihood, then the pose of a particle of weight > 0).
+__global__ void __launch_bounds__(256) k_pf_cluster_insert(const b2_transform* __restrict__ poses, const b2_particle_attr* __restrict__ attrs, uint32_t n, double L_max,
+                                                           KldBins bins, unsigned long long* __restrict__ keys, uint64_t mask, unsigned int* __restrict__ parent,
+                                                           unsigned long long* __restrict__ w, unsigned int* __restrict__ cnt, uint32_t* __restrict__ slot_of,
+                                                           PfClusterState* __restrict__ st)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned long long wi = 0ull;
+    uint32_t s = B2_CLUSTER_NONE;
+    if (i < n) {
+        wi = kld_weight(attrs[i].likelihood.mean, L_max);
+        const uint64_t key = wi > 0ull ? kld_key(poses[i], bins) : B2_KLD_NONFINITE_KEY;
+        if (key != B2_KLD_NONFINITE_KEY) {
+            const unsigned long long v = key ^ 0x8000ull;
+            uint64_t t = kld_hash(v) & mask;
+            for (uint64_t probe = 0; probe <= mask; probe++) {          // at most n of the 2 n and more slots are taken: a free one turns up
+                const unsigned long long old = atomicCAS(keys + t, 0ull, v);
+                if (old == 0ull) parent[t] = (unsigned int)t;
+                if (old == 0ull || old == v) { s = (uint32_t)t; break; }
+                t = (t + 1u) & mask;
+            }
+            if (s == B2_CLUSTER_NONE) st->fault = 1u;
+        }
+        if (s == B2_CLUSTER_NONE) wi = 0ull;
+        slot_of[i] = s;
+    }
+    cluster_warp_add(s, wi, 1u, 0u, w, cnt, nullptr);
+    const uint32_t members = __popc(__ballot_sync(0xffffffffu, s != B2_CLUSTER_NONE));
+    #pragma unroll
+    for (int o = 16; o > 0; o >>= 1) wi += __shfl_xor_sync(0xffffffffu, wi, o);
+    if ((threadIdx.x & 31u) == 0u && members) { atomicAdd(&st->weight_total, wi); atomicAdd(&st->n_clustered, members); }
+}
+// the root of slot x, halving the path on the way.  Keys fall strictly along the links, so a path is shorter than the table.
+__device__ __forceinline__ uint32_t cluster_find(volatile unsigned int* parent, uint32_t x, uint64_t mask)
+{
+    for (uint64_t it = 0; it <= mask; it++) {
+        const uint32_t p = parent[x];
+        if (p == x) break;
+        const uint32_t g = parent[p];
+        if (g != p) parent[x] = g;
+        x = g;
+    }
+    return x;
+}
+// one thread per slot: joins an occupied slot with each occupied neighbour of smaller key (so every pair is joined once, from its larger
+// end).  The root with the larger key is hooked under the other tree by one atomicCAS; when another thread hooked it first, the walk goes on
+// from where that thread put it, to a strictly smaller key.  Nothing waits for another thread, and every loop ends within the table's size.
+__global__ void __launch_bounds__(256) k_pf_cluster_hook(const unsigned long long* __restrict__ keys, uint64_t mask, uint32_t K, int has_z, unsigned int* parent,
+                                                         unsigned int* __restrict__ aux, PfClusterState* __restrict__ st)
+{
+    const uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (s > mask) return;
+    const unsigned long long v = keys[s];
+    if (v == 0ull) return;
+    aux[s] = 0u;
+    const uint64_t key = v ^ 0x8000ull;
+    const uint32_t n_off = has_z ? 81u : 27u;
+    for (uint32_t o = 0; o < n_off; o++) {
+        const uint64_t nk = kld_key_offset(key, o, K, has_z != 0);
+        if (nk >= key) continue;                                          // none, the bin itself, or a pair its other end joins
+        const unsigned long long nv = nk ^ 0x8000ull;
+        uint64_t t = kld_hash(nv) & mask;
+        bool found = false;
+        for (uint64_t probe = 0; probe <= mask; probe++) {
+            const unsigned long long cur = keys[t];
+            if (cur == 0ull) break;
+            if (cur == nv) { found = true; break; }
+            t = (t + 1u) & mask;
+        }
+        if (!found) continue;
+        uint32_t a = cluster_find(parent, (uint32_t)s, mask), b = cluster_find(parent, (uint32_t)t, mask);
+        bool joined = false;
+        for (uint64_t it = 0; it <= mask; it++) {
+            if (a == b) { joined = true; break; }
+            if (keys[a] < keys[b]) { const uint32_t c = a; a = b; b = c; }   // a has the larger key
+            const uint32_t old = atomicCAS(parent + a, a, b);
+            if (old == a) { joined = true; break; }
+            a = old;
+        }
+        if (!joined) st->retry = 1u;
+    }
+}
+// one thread per slot, after a round that ran to its end: the slot's root (read only: the forest no longer changes but for these writes,
+// which point a slot at its own root), then weight, members and one bin added to the root, and each root appended to the list of clusters
+// (in no particular order: the sort that follows has distinct keys)
+__global__ void __launch_bounds__(256) k_pf_cluster_flatten(const unsigned long long* __restrict__ keys, uint64_t mask, volatile unsigned int* parent,
+                                                            unsigned long long* __restrict__ w, unsigned int* __restrict__ cnt, unsigned int* __restrict__ aux,
+                                                            uint32_t* __restrict__ roots, unsigned long long* __restrict__ root_keys, PfClusterState* __restrict__ st)
+{
+    if (st->retry) return;
+    const uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const unsigned long long v = s <= mask ? keys[s] : 0ull;
+    uint32_t r = B2_CLUSTER_NONE;
+    if (v != 0ull) {
+        r = (uint32_t)s;
+        for (uint64_t it = 0; it <= mask; it++) { const uint32_t p = parent[r]; if (p == r) break; r = p; }
+        parent[s] = r;
+    }
+    const bool moved = v != 0ull && r != (uint32_t)s;                      // nothing is ever added to a slot that is not a root
+    cluster_warp_add(r, moved ? w[s] : 0ull, moved ? cnt[s] : 0u, v != 0ull ? 1u : 0u, w, cnt, aux);
+    const uint32_t occupied = __popc(__ballot_sync(0xffffffffu, v != 0ull));
+    if ((threadIdx.x & 31u) == 0u && occupied) atomicAdd(&st->bins, occupied);
+    if (v != 0ull && r == (uint32_t)s) {
+        const uint32_t j = atomicAdd(&st->n_clusters, 1u);
+        roots[j] = r; root_keys[j] = v ^ 0x8000ull;
+    }
+}
+// the second sort key of the clusters, already in key order: the complement of the weight, so that the heaviest comes first
+__global__ void __launch_bounds__(256) k_pf_cluster_weight_keys(const uint32_t* __restrict__ roots, const unsigned long long* __restrict__ w, uint32_t m,
+                                                                unsigned long long* __restrict__ out)
+{
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < m) out[j] = ~w[roots[j]];
+}
+// one thread per cluster in rank order: the head of a recorded cluster, then the rank takes the place of the root's bin count
+__global__ void __launch_bounds__(256) k_pf_cluster_rank(const uint32_t* __restrict__ roots, uint32_t m, uint32_t n_records, const unsigned long long* __restrict__ keys,
+                                                         const unsigned long long* __restrict__ w, const unsigned int* __restrict__ cnt, unsigned int* __restrict__ aux,
+                                                         PfClusterHead* __restrict__ heads)
+{
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= m) return;
+    const uint32_t r = roots[j];
+    if (j < n_records) { PfClusterHead hd; hd.weight_int = w[r]; hd.key = keys[r] ^ 0x8000ull; hd.bins = aux[r]; hd.members = cnt[r]; heads[j] = hd; }
+    aux[r] = j;
+}
+// one thread per particle: its label, and its place in the sort that gathers the recorded clusters (every other particle sorts behind them)
+__global__ void __launch_bounds__(256) k_pf_cluster_labels(const uint32_t* __restrict__ slot_of, uint32_t n, const unsigned int* __restrict__ parent,
+                                                           const unsigned int* __restrict__ aux, uint32_t n_records, uint32_t* __restrict__ labels,
+                                                           uint32_t* __restrict__ sort_keys, uint32_t* __restrict__ index)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t s = slot_of[i];
+    const uint32_t label = s == B2_CLUSTER_NONE ? B2_CLUSTER_NONE : aux[parent[s]];
+    if (labels) labels[i] = label;
+    sort_keys[i] = label < n_records ? label : n_records;
+    index[i] = i;
+}
+// one thread per member of a recorded cluster: 68 B gathered and 68 B written
+__global__ void __launch_bounds__(256) k_pf_cluster_gather(const uint32_t* __restrict__ index, uint32_t total, const b2_transform* __restrict__ poses,
+                                                           const b2_particle_attr* __restrict__ attrs, b2_transform* __restrict__ poses_out,
+                                                           b2_particle_attr* __restrict__ attrs_out)
+{
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= total) return;
+    const uint32_t i = index[p];
+    poses_out[p] = poses[i]; attrs_out[p] = attrs[i];
+}
+#endif
+
 #include "icp_loop.cuh"

@@ -371,6 +371,12 @@ assert RESIDUAL_RESULT_DTYPE.itemsize == 32
 # b2_kld_result: what PCDSensorUpdaterB200.resampleKLD returns
 KLD_RESULT_DTYPE = np.dtype([("n_particles", np.uint64), ("bins", np.uint64), ("weight_sum", np.float64), ("weight_max", np.float64)])
 assert KLD_RESULT_DTYPE.itemsize == 32
+# b2_cluster_record / b2_cluster_result: what PCDSensorUpdaterB200.estimateClusters returns
+CLUSTER_RECORD_DTYPE = np.dtype([("stats", PARTICLE_STATS_DTYPE), ("weight", np.float64), ("weight_int", np.uint64), ("bins", np.uint64), ("key", np.uint64)])
+assert CLUSTER_RECORD_DTYPE.itemsize == 472
+CLUSTER_RESULT_DTYPE = np.dtype([("n_clusters", np.uint64), ("n_records", np.uint64), ("bins", np.uint64), ("n_clustered", np.uint64), ("weight_total", np.uint64),
+                                 ("rounds", np.uint64), ("weight_sum", np.float64), ("weight_max", np.float64)])
+assert CLUSTER_RESULT_DTYPE.itemsize == 64
 
 
 def quat_from_rpy(roll, pitch, yaw):
