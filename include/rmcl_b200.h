@@ -265,6 +265,44 @@ typedef struct {
 B2_API int b2_micp_correct(b2_rcc* const* sensors, const b2_transform* Tbo, const double* merge_weights, uint32_t n_sensors,
                            b2_transform* Tom_inout, double* convergence_progress_inout, int adaptive_max_dist,
                            uint32_t n_corrections, uint32_t iterations, b2_micp_step* steps_out);
+/* The covariance of a MICP-L correction, from the point-to-plane information of its final correspondences (the reference publishes a guess,
+ * micp_localization.cpp:1053-1084; no reference implementation, SURVEY appendix I).  Inputs: the sensors, Tbo and merge weights w_k (NULL = all
+ * 1.0) of a correction that just ran, its T_onew_oold and the convergence_progress it gated with, and the reference frame Tbo_ref (NULL = Tbo[0]).
+ * The published pose is Tbm = Tom_new * Tbo_ref; the covariance is about it, in its body frame: Tbm' = Tbm * Exp(d), d = (x, y, z, roll, pitch,
+ * yaw), the order and frame of PoseWithCovariance and of b2_pf_estimate_stats.
+ *  - Pairs: sensor k's loop pre-transform T_k = Tso_k * T_onew_oold * Tos_k (Tos = Tbo * Tsb, float, as the ICP loop composes it).  Pair i is
+ *    used iff dataset mask > 0, model hit > 0 and the P2L gate of b2_rcc_cross_statistics(T_k, convergence_progress) accepts it, so n_pairs[k]
+ *    equals that call's n_meas.  Its residual r is the signed point-to-plane distance of the gate.
+ *  - Jacobian: U_k = ~Tbo_ref * Tbo_k * Tsb_k (composed in double, rounded to float once), q = U_k d (the raw dataset point), n = R(U_k) R(T_k)^T N
+ *    (the model normal), J = (n, q x n), all in float.
+ *  - Sums in FP64, per sensor, then weighted: H = sum_k w_k sum_i J J^T, R2 = sum_k w_k sum_i r^2, Q2 = sum_k w_k sum_i |q|^2, W = sum_k w_k n_k.
+ *    sigma2 = R2 / (W - 6) (NaN when W <= 6), L = sqrt(Q2 / W) (1 when that is not > 0).
+ *  - Scaling S = diag(1, 1, 1, 1/L, 1/L, 1/L); S H S is decomposed by cyclic Jacobi in FP64 (at most 32 sweeps; stops when the off-diagonal sum of
+ *    squares is <= 1e-30 times the matrix's), eigenvalues ascending, each eigenvector's largest-magnitude component positive (first one on ties).
+ *    Direction i is degenerate iff eigenvalues[i] <= tau * eigenvalues[5].
+ *  - covariance = S (sigma2 sum_nondeg v v^T / lambda + degenerate_variance sum_deg v v^T) S: a degenerate direction gets degenerate_variance m^2
+ *    along translation and degenerate_variance / L^2 rad^2 along rotation.
+ *  - W == 0 (no pairs): information and the eigen data are 0, covariance and sigma2 NaN, length_scale 0, all six directions degenerate; B2_OK.
+ * To describe the last step of b2_micp_correct, pass steps[-1].T_onew_oold with the progress that step gated with: the input progress for one
+ * step, else steps[-2].convergence_progress.  Reads each handle's current dataset and model buffers (own or bound) and writes nothing into any
+ * handle.  One launch on the lead handle's stream, ordered against the other handles' streams as b2_micp_correct_once orders them, then one copy of
+ * the record and a synchronise.  Works for ray-casting and closest-point handles in every exec mode.  Refused (B2_ERR_INVALID, no launch, nothing
+ * written): null sensors, Tbo, T_onew_oold, cfg or out_host; n_sensors outside 1..4, a handle given twice, handles on different devices; a handle
+ * with calls in flight, with no find yet, or whose dataset size differs from its model size; non-finite transforms; a negative or non-finite
+ * weight; tau outside (0, 1); degenerate_variance not finite and > 0.  Suggested values (not tuned on data): tau 1e-3, degenerate_variance 1e2. */
+typedef struct { double tau, degenerate_variance; } b2_micp_cov_config;                                          /* 16 B */
+typedef char b2_micp_cov_config_is_16_bytes[sizeof(b2_micp_cov_config) == 16 ? 1 : -1];
+typedef struct {
+    double   information[36], covariance[36];   /* row-major, x y z roll pitch yaw, body frame of Tom_new * Tbo_ref */
+    double   eigenvalues[6], eigenvectors[36];  /* of S H S, ascending; row i = unit eigenvector i (scaled coordinates) */
+    double   sigma2, residual_sq_sum, weight_sum, length_scale;
+    uint64_t n_pairs[4];                        /* gated pairs per sensor */
+    uint32_t n_degenerate, degenerate_mask;     /* bit i: eigenvalues[i] <= tau * eigenvalues[5] */
+} b2_micp_covariance;                                                                                            /* 984 B */
+typedef char b2_micp_covariance_is_984_bytes[sizeof(b2_micp_covariance) == 984 ? 1 : -1];
+B2_API int b2_micp_pose_covariance(b2_rcc* const* sensors, const b2_transform* Tbo, const double* merge_weights, uint32_t n_sensors,
+                                   const b2_transform* T_onew_oold, double convergence_progress, const b2_transform* Tbo_ref,
+                                   const b2_micp_cov_config* cfg, b2_micp_covariance* out_host);
 /* How b2_rcc_correct_once* runs the inner iterations: 2 (default) one kernel for all of them, launched programmatically behind find; the block
  * sums cross the grid as 64-bit fixed-point atomics (every block must be co-resident: one block per SM).  1 the same kernel through a cooperative
  * launch, the sums as FP64 slots behind a grid sync.  0 one reduction launch per inner iteration in the reference's own frame-algebra order

@@ -331,6 +331,24 @@ inline void micp_correct(const std::vector<CorrespondencesB200*>& sensors, const
     for (CorrespondencesB200* s : sensors) s->outdated = false;
 }
 
+// The covariance of the correction that just ran on `sensors` (b2_micp_pose_covariance: point-to-plane information of the final correspondences),
+// about Tom_new * Tbo_ref in its body frame (Tbo_ref null: Tbo[0]), x y z roll pitch yaw: what publishPose (micp_localization.cpp:1053-1084)
+// puts into PoseWithCovariance.  After micp_correct pass steps.back().T_onew_oold and the progress that step gated with (the input progress for
+// one step, else steps[n - 2].convergence_progress).
+inline b2_micp_covariance micp_pose_covariance(const std::vector<CorrespondencesB200*>& sensors, const std::vector<rm::Transform>& Tbo,
+                                               const std::vector<double>& merge_weights, const rm::Transform& T_onew_oold, double convergence_progress,
+                                               const rm::Transform* Tbo_ref = nullptr, b2_micp_cov_config cfg = {1e-3, 1e2})
+{
+    if (sensors.size() != Tbo.size() || (!merge_weights.empty() && merge_weights.size() != sensors.size())) throw std::invalid_argument("micp_pose_covariance: one Tbo / weight per sensor");
+    std::vector<b2_rcc*> h;
+    for (CorrespondencesB200* s : sensors) h.push_back(s->handle());
+    b2_micp_covariance out;
+    b2_check(b2_micp_pose_covariance(h.data(), reinterpret_cast<const b2_transform*>(Tbo.data()), merge_weights.empty() ? nullptr : merge_weights.data(),
+                                     (uint32_t)h.size(), reinterpret_cast<const b2_transform*>(&T_onew_oold), convergence_progress,
+                                     reinterpret_cast<const b2_transform*>(Tbo_ref), &cfg, &out), "micp_pose_covariance");
+    return out;
+}
+
 // --- particle filter sensor update ------------------------------------------------------------------------------------------------
 class PCDSensorUpdaterB200
 #if defined(RMCL_B200_WITH_RMAGINE) && defined(RMCL_B200_WITH_RMCL_ROS)

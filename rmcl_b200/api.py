@@ -157,7 +157,7 @@ EXPORTS = [
     "b2_rcc_correct_once_async", "b2_rcc_correct_once_wait", "b2_micp_correct_once", "b2_rcc_set_exec_mode", "b2_debug_read_bandwidth", "b2_rcc_set_sim_options", "b2_rcc_bind_dataset", "b2_rcc_bind_model_buffers", "b2_rcc_benchmark_batch", "b2_pf_p2p_init", "b2_pf_p2p_connect", "b2_pf_p2p_publish", "b2_pf_resample_gladiator_p2p", "b2_pf_p2p_connect_local", "b2_rcc_set_cpc_options", "b2_pf_set_mapping", "b2_pf_get_mapping",
     "b2_micp_correct", "b2_pf_init_uniform", "b2_pf_init_gaussian", "b2_pf_estimate_stats", "b2_rcc_set_cloud_o1dn",
     "b2_rcc_set_cloud_spherical", "b2_pf_sample_cloud", "b2_pf_resample_residual", "b2_pf_project_to_surface",
-    "b2_pf_resample_kld", "b2_pf_cluster_stats",
+    "b2_pf_resample_kld", "b2_pf_cluster_stats", "b2_micp_pose_covariance",
 ]
 
 
@@ -668,6 +668,31 @@ def micp_correct(sensors, Tbo, Tom, n_corrections=3, iterations=5, convergence_p
     for s in sensors:
         s.outdated = False
     return T, cp.value, steps
+
+
+# b2_micp_covariance (rmcl_b200.h): the pose covariance of a correction and the information it comes from
+MICP_COVARIANCE_DTYPE = np.dtype([("information", np.float64, 36), ("covariance", np.float64, 36), ("eigenvalues", np.float64, 6),
+                                  ("eigenvectors", np.float64, 36), ("sigma2", np.float64), ("residual_sq_sum", np.float64), ("weight_sum", np.float64),
+                                  ("length_scale", np.float64), ("n_pairs", np.uint64, 4), ("n_degenerate", np.uint32), ("degenerate_mask", np.uint32)])
+assert MICP_COVARIANCE_DTYPE.itemsize == 984
+
+
+class _MicpCovConfig(C.Structure):
+    _fields_ = [("tau", C.c_double), ("degenerate_variance", C.c_double)]
+
+
+def micp_pose_covariance(sensors, Tbo, T_onew_oold, convergence_progress=0.0, merge_weights=None, Tbo_ref=None, tau=1e-3, degenerate_variance=1e2):
+    """The covariance of the correction that just ran on `sensors` (b2_micp_pose_covariance, SURVEY appendix I): from the point-to-plane
+    information of the final correspondences, about Tom_new * Tbo_ref (default Tbo[0]) in its body frame, x y z roll pitch yaw.  Pass the
+    correction's T_onew_oold and the progress it gated with (after micp_correct: steps[-1]["T_onew_oold"] and the input progress for one step,
+    else steps[-2]["convergence_progress"]).  -> a MICP_COVARIANCE_DTYPE record."""
+    n, hs, Tb, w = _sensor_args(sensors, Tbo, merge_weights)
+    ref = None if Tbo_ref is None else _tf(np.asarray(Tbo_ref, TRANSFORM_DTYPE).reshape(()))
+    cfg = _MicpCovConfig(float(tau), float(degenerate_variance))
+    out = np.zeros((), MICP_COVARIANCE_DTYPE)
+    _chk(load_library().b2_micp_pose_covariance(hs, _p(Tb), _p(w), C.c_uint32(n), _p(_tf(np.asarray(T_onew_oold, TRANSFORM_DTYPE).reshape(()))),
+                                                C.c_double(float(convergence_progress)), _p(ref), C.byref(cfg), _p(out)))
+    return out
 
 
 def umeyama_transform(stats, device=0):

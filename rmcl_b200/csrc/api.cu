@@ -400,6 +400,7 @@ struct b2_rcc {
     std::deque<PendingCall> pending;    // enqueued, not yet collected (oldest first), at most B2_RING
     unsigned int slot_counter = 0;
     DevBuf<unsigned char> d_chain;      // b2_micp_correct with this handle in the lead: IcpChainState, then one b2_micp_step per correction
+    DevBuf<double> d_cov_part; DevBuf<unsigned int> d_cov_ticket; DevBuf<b2_micp_covariance> d_cov_rec;   // b2_micp_pose_covariance with this handle in the lead
     bool timing = false; cudaEvent_t ev[3] = {nullptr, nullptr, nullptr}; bool timing_valid = false;
     cudaStream_t aux = nullptr; cudaEvent_t ev_aux = nullptr;     // side stream: scan upload + unpack overlap the find kernel
     cudaEvent_t ev_join = nullptr;      // multi-sensor correctOnce: orders this handle's stream against the lead handle's
@@ -494,6 +495,7 @@ extern "C" int b2_rcc_destroy(b2_rcc* h)
     h->d_mpts.release(); h->d_mnrm.release(); h->d_mranges.release(); h->d_mhits.release(); h->d_mfaces.release();
     h->d_partials.release(); h->d_ticket.release(); h->d_stats.release(); h->d_icp.release(); h->d_bar.release(); h->d_res.release(); h->d_dbg.release(); h->d_slots.release(); h->d_tile_cost.release(); h->d_tile_perm.release();
     h->d_chain.release(); h->d_cloud.release(); h->d_scan_keys.release();
+    h->d_cov_part.release(); h->d_cov_ticket.release(); h->d_cov_rec.release();
     { DeviceCtx& dc = g_dev[h->map->device & 63]; std::lock_guard<std::mutex> lk(dc.m); dc.n_handles--; if (dc.last == h) { dc.last = nullptr; dc.recorded = false; } }
     h->d_poses.release(); h->d_tdelta.release(); h->d_ncorr.release(); h->d_bstats.release();
     if (h->pin) cudaFreeHost(h->pin);
@@ -1183,24 +1185,34 @@ static int launch_icp_loop(b2_rcc* H, const IcpLaunch& L, int grid, size_t smem,
 // with pairs.  A sensor without pairs gets none, so the other sensors' pairs are summed by exactly the blocks a call without it would use: its
 // presence cannot change a bit of the result.  Then per sensor the pairs per thread in shared memory, merge weight, range limits, frames and
 // dataset; the gate (max_dist) is the caller's.
-static int loop_layout(const b2_rcc* H, const SensorCall* sc, uint32_t ns, uint64_t total, const b2_transform& Tom, uint32_t iterations, IcpLaunch& L)
+// The blocks of a grid of at most grid_cap blocks of `block` threads, split among ns sensors with n[k] pairs (total in all) as described above.
+// Returns the grid; nblk[k] receives sensor k's blocks.
+static int split_blocks(const uint32_t* n, uint32_t ns, uint64_t total, int grid_cap, int block, uint32_t* nblk)
 {
-    memset(&L, 0, sizeof(L));
-    L.Tom = Tom; L.n_sensors = ns; L.iterations = iterations;
-    uint32_t ns_busy = 0, nblk[B2_MAX_SENSORS];
-    for (uint32_t k = 0; k < ns; k++) if (sc[k].h->work_n() > 0) ns_busy++;
-    const int grid = std::min<int>(H->fused_grid, (int)std::max<uint64_t>((total + B2_ICP_BLOCK - 1) / B2_ICP_BLOCK, ns_busy));
+    uint32_t ns_busy = 0;
+    for (uint32_t k = 0; k < ns; k++) if (n[k] > 0) ns_busy++;
+    const int grid = std::min<int>(grid_cap, (int)std::max<uint64_t>((total + block - 1) / block, ns_busy));
     int assigned = 0;
     for (uint32_t k = 0; k < ns; k++) {
-        const uint32_t nw = sc[k].h->work_n();
+        const uint32_t nw = n[k];
         nblk[k] = nw ? std::max<uint32_t>(1u, (uint32_t)((uint64_t)grid * nw / total)) : 0u; assigned += (int)nblk[k];
     }
     while (assigned > grid) { uint32_t big = 0; for (uint32_t k = 1; k < ns; k++) if (nblk[k] > nblk[big]) big = k; nblk[big]--; assigned--; }
     while (assigned < grid) {
         uint32_t best = 0; double load = -1.0;
-        for (uint32_t k = 0; k < ns; k++) { if (!nblk[k]) continue; const double l = (double)sc[k].h->work_n() / nblk[k]; if (l > load) { load = l; best = k; } }
+        for (uint32_t k = 0; k < ns; k++) { if (!nblk[k]) continue; const double l = (double)n[k] / nblk[k]; if (l > load) { load = l; best = k; } }
         nblk[best]++; assigned++;
     }
+    return grid;
+}
+
+static int loop_layout(const b2_rcc* H, const SensorCall* sc, uint32_t ns, uint64_t total, const b2_transform& Tom, uint32_t iterations, IcpLaunch& L)
+{
+    memset(&L, 0, sizeof(L));
+    L.Tom = Tom; L.n_sensors = ns; L.iterations = iterations;
+    uint32_t nw[B2_MAX_SENSORS], nblk[B2_MAX_SENSORS];
+    for (uint32_t k = 0; k < ns; k++) nw[k] = sc[k].h->work_n();
+    const int grid = split_blocks(nw, ns, total, H->fused_grid, B2_ICP_BLOCK, nblk);
     uint32_t blk0 = 0;
     for (uint32_t k = 0; k < ns; k++) {
         const b2_rcc* h = sc[k].h;
@@ -1608,6 +1620,96 @@ extern "C" int b2_micp_correct(b2_rcc* const* sensors, const b2_transform* Tbo, 
     *Tom_inout = got->find[0].Tom;
     *cp_inout = got->cp;
     if (steps_out) memcpy(steps_out, rec, sizeof(b2_micp_step) * (size_t)n_corrections);
+    return B2_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// b2_micp_pose_covariance (SURVEY appendix I): one k_micp_information launch over the final correspondences of all sensors
+// ---------------------------------------------------------------------------------------------------------------------
+// row-major rotation matrix of a float quaternion, normalised in double
+static void quat_to_mat_d(const b2_quat& q, double R[9])
+{
+    const double n = std::sqrt((double)q.x * q.x + (double)q.y * q.y + (double)q.z * q.z + (double)q.w * q.w);
+    const double x = q.x / n, y = q.y / n, z = q.z / n, w = q.w / n;
+    R[0] = 1.0 - 2.0 * (y * y + z * z); R[1] = 2.0 * (x * y - z * w); R[2] = 2.0 * (x * z + y * w);
+    R[3] = 2.0 * (x * y + z * w); R[4] = 1.0 - 2.0 * (x * x + z * z); R[5] = 2.0 * (y * z - x * w);
+    R[6] = 2.0 * (x * z - y * w); R[7] = 2.0 * (y * z + x * w); R[8] = 1.0 - 2.0 * (x * x + y * y);
+}
+// C = A B (transpose_a: A^T B, transpose_b: A B^T), 3x3 row-major
+static void mat3_mul_d(const double* A, bool transpose_a, const double* B, bool transpose_b, double* C)
+{
+    for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) {
+        double s = 0.0;
+        for (int k = 0; k < 3; k++) s += (transpose_a ? A[k * 3 + i] : A[i * 3 + k]) * (transpose_b ? B[j * 3 + k] : B[k * 3 + j]);
+        C[i * 3 + j] = s;
+    }
+}
+
+extern "C" int b2_micp_pose_covariance(b2_rcc* const* sensors, const b2_transform* Tbo, const double* merge_weights, uint32_t n_sensors,
+                                       const b2_transform* T_onew_oold, double cp, const b2_transform* Tbo_ref, const b2_micp_cov_config* cfg,
+                                       b2_micp_covariance* out_host)
+{
+    NOTNULL(sensors); NOTNULL(Tbo); NOTNULL(T_onew_oold); NOTNULL(cfg); NOTNULL(out_host);
+    static const char* what = "micp_pose_covariance";
+    if (!(cfg->tau > 0.0 && cfg->tau < 1.0)) return fail(B2_ERR_INVALID, "%s: tau %g outside (0, 1)", what, cfg->tau);
+    if (!(std::isfinite(cfg->degenerate_variance) && cfg->degenerate_variance > 0.0))
+        return fail(B2_ERR_INVALID, "%s: degenerate_variance %g is not finite and > 0", what, cfg->degenerate_variance);
+    SensorCall sc[B2_MAX_SENSORS];
+    RES(sensor_list(__func__, what, sensors, Tbo, merge_weights, nullptr, n_sensors, sc));
+    b2_rcc* H = sc[0].h;
+    const uint32_t ns = n_sensors;
+    const b2_transform Tref = Tbo_ref ? *Tbo_ref : Tbo[0];
+    if (!all_finite(&T_onew_oold->R.x, 7) || !all_finite(&Tref.R.x, 7)) return fail(B2_ERR_INVALID, "%s: non-finite T_onew_oold or Tbo_ref", what);
+    uint32_t n[B2_MAX_SENSORS]; uint64_t total = 0;
+    for (uint32_t k = 0; k < ns; k++) {
+        const b2_rcc* h = sc[k].h;
+        if (h->map->device != H->map->device) return fail(B2_ERR_INVALID, "%s: all sensors must live on the same device", what);
+        if (!h->pending.empty()) return fail(B2_ERR_INVALID, "%s: asynchronous calls are still in flight on sensor %u, collect them first", what, k);
+        if (!h->found) return fail(B2_ERR_INVALID, "%s: sensor %u has no correspondences (find first)", what, k);
+        if (h->n_dataset != h->n_model) return fail(B2_ERR_INVALID, "%s: sensor %u: dataset size %u != model size %u", what, k, h->n_dataset, h->n_model);
+        if (!all_finite(&sc[k].Tbo.R.x, 7) || !all_finite(&h->Tsb.R.x, 7)) return fail(B2_ERR_INVALID, "%s: sensor %u: non-finite Tbo or Tsb", what, k);
+        if (!(std::isfinite(sc[k].weight) && sc[k].weight >= 0.0)) return fail(B2_ERR_INVALID, "%s: sensor %u: merge weight %g is negative or not finite", what, k, sc[k].weight);
+        n[k] = h->n_model; total += n[k];
+    }
+    MicpCovLaunch L; memset(&L, 0, sizeof(L));
+    L.n_sensors = ns; L.tau = cfg->tau; L.degenerate_variance = cfg->degenerate_variance;
+    uint32_t nblk[B2_MAX_SENSORS];
+    const int grid = std::max(1, split_blocks(n, ns, total, H->red_grid, B2_COV_BLOCK, nblk));      // no pairs: one block writes the record
+    double Rref[9]; quat_to_mat_d(Tref.R, Rref);
+    uint32_t blk0 = 0;
+    for (uint32_t k = 0; k < ns; k++) {
+        const b2_rcc* h = sc[k].h;
+        MicpCovSensor& S = L.s[k];
+        S.dpts = h->dpts(); S.dmask = h->dmask(); S.mpts = h->mpts(); S.mnrm = h->mnrm(); S.mmask = h->mhits();
+        S.n = n[k]; S.blk0 = blk0; S.nblk = nblk[k]; blk0 += nblk[k];
+        S.max_dist = adaptive_max_dist(h, cp); S.weight = sc[k].weight;
+        const Tf Tos = tf_mul(tf_from_pod(sc[k].Tbo), tf_from_pod(h->Tsb));
+        const Tf Tpre = tf_mul(tf_mul(tf_inv(Tos), tf_from_pod(*T_onew_oold)), Tos);              // icp_tail_rest's pre-transform
+        tf_store(&S.Tpre, Tpre);
+        // U = ~Tbo_ref * Tbo * Tsb and R(U) R(Tpre)^T in double, each rounded to float once
+        double Rbo[9], Rsb[9], Rpre[9], Rbs[9], RU[9], RN[9];
+        quat_to_mat_d(sc[k].Tbo.R, Rbo); quat_to_mat_d(h->Tsb.R, Rsb);
+        b2_quat qp; qp.x = Tpre.R.x; qp.y = Tpre.R.y; qp.z = Tpre.R.z; qp.w = Tpre.R.w;
+        quat_to_mat_d(qp, Rpre);
+        mat3_mul_d(Rbo, false, Rsb, false, Rbs);
+        mat3_mul_d(Rref, true, Rbs, false, RU);
+        mat3_mul_d(RU, false, Rpre, true, RN);
+        const double tb[3] = {sc[k].Tbo.t.x, sc[k].Tbo.t.y, sc[k].Tbo.t.z}, ts[3] = {h->Tsb.t.x, h->Tsb.t.y, h->Tsb.t.z}, tr[3] = {Tref.t.x, Tref.t.y, Tref.t.z};
+        double p[3];
+        for (int i = 0; i < 3; i++) p[i] = Rbo[i * 3] * ts[0] + Rbo[i * 3 + 1] * ts[1] + Rbo[i * 3 + 2] * ts[2] + tb[i] - tr[i];
+        for (int i = 0; i < 9; i++) { S.U[i] = (float)RU[i]; S.RN[i] = (float)RN[i]; }
+        for (int i = 0; i < 3; i++) S.U[9 + i] = (float)(Rref[i] * p[0] + Rref[3 + i] * p[1] + Rref[6 + i] * p[2]);
+    }
+    RES(H->d_cov_part.reserve((size_t)B2_COV_NACC * std::max(H->red_grid, 1))); RES(H->d_cov_rec.reserve(1));
+    if (!H->d_cov_ticket.p) { RES(H->d_cov_ticket.reserve(1)); CU(cudaMemset(H->d_cov_ticket.p, 0, sizeof(unsigned int))); }
+    RES(join_streams(sc, ns, true));
+    k_micp_information<<<grid, B2_COV_BLOCK, 0, H->stream>>>(L, H->d_cov_part.p, H->d_cov_ticket.p, H->d_cov_rec.p);
+    LAUNCHED();
+    b2_micp_covariance rec;
+    CU(cudaMemcpyAsync(&rec, H->d_cov_rec.p, sizeof(rec), cudaMemcpyDeviceToHost, H->stream));
+    RES(join_streams(sc, ns, false));
+    CU(cudaStreamSynchronize(H->stream));
+    *out_host = rec;
     return B2_OK;
 }
 

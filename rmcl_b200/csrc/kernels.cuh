@@ -2360,4 +2360,210 @@ __global__ void __launch_bounds__(256) k_pf_cluster_gather(const uint32_t* __res
 }
 #endif
 
+// ---------------------------------------------------------------------------------------------------------------------
+// b2_micp_pose_covariance (SURVEY appendix I): the point-to-plane information of a correction's final correspondences, in the body frame of
+// the published pose, and its covariance
+// ---------------------------------------------------------------------------------------------------------------------
+#define B2_COV_NACC 24                 // per sensor: the 21 entries of J J^T on and above the diagonal (row-major), r^2, |q|^2, pairs
+#define B2_COV_BLOCK 256
+#define B2_COV_SENSORS 4               // = B2_MAX_SENSORS, the n_pairs of the record
+struct MicpCovSensor {
+    const float* dpts; const uint8_t* dmask; const float* mpts; const float* mnrm; const uint8_t* mmask;
+    b2_transform Tpre;                 // T_snew_sold = Tso * T_onew_oold * Tos, as the ICP loop composes it
+    float U[12];                       // ~Tbo_ref * Tbo * Tsb: rotation row-major, then translation (dataset point -> reference body frame)
+    float RN[9];                       // R(U) R(Tpre)^T, row-major (model normal -> reference body frame)
+    float max_dist;
+    uint32_t n, blk0, nblk;            // pairs; blocks [blk0, blk0 + nblk)
+    double weight;
+};
+struct MicpCovLaunch { MicpCovSensor s[B2_COV_SENSORS]; uint32_t n_sensors; double tau, degenerate_variance; };
+
+// one accepted pair: q = U d, n = RN N, J = (n, q x n) in float, the sums in FP64
+B2_DEV void micp_cov_add_pair(double* a, const float* U, const float* RN, V3 d, V3 N, float r)
+{
+    const V3 q = mk3(add(add(add(mul(U[0], d.x), mul(U[1], d.y)), mul(U[2], d.z)), U[9]),
+                     add(add(add(mul(U[3], d.x), mul(U[4], d.y)), mul(U[5], d.z)), U[10]),
+                     add(add(add(mul(U[6], d.x), mul(U[7], d.y)), mul(U[8], d.z)), U[11]));
+    const V3 n = mk3(add(add(mul(RN[0], N.x), mul(RN[1], N.y)), mul(RN[2], N.z)),
+                     add(add(mul(RN[3], N.x), mul(RN[4], N.y)), mul(RN[5], N.z)),
+                     add(add(mul(RN[6], N.x), mul(RN[7], N.y)), mul(RN[8], N.z)));
+    const double J[6] = {(double)n.x, (double)n.y, (double)n.z, (double)sub(mul(q.y, n.z), mul(q.z, n.y)),
+                         (double)sub(mul(q.z, n.x), mul(q.x, n.z)), (double)sub(mul(q.x, n.y), mul(q.y, n.x))};
+    int e = 0;
+    #pragma unroll
+    for (int i = 0; i < 6; i++)
+        #pragma unroll
+        for (int j = i; j < 6; j++) a[e++] += J[i] * J[j];
+    a[21] += (double)r * (double)r;
+    a[22] += (double)q.x * (double)q.x + (double)q.y * (double)q.y + (double)q.z * (double)q.z;
+    a[23] += 1.0;
+}
+
+// The record from the per-sensor sums (sums[k * B2_COV_NACC ..]): weighted information, scaling, cyclic Jacobi, pseudo-inverse.  One thread.
+// The main loops stay rolled so that the 6x6 arrays live in local memory: unrolled, they would take ~160 registers of the calling kernel.
+B2_DEV void micp_cov_finalize(const double* sums, const double* weights, uint32_t n_sensors, double tau, double degenerate_variance, b2_micp_covariance* o)
+{
+#if B2_ON_DEVICE
+    const double qnan = __longlong_as_double(0x7ff8000000000000ll);
+#else
+    const double qnan = std::nan("");
+#endif
+    double H[36], R2 = 0.0, Q2 = 0.0, W = 0.0;
+    for (int i = 0; i < 36; i++) H[i] = 0.0;
+    for (int k = 0; k < B2_COV_SENSORS; k++) o->n_pairs[k] = 0;
+    #pragma unroll 1
+    for (uint32_t k = 0; k < n_sensors; k++) {
+        const double* s = sums + (size_t)k * B2_COV_NACC;
+        const double w = weights[k];
+        int e = 0;
+        #pragma unroll 1
+        for (int i = 0; i < 6; i++) for (int j = i; j < 6; j++) H[i * 6 + j] += w * s[e++];
+        R2 += w * s[21]; Q2 += w * s[22]; W += w * s[23];
+        o->n_pairs[k] = (uint64_t)s[23];
+    }
+    #pragma unroll 1
+    for (int i = 1; i < 6; i++) for (int j = 0; j < i; j++) H[i * 6 + j] = H[j * 6 + i];
+    for (int i = 0; i < 36; i++) o->information[i] = H[i];
+    o->residual_sq_sum = R2; o->weight_sum = W;
+    o->sigma2 = W > 6.0 ? R2 / (W - 6.0) : qnan;
+    if (!(W > 0.0)) {                                              // no pairs: nothing is known
+        for (int i = 0; i < 36; i++) { o->eigenvectors[i] = 0.0; o->covariance[i] = qnan; }
+        for (int i = 0; i < 6; i++) o->eigenvalues[i] = 0.0;
+        o->length_scale = 0.0; o->n_degenerate = 6; o->degenerate_mask = 0x3f;
+        return;
+    }
+    double L = sqrt(Q2 / W);
+    if (!(L > 0.0)) L = 1.0;
+    const double sc[6] = {1.0, 1.0, 1.0, 1.0 / L, 1.0 / L, 1.0 / L};
+    double A[36], V[36], total = 0.0;
+    #pragma unroll 1
+    for (int i = 0; i < 6; i++) for (int j = 0; j < 6; j++) { A[i * 6 + j] = sc[i] * H[i * 6 + j] * sc[j]; V[i * 6 + j] = i == j ? 1.0 : 0.0; }
+    for (int i = 0; i < 36; i++) total += A[i] * A[i];
+    // cyclic Jacobi: rotation (p, q) zeroes A[p][q] (theta = (a_qq - a_pp) / (2 a_pq), t = tan of the smaller angle); at most 32 sweeps, until the
+    // off-diagonal sum of squares is at most 1e-30 of the whole (an off-diagonal entry 1e-15 of the norm)
+    #pragma unroll 1
+    for (int sweep = 0; sweep < 32; sweep++) {
+        double off = 0.0;
+        #pragma unroll 1
+        for (int p = 0; p < 5; p++) for (int q = p + 1; q < 6; q++) off += A[p * 6 + q] * A[p * 6 + q];
+        if (!(off > 1e-30 * total)) break;
+        #pragma unroll 1
+        for (int p = 0; p < 5; p++) for (int q = p + 1; q < 6; q++) {
+            const double apq = A[p * 6 + q];
+            if (apq == 0.0) continue;
+            const double theta = (A[q * 6 + q] - A[p * 6 + p]) / (2.0 * apq);
+            const double t = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
+            const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+            for (int k = 0; k < 6; k++) { const double x = A[k * 6 + p], y = A[k * 6 + q]; A[k * 6 + p] = c * x - s * y; A[k * 6 + q] = s * x + c * y; }
+            for (int k = 0; k < 6; k++) { const double x = A[p * 6 + k], y = A[q * 6 + k]; A[p * 6 + k] = c * x - s * y; A[q * 6 + k] = s * x + c * y; }
+            for (int k = 0; k < 6; k++) { const double x = V[k * 6 + p], y = V[k * 6 + q]; V[k * 6 + p] = c * x - s * y; V[k * 6 + q] = s * x + c * y; }
+            A[p * 6 + q] = 0.0; A[q * 6 + p] = 0.0;
+        }
+    }
+    int idx[6] = {0, 1, 2, 3, 4, 5};
+    #pragma unroll 1
+    for (int a = 0; a < 5; a++) for (int b = a + 1; b < 6; b++) if (A[idx[b] * 7] < A[idx[a] * 7]) { const int t = idx[a]; idx[a] = idx[b]; idx[b] = t; }
+    double lam[6], ev[36];
+    #pragma unroll 1
+    for (int i = 0; i < 6; i++) {
+        lam[i] = A[idx[i] * 7];
+        int m = 0;
+        for (int k = 1; k < 6; k++) if (fabs(V[k * 6 + idx[i]]) > fabs(V[m * 6 + idx[i]])) m = k;
+        const double sg = V[m * 6 + idx[i]] < 0.0 ? -1.0 : 1.0;
+        for (int k = 0; k < 6; k++) ev[i * 6 + k] = sg * V[k * 6 + idx[i]];
+    }
+    double Cs[36];
+    for (int i = 0; i < 36; i++) Cs[i] = 0.0;
+    uint32_t mask = 0, n_deg = 0;
+    #pragma unroll 1
+    for (int i = 0; i < 6; i++) {
+        const bool deg = lam[i] <= tau * lam[5];
+        if (deg) { mask |= 1u << i; n_deg++; }
+        const double f = deg ? degenerate_variance : o->sigma2 / lam[i];
+        #pragma unroll 1
+        for (int a = 0; a < 6; a++) for (int b = 0; b < 6; b++) Cs[a * 6 + b] += f * (ev[i * 6 + a] * ev[i * 6 + b]);
+    }
+    for (int a = 0; a < 6; a++) for (int b = 0; b < 6; b++) o->covariance[a * 6 + b] = sc[a] * Cs[a * 6 + b] * sc[b];
+    for (int i = 0; i < 6; i++) o->eigenvalues[i] = lam[i];
+    for (int i = 0; i < 36; i++) o->eigenvectors[i] = ev[i];
+    o->length_scale = L; o->n_degenerate = n_deg; o->degenerate_mask = mask;
+}
+
+#if defined(__CUDACC__)
+// One launch over all sensors; blocks [blk0, blk0 + nblk) read sensor k's pairs with k_p2l_reduce's loads and gate.  Block partials go to
+// `partials`; the last block to finish sums them per sensor in a fixed order (repeated calls give the same bytes) and writes the record.
+__global__ void __launch_bounds__(B2_COV_BLOCK) k_micp_information(const __grid_constant__ MicpCovLaunch L, double* __restrict__ partials,
+                                                                   unsigned int* __restrict__ ticket, b2_micp_covariance* __restrict__ out)
+{
+    constexpr int NW = B2_COV_BLOCK / 32, NG = B2_COV_BLOCK / B2_COV_NACC;
+    __shared__ double smem[B2_COV_NACC][NW];
+    __shared__ double s_grp[NG][B2_COV_NACC];
+    __shared__ double s_sum[B2_COV_SENSORS][B2_COV_NACC];
+    __shared__ bool is_last;
+    double acc[B2_COV_NACC];
+    #pragma unroll
+    for (int j = 0; j < B2_COV_NACC; j++) acc[j] = 0.0;
+    for (uint32_t k = 0; k < L.n_sensors; k++) {
+        const MicpCovSensor& S = L.s[k];
+        if (blockIdx.x < S.blk0 || blockIdx.x >= S.blk0 + S.nblk) continue;
+        const Tf Tpre = tf_from_pod(S.Tpre);
+        const uint32_t stride = S.nblk * B2_COV_BLOCK;
+        #pragma unroll 1
+        for (uint32_t i = (blockIdx.x - S.blk0) * B2_COV_BLOCK + threadIdx.x; i < S.n; i += stride) {
+            const uint8_t dm = S.dmask[i], mm = S.mmask[i];
+            const V3 d = mk3(S.dpts[3 * i], S.dpts[3 * i + 1], S.dpts[3 * i + 2]);
+            const V3 I = mk3(S.mpts[3 * i], S.mpts[3 * i + 1], S.mpts[3 * i + 2]);
+            const V3 N = mk3(S.mnrm[3 * i], S.mnrm[3 * i + 1], S.mnrm[3 * i + 2]);
+            V3 D, M;
+            if ((dm > 0) && (mm > 0) && p2l_pair(Tpre, d, I, N, S.max_dist, D, M)) micp_cov_add_pair(acc, S.U, S.RN, d, N, v_dot(v_sub(I, D), N));
+        }
+    }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    #pragma unroll
+    for (int j = 0; j < B2_COV_NACC; j++) {
+        double v = acc[j];
+        #pragma unroll
+        for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+        if (lane == 0) smem[j][warp] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < B2_COV_NACC) {
+        double x = 0.0;
+        #pragma unroll
+        for (int w = 0; w < NW; w++) x += smem[threadIdx.x][w];
+        partials[(size_t)blockIdx.x * B2_COV_NACC + threadIdx.x] = x;
+        __threadfence();
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) is_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+    __syncthreads();
+    if (!is_last) return;
+    __threadfence();
+    // per sensor: thread (g, i) adds value i of blocks blk0 + g, blk0 + g + NG, ...; then the NG group sums in order
+    for (uint32_t k = 0; k < L.n_sensors; k++) {
+        const MicpCovSensor& S = L.s[k];
+        if (threadIdx.x < NG * B2_COV_NACC) {
+            const uint32_t i = threadIdx.x % B2_COV_NACC, g = threadIdx.x / B2_COV_NACC;
+            double a = 0.0;
+            for (uint32_t b = S.blk0 + g; b < S.blk0 + S.nblk; b += NG) a += __ldcg(partials + (size_t)b * B2_COV_NACC + i);
+            s_grp[g][i] = a;
+        }
+        __syncthreads();
+        if (threadIdx.x < B2_COV_NACC) {
+            double a = 0.0;
+            #pragma unroll
+            for (int g = 0; g < NG; g++) a += s_grp[g][threadIdx.x];
+            s_sum[k][threadIdx.x] = a;
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        double w[B2_COV_SENSORS];
+        for (uint32_t k = 0; k < L.n_sensors; k++) w[k] = L.s[k].weight;
+        micp_cov_finalize(&s_sum[0][0], w, L.n_sensors, L.tau, L.degenerate_variance, out);
+        *ticket = 0u;
+    }
+}
+#endif
+
 #include "icp_loop.cuh"
