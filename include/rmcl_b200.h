@@ -556,6 +556,60 @@ B2_API int b2_pf_cluster_stats(b2_pf* h, const b2_transform* poses_dev, const b2
 typedef struct { float probe_above, probe_below, base_height, max_slope; int32_t align; } b2_surface_config;      /* 20 B */
 B2_API int b2_pf_project_to_surface(b2_pf* h, b2_transform* poses_dev, b2_particle_attr* attrs_dev, uint32_t n_particles, const b2_surface_config* cfg);
 
+/* Recovery from a kidnapping: Augmented MCL (Thrun, Burgard, Fox, Probabilistic Robotics, 8.3.5; AMCL's recovery_alpha_slow / _fast; no
+ * reference implementation, SURVEY appendix J).  A converged set only copies and perturbs its own particles, so once the robot is lifted,
+ * slips or its odometry jumps, nothing puts a particle where it really is.  These calls keep a slow and a fast average of the set's mean
+ * likelihood and, when the fast one drops below the slow one, replace a fraction p = max(0, 1 - w_fast / w_slow) of the particles with
+ * random poses.  One cycle: motion, sensor update, b2_pf_recovery_observe, resampling, b2_pf_recovery_inject, (surface projection).
+ * The handle keeps a device-resident record {w_slow, w_fast, p_inject}, zero at creation.
+ *
+ * b2_pf_recovery_reset: sets the record to 0, enqueued on the handle's stream.  Call it after (re)initialising the set.
+ *
+ * b2_pf_recovery_observe: call it once after each sensor update, on the whole set (a sharded set passes the all-gathered set, as
+ * b2_pf_resample_kld takes it, so every rank holds the same record).
+ *  - w_avg = S / n, S the FP64 sum of likelihood.mean that b2_pf_resample_residual computes (bit-equal to b2_pf_estimate_stats' sum).
+ *    likelihood.mean is the filter's running, forgotten fit, not the latest scan's likelihood: the recovery reacts at the pace the forget
+ *    settings give the filter's memory.
+ *  - w_avg not finite or below 0: the record is left unchanged.  Otherwise each average w of rate alpha becomes w_avg when w == 0, else
+ *    w + alpha (w_avg - w); then p_inject = w_slow > 0 ? max(0, 1 - w_fast / w_slow) : 0, all in FP64.
+ *  - One statistics pass and a one-thread update kernel that reads its result in device memory: no read-back.  state_host (may be NULL)
+ *    receives {w_avg, w_slow, w_fast, p_inject} and the call synchronises; otherwise it only enqueues.
+ *  Refused (B2_ERR_INVALID, no launch): null h, attrs_dev or cfg; n == 0; an alpha not finite or outside [0, 1]; alpha_slow > alpha_fast.
+ *  Suggested values: alpha_slow 0.001, alpha_fast 0.1 (AMCL's recovery_alpha_slow / _fast).
+ *
+ * b2_pf_recovery_inject: call it after resampling.  In place on the slice [first, first + n_local) of the set (poses_dev / attrs_dev hold
+ * n_local entries, DEVICE pointers), with p = p_inject read from the record on the device.  Particle g (global index), Philox4x32-10 with key
+ * `seed` and counter (g, 7, step, block):
+ *  1. replaced iff (double)word0 of block 0 * 2^-32 < p (p == 0: nothing is touched);
+ *  2. try t < max_tries draws the six words 0-3 of block 1 + 2t and 0-1 of block 2 + 2t and maps them into the box [bb_min, bb_max] (x, y,
+ *     z, roll, pitch, yaw) as b2_pf_init_uniform does;
+ *  3. surface NULL: the first candidate is taken.  Otherwise a candidate is taken iff b2_pf_project_to_surface's rule finds ground under it,
+ *     and it is taken as that rule moved it;
+ *  4. a taken candidate overwrites the pose (stamp 0, as the initialiser writes it) and the attributes become {mean 0, sigma 0, n_meas 0},
+ *     state_sigma 0: an unevaluated particle carries no weight in the estimates and resamplers until the next sensor update, whose merge
+ *     takes the fresh likelihood alone.  (The wall check's mark is {0, 0, MAX_N_MEAS}.)
+ *  5. no candidate taken within max_tries: the particle stays exactly as it was and counts as failed.
+ * After the call, if p > 0, the record is reset to 0 (AMCL resets the averages after it injects, so that it does not spiral into complete
+ * randomness).  out_host (may be NULL) receives {p used, n_replaced, n_failed} of the slice and the call synchronises; otherwise it only
+ * enqueues.  Draws depend on (seed, step, g, try) only, so slices concatenate to the whole result bit for bit.  n_local == 0 launches nothing
+ * and so leaves the record as it is: in a sharded set give every rank a non-empty slice (equal shards do), or a rank with an empty one keeps
+ * p > 0 while the others reset, and their records differ from then on.
+ * Limit: the surface test puts a candidate on walkable ground; it does not prove the robot fits there (under a table, say).
+ *  Refused (B2_ERR_INVALID, no launch, buffers untouched): null h, bb_min or bb_max; the box refusals of b2_pf_init_uniform; the refusals
+ *  of b2_pf_project_to_surface when surface is given; max_tries outside [1, 64]; null buffers with n_local > 0; first + n_local > 2^32.
+ *  Suggested values: max_tries 16; the map's box with roll and pitch 0 and yaw [-pi, pi); b2_pf_project_to_surface's suggested config. */
+typedef struct { double alpha_slow, alpha_fast; } b2_recovery_config;                                          /* 16 B */
+typedef char b2_recovery_config_is_16_bytes[sizeof(b2_recovery_config) == 16 ? 1 : -1];
+typedef struct { double w_avg, w_slow, w_fast, p_inject; } b2_recovery_state;                                  /* 32 B */
+typedef char b2_recovery_state_is_32_bytes[sizeof(b2_recovery_state) == 32 ? 1 : -1];
+typedef struct { double p_inject; uint64_t n_replaced, n_failed; } b2_recovery_result;                         /* 24 B */
+typedef char b2_recovery_result_is_24_bytes[sizeof(b2_recovery_result) == 24 ? 1 : -1];
+B2_API int b2_pf_recovery_reset(b2_pf* h);
+B2_API int b2_pf_recovery_observe(b2_pf* h, const b2_particle_attr* attrs_dev, uint32_t n, const b2_recovery_config* cfg, b2_recovery_state* state_host /* nullable */);
+B2_API int b2_pf_recovery_inject(b2_pf* h, b2_transform* poses_dev, b2_particle_attr* attrs_dev, uint32_t first, uint32_t n_local, const double bb_min[6],
+                                 const double bb_max[6], const b2_surface_config* surface /* nullable */, uint32_t max_tries, uint64_t seed, uint32_t step,
+                                 b2_recovery_result* out_host /* nullable */);
+
 /* ---------------------------------------------------------------- introspection ------------------------------ */
 /* CUDA-event timing of the kernels inside b2_rcc_correct_once*(): when enabled, events are recorded on the handle's stream around the
  * find kernel and around the reduction/Umeyama kernels; b2_rcc_last_timing returns the two durations of the most recent call (ms). */

@@ -422,6 +422,28 @@ public:
         b2_check(b2_pf_project_to_surface(h_, reinterpret_cast<b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(), &cfg),
                  "projectToSurface");
     }
+    // Recovery from a kidnapping (Augmented MCL, b2_pf_recovery_*): recoveryObserve after each update keeps a slow and a fast average of the
+    // set's mean likelihood at recovery_config's rates (AMCL's recovery_alpha_slow / _fast); recoveryInject after resampling replaces a
+    // fraction p_inject = max(0, 1 - w_fast / w_slow) of the particles with random poses of the box (on the map's ground when `surface` is
+    // given).  Call recoveryReset after (re)initialising the set.  With want_state / want_result the call reads the record back into
+    // last_recovery_state / last_recovery and synchronises; otherwise it only enqueues.
+    b2_recovery_config recovery_config{0.001, 0.1};
+    b2_recovery_state last_recovery_state{};
+    b2_recovery_result last_recovery{};
+    void recoveryReset() { b2_check(b2_pf_recovery_reset(h_), "recoveryReset"); }
+    void recoveryObserve(rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs, bool want_state = false)
+    {
+        b2_check(b2_pf_recovery_observe(h_, reinterpret_cast<const b2_particle_attr*>(attrs.raw()), (uint32_t)attrs.size(), &recovery_config,
+                                        want_state ? &last_recovery_state : nullptr), "recoveryObserve");
+    }
+    void recoveryInject(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs,
+                        const std::array<double, 6>& bb_min, const std::array<double, 6>& bb_max, const b2_surface_config* surface = nullptr,
+                        uint32_t max_tries = 16, uint64_t seed = 1234, uint32_t step = 0, uint32_t first = 0, bool want_result = false)
+    {
+        if (poses.size() != attrs.size()) throw std::invalid_argument("recoveryInject: poses and attrs differ in size");
+        b2_check(b2_pf_recovery_inject(h_, reinterpret_cast<b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), first, (uint32_t)poses.size(),
+                                       bb_min.data(), bb_max.data(), surface, max_tries, seed, step, want_result ? &last_recovery : nullptr), "recoveryInject");
+    }
     struct SimpleLikelihoodStats { float sum = 0.0f; float max = -1.0f; };                       // resampling.cuh:26-30
     SimpleLikelihoodStats computeStats(rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs)
     {

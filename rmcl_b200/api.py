@@ -10,7 +10,8 @@ import os
 
 import numpy as np
 
-from .synth import CLUSTER_RECORD_DTYPE, CLUSTER_RESULT_DTYPE, CROSS_STATS_DTYPE, KLD_RESULT_DTYPE, PARTICLE_ATTR_DTYPE, PARTICLE_STATS_DTYPE, RANGE_MEAS_DTYPE, RESIDUAL_RESULT_DTYPE, TRANSFORM_DTYPE
+from .synth import (CLUSTER_RECORD_DTYPE, CLUSTER_RESULT_DTYPE, CROSS_STATS_DTYPE, KLD_RESULT_DTYPE, PARTICLE_ATTR_DTYPE, PARTICLE_STATS_DTYPE, RANGE_MEAS_DTYPE,
+                    RECOVERY_RESULT_DTYPE, RECOVERY_STATE_DTYPE, RESIDUAL_RESULT_DTYPE, TRANSFORM_DTYPE)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.environ.get("B2_LIB_PATH") or os.path.join(_HERE, "lib", "librmcl_b200.so")     # B2_LIB_PATH: experiment builds (scripts/)
@@ -93,6 +94,16 @@ class ClusterConfig(C.Structure):
         return ClusterConfig(0.5, 0.0, math.radians(10.0), 8)
 
 
+class RecoveryConfig(C.Structure):
+    """b2_recovery_config: the rates of the slow and the fast average of the recovery (recoveryObserve), 0 <= alpha_slow <= alpha_fast <= 1.
+    defaults() are AMCL's recovery_alpha_slow and recovery_alpha_fast."""
+    _fields_ = [("alpha_slow", C.c_double), ("alpha_fast", C.c_double)]
+
+    @staticmethod
+    def defaults():
+        return RecoveryConfig(0.001, 0.1)
+
+
 class _CloudLayout(C.Structure):
     _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("point_step", C.c_uint32), ("row_step", C.c_uint32), ("offset_x", C.c_uint32),
                 ("offset_y", C.c_uint32), ("offset_z", C.c_uint32), ("datatype", C.c_uint8), ("is_bigendian", C.c_uint8), ("pad", C.c_uint8 * 2)]
@@ -157,7 +168,8 @@ EXPORTS = [
     "b2_rcc_correct_once_async", "b2_rcc_correct_once_wait", "b2_micp_correct_once", "b2_rcc_set_exec_mode", "b2_debug_read_bandwidth", "b2_rcc_set_sim_options", "b2_rcc_bind_dataset", "b2_rcc_bind_model_buffers", "b2_rcc_benchmark_batch", "b2_pf_p2p_init", "b2_pf_p2p_connect", "b2_pf_p2p_publish", "b2_pf_resample_gladiator_p2p", "b2_pf_p2p_connect_local", "b2_rcc_set_cpc_options", "b2_pf_set_mapping", "b2_pf_get_mapping",
     "b2_micp_correct", "b2_pf_init_uniform", "b2_pf_init_gaussian", "b2_pf_estimate_stats", "b2_rcc_set_cloud_o1dn",
     "b2_rcc_set_cloud_spherical", "b2_pf_sample_cloud", "b2_pf_resample_residual", "b2_pf_project_to_surface",
-    "b2_pf_resample_kld", "b2_pf_cluster_stats", "b2_micp_pose_covariance",
+    "b2_pf_resample_kld", "b2_pf_cluster_stats", "b2_micp_pose_covariance", "b2_pf_recovery_reset", "b2_pf_recovery_observe",
+    "b2_pf_recovery_inject",
 ]
 
 
@@ -883,6 +895,41 @@ class PCDSensorUpdaterB200:
         _chk(load_library().b2_pf_cluster_stats(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(n), C.byref(cfg), _p(recs),
                                                 None if labels is None else _devptr(labels), _p(out)))
         return out, recs[:int(out["n_records"])]
+
+    def recoveryReset(self):
+        """Zero the recovery's record {w_slow, w_fast, p_inject} (b2_pf_recovery_reset), on the handle's stream.  Call it after
+        (re)initialising the set: initSamples and initSamplesUniform leave the record as it is."""
+        _chk(load_library().b2_pf_recovery_reset(self._h))
+
+    def recoveryObserve(self, particle_attrs, cfg=None, want_state=False):
+        """Augmented MCL's averages (b2_pf_recovery_observe): call once after each update(), on the whole (n, 9) float32 CUDA tensor of
+        attributes (a sharded set passes the all-gathered set).  The slow and the fast average of the set's mean likelihood follow it at
+        `cfg`'s rates (a RecoveryConfig, default defaults()), and p_inject = max(0, 1 - w_fast / w_slow) is kept on the device for
+        recoveryInject.  want_state: -> a synth.RECOVERY_STATE_DTYPE record (w_avg, w_slow, w_fast, p_inject), read back with a
+        synchronise; otherwise the call only enqueues and returns None."""
+        c = cfg or RecoveryConfig.defaults()
+        n = particle_attrs.numel() * particle_attrs.element_size() // 36
+        out = np.zeros((), RECOVERY_STATE_DTYPE) if want_state else None
+        _chk(load_library().b2_pf_recovery_observe(self._h, _devptr(particle_attrs), C.c_uint32(n), C.byref(c), _p(out)))
+        return out
+
+    def recoveryInject(self, particle_poses, particle_attrs, bb_min, bb_max, surface=None, max_tries=16, seed=1234, step=0, first=0, want_result=False):
+        """Augmented MCL's injection (b2_pf_recovery_inject): call after resampling.  In place on the (n, 8) / (n, 9) float32 CUDA tensors,
+        particles first .. first+n-1 of the set: each is replaced with the probability p_inject of the last recoveryObserve by a pose drawn
+        uniformly from the box (x, y, z, roll, pitch, yaw) as initSamplesUniform draws it; with `surface` (a SurfaceConfig) a candidate is
+        taken only where projectToSurface finds ground, as it moves it, and up to max_tries candidates are drawn.  A replaced particle has
+        the likelihood {0, 0, 0}: no weight until the next update() evaluates it.  After an injection the averages restart from 0.
+        want_result: -> a synth.RECOVERY_RESULT_DTYPE record (p_inject, n_replaced, n_failed), read back with a synchronise; otherwise the
+        call only enqueues and returns None."""
+        lo, hi = np.ascontiguousarray(bb_min, np.float64).reshape(6), np.ascontiguousarray(bb_max, np.float64).reshape(6)
+        n = particle_poses.numel() * particle_poses.element_size() // 32
+        if particle_attrs.numel() * particle_attrs.element_size() != 36 * n:
+            raise ValueError("recoveryInject: poses and attrs differ in length")
+        out = np.zeros((), RECOVERY_RESULT_DTYPE) if want_result else None
+        _chk(load_library().b2_pf_recovery_inject(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(first), C.c_uint32(n), _p(lo), _p(hi),
+                                                  None if surface is None else C.byref(surface), C.c_uint32(max_tries), C.c_uint64(seed),
+                                                  C.c_uint32(step), _p(out)))
+        return out
 
     def gladiatorRandoms(self, seed, step, first, n, device=None):
         """The draws resample() uses for champions first..first+n-1 (raw u32 opponent word + 6 normals each), as torch CUDA tensors."""

@@ -1909,6 +1909,9 @@ struct b2_pf {
     DevBuf<unsigned long long> d_cl_w; DevBuf<unsigned int> d_cl_cnt, d_cl_aux; DevBuf<uint32_t> d_cl_slot, d_cl_key, d_cl_key2, d_cl_idx, d_cl_idx2;
     DevBuf<b2_transform> d_cl_poses; DevBuf<b2_particle_attr> d_cl_attrs; DevBuf<PfClusterHead> d_cl_heads; DevBuf<b2_particle_stats> d_cl_recs;
     DevBuf<PfClusterState> d_cl; unsigned char* h_cl = nullptr;
+    // recovery (b2_pf_recovery_*), allocated at the first of its calls: the record {w_avg, w_slow, w_fast, p_inject}, the result of an
+    // injection, and one pinned host block for either read-back
+    DevBuf<b2_recovery_state> d_rec; DevBuf<b2_recovery_result> d_rec_res; unsigned char* h_rec = nullptr;
 };
 
 extern "C" int b2_pf_destroy(b2_pf* h);
@@ -1978,6 +1981,8 @@ extern "C" int b2_pf_destroy(b2_pf* h)
     h->d_cl_w.release(); h->d_cl_cnt.release(); h->d_cl_aux.release(); h->d_cl_slot.release(); h->d_cl_key.release(); h->d_cl_key2.release(); h->d_cl_idx.release();
     h->d_cl_idx2.release(); h->d_cl_poses.release(); h->d_cl_attrs.release(); h->d_cl_heads.release(); h->d_cl_recs.release(); h->d_cl.release();
     if (h->h_cl) cudaFreeHost(h->h_cl);
+    h->d_rec.release(); h->d_rec_res.release();
+    if (h->h_rec) cudaFreeHost(h->h_rec);
     b2_mesh* map = h->map;
     delete h;
     (void)cudaGetLastError();
@@ -2233,23 +2238,31 @@ extern "C" int b2_pf_motion_update(b2_pf* h, b2_transform* poses_dev, b2_particl
     return B2_OK;
 }
 
+// the checks of a surface config (`what` names the caller in the message), and the constants the rule takes from it
+static int surface_config_check(const b2_surface_config& c, const char* what, float* cos_max, float* tfar)
+{
+    const float f[4] = {c.probe_above, c.probe_below, c.base_height, c.max_slope};
+    if (!all_finite(f, 4)) return fail(B2_ERR_INVALID, "%s: a config field is not finite (%g, %g, %g, %g)", what, f[0], f[1], f[2], f[3]);
+    *tfar = c.probe_above + c.probe_below;
+    if (c.probe_above < 0.0f || c.probe_below < 0.0f || !(*tfar > 0.0f))
+        return fail(B2_ERR_INVALID, "%s: probe_above %g and probe_below %g must be >= 0 with a positive sum", what, f[0], f[1]);
+    if (c.base_height < 0.0f) return fail(B2_ERR_INVALID, "%s: base_height %g < 0", what, f[2]);
+    if (!(c.max_slope >= 0.0f && c.max_slope <= (float)1.5707963267948966))           // pi/2 rounded to float, as a caller passes it
+        return fail(B2_ERR_INVALID, "%s: max_slope %g outside [0, pi/2]", what, f[3]);
+    if (c.align != 0 && c.align != 1) return fail(B2_ERR_INVALID, "%s: align is 0 or 1, not %d", what, (int)c.align);
+    *cos_max = (float)std::cos((double)c.max_slope);
+    return B2_OK;
+}
+
 // the motion stage's surface constraint (docs/RMCL.md:72; SURVEY appendix F): one downward ray per particle, in place
 extern "C" int b2_pf_project_to_surface(b2_pf* h, b2_transform* poses_dev, b2_particle_attr* attrs_dev, uint32_t n, const b2_surface_config* cfg)
 {
     NOTNULL(h); NOTNULL(cfg);
     if (n > 0) { NOTNULL(poses_dev); NOTNULL(attrs_dev); }
     const b2_surface_config c = *cfg;
-    const float f[4] = {c.probe_above, c.probe_below, c.base_height, c.max_slope};
-    if (!all_finite(f, 4)) return fail(B2_ERR_INVALID, "project to surface: a config field is not finite (%g, %g, %g, %g)", f[0], f[1], f[2], f[3]);
-    const float tfar = c.probe_above + c.probe_below;
-    if (c.probe_above < 0.0f || c.probe_below < 0.0f || !(tfar > 0.0f))
-        return fail(B2_ERR_INVALID, "project to surface: probe_above %g and probe_below %g must be >= 0 with a positive sum", f[0], f[1]);
-    if (c.base_height < 0.0f) return fail(B2_ERR_INVALID, "project to surface: base_height %g < 0", f[2]);
-    if (!(c.max_slope >= 0.0f && c.max_slope <= (float)1.5707963267948966))           // pi/2 rounded to float, as a caller passes it
-        return fail(B2_ERR_INVALID, "project to surface: max_slope %g outside [0, pi/2]", f[3]);
-    if (c.align != 0 && c.align != 1) return fail(B2_ERR_INVALID, "project to surface: align is 0 or 1, not %d", (int)c.align);
+    float cos_max, tfar;
+    RES(surface_config_check(c, "project to surface", &cos_max, &tfar));
     if (n == 0) return B2_OK;
-    const float cos_max = (float)std::cos((double)c.max_slope);
     CU(cudaSetDevice(h->map->device));
     k_pf_surface<<<(n + 127) / 128, 128, 0, h->stream>>>(h->map->view(), poses_dev, attrs_dev, n, c, cos_max, tfar);
     LAUNCHED();
@@ -2384,19 +2397,26 @@ static int pf_init_range(uint32_t first, uint32_t n)
     return B2_OK;
 }
 
+// the box of the uniform initialiser and of the recovery's candidates, narrowed to float and checked (`what` names the caller)
+static int pf_box_check(const double* bb_min, const double* bb_max, const char* what, PfInitBox* box)
+{
+    static const char* dim[6] = {"x", "y", "z", "roll", "pitch", "yaw"};
+    for (int k = 0; k < 6; k++) {
+        box->lo[k] = (float)bb_min[k]; box->hi[k] = (float)bb_max[k];         // uniform_real_distribution<float> of the double parameters
+        if (!std::isfinite(box->lo[k]) || !std::isfinite(box->hi[k]))
+            return fail(B2_ERR_INVALID, "%s: %s bounds [%g, %g] are not finite in float", what, dim[k], bb_min[k], bb_max[k]);
+        if (box->lo[k] > box->hi[k]) return fail(B2_ERR_INVALID, "%s: %s bounds [%g, %g] have min > max", what, dim[k], bb_min[k], bb_max[k]);
+        if (!std::isfinite(box->hi[k] - box->lo[k])) return fail(B2_ERR_INVALID, "%s: the %s extent %g overflows float", what, dim[k], bb_max[k] - bb_min[k]);
+    }
+    return B2_OK;
+}
+
 extern "C" int b2_pf_init_uniform(b2_pf* h, b2_transform* poses_dev, b2_particle_attr* attrs_dev, uint32_t first, uint32_t n, const double* bb_min, const double* bb_max,
                                   uint64_t seed)
 {
     NOTNULL(h); NOTNULL(bb_min); NOTNULL(bb_max);
-    static const char* dim[6] = {"x", "y", "z", "roll", "pitch", "yaw"};
     PfInitBox box;
-    for (int k = 0; k < 6; k++) {
-        box.lo[k] = (float)bb_min[k]; box.hi[k] = (float)bb_max[k];           // uniform_real_distribution<float> of the double parameters
-        if (!std::isfinite(box.lo[k]) || !std::isfinite(box.hi[k]))
-            return fail(B2_ERR_INVALID, "init uniform: %s bounds [%g, %g] are not finite in float", dim[k], bb_min[k], bb_max[k]);
-        if (box.lo[k] > box.hi[k]) return fail(B2_ERR_INVALID, "init uniform: %s bounds [%g, %g] have min > max", dim[k], bb_min[k], bb_max[k]);
-        if (!std::isfinite(box.hi[k] - box.lo[k])) return fail(B2_ERR_INVALID, "init uniform: the %s extent %g overflows float", dim[k], bb_max[k] - bb_min[k]);
-    }
+    RES(pf_box_check(bb_min, bb_max, "init uniform", &box));
     RES(pf_init_range(first, n));
     if (n == 0) return B2_OK;
     NOTNULL(poses_dev); NOTNULL(attrs_dev);
@@ -2449,6 +2469,95 @@ extern "C" int b2_pf_init_gaussian(b2_pf* h, b2_transform* poses_dev, b2_particl
     CU(cudaSetDevice(h->map->device));
     k_pf_init_gaussian<<<(n + 255) / 256, 256, 0, h->stream>>>(poses_dev, attrs_dev, first, n, g, seed);
     LAUNCHED();
+    return B2_OK;
+}
+
+// ---- recovery from a kidnapping (Augmented MCL; SURVEY appendix J) ---------------------------------------------------------------------------
+// the record, zeroed on the handle's stream when it is first needed
+static int recovery_record(b2_pf* h)
+{
+    if (h->d_rec.p) return B2_OK;
+    RES(h->d_rec.reserve(1)); RES(h->d_rec_res.reserve(1));
+    CU(cudaMemsetAsync(h->d_rec.p, 0, sizeof(b2_recovery_state), h->stream));
+    CU(cudaMallocHost((void**)&h->h_rec, std::max(sizeof(b2_recovery_state), sizeof(b2_recovery_result))));
+    return B2_OK;
+}
+
+extern "C" int b2_pf_recovery_reset(b2_pf* h)
+{
+    NOTNULL(h);
+    CU(cudaSetDevice(h->map->device));
+    RES(recovery_record(h));
+    CU(cudaMemsetAsync(h->d_rec.p, 0, sizeof(b2_recovery_state), h->stream));
+    return B2_OK;
+}
+
+extern "C" int b2_pf_recovery_observe(b2_pf* h, const b2_particle_attr* attrs_dev, uint32_t n, const b2_recovery_config* cfg, b2_recovery_state* state_host)
+{
+    NOTNULL(h); NOTNULL(attrs_dev); NOTNULL(cfg);
+    if (n == 0) return fail(B2_ERR_INVALID, "recovery observe: no particles (n = 0)");
+    const double as = cfg->alpha_slow, af = cfg->alpha_fast;
+    if (!(std::isfinite(as) && as >= 0.0 && as <= 1.0) || !(std::isfinite(af) && af >= 0.0 && af <= 1.0))
+        return fail(B2_ERR_INVALID, "recovery observe: alpha_slow = %g and alpha_fast = %g must lie in [0, 1]", as, af);
+    if (as > af) return fail(B2_ERR_INVALID, "recovery observe: alpha_slow = %g > alpha_fast = %g", as, af);
+    CU(cudaSetDevice(h->map->device));
+    RES(recovery_record(h));
+    const uint32_t grid = std::min<uint32_t>((uint32_t)h->n_sm * 4u, (n + 255) / 256);
+    if (!h->d_res.p) {
+        RES(h->d_res_part.reserve((size_t)B2_RES_NV * 4 * (size_t)h->n_sm)); RES(h->d_res.reserve(1));
+        CU(cudaMemsetAsync(h->d_res.p, 0, sizeof(PfResidualState), h->stream));
+        CU(cudaMallocHost((void**)&h->h_res, sizeof(PfResidualState)));
+    }
+    k_pf_residual_stats<<<grid, 256, 0, h->stream>>>(attrs_dev, n, h->d_res_part.p, h->d_res.p);
+    LAUNCHED();
+    k_pf_recovery_filter<<<1, 1, 0, h->stream>>>(&h->d_res.p->S, n, as, af, h->d_rec.p);
+    LAUNCHED();
+    if (state_host) {
+        CU(cudaMemcpyAsync(h->h_rec, h->d_rec.p, sizeof(b2_recovery_state), cudaMemcpyDeviceToHost, h->stream));
+        CU(cudaStreamSynchronize(h->stream));
+        memcpy(state_host, h->h_rec, sizeof(b2_recovery_state));
+    }
+    return B2_OK;
+}
+
+extern "C" int b2_pf_recovery_inject(b2_pf* h, b2_transform* poses_dev, b2_particle_attr* attrs_dev, uint32_t first, uint32_t n_local, const double* bb_min,
+                                     const double* bb_max, const b2_surface_config* surface, uint32_t max_tries, uint64_t seed, uint32_t step,
+                                     b2_recovery_result* out_host)
+{
+    NOTNULL(h); NOTNULL(bb_min); NOTNULL(bb_max);
+    PfInitBox box;
+    RES(pf_box_check(bb_min, bb_max, "recovery inject", &box));
+    b2_surface_config sc{};
+    float cos_max = 0.0f, tfar = 0.0f;
+    if (surface) { sc = *surface; RES(surface_config_check(sc, "recovery inject", &cos_max, &tfar)); }
+    if (max_tries < 1 || max_tries > B2_RECOVERY_MAX_TRIES) return fail(B2_ERR_INVALID, "recovery inject: max_tries = %u outside [1, %u]", max_tries, B2_RECOVERY_MAX_TRIES);
+    if (n_local > 0) { NOTNULL(poses_dev); NOTNULL(attrs_dev); }
+    RES(pf_init_range(first, n_local));
+    CU(cudaSetDevice(h->map->device));
+    RES(recovery_record(h));
+    if (n_local == 0) {
+        if (out_host) {                                   // nothing to replace: the p a slice would have used
+            CU(cudaMemcpyAsync(h->h_rec, &h->d_rec.p->p_inject, sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+            CU(cudaStreamSynchronize(h->stream));
+            b2_recovery_result r{0.0, 0, 0};
+            memcpy(&r.p_inject, h->h_rec, sizeof(double));
+            *out_host = r;
+        }
+        return B2_OK;
+    }
+    b2_recovery_result* res = out_host ? h->d_rec_res.p : nullptr;
+    if (res) CU(cudaMemsetAsync(res, 0, sizeof(b2_recovery_result), h->stream));
+    const uint32_t grid = (n_local + 127) / 128;
+    if (surface) k_pf_recovery_inject<true><<<grid, 128, 0, h->stream>>>(h->map->view(), poses_dev, attrs_dev, first, n_local, box, sc, cos_max, tfar, max_tries, seed, step, h->d_rec.p, res);
+    else         k_pf_recovery_inject<false><<<grid, 128, 0, h->stream>>>(h->map->view(), poses_dev, attrs_dev, first, n_local, box, sc, cos_max, tfar, max_tries, seed, step, h->d_rec.p, res);
+    LAUNCHED();
+    k_pf_recovery_clear<<<1, 1, 0, h->stream>>>(h->d_rec.p);
+    LAUNCHED();
+    if (out_host) {
+        CU(cudaMemcpyAsync(h->h_rec, res, sizeof(b2_recovery_result), cudaMemcpyDeviceToHost, h->stream));
+        CU(cudaStreamSynchronize(h->stream));
+        memcpy(out_host, h->h_rec, sizeof(b2_recovery_result));
+    }
     return B2_OK;
 }
 

@@ -1221,9 +1221,9 @@ __global__ void __launch_bounds__(128) k_pf_motion(BvhView bvh, b2_transform* __
 // to face the ray origin, has n.z >= cos_max.  On ground the particle is put base_height over it (along +z, or along n with align, where
 // the smallest rotation also takes the body z-axis onto n); else it keeps its pose and gets the wall check's mark {0, 0, MAX_N_MEAS}.
 // The stamp and the rest of the attributes are left as they are.  cos_max = (float)cos((double)max_slope), tfar = probe_above + probe_below.
-B2_DEV void pf_surface_one(const BvhView& bvh, b2_transform* pose_io, b2_particle_attr* attr_io, const b2_surface_config& cfg, float cos_max, float tfar)
+// pf_surface_pose applies the rule to a pose in registers and reports the ground test; pf_surface_one applies it to a particle in memory.
+B2_DEV bool pf_surface_pose(const BvhView& bvh, Tf& T, const b2_surface_config& cfg, float cos_max, float tfar)
 {
-    const Tf T = tf_load(pose_io);
     const float oz = add(T.t.z, cfg.probe_above);
     HitRec h = trace_init(tfar);
     // A non-finite pose is off surface.  A non-finite origin hits no triangle anyway, but its box tests pass everywhere (fmaxf / fminf drop
@@ -1240,12 +1240,7 @@ B2_DEV void pf_surface_one(const BvhView& bvh, b2_transform* pose_io, b2_particl
         n = v_normalize(tri_ng(bvh, h.tri));
         if (n.z < 0.0f) n = v_neg(n);
     }
-    if (!(h.face != B2_NOFACE && n.z >= cos_max)) {                                   // no hit, too steep, or a NaN normal
-        b2_gaussian1d lk = attr_io->likelihood;
-        lk.mean = 0.0f; lk.sigma = 0.0f; lk.n_meas = 10000u;
-        attr_io->likelihood = lk;
-        return;
-    }
+    if (!(h.face != B2_NOFACE && n.z >= cos_max)) return false;                       // no hit, too steep, or a NaN normal
     const V3 g = mk3(T.t.x, T.t.y, sub(oz, h.t));
     Tf out;
     if (cfg.align) {
@@ -1264,9 +1259,23 @@ B2_DEV void pf_surface_one(const BvhView& bvh, b2_transform* pose_io, b2_particl
         out.R = T.R;
         out.t = mk3(g.x, g.y, add(g.z, cfg.base_height));
     }
+    T = out;
+    return true;
+}
+// true iff the particle stood on ground and was moved; else it is marked
+B2_DEV bool pf_surface_one(const BvhView& bvh, b2_transform* pose_io, b2_particle_attr* attr_io, const b2_surface_config& cfg, float cos_max, float tfar)
+{
+    Tf T = tf_load(pose_io);
+    if (!pf_surface_pose(bvh, T, cfg, cos_max, tfar)) {
+        b2_gaussian1d lk = attr_io->likelihood;
+        lk.mean = 0.0f; lk.sigma = 0.0f; lk.n_meas = 10000u;
+        attr_io->likelihood = lk;
+        return false;
+    }
     // R and t only: the stamp stays
-    pose_io->R.x = out.R.x; pose_io->R.y = out.R.y; pose_io->R.z = out.R.z; pose_io->R.w = out.R.w;
-    pose_io->t.x = out.t.x; pose_io->t.y = out.t.y; pose_io->t.z = out.t.z;
+    pose_io->R.x = T.R.x; pose_io->R.y = T.R.y; pose_io->R.z = T.R.z; pose_io->R.w = T.R.w;
+    pose_io->t.x = T.t.x; pose_io->t.y = T.t.y; pose_io->t.z = T.t.z;
+    return true;
 }
 #ifdef __CUDACC__
 __global__ void __launch_bounds__(128) k_pf_surface(BvhView bvh, b2_transform* __restrict__ poses, b2_particle_attr* __restrict__ attrs, uint32_t n,
@@ -1414,17 +1423,22 @@ B2_DEV void pf_init_attr(b2_particle_attr* a)
     #pragma unroll
     for (int k = 0; k < 6; k++) a->state_sigma[k] = 0.0f;
 }
-// uniform_real_distribution<float>(lo, hi) per dimension (:287-292, :318-319): lo + (hi - lo) u, u in [0, 1), never above hi
+// uniform_real_distribution<float>(lo, hi) per dimension (:287-292, :318-319): lo + (hi - lo) u, u in [0, 1), never above hi; words r[0..5]
+// give x, y, z, roll, pitch, yaw, the angles Euler ZYX.  Shared by the initialiser and the recovery's candidates.
+B2_DEV Tf pf_box_pose(const PfInitBox& box, const uint32_t r[6])
+{
+    float v[6];
+    #pragma unroll
+    for (int k = 0; k < 6; k++) v[k] = fminf(add(box.lo[k], mul(sub(box.hi[k], box.lo[k]), u01_closed_open(r[k]))), box.hi[k]);
+    Tf T; T.t = mk3(v[0], v[1], v[2]); T.R = euler_to_quat(v[3], v[4], v[5]);
+    return T;
+}
 B2_DEV void pf_init_uniform_one(uint64_t seed, uint32_t gidx, const PfInitBox& box, b2_transform* out_p, b2_particle_attr* out_a)
 {
     uint32_t r[8];
     philox4x32_10(gidx, B2_PF_INIT_TAG_UNIFORM, 0u, 0u, (uint32_t)seed, (uint32_t)(seed >> 32), r);
     philox4x32_10(gidx, B2_PF_INIT_TAG_UNIFORM, 0u, 1u, (uint32_t)seed, (uint32_t)(seed >> 32), r + 4);
-    float v[6];
-    #pragma unroll
-    for (int k = 0; k < 6; k++) v[k] = fminf(add(box.lo[k], mul(sub(box.hi[k], box.lo[k]), u01_closed_open(r[k]))), box.hi[k]);
-    Tf T; T.t = mk3(v[0], v[1], v[2]); T.R = euler_to_quat(v[3], v[4], v[5]);
-    tf_store(out_p, T);
+    tf_store(out_p, pf_box_pose(box, r));
     pf_init_attr(out_a);
 }
 // x = L N(0, I6) (rm::Matrix_ product, sums over k = 0..5 in order), pose = Tlm * Transform{EulerAngles{x3, x4, x5}, {x0, x1, x2}} (:231-251)
@@ -1459,6 +1473,93 @@ __global__ void __launch_bounds__(256) k_pf_init_gaussian(b2_transform* __restri
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     pf_init_gaussian_one(seed, first + i, g, poses + i, attrs + i);
+}
+#endif
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Recovery from a kidnapping: Augmented MCL (Thrun, Burgard, Fox, Probabilistic Robotics, 8.3.5; AMCL's recovery_alpha_slow / _fast; no
+// reference implementation, SURVEY appendix J).  The handle's record {w_avg, w_slow, w_fast, p_inject} (b2_recovery_state) follows the mean
+// likelihood of the set (pf_recovery_filter, after each sensor update); after resampling each particle is replaced with probability
+// p_inject by a random pose of a box, on the map's ground when a surface config is given (pf_recovery_one).  Draws: Philox4x32-10 with
+// counter (global particle index, B2_PF_RECOVERY_TAG, step, block) and key = seed: block 0 word 0 decides, blocks 1 + 2t and 2 + 2t give try
+// t's six words.  They depend on (seed, step, index, try) only, so slices of a sharded set concatenate to the whole result.
+// ---------------------------------------------------------------------------------------------------------------------
+#define B2_PF_RECOVERY_TAG 7u
+#define B2_RECOVERY_MAX_TRIES 64u
+// AMCL's recurrence on the record, all in FP64: w_avg = S / n; a non-finite or negative w_avg leaves the record as it is; each average w of
+// rate alpha becomes w_avg when w == 0, else w + alpha (w_avg - w); p_inject = w_slow > 0 ? max(0, 1 - w_fast / w_slow) : 0
+B2_DEV void pf_recovery_filter(double S, uint32_t n, double alpha_slow, double alpha_fast, b2_recovery_state* st)
+{
+    const double w_avg = S / (double)n;
+    st->w_avg = w_avg;
+    if (!(w_avg >= 0.0 && w_avg <= 1.7976931348623157e308)) return;
+    st->w_slow = st->w_slow == 0.0 ? w_avg : st->w_slow + alpha_slow * (w_avg - st->w_slow);
+    st->w_fast = st->w_fast == 0.0 ? w_avg : st->w_fast + alpha_fast * (w_avg - st->w_fast);
+    const double p = st->w_slow > 0.0 ? 1.0 - st->w_fast / st->w_slow : 0.0;
+    st->p_inject = p > 0.0 ? p : 0.0;
+}
+// what happened to one particle
+#define B2_RECOVERY_KEPT 0u          // not chosen
+#define B2_RECOVERY_REPLACED 1u
+#define B2_RECOVERY_FAILED 2u        // chosen, but no candidate of max_tries was taken: the particle is unchanged
+// particle g of the set with the record's p: chosen iff (double)word * 2^-32 < p; try t's candidate is pf_box_pose of its six words, taken
+// as it is without a surface (bvh == nullptr), else iff pf_surface_pose finds ground under it, as it moved it.  A taken candidate is written
+// with stamp 0 (tf_store, as the initialiser writes it) and the attributes {0, 0, 0}, state_sigma 0: no weight until a sensor update
+// evaluates it, whose Gaussian merge then takes the fresh likelihood alone (n_meas 0).
+B2_DEV uint32_t pf_recovery_one(const BvhView* bvh, b2_transform* pose_io, b2_particle_attr* attr_io, uint32_t g, double p, const PfInitBox& box,
+                                const b2_surface_config& cfg, float cos_max, float tfar, uint32_t max_tries, uint64_t seed, uint32_t step)
+{
+    const uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
+    uint32_t r[8];
+    philox4x32_10(g, B2_PF_RECOVERY_TAG, step, 0u, k0, k1, r);
+    if (!((double)r[0] * 2.3283064365386963e-10 < p)) return B2_RECOVERY_KEPT;
+    for (uint32_t t = 0; t < max_tries; t++) {
+        philox4x32_10(g, B2_PF_RECOVERY_TAG, step, 1u + 2u * t, k0, k1, r);
+        philox4x32_10(g, B2_PF_RECOVERY_TAG, step, 2u + 2u * t, k0, k1, r + 4);
+        Tf T = pf_box_pose(box, r);
+        if (bvh && !pf_surface_pose(*bvh, T, cfg, cos_max, tfar)) continue;
+        tf_store(pose_io, T);
+        b2_particle_attr a;
+        a.likelihood.mean = 0.0f; a.likelihood.sigma = 0.0f; a.likelihood.n_meas = 0u;
+        #pragma unroll
+        for (int k = 0; k < 6; k++) a.state_sigma[k] = 0.0f;
+        *attr_io = a;
+        return B2_RECOVERY_REPLACED;
+    }
+    return B2_RECOVERY_FAILED;
+}
+#ifdef __CUDACC__
+// one thread: the record's update from the S that k_pf_residual_stats left in device memory (bit-equal to the estimate's L_sum)
+__global__ void k_pf_recovery_filter(const double* __restrict__ S, uint32_t n, double alpha_slow, double alpha_fast, b2_recovery_state* __restrict__ st)
+{
+    pf_recovery_filter(*S, n, alpha_slow, alpha_fast, st);
+}
+// one thread per particle first + i of the slice; 128 threads per block as k_pf_surface, since replaced particles trace rays.  res (may be
+// null) receives the p used and the counts: every lane of a warp votes (lanes past the slice with "kept"), lane 0 adds the warp's counts.
+template <bool SURFACE>
+__global__ void __launch_bounds__(128) k_pf_recovery_inject(BvhView bvh, b2_transform* __restrict__ poses, b2_particle_attr* __restrict__ attrs, uint32_t first,
+                                                            uint32_t n, PfInitBox box, b2_surface_config cfg, float cos_max, float tfar, uint32_t max_tries,
+                                                            uint64_t seed, uint32_t step, const b2_recovery_state* __restrict__ st, b2_recovery_result* __restrict__ res)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    uint32_t what = B2_RECOVERY_KEPT;
+    if (i < n) {
+        const double p = st->p_inject;
+        if (res && i == 0) res->p_inject = p;
+        what = pf_recovery_one(SURFACE ? &bvh : nullptr, poses + i, attrs + i, first + i, p, box, cfg, cos_max, tfar, max_tries, seed, step);
+    }
+    if (res) {                                                          // uniform over the grid; blocks are whole warps
+        const unsigned rep = __ballot_sync(0xffffffffu, what == B2_RECOVERY_REPLACED), fl = __ballot_sync(0xffffffffu, what == B2_RECOVERY_FAILED);
+        if ((threadIdx.x & 31u) == 0u) {
+            if (rep) atomicAdd((unsigned long long*)&res->n_replaced, (unsigned long long)__popc(rep));
+            if (fl) atomicAdd((unsigned long long*)&res->n_failed, (unsigned long long)__popc(fl));
+        }
+    }
+}
+// one thread, after k_pf_recovery_inject has read p: AMCL resets both averages after an injection
+__global__ void k_pf_recovery_clear(b2_recovery_state* __restrict__ st)
+{
+    if (st->p_inject > 0.0) { st->w_slow = 0.0; st->w_fast = 0.0; st->p_inject = 0.0; }
 }
 #endif
 

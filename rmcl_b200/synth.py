@@ -371,6 +371,11 @@ assert RESIDUAL_RESULT_DTYPE.itemsize == 32
 # b2_kld_result: what PCDSensorUpdaterB200.resampleKLD returns
 KLD_RESULT_DTYPE = np.dtype([("n_particles", np.uint64), ("bins", np.uint64), ("weight_sum", np.float64), ("weight_max", np.float64)])
 assert KLD_RESULT_DTYPE.itemsize == 32
+# b2_recovery_state / b2_recovery_result: what PCDSensorUpdaterB200.recoveryObserve / recoveryInject return
+RECOVERY_STATE_DTYPE = np.dtype([("w_avg", np.float64), ("w_slow", np.float64), ("w_fast", np.float64), ("p_inject", np.float64)])
+assert RECOVERY_STATE_DTYPE.itemsize == 32
+RECOVERY_RESULT_DTYPE = np.dtype([("p_inject", np.float64), ("n_replaced", np.uint64), ("n_failed", np.uint64)])
+assert RECOVERY_RESULT_DTYPE.itemsize == 24
 # b2_cluster_record / b2_cluster_result: what PCDSensorUpdaterB200.estimateClusters returns
 CLUSTER_RECORD_DTYPE = np.dtype([("stats", PARTICLE_STATS_DTYPE), ("weight", np.float64), ("weight_int", np.uint64), ("bins", np.uint64), ("key", np.uint64)])
 assert CLUSTER_RECORD_DTYPE.itemsize == 472
