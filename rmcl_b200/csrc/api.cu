@@ -388,7 +388,8 @@ struct b2_rcc {
     int smem_u_cap = 0;                 // pairs per thread k_icp_loop can keep in shared memory (beyond the two in registers)
     int exec_mode = 2;                  // b2_rcc_set_exec_mode: 2 software grid barrier + programmatic launch (default), 1 cooperative launch, 0 one launch per reduction
     bool pdl_next = false, pdl_armed = false;   // the next find is followed by k_icp_loop launched with programmatic stream serialization / the find let it start early
-    DevBuf<uint32_t> d_tile_cost; DevBuf<uint16_t> d_tile_perm; uint32_t perm_tiles = 0, cost_tiles = 0;    // tile schedule of k_rcc_find: warp durations of the last launch (cost_tiles of them if it recorded any), order for the next (always a permutation of perm_tiles tiles)
+    DevBuf<uint32_t> d_tile_cost; DevBuf<uint16_t> d_tile_perm; uint32_t perm_tiles = 0, cost_tiles = 0;    // tile schedule of k_rcc_find: tile durations of the last launch (cost_tiles of them if it recorded any), order for the next (always a permutation of perm_tiles tiles)
+    DevBuf<unsigned int> d_find_tickets; unsigned int find_ticket = 0; uint32_t find_grid = 0;   // k_rcc_find's tile queue: device counter, its value at the next launch, grid of the last launch
     DevBuf<uint8_t> d_cloud; bool model_from_cloud = false;      // b2_rcc_set_cloud_o1dn: uploaded host cloud; the model came from that call (its tile schedule carries over)
     b2_spherical_model sph{}; bool model_spherical = false;    // the model b2_rcc_set_model_spherical set, while it is the current one (b2_rcc_set_cloud_spherical bins into it)
     DevBuf<unsigned long long> d_scan_keys;                     // b2_rcc_set_cloud_spherical: one key per cell, all 0 between calls
@@ -457,7 +458,9 @@ static int rcc_init(b2_rcc* h)
     { const char* e = getenv("B2_FUSED"); h->exec_mode = e ? atoi(e) : 2; if (h->exec_mode < 0 || h->exec_mode > 2) h->exec_mode = 2; }
     RES(h->d_partials.reserve((size_t)(B2_NACC + 1) * std::max(h->red_grid, 2 * B2_ICP_MAX_GRID))); RES(h->d_ticket.reserve(1)); RES(h->d_stats.reserve(1)); RES(h->d_icp.reserve(1));
     RES(h->d_bar.reserve(2)); RES(h->d_res.reserve(1)); RES(h->d_dbg.reserve(16 + 4 * B2_ICP_MAX_GRID)); RES(h->d_slots.reserve((size_t)B2_ICP_ACC_WORDS + B2_ICP_BASE_WORDS + B2_ICP_SLOT_WORDS));
+    RES(h->d_find_tickets.reserve(1));
     CU(cudaMemset(h->d_ticket.p, 0, sizeof(unsigned int)));
+    CU(cudaMemset(h->d_find_tickets.p, 0, sizeof(unsigned int)));
     CU(cudaMemset(h->d_bar.p, 0, 2 * sizeof(unsigned int)));
     CU(cudaMemset(h->d_slots.p, 0, ((size_t)B2_ICP_ACC_WORDS + B2_ICP_BASE_WORDS + B2_ICP_SLOT_WORDS) * sizeof(unsigned long long)));      // accumulators and base agree (0); slot tag 0 is never used
     CU(cudaMemset(h->d_dbg.p, 0, (16 + 4 * B2_ICP_MAX_GRID) * sizeof(unsigned long long)));
@@ -493,7 +496,7 @@ extern "C" int b2_rcc_destroy(b2_rcc* h)
     cudaStreamSynchronize(h->stream);
     h->d_dirs.release(); h->d_origs.release(); h->d_dpts.release(); h->d_dmask.release(); h->d_ranges_in.release();
     h->d_mpts.release(); h->d_mnrm.release(); h->d_mranges.release(); h->d_mhits.release(); h->d_mfaces.release();
-    h->d_partials.release(); h->d_ticket.release(); h->d_stats.release(); h->d_icp.release(); h->d_bar.release(); h->d_res.release(); h->d_dbg.release(); h->d_slots.release(); h->d_tile_cost.release(); h->d_tile_perm.release();
+    h->d_partials.release(); h->d_ticket.release(); h->d_stats.release(); h->d_icp.release(); h->d_bar.release(); h->d_res.release(); h->d_dbg.release(); h->d_slots.release(); h->d_tile_cost.release(); h->d_tile_perm.release(); h->d_find_tickets.release();
     h->d_chain.release(); h->d_cloud.release(); h->d_scan_keys.release();
     h->d_cov_part.release(); h->d_cov_ticket.release(); h->d_cov_rec.release();
     { DeviceCtx& dc = g_dev[h->map->device & 63]; std::lock_guard<std::mutex> lk(dc.m); dc.n_handles--; if (dc.last == h) { dc.last = nullptr; dc.recorded = false; } }
@@ -579,6 +582,30 @@ extern "C" __attribute__((visibility("default"))) int b2_rcc_debug_model_tables(
     if (ranges && *n && h->n_ranges_in == *n) CU(cudaMemcpy(ranges, h->d_ranges_in.p, sizeof(float) * *n, cudaMemcpyDeviceToHost));
     return B2_OK;
 }
+// test aid (not part of the public header): k_rcc_find's tile queue.  set != nullptr: after the stream drains, the device counter and the
+// handle's copy both become *set (a test starts them just below 2^32 to cross the wrap).  out (may be null): {device counter, handle's
+// value for the next launch, grid of the last launch}.
+extern "C" __attribute__((visibility("default"))) int b2_rcc_debug_find_tickets(b2_rcc* h, const unsigned int* set, unsigned int* out)
+{
+    NOTNULL(h);
+    CU(cudaSetDevice(h->map->device));
+    CU(cudaStreamSynchronize(h->stream));
+    if (set) { CU(cudaMemcpy(h->d_find_tickets.p, set, sizeof(unsigned int), cudaMemcpyHostToDevice)); h->find_ticket = *set; }
+    if (out) { CU(cudaMemcpy(out, h->d_find_tickets.p, sizeof(unsigned int), cudaMemcpyDeviceToHost)); out[1] = h->find_ticket; out[2] = h->find_grid; }
+    return B2_OK;
+}
+// test aid (not part of the public header): host copy of the tile durations the last find recorded (*n_tiles = 0 when it recorded none);
+// poison != 0: afterwards every entry is set to 0xffffffff on the device, so that the next find must rewrite each one
+extern "C" __attribute__((visibility("default"))) int b2_rcc_debug_tile_cost(b2_rcc* h, uint32_t* out, uint32_t capacity, uint32_t* n_tiles, int poison)
+{
+    NOTNULL(h); NOTNULL(n_tiles);
+    CU(cudaSetDevice(h->map->device));
+    CU(cudaStreamSynchronize(h->stream));
+    *n_tiles = h->cost_tiles;
+    if (out && h->cost_tiles && capacity >= h->cost_tiles) CU(cudaMemcpy(out, h->d_tile_cost.p, h->cost_tiles * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    if (poison && h->cost_tiles) CU(cudaMemset(h->d_tile_cost.p, 0xff, h->cost_tiles * sizeof(uint32_t)));
+    return B2_OK;
+}
 // make PROFILE=1 only: per block {ns at publish, ns at collect, cycles since the block reduce at publish, at collect} of iteration 1
 extern "C" __attribute__((visibility("default"))) int b2_rcc_debug_blocks(b2_rcc* h, unsigned long long* out /* 4 * B2_ICP_MAX_GRID */)
 {
@@ -589,8 +616,8 @@ extern "C" __attribute__((visibility("default"))) int b2_rcc_debug_blocks(b2_rcc
     return B2_OK;
 }
 
-// profiling aid (not part of the public header): per-warp {start, end} %globaltimer stamps of the NEXT k_rcc_find launches.
-// buf_dev: device buffer of 2 x ceil(n_rays / 32) u64, or nullptr to switch the stamps off again.
+// profiling aid (not part of the public header): per-tile {start, end} %globaltimer stamps of the NEXT k_rcc_find launches.
+// buf_dev: device buffer of 2 x ceil(n_rays / 32) u64 (one pair per tile of 32 rays), or nullptr to switch the stamps off again.
 extern "C" __attribute__((visibility("default"))) int b2_rcc_debug_find_warp_times(b2_rcc* h, unsigned long long* buf_dev)
 {
     NOTNULL(h);
@@ -875,6 +902,42 @@ static ModelBuffers model_buffers(const b2_rcc* h)
     ModelBuffers b; b.pts = h->mpts(); b.nrm = h->mnrm(); b.hits = h->mhits(); b.faces = h->d_mfaces.p; b.ranges = h->d_mranges.p; return b;
 }
 
+// k_rcc_find as one resident wave (kernels.cuh): the blocks that fit on the device at once, computed once per device
+static int find_slots(int device, uint32_t* slots)
+{
+    static std::atomic<uint32_t> per_device[64];
+    uint32_t v = per_device[device & 63].load(std::memory_order_relaxed);
+    if (v == 0) {
+        int per_sm = 0, n_sm = 0;
+        CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_rcc_find, B2_FIND_BLOCK, 0));
+        CU(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, device));
+        if (per_sm < 1 || n_sm < 1) return fail(B2_ERR_CUDA, "k_rcc_find cannot be resident on device %d", device);
+        v = (uint32_t)per_sm * (uint32_t)n_sm;
+        per_device[device & 63].store(v, std::memory_order_relaxed);
+    }
+    *slots = v;
+    return B2_OK;
+}
+
+// k_rcc_find over `total` rays (all poses) on h's stream: the grid is one resident wave, at most one warp per tile, and the tickets
+// of the launch are taken from h's queue counter.  The launch consumes exactly n_tiles tickets (kernels.cuh); h->find_ticket follows
+// the device counter modulo 2^32.
+static int launch_rcc_find(b2_rcc* h, uint64_t total, int prefetch_mode, const b2_transform* Tbm_dev, const IcpState* icp_dev, const b2_transform& Tbm_val,
+                           uint32_t n_poses, const ModelBuffers& out, int early, const uint16_t* perm, uint32_t* cost)
+{
+    const uint64_t n_tiles = (total + 31u) / 32u;
+    if (n_tiles > 0x7fffffffull) return fail(B2_ERR_INVALID, "too many rays for one find (%llu)", (unsigned long long)total);
+    uint32_t slots = 0;
+    RES(find_slots(h->map->device, &slots));
+    const uint32_t warps_per_block = B2_FIND_BLOCK / 32u, grid = (uint32_t)std::min<uint64_t>(slots, (n_tiles + warps_per_block - 1u) / warps_per_block);
+    const unsigned int base = h->find_ticket;
+    k_rcc_find<<<grid, B2_FIND_BLOCK, 0, h->stream>>>(h->map->view(), h->map->n_nodes, h->map->n_tris, prefetch_mode, Tbm_dev, icp_dev, Tbm_val, h->Tsb, ray_model(h), n_poses, out, early,
+                                                      perm, cost, h->d_find_tickets.p, base, (uint32_t)n_tiles);
+    h->find_ticket = base + (unsigned int)n_tiles;                              // unsigned: wraps like the device counter
+    h->find_grid = grid;
+    return B2_OK;
+}
+
 static int launch_find(b2_rcc* h, const b2_transform* Tbm_host, const IcpState* icp_dev)
 {
     static const int prefetch_mode_cp = [] { const char* e = getenv("B2_FIND_PREFETCH"); return e ? atoi(e) : 0; }();
@@ -892,18 +955,16 @@ static int launch_find(b2_rcc* h, const b2_transform* Tbm_host, const IcpState* 
     if (!h->has_model) return fail(B2_ERR_INVALID, "find before setModel");
     if (h->n == 0) return B2_OK;
     RES(reserve_model(h, h->n));
-    const uint32_t grid = (h->n + B2_FIND_BLOCK - 1) / B2_FIND_BLOCK;
     // no L2 prefetch by default: on an H100 (50 MB L2) prefetching the 37 MB node array of a 1M-triangle map slowed the C2 step from
     // 80 to 86 us (nodes + triangles, mode 2: 91 us)
     static const int prefetch_mode = [] { const char* e = getenv("B2_FIND_PREFETCH"); return e ? atoi(e) : 0; }();
-    // early_dependents: only when every block of this grid is resident in the first wave (14 blocks per SM), so that an early-resident
-    // dependent block can never take an SM slot a find block is still waiting for
-    const int early = (h->pdl_next && grid <= 14u * (uint32_t)h->red_grid) ? 1 : 0;
+    // early_dependents: the grid is one resident wave, so an early-resident dependent block never takes a slot a find block waits for
+    const int early = h->pdl_next ? 1 : 0;
     h->pdl_armed = early != 0;
     // tile schedule (kernels.cuh): whole tiles only, as many as the ICP loop's idle warps sort in the time they have (icp_loop.cuh)
     static const int use_sched = [] { const char* e = getenv("B2_FIND_SCHED"); return e ? atoi(e) : 1; }();
     const uint32_t n_tiles = h->n / 32u;
-    const bool sched = use_sched && (h->n % 32u) == 0u && n_tiles >= 2u && n_tiles <= (uint32_t)B2_PERM_MAX_TILES && grid * (B2_FIND_BLOCK / 32u) == n_tiles;
+    const bool sched = use_sched && (h->n % 32u) == 0u && n_tiles >= 2u && n_tiles <= (uint32_t)B2_PERM_MAX_TILES;
     uint32_t* cost = nullptr; const uint16_t* perm = nullptr;
     if (sched) {
         if (h->perm_tiles != n_tiles) {      // first launch with this model: identity order; from then on d_tile_perm always holds a permutation of the tiles
@@ -914,8 +975,7 @@ static int launch_find(b2_rcc* h, const b2_transform* Tbm_host, const IcpState* 
         }
         cost = h->d_tile_cost.p; perm = h->d_tile_perm.p; h->cost_tiles = n_tiles;
     } else h->cost_tiles = 0;
-    k_rcc_find<<<grid, B2_FIND_BLOCK, 0, h->stream>>>(h->map->view(), h->map->n_nodes, h->map->n_tris, prefetch_mode, nullptr, icp_dev, Tbm_host ? *Tbm_host : tf_identity_pod(), h->Tsb, ray_model(h), 1u, model_buffers(h), early,
-                                                      perm, cost);
+    RES(launch_rcc_find(h, h->n, prefetch_mode, nullptr, icp_dev, Tbm_host ? *Tbm_host : tf_identity_pod(), 1u, model_buffers(h), early, perm, cost));
     LAUNCHED();
     h->n_model = h->n; h->found = true;
     return B2_OK;
@@ -1777,8 +1837,7 @@ extern "C" int b2_rcc_benchmark_batch(b2_rcc* h, const b2_transform* Tbm_host, u
     ModelBuffers out; out.pts = pts.p; out.nrm = nrm.p; out.hits = hits.p; out.faces = faces.p; out.ranges = rng.p;
     for (uint32_t r = 0; r < n_runs && e == cudaSuccess; r++) {
         cudaEventRecord(ev[0], h->stream);
-        k_rcc_find<<<(uint32_t)((total + B2_FIND_BLOCK - 1) / B2_FIND_BLOCK), B2_FIND_BLOCK, 0, h->stream>>>(h->map->view(), h->map->n_nodes, h->map->n_tris, 0, h->d_poses.p, nullptr,
-                                                                                                        tf_identity_pod(), h->Tsb, ray_model(h), n_poses, out, 0, nullptr, nullptr);
+        if ((rc = launch_rcc_find(h, total, 0, h->d_poses.p, nullptr, tf_identity_pod(), n_poses, out, 0, nullptr, nullptr)) != B2_OK) break;
         cudaEventRecord(ev[1], h->stream);
         k_p2l_batch<<<bpp * n_poses, B2_FUSED_BLOCK, 0, h->stream>>>(pts.p, nrm.p, hits.p, h->n, h->dpts(), h->dmask(), h->max_dist, bpp, rays_per_block, h->d_partials.p);
         cudaEventRecord(ev[2], h->stream);
@@ -1790,7 +1849,9 @@ extern "C" int b2_rcc_benchmark_batch(b2_rcc* h, const b2_transform* Tbm_host, u
         if (e == cudaSuccess) e = cudaGetLastError();
     }
     for (int i = 0; i < 4; i++) if (ev[i]) cudaEventDestroy(ev[i]);
+    if (rc != B2_OK) CU(cudaStreamSynchronize(h->stream));
     cleanup();
+    if (rc != B2_OK) return rc;
     if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(B2_ERR_CUDA, "b2_rcc_benchmark_batch: %s", cudaGetErrorString(e)); }
     if (sim_s) *sim_s = acc[0]; if (red_s) *red_s = acc[1]; if (svd_s) *svd_s = acc[2];
     return B2_OK;

@@ -38,7 +38,7 @@ struct IcpSensor {
     float max_dist, range_min, range_max;
     uint32_t n, blk0, nblk, zc_n_origs, smem_u;                 // pairs; blocks [blk0, blk0+nblk); pairs per thread kept in shared memory
     uint32_t zc_seq;
-    const uint32_t* tile_cost; uint16_t* tile_perm;             // != nullptr: the idle warps of this sensor's first block turn the warp durations of the find
+    const uint32_t* tile_cost; uint16_t* tile_perm;             // != nullptr: the idle warps of this sensor's first block turn the tile durations of the find
     uint32_t n_tiles;                                           //   kernel into the tile order of the NEXT find (kernels.cuh: tile schedule)
     float max_dist_min;                                         // chain steps only: adaptive_max_dist_min (Correspondences.hpp:23); max_dist is then params.max_dist
 };
@@ -527,23 +527,37 @@ __global__ void __launch_bounds__(B2_ICP_BLOCK) k_icp_loop(const __grid_constant
             if (u < B2_ICP_REG_PAIRS) { if (u == 0) c_d[0] = d; else c_d[1] = d; }
             else { float* p = s_pairs + (size_t)(u - B2_ICP_REG_PAIRS) * 9 * B2_ICP_BLOCK + tid; p[0] = d.x; p[B2_ICP_BLOCK] = d.y; p[2 * B2_ICP_BLOCK] = d.z; }
         }
+    } else {
+        // the dataset half of this thread's pairs (written before the find was launched), with its own validity folded in.  Each block first
+        // pulls one slice of its sensor's whole dataset into L2: a block that becomes resident early behind the find then warms the pairs of
+        // the block that lands last (on the SM the find leaves last), whose loads are on the critical path.
+        if (tid == 0u) bulk_prefetch_slice(S.dpts, 12ull * n, blockIdx.x - S.blk0, S.nblk);
+        else if (tid == 32u) bulk_prefetch_slice(S.dmask, n, blockIdx.x - S.blk0, S.nblk);
+        for (uint32_t u = 0; u < n_cached; u++) {
+            const uint32_t i = lid + u * stride;
+            const bool in = i < n;
+            const uint32_t j = in ? i : 0u;
+            V3 d = mk3(S.dpts[3 * j], S.dpts[3 * j + 1], S.dpts[3 * j + 2]);
+            if (!(in && (S.dmask[j] > 0))) d.x = qnan;
+            if (u < B2_ICP_REG_PAIRS) { if (u == 0) c_d[0] = d; else c_d[1] = d; }
+            else { float* p = s_pairs + (size_t)(u - B2_ICP_REG_PAIRS) * 9 * B2_ICP_BLOCK + tid; p[0] = d.x; p[B2_ICP_BLOCK] = d.y; p[2 * B2_ICP_BLOCK] = d.z; }
+        }
     }
+    unsigned long long* const acc_w = xbuf;
+    unsigned long long* const base_w = xbuf + B2_ICP_ACC_WORDS;
+    ulonglong2* const slots = reinterpret_cast<ulonglong2*>(xbuf + B2_ICP_ACC_WORDS + B2_ICP_BASE_WORDS);
+    // written by block 0 of the previous launch, which completed before the find this launch follows was started
+    if (!COOP && tid < 2u * B2_MAX_SENSORS * 32u) (&s_prev[0][0][0])[tid] = __ldcg(base_w + tid);
     if (!COOP) asm volatile("griddepcontrol.wait;" ::: "memory");
-    // ---- load this thread's pairs once: validity is folded into the dataset point (NaN fails the P2L gate like a masked pair) ----
+    // ---- the model half of this thread's pairs, from the find: validity is folded into the dataset point (NaN fails the P2L gate like a masked pair) ----
     // Slots beyond the sensor's pairs read pair 0 (and are then masked): every sensor that is given blocks has at least one pair (api.cu: loop_layout).
     for (uint32_t u = 0; u < n_cached; u++) {
         const uint32_t i = lid + u * stride;
-        const bool in = i < n;
-        const uint32_t j = in ? i : 0u;
+        const uint32_t j = i < n ? i : 0u;
         V3 d;
-        if (S.zc_ranges) {
-            if (u < B2_ICP_REG_PAIRS) d = (u == 0) ? c_d[0] : c_d[1];
-            else { const float* p = s_pairs + (size_t)(u - B2_ICP_REG_PAIRS) * 9 * B2_ICP_BLOCK + tid; d = mk3(p[0], p[B2_ICP_BLOCK], p[2 * B2_ICP_BLOCK]); }
-            if (!(S.mmask[j] > 0)) d.x = qnan;
-        } else {
-            d = mk3(S.dpts[3 * j], S.dpts[3 * j + 1], S.dpts[3 * j + 2]);
-            if (!(in && (S.dmask[j] > 0) && (S.mmask[j] > 0))) d.x = qnan;
-        }
+        if (u < B2_ICP_REG_PAIRS) d = (u == 0) ? c_d[0] : c_d[1];
+        else { const float* p = s_pairs + (size_t)(u - B2_ICP_REG_PAIRS) * 9 * B2_ICP_BLOCK + tid; d = mk3(p[0], p[B2_ICP_BLOCK], p[2 * B2_ICP_BLOCK]); }
+        if (!(S.mmask[j] > 0)) d.x = qnan;
         const V3 I = mk3(S.mpts[3 * j], S.mpts[3 * j + 1], S.mpts[3 * j + 2]), N = mk3(S.mnrm[3 * j], S.mnrm[3 * j + 1], S.mnrm[3 * j + 2]);
         if (u < B2_ICP_REG_PAIRS) { if (u == 0) { c_d[0] = d; c_I[0] = I; c_N[0] = N; } else { c_d[1] = d; c_I[1] = I; c_N[1] = N; } }
         else {
@@ -553,10 +567,6 @@ __global__ void __launch_bounds__(B2_ICP_BLOCK) k_icp_loop(const __grid_constant
             p[6 * B2_ICP_BLOCK] = N.x; p[7 * B2_ICP_BLOCK] = N.y; p[8 * B2_ICP_BLOCK] = N.z;
         }
     }
-    unsigned long long* const acc_w = xbuf;
-    unsigned long long* const base_w = xbuf + B2_ICP_ACC_WORDS;
-    ulonglong2* const slots = reinterpret_cast<ulonglong2*>(xbuf + B2_ICP_ACC_WORDS + B2_ICP_BASE_WORDS);
-    if (!COOP && tid < 2u * B2_MAX_SENSORS * 32u) (&s_prev[0][0][0])[tid] = __ldcg(base_w + tid);     // written by block 0 of the previous launch
     __syncthreads();
     // a chain step gates with the progress the previous step left (written before this grid's find was launched)
     const float max_dist = L.chain ? icp_adaptive_max_dist(S.max_dist, S.max_dist_min, L.chain->cp) : S.max_dist;

@@ -658,12 +658,13 @@ B2_DEV void find_one(const BvhView& bvh, Tf Tsm, const RayModel& model, uint32_t
     }
 }
 
-// bulk prefetch of this block's slice of the node array into L2 (UBLKPF): after a cold start the top of the tree then comes from
-// L2 instead of one DRAM round trip per level.  16-byte granularity, fire and forget.
-__device__ __forceinline__ void bulk_prefetch_slice(const void* base, uint64_t total)
+// bulk prefetch of slice `part` of `parts` of an array into L2 (UBLKPF): e.g. after a cold start the top of the tree then comes from
+// L2 instead of one DRAM round trip per level.  16-byte granularity (a base that is not 16-byte aligned is not prefetched), fire and forget.
+__device__ __forceinline__ void bulk_prefetch_slice(const void* base, uint64_t total, uint32_t part, uint32_t parts)
 {
-    const uint64_t per = ((total + gridDim.x - 1) / gridDim.x + 15ull) & ~15ull;
-    const uint64_t beg = (uint64_t)blockIdx.x * per;
+    if (reinterpret_cast<uintptr_t>(base) & 15u) return;
+    const uint64_t per = ((total + parts - 1) / parts + 15ull) & ~15ull;
+    const uint64_t beg = (uint64_t)part * per;
     if (beg < total) {
         const uint32_t bytes = (uint32_t)min(per, total - beg) & ~15u;
         const char* ptr = reinterpret_cast<const char*>(base) + beg;
@@ -673,52 +674,68 @@ __device__ __forceinline__ void bulk_prefetch_slice(const void* base, uint64_t t
 // mode 1: node array; mode 2: node array + leaf triangle records (the whole map: 85 MB for 1M triangles, more than the 50 MB L2 of an H100)
 __device__ __forceinline__ void prefetch_map_l2(const BvhView& bvh, uint32_t n_nodes, uint32_t n_tris, int mode)
 {
-    if (threadIdx.x == 0 && mode >= 1) bulk_prefetch_slice(bvh.nodes, (uint64_t)n_nodes * (uint64_t)B2_NODE_BYTES);
-    if (threadIdx.x == 32 % blockDim.x && mode >= 2) bulk_prefetch_slice(bvh.tris, (uint64_t)n_tris * 48ull);
+    if (threadIdx.x == 0 && mode >= 1) bulk_prefetch_slice(bvh.nodes, (uint64_t)n_nodes * (uint64_t)B2_NODE_BYTES, blockIdx.x, gridDim.x);
+    if (threadIdx.x == 32 % blockDim.x && mode >= 2) bulk_prefetch_slice(bvh.tris, (uint64_t)n_tris * 48ull, blockIdx.x, gridDim.x);
 }
 
 #define B2_FIND_BLOCK 64
-// profiling aid: when set (b2_rcc_debug_find_warp_times), lane 0 of every warp stores {start, end} in %globaltimer nanoseconds
+// profiling aid: when set (b2_rcc_debug_find_warp_times), lane 0 of the warp that traces a tile stores its {start, end} in %globaltimer nanoseconds
 __device__ unsigned long long* g_find_warp_times = nullptr;
 __device__ __forceinline__ unsigned long long globaltimer_ns() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 
-// 14 blocks per SM (72 registers).  On an H100 the 2048 blocks of the C2 scan need 15.5 per SM on 132 SMs to be resident in one wave;
-// 16 blocks per SM (64 registers, twice the spill traffic) was measured slower there: with the shipped setting (no L2 prefetch), alternating
-// runs of bench.py --no-extra on one H100 SXM (400 W power limit) gave a find alone of 49.6-50.0 vs 51.8-52.4 us and a C2 step of 81.2 vs
-// 82.4-82.7 us; with the node-array prefetch on, 55 vs 60 us and 85.6 vs 90.0 us.
-// Tile schedule (single-pose launches): the block scheduler hands out blocks in index order over a few microseconds, and the kernel ends
-// with its slowest warp -- so the tiles that took longest in the PREVIOUS launch of this handle (same model, nearly the same pose: MICP-L
-// corrects continuously) go first.  Each warp leaves its duration in `tile_cost`; the ICP loop that follows the find turns the durations
-// into the order `tile_perm` of the next launch (icp_loop.cuh: tile_perm_group, idle warps of one block).  Purely a schedule: every tile is traced exactly once, results do not depend on it.
+// 14 blocks per SM (72 registers).  16 blocks per SM (64 registers, twice the spill traffic) was measured slower on an H100 SXM (400 W power
+// limit): with the shipped setting (no L2 prefetch), alternating runs of bench.py --no-extra gave a find alone of 49.6-50.0 vs 51.8-52.4 us and
+// a C2 step of 81.2 vs 82.4-82.7 us; with the node-array prefetch on, 55 vs 60 us and 85.6 vs 90.0 us.
+// One resident wave with a per-warp tile queue: the grid is the blocks that fit on the device at once (api.cu: find_slots).  Warp w traces
+// tile w first, then takes tiles (8x4 rays) one after another from a per-handle ticket counter until the tickets pass the last tile: a warp
+// that finishes early takes the next tile at once instead of idling beside the other warp of its block, and since every block is resident
+// from the start, a dependent kernel that becomes resident early (k_icp_loop) never takes a slot a find block is waiting for.  The first
+// tiles take no ticket because every warp asking for one at the same moment serialises on the counter's address (on an H100, tickets for
+// the first tiles too delayed the median tile start by 1.3 us and made the C2 find ~4 us slower).
+// Tickets: ticket k of a launch stands for tile warps + k, and every warp that traced a tile ends on one ticket past the last tile, so a
+// launch takes exactly n_tiles tickets.  The host passes the counter's value at the launch (`ticket_base`) and advances its copy by
+// n_tiles; no reset between launches.  k is an unsigned 32-bit difference, which stays right when the counter wraps around 2^32.
+// Tile schedule (single-pose launches): the kernel ends with its slowest warp -- so the tiles that took longest in the PREVIOUS launch of
+// this handle (same model, nearly the same pose: MICP-L corrects continuously) are handed out first.  Each tile leaves its duration (SM
+// cycles from its ticket to its last write) in `tile_cost[tile]`; the ICP loop that follows the find turns the durations into the order
+// `tile_perm` of the next launch (icp_loop.cuh: tile_perm_group, idle warps of one block).  Without a schedule tiles go in raster order.
+// Purely a schedule: every tile is traced exactly once, at its own buffer index, so results do not depend on it.
 __global__ void __launch_bounds__(B2_FIND_BLOCK, 14) k_rcc_find(BvhView bvh, uint32_t n_nodes, uint32_t n_tris, int prefetch_mode, const b2_transform* __restrict__ Tbm_dev,
                                                                 const IcpState* __restrict__ icp, b2_transform Tbm_val, b2_transform Tsb_val, RayModel model, uint32_t n_poses,
-                                                                ModelBuffers out, int early_dependents, const uint16_t* __restrict__ tile_perm, uint32_t* __restrict__ tile_cost)
+                                                                ModelBuffers out, int early_dependents, const uint16_t* __restrict__ tile_perm, uint32_t* __restrict__ tile_cost,
+                                                                unsigned int* __restrict__ tickets, unsigned int ticket_base, uint32_t n_tiles)
 {
-    __shared__ uint32_t s_t0[B2_FIND_BLOCK / 32];
-    uint64_t gid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (tile_perm) gid = ((uint64_t)tile_perm[gid >> 5] << 5) | (gid & 31u);                      // n_poses == 1; a permutation of the tiles
-    if (tile_cost && (threadIdx.x & 31u) == 0u) { uint32_t c; asm volatile("mov.u32 %0, %%clock;" : "=r"(c)); s_t0[threadIdx.x >> 5] = c; }
     // let a dependent kernel launched with programmatic stream serialization (k_icp_loop) become resident as SMs drain; it still waits
     // (griddepcontrol.wait) for this grid to complete and flush before it reads the model buffers
     if (early_dependents) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    if (g_find_warp_times && (threadIdx.x & 31u) == 0u) g_find_warp_times[2 * (((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5)] = globaltimer_ns();      // nothing stays live across the trace
     prefetch_map_l2(bvh, n_nodes, n_tris, prefetch_mode);
-    const uint64_t total = (uint64_t)model.n * n_poses;
-    if (gid < total) {
-        const uint32_t pose = (uint32_t)(gid / model.n), i = tile_order((uint32_t)(gid % model.n), model.width, model.height);
-        Tf Tbm;
-        if (icp) Tbm = tf_mul(tf_load(&icp->Tom), tf_load(&icp->Tbo));           // MICPSensor.hpp:148
-        else if (Tbm_dev) Tbm = tf_load(Tbm_dev + pose);
-        else Tbm = tf_from_pod(Tbm_val);
-        find_one(bvh, tf_mul(Tbm, tf_from_pod(Tsb_val)), model, i, (uint64_t)pose * model.n + i, out);
-    }
-    if (tile_cost) {
+    __shared__ uint32_t s_t0[B2_FIND_BLOCK / 32], s_tile[B2_FIND_BLOCK / 32];                     // the tile's start clock and number: nothing extra stays live across the trace
+    const uint32_t lane = threadIdx.x & 31u, warps = gridDim.x * (B2_FIND_BLOCK / 32u);
+    uint32_t t = (blockIdx.x * B2_FIND_BLOCK + threadIdx.x) >> 5;                                  // first tile: the warp's own index, no ticket
+    while (t < n_tiles) {
+        const uint32_t tile = tile_perm ? (uint32_t)tile_perm[t] : t;                               // n_poses == 1 with a schedule; a permutation of the tiles
+        if (lane == 0u) s_tile[threadIdx.x >> 5] = tile;
+        if (tile_cost && lane == 0u) { uint32_t c; asm volatile("mov.u32 %0, %%clock;" : "=r"(c)); s_t0[threadIdx.x >> 5] = c; }
+        if (g_find_warp_times && lane == 0u) g_find_warp_times[2 * (uint64_t)tile] = globaltimer_ns();
+        const uint64_t gid = ((uint64_t)tile << 5) | (threadIdx.x & 31u);
+        const uint32_t pose = (uint32_t)(gid / model.n);
+        if (pose < n_poses) {
+            const uint32_t i = tile_order((uint32_t)(gid % model.n), model.width, model.height);
+            Tf Tbm;
+            if (icp) Tbm = tf_mul(tf_load(&icp->Tom), tf_load(&icp->Tbo));           // MICPSensor.hpp:148
+            else if (Tbm_dev) Tbm = tf_load(Tbm_dev + pose);
+            else Tbm = tf_from_pod(Tbm_val);
+            find_one(bvh, tf_mul(Tbm, tf_from_pod(Tsb_val)), model, i, (uint64_t)pose * model.n + i, out);
+        }
         __syncwarp();
-        if ((threadIdx.x & 31u) == 0u) { uint32_t c; asm volatile("mov.u32 %0, %%clock;" : "=r"(c)); tile_cost[gid >> 5] = c - s_t0[threadIdx.x >> 5]; }
-    }
-    if (g_find_warp_times) {
-        __syncwarp();
-        if ((threadIdx.x & 31u) == 0u) g_find_warp_times[2 * (((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5) + 1] = globaltimer_ns();
+        if ((threadIdx.x & 31u) == 0u) {
+            const uint32_t done = s_tile[threadIdx.x >> 5];
+            if (tile_cost) { uint32_t c; asm volatile("mov.u32 %0, %%clock;" : "=r"(c)); tile_cost[done] = c - s_t0[threadIdx.x >> 5]; }
+            if (g_find_warp_times) g_find_warp_times[2 * (uint64_t)done + 1] = globaltimer_ns();
+        }
+        uint32_t k = 0;
+        if (lane == 0u) k = atomicAdd(tickets, 1u) - ticket_base;
+        t = warps + __shfl_sync(0xffffffffu, k, 0);
     }
 }
 
