@@ -19,6 +19,24 @@
 //   this test is at least as permissive as the oracle's visit rule V (tn <= tbest*C1 && tf >= max(0, tn*C3), C3 = 1-2^-12): if tn_F > 0,
 //   tn' <= tn_F*C3' <= fl(tn_F*C3) <= tf_F <= tf'; if tn_F <= 0, tn' <= 0 <= tf_F.  Hence every HIT's leaf is visited and the result
 //   equals the brute-force answer.
+// INTEGER BOX TEST: the same predicate, tn = max(tn'_x, tn'_y, tn'_z, 0) <= tf = min(tf'_x, tf'_y, tf'_z, tlim), reduced on the float BIT
+//   PATTERNS as signed ints: tn_i = __vimax3_s32_relu(near planes), tf_i = __vimin3_s32(far planes, tlim_i) (VIMNMX3 on sm_90), hit iff
+//   tn_i <= tf_i.  Signed-int order equals float order on non-negative non-NaN floats (+0 .. +inf); every float with the sign bit set is a
+//   negative int, -0 the smallest.  fmaxf / fminf drop a NaN operand.  The bits are the float test's exactly when (a) no near plane is NaN
+//   and (b) no far plane is NaN or -0, and tlim_i maps tlim = -0 to 0 and NaN to INT_MAX:
+//     tn: a negative or -0 near plane counts as 0 both ways (relu / fmaxf(., 0)); otherwise order is preserved, so tn_i = bits(tn) with
+//         tn = +-0 -> 0.
+//     tf: if some far plane or tlim is negative (< -0), tf_i < 0 <= tn_i and tf < 0 <= tn: miss both ways.  Otherwise every operand is
+//         +0 .. +inf (or tlim NaN, dropped by fminf, INT_MAX here) and tf_i = bits(tf), so tn_i <= tf_i iff tn <= tf.
+//   (a) and (b) hold for every node plane (finite, or +-inf in empty slots: the builders refuse non-finite vertices) when, per axis,
+//   idir, idn, ncn, ncf are finite, idn != 0, and ncf is +0 with |idir| >= 1 or |ncf| >= 2^-100 (ray_setup flags such rays B2_RAY_INTBOX):
+//     NaN needs a NaN operand, inf * 0 or inf - inf: none with finite nonzero slopes and finite addends.
+//     -0: ncf is computed as dl - oi, never -0 (dl >= +0).  With ncf = +0 the FMA is +-0 + +0 = +0 for a zero plane and |plane * idir|
+//     >= 2^-149 (not rounding to 0) for any other.  With |ncf| >= 2^-100: if |plane * idir| < 2^-101 the sum is nonzero and above 2^-101;
+//     otherwise plane * idir is an integer multiple of 2^-148 (a product of two floats m1 2^e1 * m2 2^e2, m < 2^24, at least 2^-101 in
+//     magnitude has e1 + e2 >= -148) and ncf one of 2^-149, so the exact sum is 0 (rounded to +0) or at least 2^-149 in magnitude.
+//   Any other ray (NaN or inf components, denormal-scale addends; never a unit direction from a finite origin in practice) runs the
+//   float reduction: trace_closest picks the instantiation once per ray.
 #pragma once
 #include "b2_math.cuh"
 #include "bvh8.h"
@@ -44,9 +62,11 @@ struct RaySetup {
     V3 o, d, idir;
     V3 idn, ncn, ncf;       // near-plane slope (idir*C3'), NEGATED near / far constants of the box test (see header): the FMA addends
     uint32_t oct;           // bit k set iff idir_k >= 0
-    uint32_t noff;          // float4 offsets of the near planes inside a node, one byte per axis (lo arrays for positive directions, hi arrays
-                            // otherwise); the far planes sit at 6 - onx, 10 - ony, 14 - onz
+    uint32_t noff;          // byte offsets of the near planes inside a node, bits 0..23 one byte per axis (lo arrays for positive directions,
+                            // hi arrays otherwise; the far planes sit at 96 - bnx, 160 - bny, 224 - bnz); bit 31 = B2_RAY_INTBOX
 };
+
+#define B2_RAY_INTBOX 0x80000000u    // noff flag: the box test of this ray may reduce on integer bit patterns (see header)
 
 #define B2_C3P 0.99951171875f          // 1 - 2^-11
 
@@ -103,6 +123,14 @@ B2_DEV V3 tri_ng(const BvhView& bvh, uint32_t tri_idx)
     return cross_fma(v_sub(mk3(b.x, b.y, b.z), v0), v_sub(mk3(c.x, c.y, c.z), v0));
 }
 
+// One axis of a ray admits the integer box test (header): slopes and addends finite, slopes nonzero, and the far addend either at least 2^-100
+// in magnitude or +0 with |idir| >= 1 -- then no near plane is NaN and no far plane is NaN or -0.
+B2_DEV bool intbox_axis(float idir, float idn, float ncn, float ncf)
+{
+    const float inf = u2f(0x7f800000u), afar = fabsf(ncf);
+    return fabsf(idn) < inf && idn != 0.0f && fabsf(ncn) < inf && afar < inf && (afar >= u2f(0x0d800000u) || (ncf == 0.0f && fabsf(idir) >= 1.0f));
+}
+
 B2_DEV RaySetup ray_setup(V3 o, V3 d, const BvhView& bvh)
 {
     RaySetup r; r.o = o; r.d = d;
@@ -117,9 +145,11 @@ B2_DEV RaySetup ray_setup(V3 o, V3 d, const BvhView& bvh)
     const float dlx = (fabsf(oix) + bvh.bx * fabsf(r.idir.x)) * k20, dly = (fabsf(oiy) + bvh.by * fabsf(r.idir.y)) * k20, dlz = (fabsf(oiz) + bvh.bz * fabsf(r.idir.z)) * k20;
     r.idn = mk3(r.idir.x * B2_C3P, r.idir.y * B2_C3P, r.idir.z * B2_C3P);
     r.ncn = mk3(-((oix + dlx) * B2_C3P), -((oiy + dly) * B2_C3P), -((oiz + dlz) * B2_C3P));
-    r.ncf = mk3(-(oix - dlx), -(oiy - dly), -(oiz - dlz));
-    // node layout in float4 units: lo_x 0..1, lo_y 2..3, lo_z 4..5, hi_x 6..7, hi_y 8..9, hi_z 10..11
-    r.noff = ((r.oct & 1u) ? 0u : 6u) | (((r.oct & 2u) ? 2u : 8u) << 8) | (((r.oct & 4u) ? 4u : 10u) << 16);
+    r.ncf = mk3(dlx - oix, dly - oiy, dlz - oiz);   // = -(oi - dl), but +0 rather than -0 when oi == dl (INTEGER BOX TEST in the header)
+    // node layout in bytes: lo_x 0, lo_y 32, lo_z 64, hi_x 96, hi_y 128, hi_z 160 (two quads each), header 192
+    r.noff = ((r.oct & 1u) ? 0u : 96u) | (((r.oct & 2u) ? 32u : 128u) << 8) | (((r.oct & 4u) ? 64u : 160u) << 16);
+    if (intbox_axis(r.idir.x, r.idn.x, r.ncn.x, r.ncf.x) && intbox_axis(r.idir.y, r.idn.y, r.ncn.y, r.ncf.y) && intbox_axis(r.idir.z, r.idn.z, r.ncn.z, r.ncf.z))
+        r.noff |= B2_RAY_INTBOX;
 #if B2_ON_DEVICE
     // Per-ray constants of the box test are made opaque to the optimiser: under the 72-register cap of the traversal kernels it otherwise
     // RE-DERIVES them from o / d in every node visit (octant, plane offsets, slack constants: ~45 of ~190 instructions per visit in the round-1
@@ -154,27 +184,64 @@ B2_DEV uint32_t spread3x(uint32_t x)
 // same space (record index of bit b = tri_base + popc(trimask & ((1 << b) - 1))).
 // 13 quads per visit (12 plane quads + one header quad); the masks come from the eight box-test bits with ~30 bit operations -- the first
 // version decoded one meta byte per child (~60 instructions, a third of the visit in its SASS).
-B2_DEV void node_test(const float4* __restrict__ np, const RaySetup& r, float tbest, uint32_t& child_base, uint32_t& tri_base, uint32_t& inner, uint32_t& tris, uint32_t& trimask)
+// Load order: the header and quad a (children 0..3) of all six plane arrays first -- one 16-byte load in each of the node's seven 32-byte
+// sectors, so a node that misses L1 costs one round trip to L2 / DRAM -- then quad b (children 4..7), which the first loads brought into L1.
+// INTBOX: reduce each child's six planes on their bit patterns (header, INTEGER BOX TEST); only for rays flagged B2_RAY_INTBOX.
+B2_DEV int imin(int a, int b) { return a < b ? a : b; }
+
+// Read-only 16-byte load that the compiler keeps in source order with the other ordered loads (volatile asm): the node visit issues the
+// loads that touch all seven sectors of a node before any that does not.
+B2_DEV float4 ldg_ordered(const float4* p)
 {
-    // near planes: the "lo" arrays for positive directions, the "hi" arrays otherwise; far planes: the other one (offset 6 quads apart)
-    // derived HERE, per visit (three bit-field extracts), not hoisted out of the traversal loop into three more live registers (or spill slots)
-    uint32_t onx, ony, onz;
 #if B2_ON_DEVICE
-    asm volatile("bfe.u32 %0, %3, 0, 8;\n\tbfe.u32 %1, %3, 8, 8;\n\tbfe.u32 %2, %3, 16, 8;" : "=r"(onx), "=r"(ony), "=r"(onz) : "r"(r.noff));
+    float4 v;
+    asm volatile("ld.global.nc.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
+    return v;
 #else
-    onx = r.noff & 0xffu; ony = (r.noff >> 8) & 0xffu; onz = r.noff >> 16;
+    return *p;
 #endif
-    const float4 nxa = ldg(np + onx), nxb = ldg(np + onx + 1), fxa = ldg(np + (6u - onx)), fxb = ldg(np + (7u - onx));
-    const float4 nya = ldg(np + ony), nyb = ldg(np + ony + 1), fya = ldg(np + (10u - ony)), fyb = ldg(np + (11u - ony));
-    const float4 nza = ldg(np + onz), nzb = ldg(np + onz + 1), fza = ldg(np + (14u - onz)), fzb = ldg(np + (15u - onz));
-    const float4 h = ldg(np + 12);
+}
+
+template <bool INTBOX>
+B2_DEV void node_test(const float4* __restrict__ nodes, uint32_t node_idx, const RaySetup& r, float tbest, uint32_t& child_base, uint32_t& tri_base,
+                      uint32_t& inner, uint32_t& tris, uint32_t& trimask)
+{
+    // one 64-bit node base; the plane arrays are reached by per-ray byte offsets, quad b (+16) and the header (+192) by immediates.  Near planes:
+    // the "lo" arrays for positive directions, the "hi" arrays otherwise; far planes: the other one (96 bytes apart).  The offsets are
+    // extracted HERE, per visit, not hoisted out of the traversal loop into six more live registers (or spill slots).
+    const char* const nb = reinterpret_cast<const char*>(nodes) + (size_t)node_idx * (16u * B2_NODE_QUADS);
+    uint32_t bnx, bny, bnz;
+#if B2_ON_DEVICE
+    asm volatile("bfe.u32 %0, %3, 0, 8;\n\tbfe.u32 %1, %3, 8, 8;\n\tbfe.u32 %2, %3, 16, 8;" : "=r"(bnx), "=r"(bny), "=r"(bnz) : "r"(r.noff));
+#else
+    bnx = r.noff & 0xffu; bny = (r.noff >> 8) & 0xffu; bnz = (r.noff >> 16) & 0xffu;
+#endif
+    const char* const pnx = nb + bnx; const char* const pfx = nb + (96u - bnx);
+    const char* const pny = nb + bny; const char* const pfy = nb + (160u - bny);
+    const char* const pnz = nb + bnz; const char* const pfz = nb + (224u - bnz);
+#define B2_Q(P, OFF) ldg_ordered(reinterpret_cast<const float4*>((P) + (OFF)))
+    const float4 h = B2_Q(nb, 192);
+    const float4 nxa = B2_Q(pnx, 0), nya = B2_Q(pny, 0), nza = B2_Q(pnz, 0), fxa = B2_Q(pfx, 0), fya = B2_Q(pfy, 0), fza = B2_Q(pfz, 0);
     child_base = f2u(h.x); tri_base = f2u(h.y);
     const uint32_t masks = f2u(h.z), imask = masks & 0xffu;
     trimask = masks >> 8;
     const float tlim = tbest * B2_C1;
+    int tl = (int)f2u(tlim);                   // integer reduction: tlim = -0 (a tfar of -0) compares as +0, NaN (ignored by fminf) as the maximum
+    if (INTBOX) { if (tlim == 0.0f) tl = 0; if (tlim != tlim) tl = 0x7fffffff; }
+    // every box test waits for the header: bits 24..30 of noff are zero but opaque to the compiler, so the header load is issued with the
+    // quad-a loads instead of being sunk to the end of the visit, where its miss would be a second round trip
+    tl |= (int)(masks & r.noff & 0x7f000000u);
     uint32_t hit8 = 0;
     // Two children per step, one plane of two neighbouring slots from the .xy / .zw halves of a 128-bit node load; slope and addend are
     // per-ray scalars.  Every plane is one round-to-nearest FMA, the same bits as the CPU emulation.
+#define B2_HIT(BIT, NX, NY, NZ, FX, FY, FZ)                                                                            \
+    if (INTBOX) {                                                                                                      \
+        const int tn = __vimax3_s32_relu((int)f2u(NX), (int)f2u(NY), (int)f2u(NZ));                                    \
+        const int tf = __vimin3_s32((int)f2u(FX), (int)f2u(FY), imin((int)f2u(FZ), tl));                                \
+        hit8 |= (tn <= tf) ? (BIT) : 0u;                                                                               \
+    } else {                                                                                                           \
+        hit8 |= (fmaxf(fmaxf(NX, NY), fmaxf(NZ, 0.0f)) <= fminf(fminf(FX, FY), fminf(FZ, tlim))) ? (BIT) : 0u;         \
+    }
 #define B2_PAIR(S, NX0, NX1, NY0, NY1, NZ0, NZ1, FX0, FX1, FY0, FY1, FZ0, FZ1)                                        \
     {                                                                                                                  \
         const float nx0 = fma_rn(NX0, r.idn.x, r.ncn.x), nx1 = fma_rn(NX1, r.idn.x, r.ncn.x);                          \
@@ -183,23 +250,23 @@ B2_DEV void node_test(const float4* __restrict__ np, const RaySetup& r, float tb
         const float fx0 = fma_rn(FX0, r.idir.x, r.ncf.x), fx1 = fma_rn(FX1, r.idir.x, r.ncf.x);                        \
         const float fy0 = fma_rn(FY0, r.idir.y, r.ncf.y), fy1 = fma_rn(FY1, r.idir.y, r.ncf.y);                        \
         const float fz0 = fma_rn(FZ0, r.idir.z, r.ncf.z), fz1 = fma_rn(FZ1, r.idir.z, r.ncf.z);                        \
-        const float tn0 = fmaxf(fmaxf(nx0, ny0), fmaxf(nz0, 0.0f)), tn1 = fmaxf(fmaxf(nx1, ny1), fmaxf(nz1, 0.0f));    \
-        const float tf0 = fminf(fminf(fx0, fy0), fminf(fz0, tlim)), tf1 = fminf(fminf(fx1, fy1), fminf(fz1, tlim));    \
-        hit8 |= (tn0 <= tf0) ? (1u << (S)) : 0u;                                                                       \
-        hit8 |= (tn1 <= tf1) ? (2u << (S)) : 0u;                                                                       \
+        B2_HIT(1u << (S), nx0, ny0, nz0, fx0, fy0, fz0)                                                                \
+        B2_HIT(2u << (S), nx1, ny1, nz1, fx1, fy1, fz1)                                                                \
     }
     B2_PAIR(0, nxa.x, nxa.y, nya.x, nya.y, nza.x, nza.y, fxa.x, fxa.y, fya.x, fya.y, fza.x, fza.y)
     B2_PAIR(2, nxa.z, nxa.w, nya.z, nya.w, nza.z, nza.w, fxa.z, fxa.w, fya.z, fya.w, fza.z, fza.w)
+    const float4 nxb = B2_Q(pnx, 16), nyb = B2_Q(pny, 16), nzb = B2_Q(pnz, 16), fxb = B2_Q(pfx, 16), fyb = B2_Q(pfy, 16), fzb = B2_Q(pfz, 16);
     B2_PAIR(4, nxb.x, nxb.y, nyb.x, nyb.y, nzb.x, nzb.y, fxb.x, fxb.y, fyb.x, fyb.y, fzb.x, fzb.y)
     B2_PAIR(6, nxb.z, nxb.w, nyb.z, nyb.w, nzb.z, nzb.w, fxb.z, fxb.w, fyb.z, fyb.w, fzb.z, fzb.w)
 #undef B2_PAIR
+#undef B2_HIT
+#undef B2_Q
     inner = (xor_permute8(hit8 & imask, r.oct) << 24) | imask;
     tris = spread3x(hit8 & ~imask) & trimask;           // empty slots never pass the box test (lo = +inf, hi = -inf) and have no trimask bits
 }
 
-// Closest hit. best.t must be initialised to tfar, best.face to B2_NOFACE by the caller (see trace_init).
-template <bool STATS>
-B2_DEV void trace_closest(const BvhView& bvh, const RaySetup& r, HitRec& best, uint32_t& n_nodes, uint32_t& n_tris)
+template <bool STATS, bool INTBOX>
+B2_DEV void trace_closest_box(const BvhView& bvh, const RaySetup& r, HitRec& best, uint32_t& n_nodes, uint32_t& n_tris)
 {
     uint2 stack[B2_TRAVERSAL_STACK];
     int sp = 0;
@@ -230,12 +297,22 @@ B2_DEV void trace_closest(const BvhView& bvh, const RaySetup& r, HitRec& best, u
             const uint32_t node_idx = G.x + rel;
             if (G.y & 0xff000000u) stack[sp++] = G;
             uint32_t child_base, tri_base, inner, tris;
-            node_test(bvh.nodes + B2_NODE_QUADS * (size_t)node_idx, r, best.t, child_base, tri_base, inner, tris, Gm);
+            node_test<INTBOX>(bvh.nodes, node_idx, r, best.t, child_base, tri_base, inner, tris, Gm);
             if (STATS) n_nodes++;
             G = make_uint2(child_base, inner);
             Gt = make_uint2(tri_base, tris);
         }
     }
+}
+
+// Closest hit. best.t must be initialised to tfar, best.face to B2_NOFACE by the caller (see trace_init).  A ray whose box-test constants
+// are outside the integer test's domain (non-finite or denormal-scale; never a unit direction from a finite origin in practice) walks the
+// same tree with the float reduction.
+template <bool STATS>
+B2_DEV void trace_closest(const BvhView& bvh, const RaySetup& r, HitRec& best, uint32_t& n_nodes, uint32_t& n_tris)
+{
+    if (r.noff & B2_RAY_INTBOX) trace_closest_box<STATS, true>(bvh, r, best, n_nodes, n_tris);
+    else                        trace_closest_box<STATS, false>(bvh, r, best, n_nodes, n_tris);
 }
 
 B2_DEV HitRec trace_init(float tfar) { HitRec h; h.t = tfar; h.face = B2_NOFACE; h.tri = 0u; return h; }
