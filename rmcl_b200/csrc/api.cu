@@ -1932,11 +1932,27 @@ extern "C" int b2_debug_read_bandwidth(int device, uint64_t bytes, int iters, do
 // ---------------------------------------------------------------------------------------------------------------------
 // particle filter
 // ---------------------------------------------------------------------------------------------------------------------
+// the fixed-size device records of the particle-filter entry points: one device block, zeroed at the handle's creation, and one pinned
+// host mirror of the same layout that pf_fetch reads members back into
+struct PfRecords {
+    PfEstimateScratch est;                              // the estimate's two passes: record, Tbm, L_sum, tickets
+    PfResidualState res;                                // the weight statistics (pf_weight_stats) and the residual's chunk record
+    PfKldState kld;                                     // KLD's chunk record
+    PfClusterState cl;                                  // the cluster labelling's record
+    PfClusterHead heads[B2_CLUSTER_MAX_RECORDS];        // the recorded clusters' heads ...
+    b2_particle_stats recs[B2_CLUSTER_MAX_RECORDS];     // ... and their estimates
+    b2_recovery_state rec;                              // the recovery's {w_avg, w_slow, w_fast, p_inject}
+    b2_recovery_result rec_res;                         // the result of an injection
+    unsigned long long traffic;                         // remote bytes read by the p2p Gladiator kernel
+};
+
+// The scratch below (partials, records, the resamplers' and the clusters' buffers) is shared by the entry points: a handle serves one call at
+// a time, and each call's work runs in h->stream order.
 struct b2_pf {
     b2_mesh* map = nullptr; cudaStream_t stream = 0;
     DevBuf<PfBeam> d_beams; PfBeam* h_beams = nullptr; size_t h_beams_cap = 0;
     DevBuf<b2_transform> d_poses; DevBuf<b2_particle_attr> d_attrs;
-    DevBuf<double> d_part; DevBuf<unsigned int> d_ticket; DevBuf<float> d_out; float* h_out = nullptr; int n_sm = 0;
+    int n_sm = 0;
     int smem_optin = 0;
     cudaStream_t side = nullptr; cudaEvent_t ev_beams = nullptr, ev_side = nullptr;      // second stream of the chunked host variant (b2_pf_sensor_update_host)
     // ray mapping of k_pf_update (kernels.cuh): 0 lanes = beams, 1 lanes = particles, 2 lanes = particles sorted by pose, 3 (default) whichever of 0 / 2
@@ -1947,32 +1963,26 @@ struct b2_pf {
     DevBuf<uint32_t> d_keys, d_keys2, d_idx, d_idx2; DevBuf<unsigned char> d_sort_tmp;
     // sharded resampling over NVLink peer memory (b2_pf_p2p_*): own exchange buffers (cudaMalloc: exportable through CUDA IPC) + the peers' mappings
     b2_transform* x_poses = nullptr; b2_particle_attr* x_attrs = nullptr; uint32_t x_cap = 0;
-    PfPeers peers{}; bool peers_open = false; DevBuf<unsigned long long> d_traffic;
-    // pose estimate (b2_pf_estimate_stats), allocated at its first call: block partials of both passes, the record, Tbm and tickets
-    DevBuf<double> d_est_part; DevBuf<PfEstimateScratch> d_est; b2_particle_stats* h_est = nullptr;
+    PfPeers peers{}; bool peers_open = false;
+    // the records (PfRecords) and their pinned mirror; block partials of the grid reductions (k_pf_residual_stats and the estimate's two
+    // passes): B2_EST_NV_MAX per block of at most 4 n_sm blocks
+    DevBuf<PfRecords> d_recs; PfRecords* h_recs = nullptr; DevBuf<double> d_part;
     // beam sampling from a device cloud (b2_pf_sample_cloud): one record per sample, and its pinned host copy
     DevBuf<PfBeamSample> d_samples; PfBeamSample* h_samples = nullptr; uint32_t h_samples_cap = 0;
-    // residual resampling (b2_pf_resample_residual), grown at its calls: statistics partials, per-draw parents, counts and their prefix for
-    // the largest chunk, the scan's temporary storage, and the state record with its pinned host copy
-    DevBuf<double> d_res_part; DevBuf<uint32_t> d_res_parents; DevBuf<unsigned long long> d_res_counts, d_res_prefix; DevBuf<unsigned char> d_res_tmp;
-    DevBuf<PfResidualState> d_res; PfResidualState* h_res = nullptr;
-    // KLD-sampling (b2_pf_resample_kld), grown at its calls (its statistics pass uses the residual's buffers above): integer weights and their
-    // prefix, the hash set (keys, first draws), per-draw parents, hash slots, flags and their prefix for the largest chunk, the scan's
-    // temporary storage, the yaw-sector table of kld_K sectors with its host copy, and the state record with its pinned host copy
+    // residual resampling (b2_pf_resample_residual), grown at its calls: per-draw parents, counts and their prefix for the largest chunk, and
+    // the scan's temporary storage
+    DevBuf<uint32_t> d_res_parents; DevBuf<unsigned long long> d_res_counts, d_res_prefix; DevBuf<unsigned char> d_res_tmp;
+    // KLD-sampling (b2_pf_resample_kld), grown at its calls: integer weights and their prefix, the hash set (keys, first draws), per-draw
+    // parents, hash slots, flags and their prefix for the largest chunk, the scan's temporary storage, and the yaw-sector table of kld_K
+    // sectors with its host copy
     DevBuf<unsigned long long> d_kld_w, d_kld_W, d_kld_keys, d_kld_slots; DevBuf<unsigned int> d_kld_first; DevBuf<uint32_t> d_kld_parents, d_kld_flags, d_kld_cum;
     DevBuf<unsigned char> d_kld_tmp; DevBuf<float> d_kld_tab; std::vector<float> h_kld_tab; uint32_t kld_K = 0;
-    DevBuf<PfKldState> d_kld; PfKldState* h_kld = nullptr;
     // pose hypotheses (b2_pf_cluster_stats), grown at its calls.  It shares KLD's hash set (d_kld_keys; d_kld_first holds each slot's link
     // to its root), sector table, temporary storage and, for the cluster sort's keys, d_kld_w / d_kld_W.  Its own: per slot the weight, the
     // member count and the bin count / rank; per particle the slot, the sort key and the index, each of the latter two before and after the
-    // sort (the index buffers also list the roots); the gathered members; the heads and records of the recorded clusters; the state record;
-    // and one pinned host block for the state, the heads and the records
+    // sort (the index buffers also list the roots); and the gathered members
     DevBuf<unsigned long long> d_cl_w; DevBuf<unsigned int> d_cl_cnt, d_cl_aux; DevBuf<uint32_t> d_cl_slot, d_cl_key, d_cl_key2, d_cl_idx, d_cl_idx2;
-    DevBuf<b2_transform> d_cl_poses; DevBuf<b2_particle_attr> d_cl_attrs; DevBuf<PfClusterHead> d_cl_heads; DevBuf<b2_particle_stats> d_cl_recs;
-    DevBuf<PfClusterState> d_cl; unsigned char* h_cl = nullptr;
-    // recovery (b2_pf_recovery_*), allocated at the first of its calls: the record {w_avg, w_slow, w_fast, p_inject}, the result of an
-    // injection, and one pinned host block for either read-back
-    DevBuf<b2_recovery_state> d_rec; DevBuf<b2_recovery_result> d_rec_res; unsigned char* h_rec = nullptr;
+    DevBuf<b2_transform> d_cl_poses; DevBuf<b2_particle_attr> d_cl_attrs;
 };
 
 extern "C" int b2_pf_destroy(b2_pf* h);
@@ -1983,9 +1993,9 @@ static int pf_init(b2_pf* h)
     CU(cudaDeviceGetAttribute(&h->smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, map->device));
     h->smem_optin -= 1024;              // room for the kernel's static shared memory
     CU(cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, map->device));
-    RES(h->d_part.reserve(2 * (size_t)h->n_sm * 4)); RES(h->d_ticket.reserve(1)); RES(h->d_out.reserve(2));
-    CU(cudaMemset(h->d_ticket.p, 0, sizeof(unsigned int)));
-    CU(cudaMallocHost((void**)&h->h_out, 2 * sizeof(float)));
+    RES(h->d_part.reserve((size_t)B2_EST_NV_MAX * 4 * (size_t)h->n_sm)); RES(h->d_recs.reserve(1));
+    CU(cudaMemset(h->d_recs.p, 0, sizeof(PfRecords)));
+    CU(cudaMallocHost((void**)&h->h_recs, sizeof(PfRecords)));
     CU(cudaFuncSetAttribute(k_pf_update<0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
     CU(cudaFuncSetAttribute(k_pf_update<1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
     CU(cudaFuncSetAttribute(k_pf_update<0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
@@ -2014,9 +2024,9 @@ extern "C" int b2_pf_destroy(b2_pf* h)
     if (!h) return B2_OK;
     cudaSetDevice(h->map->device);
     cudaStreamSynchronize(h->stream);
-    h->d_beams.release(); h->d_poses.release(); h->d_attrs.release(); h->d_part.release(); h->d_ticket.release(); h->d_out.release();
+    h->d_beams.release(); h->d_poses.release(); h->d_attrs.release(); h->d_part.release(); h->d_recs.release();
     if (h->h_beams) cudaFreeHost(h->h_beams);
-    if (h->h_out) cudaFreeHost(h->h_out);
+    if (h->h_recs) cudaFreeHost(h->h_recs);
     if (h->side) { cudaStreamSynchronize(h->side); cudaStreamDestroy(h->side); }
     if (h->ev_beams) cudaEventDestroy(h->ev_beams);
     if (h->ev_side) cudaEventDestroy(h->ev_side);
@@ -2029,21 +2039,13 @@ extern "C" int b2_pf_destroy(b2_pf* h)
     }
     if (h->x_poses) cudaFree(h->x_poses);
     if (h->x_attrs) cudaFree(h->x_attrs);
-    h->d_traffic.release();
-    h->d_est_part.release(); h->d_est.release();
-    if (h->h_est) cudaFreeHost(h->h_est);
     h->d_samples.release();
     if (h->h_samples) cudaFreeHost(h->h_samples);
-    h->d_res_part.release(); h->d_res_parents.release(); h->d_res_counts.release(); h->d_res_prefix.release(); h->d_res_tmp.release(); h->d_res.release();
-    if (h->h_res) cudaFreeHost(h->h_res);
+    h->d_res_parents.release(); h->d_res_counts.release(); h->d_res_prefix.release(); h->d_res_tmp.release();
     h->d_kld_w.release(); h->d_kld_W.release(); h->d_kld_keys.release(); h->d_kld_slots.release(); h->d_kld_first.release(); h->d_kld_parents.release();
-    h->d_kld_flags.release(); h->d_kld_cum.release(); h->d_kld_tmp.release(); h->d_kld_tab.release(); h->d_kld.release();
-    if (h->h_kld) cudaFreeHost(h->h_kld);
+    h->d_kld_flags.release(); h->d_kld_cum.release(); h->d_kld_tmp.release(); h->d_kld_tab.release();
     h->d_cl_w.release(); h->d_cl_cnt.release(); h->d_cl_aux.release(); h->d_cl_slot.release(); h->d_cl_key.release(); h->d_cl_key2.release(); h->d_cl_idx.release();
-    h->d_cl_idx2.release(); h->d_cl_poses.release(); h->d_cl_attrs.release(); h->d_cl_heads.release(); h->d_cl_recs.release(); h->d_cl.release();
-    if (h->h_cl) cudaFreeHost(h->h_cl);
-    h->d_rec.release(); h->d_rec_res.release();
-    if (h->h_rec) cudaFreeHost(h->h_rec);
+    h->d_cl_idx2.release(); h->d_cl_poses.release(); h->d_cl_attrs.release();
     b2_mesh* map = h->map;
     delete h;
     (void)cudaGetLastError();
@@ -2051,6 +2053,32 @@ extern "C" int b2_pf_destroy(b2_pf* h)
     return B2_OK;
 }
 extern "C" int b2_pf_set_stream(b2_pf* h, void* s) { NOTNULL(h); h->stream = (cudaStream_t)s; return B2_OK; }
+
+// read back: `count` elements starting at mirror_member (a member of h->h_recs) from the same offset of the device records, then a synchronise
+template <class T> static int pf_fetch(b2_pf* h, const T& mirror_member, size_t count = 1)
+{
+    const size_t off = (size_t)((const char*)&mirror_member - (const char*)h->h_recs);
+    CU(cudaMemcpyAsync((char*)h->h_recs + off, (const char*)h->d_recs.p + off, sizeof(T) * count, cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    return B2_OK;
+}
+
+// blocks of the grid reductions over n > 0 particles: 256 threads each, at most 4 per SM (grid-stride beyond)
+static uint32_t pf_stats_grid(const b2_pf* h, uint32_t n) { return std::min<uint32_t>((uint32_t)h->n_sm * 4u, (n + 255) / 256); }
+
+// The set's weight statistics S, L_min and L_max (k_pf_residual_stats) of n > 0 particles into h->d_recs.p->res, with read_back also into
+// h->h_recs->res.  usable: the set can be resampled or clustered -- a NaN or infinite likelihood makes S non-finite, and all zero gives
+// 0 / 0 in the reference (SURVEY D31).
+static int pf_weight_stats(b2_pf* h, const b2_particle_attr* attrs_dev, uint32_t n, bool read_back, bool* usable = nullptr)
+{
+    k_pf_residual_stats<<<pf_stats_grid(h, n), 256, 0, h->stream>>>(attrs_dev, n, h->d_part.p, &h->d_recs.p->res);
+    LAUNCHED();
+    if (!read_back) return B2_OK;
+    RES(pf_fetch(h, h->h_recs->res));
+    const PfResidualState& r = h->h_recs->res;
+    if (usable) *usable = std::isfinite(r.S) && r.S > 0.0 && r.L_min >= 0.0;
+    return B2_OK;
+}
 
 static uint32_t dir_sort_key(const b2_range_meas& m)
 {
@@ -2368,7 +2396,6 @@ extern "C" int b2_pf_p2p_init(b2_pf* h, uint32_t n_per_rank, void* handles_out_1
     CU(cudaIpcGetMemHandle(&hp, h->x_poses)); CU(cudaIpcGetMemHandle(&ha, h->x_attrs));
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "CUDA IPC handle size");
     memcpy(handles_out_128, &hp, 64); memcpy(static_cast<char*>(handles_out_128) + 64, &ha, 64);
-    RES(h->d_traffic.reserve(1));
     return B2_OK;
 }
 extern "C" int b2_pf_p2p_connect(b2_pf* h, const void* all_handles, uint32_t world, uint32_t rank, uint32_t n_per_rank)
@@ -2413,14 +2440,13 @@ extern "C" int b2_pf_resample_gladiator_p2p(b2_pf* h, b2_transform* poses_new_de
     NOTNULL(h); NOTNULL(cfg); NOTNULL(poses_new_dev); NOTNULL(attrs_new_dev);
     if (!h->peers_open && h->peers.pad != 1u) return fail(B2_ERR_INVALID, "p2p: resample before connect");
     CU(cudaSetDevice(h->map->device));
-    CU(cudaMemsetAsync(h->d_traffic.p, 0, sizeof(unsigned long long), h->stream));
-    k_pf_gladiator_p2p<<<(h->peers.n_per_rank + 255) / 256, 256, 0, h->stream>>>(h->peers, poses_new_dev, attrs_new_dev, *cfg, seed, step, h->d_traffic.p);
+    unsigned long long* traffic = &h->d_recs.p->traffic;
+    CU(cudaMemsetAsync(traffic, 0, sizeof(unsigned long long), h->stream));
+    k_pf_gladiator_p2p<<<(h->peers.n_per_rank + 255) / 256, 256, 0, h->stream>>>(h->peers, poses_new_dev, attrs_new_dev, *cfg, seed, step, traffic);
     LAUNCHED();
     if (remote_bytes_out) {
-        unsigned long long t = 0;
-        CU(cudaMemcpyAsync(&t, h->d_traffic.p, sizeof(t), cudaMemcpyDeviceToHost, h->stream));
-        CU(cudaStreamSynchronize(h->stream));
-        *remote_bytes_out = t;
+        RES(pf_fetch(h, h->h_recs->traffic));
+        *remote_bytes_out = h->h_recs->traffic;
     }
     return B2_OK;
 }
@@ -2432,7 +2458,6 @@ extern "C" int b2_pf_p2p_connect_local(b2_pf* h, const b2_transform* poses_all_d
     if (world == 0 || world > B2_MAX_PEERS || rank >= world || n_per_rank == 0) return fail(B2_ERR_INVALID, "p2p: bad local world");
     if (h->peers_open) return fail(B2_ERR_INVALID, "p2p: already connected");
     CU(cudaSetDevice(h->map->device));
-    RES(h->d_traffic.reserve(1));
     PfPeers P{}; P.world = world; P.rank = rank; P.n_per_rank = n_per_rank;
     for (uint32_t r = 0; r < world; r++) { P.poses[r] = poses_all_dev + (size_t)r * n_per_rank; P.attrs[r] = attrs_all_dev + (size_t)r * n_per_rank; }
     h->peers = P;                 // peers_open stays false: nothing to unmap, and publish is not needed
@@ -2534,22 +2559,11 @@ extern "C" int b2_pf_init_gaussian(b2_pf* h, b2_transform* poses_dev, b2_particl
 }
 
 // ---- recovery from a kidnapping (Augmented MCL; SURVEY appendix J) ---------------------------------------------------------------------------
-// the record, zeroed on the handle's stream when it is first needed
-static int recovery_record(b2_pf* h)
-{
-    if (h->d_rec.p) return B2_OK;
-    RES(h->d_rec.reserve(1)); RES(h->d_rec_res.reserve(1));
-    CU(cudaMemsetAsync(h->d_rec.p, 0, sizeof(b2_recovery_state), h->stream));
-    CU(cudaMallocHost((void**)&h->h_rec, std::max(sizeof(b2_recovery_state), sizeof(b2_recovery_result))));
-    return B2_OK;
-}
-
 extern "C" int b2_pf_recovery_reset(b2_pf* h)
 {
     NOTNULL(h);
     CU(cudaSetDevice(h->map->device));
-    RES(recovery_record(h));
-    CU(cudaMemsetAsync(h->d_rec.p, 0, sizeof(b2_recovery_state), h->stream));
+    CU(cudaMemsetAsync(&h->d_recs.p->rec, 0, sizeof(b2_recovery_state), h->stream));
     return B2_OK;
 }
 
@@ -2562,21 +2576,12 @@ extern "C" int b2_pf_recovery_observe(b2_pf* h, const b2_particle_attr* attrs_de
         return fail(B2_ERR_INVALID, "recovery observe: alpha_slow = %g and alpha_fast = %g must lie in [0, 1]", as, af);
     if (as > af) return fail(B2_ERR_INVALID, "recovery observe: alpha_slow = %g > alpha_fast = %g", as, af);
     CU(cudaSetDevice(h->map->device));
-    RES(recovery_record(h));
-    const uint32_t grid = std::min<uint32_t>((uint32_t)h->n_sm * 4u, (n + 255) / 256);
-    if (!h->d_res.p) {
-        RES(h->d_res_part.reserve((size_t)B2_RES_NV * 4 * (size_t)h->n_sm)); RES(h->d_res.reserve(1));
-        CU(cudaMemsetAsync(h->d_res.p, 0, sizeof(PfResidualState), h->stream));
-        CU(cudaMallocHost((void**)&h->h_res, sizeof(PfResidualState)));
-    }
-    k_pf_residual_stats<<<grid, 256, 0, h->stream>>>(attrs_dev, n, h->d_res_part.p, h->d_res.p);
-    LAUNCHED();
-    k_pf_recovery_filter<<<1, 1, 0, h->stream>>>(&h->d_res.p->S, n, as, af, h->d_rec.p);
+    RES(pf_weight_stats(h, attrs_dev, n, false));
+    k_pf_recovery_filter<<<1, 1, 0, h->stream>>>(&h->d_recs.p->res.S, n, as, af, &h->d_recs.p->rec);
     LAUNCHED();
     if (state_host) {
-        CU(cudaMemcpyAsync(h->h_rec, h->d_rec.p, sizeof(b2_recovery_state), cudaMemcpyDeviceToHost, h->stream));
-        CU(cudaStreamSynchronize(h->stream));
-        memcpy(state_host, h->h_rec, sizeof(b2_recovery_state));
+        RES(pf_fetch(h, h->h_recs->rec));
+        *state_host = h->h_recs->rec;
     }
     return B2_OK;
 }
@@ -2595,29 +2600,25 @@ extern "C" int b2_pf_recovery_inject(b2_pf* h, b2_transform* poses_dev, b2_parti
     if (n_local > 0) { NOTNULL(poses_dev); NOTNULL(attrs_dev); }
     RES(pf_init_range(first, n_local));
     CU(cudaSetDevice(h->map->device));
-    RES(recovery_record(h));
     if (n_local == 0) {
         if (out_host) {                                   // nothing to replace: the p a slice would have used
-            CU(cudaMemcpyAsync(h->h_rec, &h->d_rec.p->p_inject, sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-            CU(cudaStreamSynchronize(h->stream));
-            b2_recovery_result r{0.0, 0, 0};
-            memcpy(&r.p_inject, h->h_rec, sizeof(double));
-            *out_host = r;
+            RES(pf_fetch(h, h->h_recs->rec.p_inject));
+            *out_host = b2_recovery_result{h->h_recs->rec.p_inject, 0, 0};
         }
         return B2_OK;
     }
-    b2_recovery_result* res = out_host ? h->d_rec_res.p : nullptr;
+    b2_recovery_state* rec = &h->d_recs.p->rec;
+    b2_recovery_result* res = out_host ? &h->d_recs.p->rec_res : nullptr;
     if (res) CU(cudaMemsetAsync(res, 0, sizeof(b2_recovery_result), h->stream));
     const uint32_t grid = (n_local + 127) / 128;
-    if (surface) k_pf_recovery_inject<true><<<grid, 128, 0, h->stream>>>(h->map->view(), poses_dev, attrs_dev, first, n_local, box, sc, cos_max, tfar, max_tries, seed, step, h->d_rec.p, res);
-    else         k_pf_recovery_inject<false><<<grid, 128, 0, h->stream>>>(h->map->view(), poses_dev, attrs_dev, first, n_local, box, sc, cos_max, tfar, max_tries, seed, step, h->d_rec.p, res);
+    if (surface) k_pf_recovery_inject<true><<<grid, 128, 0, h->stream>>>(h->map->view(), poses_dev, attrs_dev, first, n_local, box, sc, cos_max, tfar, max_tries, seed, step, rec, res);
+    else         k_pf_recovery_inject<false><<<grid, 128, 0, h->stream>>>(h->map->view(), poses_dev, attrs_dev, first, n_local, box, sc, cos_max, tfar, max_tries, seed, step, rec, res);
     LAUNCHED();
-    k_pf_recovery_clear<<<1, 1, 0, h->stream>>>(h->d_rec.p);
+    k_pf_recovery_clear<<<1, 1, 0, h->stream>>>(rec);
     LAUNCHED();
     if (out_host) {
-        CU(cudaMemcpyAsync(h->h_rec, res, sizeof(b2_recovery_result), cudaMemcpyDeviceToHost, h->stream));
-        CU(cudaStreamSynchronize(h->stream));
-        memcpy(out_host, h->h_rec, sizeof(b2_recovery_result));
+        RES(pf_fetch(h, h->h_recs->rec_res));
+        *out_host = h->h_recs->rec_res;
     }
     return B2_OK;
 }
@@ -2629,12 +2630,8 @@ extern "C" int b2_pf_likelihood_stats(b2_pf* h, const b2_particle_attr* attrs_de
     float s = 0.f, m = 0.f;
     if (n > 0) {
         NOTNULL(attrs_dev);
-        const uint32_t grid = std::min<uint32_t>((uint32_t)h->n_sm * 4u, (n + 255) / 256);
-        k_pf_stats<<<grid, 256, 0, h->stream>>>(attrs_dev, n, h->d_part.p, h->d_ticket.p, h->d_out.p);
-        LAUNCHED();
-        CU(cudaMemcpyAsync(h->h_out, h->d_out.p, 2 * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-        CU(cudaStreamSynchronize(h->stream));
-        s = h->h_out[0]; m = h->h_out[1];
+        RES(pf_weight_stats(h, attrs_dev, n, true));
+        s = (float)h->h_recs->res.S; m = (float)h->h_recs->res.L_max;
     }
     if (sum_out) *sum_out = s;
     if (max_out) *max_out = m;
@@ -2642,18 +2639,13 @@ extern "C" int b2_pf_likelihood_stats(b2_pf* h, const b2_particle_attr* attrs_de
 }
 
 // RmclNode::estimateStats (rmcl_localization.cpp:642-731): two read passes, Tbm handed from the first to the second in device memory
-// both passes over n > 0 particles; the record is left in h->d_est.p->rec
+// both passes over n > 0 particles; the record is left in h->d_recs.p->est.rec
 static int estimate_launch(b2_pf* h, const b2_transform* poses_dev, const b2_particle_attr* attrs_dev, uint32_t n)
 {
-    const uint32_t grid = std::min<uint32_t>((uint32_t)h->n_sm * 4u, (n + 255) / 256);
-    if (!h->d_est.p) {
-        RES(h->d_est_part.reserve((size_t)B2_EST_NV_MAX * 4 * (size_t)h->n_sm)); RES(h->d_est.reserve(1));
-        CU(cudaMemset(h->d_est.p, 0, sizeof(PfEstimateScratch)));
-        CU(cudaMallocHost((void**)&h->h_est, sizeof(b2_particle_stats)));
-    }
-    k_pf_estimate_moments<<<grid, 256, 0, h->stream>>>(poses_dev, attrs_dev, n, h->d_est_part.p, h->d_est.p);
+    const uint32_t grid = pf_stats_grid(h, n);
+    k_pf_estimate_moments<<<grid, 256, 0, h->stream>>>(poses_dev, attrs_dev, n, h->d_part.p, &h->d_recs.p->est);
     LAUNCHED();
-    k_pf_estimate_cov<<<grid, 256, 0, h->stream>>>(poses_dev, attrs_dev, n, h->d_est_part.p, h->d_est.p);
+    k_pf_estimate_cov<<<grid, 256, 0, h->stream>>>(poses_dev, attrs_dev, n, h->d_part.p, &h->d_recs.p->est);
     LAUNCHED();
     return B2_OK;
 }
@@ -2663,51 +2655,49 @@ extern "C" int b2_pf_estimate_stats(b2_pf* h, const b2_transform* poses_dev, con
     if (n == 0) return fail(B2_ERR_INVALID, "estimate stats: no particles (n = 0)");
     CU(cudaSetDevice(h->map->device));
     RES(estimate_launch(h, poses_dev, attrs_dev, n));
-    CU(cudaMemcpyAsync(h->h_est, &h->d_est.p->rec, sizeof(b2_particle_stats), cudaMemcpyDeviceToHost, h->stream));
-    CU(cudaStreamSynchronize(h->stream));
-    *out_host = *h->h_est;
+    RES(pf_fetch(h, h->h_recs->est.rec));
+    *out_host = h->h_recs->est.rec;
     return B2_OK;
 }
 
-// ResidualResamplerCPU::update (ResidualResamplerCPU.cpp:55-202): a statistics pass, then the draws in chunks of doubling size, each counted,
-// scanned and searched for the draw that fills the last slot, with one read-back per chunk; the slots a chunk filled are built right after it
+// the resamplers' outputs: slots first .. first + n_local - 1 of n_out, in ranges that overlap neither an input nor each other
 static bool ranges_overlap(const void* a, size_t a_bytes, const void* b, size_t b_bytes)
 {
     const uintptr_t pa = (uintptr_t)a, pb = (uintptr_t)b;
     return a_bytes && b_bytes && pa < pb + b_bytes && pb < pa + a_bytes;
 }
+static int check_resample_outputs(const char* what, const b2_transform* poses_dev, const b2_particle_attr* attrs_dev, uint32_t n, uint32_t n_out, uint32_t first,
+                                  uint32_t n_local, const b2_transform* poses_new_dev, const b2_particle_attr* attrs_new_dev)
+{
+    if ((uint64_t)first + n_local > n_out) return fail(B2_ERR_INVALID, "%s: slots %u+%u exceed the %u output slots", what, first, n_local, n_out);
+    const size_t in_p = sizeof(b2_transform) * (size_t)n, in_a = sizeof(b2_particle_attr) * (size_t)n;
+    const size_t out_p = sizeof(b2_transform) * (size_t)n_local, out_a = sizeof(b2_particle_attr) * (size_t)n_local;
+    if (ranges_overlap(poses_new_dev, out_p, poses_dev, in_p) || ranges_overlap(poses_new_dev, out_p, attrs_dev, in_a) ||
+        ranges_overlap(attrs_new_dev, out_a, poses_dev, in_p) || ranges_overlap(attrs_new_dev, out_a, attrs_dev, in_a) ||
+        ranges_overlap(poses_new_dev, out_p, attrs_new_dev, out_a))
+        return fail(B2_ERR_INVALID, "%s: an output range overlaps an input range or the other output (the node double-buffers)", what);
+    return B2_OK;
+}
+
+// ResidualResamplerCPU::update (ResidualResamplerCPU.cpp:55-202): a statistics pass, then the draws in chunks of doubling size, each counted,
+// scanned and searched for the draw that fills the last slot, with one read-back per chunk; the slots a chunk filled are built right after it
 extern "C" int b2_pf_resample_residual(b2_pf* h, const b2_transform* poses_dev, const b2_particle_attr* attrs_dev, uint32_t n, uint32_t n_new,
                                        uint32_t first, uint32_t n_local, b2_transform* poses_new_dev, b2_particle_attr* attrs_new_dev,
                                        const b2_gladiator_config* cfg, uint64_t seed, uint32_t step, b2_residual_result* out_host)
 {
     NOTNULL(h); NOTNULL(poses_dev); NOTNULL(attrs_dev); NOTNULL(poses_new_dev); NOTNULL(attrs_new_dev); NOTNULL(cfg); NOTNULL(out_host);
     if (n == 0 || n_new == 0) return fail(B2_ERR_INVALID, "resample residual: %u particles into %u slots (both must be > 0)", n, n_new);
-    if ((uint64_t)first + n_local > n_new) return fail(B2_ERR_INVALID, "resample residual: slots %u+%u exceed the %u output slots", first, n_local, n_new);
-    const size_t in_p = sizeof(b2_transform) * (size_t)n, in_a = sizeof(b2_particle_attr) * (size_t)n;
-    const size_t out_p = sizeof(b2_transform) * (size_t)n_local, out_a = sizeof(b2_particle_attr) * (size_t)n_local;
-    if (ranges_overlap(poses_new_dev, out_p, poses_dev, in_p) || ranges_overlap(poses_new_dev, out_p, attrs_dev, in_a) ||
-        ranges_overlap(attrs_new_dev, out_a, poses_dev, in_p) || ranges_overlap(attrs_new_dev, out_a, attrs_dev, in_a) ||
-        ranges_overlap(poses_new_dev, out_p, attrs_new_dev, out_a))
-        return fail(B2_ERR_INVALID, "resample residual: an output range overlaps an input range or the other output (the node double-buffers)");
+    RES(check_resample_outputs("resample residual", poses_dev, attrs_dev, n, n_new, first, n_local, poses_new_dev, attrs_new_dev));
     CU(cudaSetDevice(h->map->device));
     const uint64_t M = n_new, nm = std::max<uint64_t>(n, M), d_max = 16 * nm;
     // draws are keyed by their index: the chunk size changes no result.  2^30 keeps a chunk within the scan's int item count.
     const uint64_t cap = std::min<uint64_t>(2 * nm, 1ull << 30);
     uint64_t chunk = std::min<uint64_t>(std::max<uint64_t>(2 * (uint64_t)n, 1ull << 16), cap);
-    const uint32_t grid = std::min<uint32_t>((uint32_t)h->n_sm * 4u, (n + 255) / 256);
-    if (!h->d_res.p) {
-        RES(h->d_res_part.reserve((size_t)B2_RES_NV * 4 * (size_t)h->n_sm)); RES(h->d_res.reserve(1));
-        CU(cudaMemset(h->d_res.p, 0, sizeof(PfResidualState)));
-        CU(cudaMallocHost((void**)&h->h_res, sizeof(PfResidualState)));
-    }
-    k_pf_residual_stats<<<grid, 256, 0, h->stream>>>(attrs_dev, n, h->d_res_part.p, h->d_res.p);
-    LAUNCHED();
-    CU(cudaMemcpyAsync(h->h_res, h->d_res.p, sizeof(PfResidualState), cudaMemcpyDeviceToHost, h->stream));
-    CU(cudaStreamSynchronize(h->stream));
-    const double S = h->h_res->S, L_min = h->h_res->L_min, L_max = h->h_res->L_max;
+    bool usable = false;
+    RES(pf_weight_stats(h, attrs_dev, n, true, &usable));
+    const double S = h->h_recs->res.S, L_max = h->h_recs->res.L_max;
     b2_residual_result res = {0, 0, S, L_max};
-    // a NaN or infinite likelihood makes S non-finite; all zero gives 0 / 0 in the reference (SURVEY D31)
-    if (!(std::isfinite(S) && S > 0.0 && L_min >= 0.0)) { *out_host = res; return B2_OK; }
+    if (!usable) { *out_host = res; return B2_OK; }
     size_t tmp_bytes = 0;
     CU(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, h->d_res_counts.p, h->d_res_prefix.p, (int)cap, h->stream));
     RES(h->d_res_parents.reserve(cap)); RES(h->d_res_counts.reserve(cap)); RES(h->d_res_prefix.reserve(cap)); RES(h->d_res_tmp.reserve(std::max<size_t>(tmp_bytes, 16)));
@@ -2719,11 +2709,10 @@ extern "C" int b2_pf_resample_residual(b2_pf* h, const b2_transform* poses_dev, 
         size_t bytes = h->d_res_tmp.cap;
         CU(cub::DeviceScan::InclusiveSum(h->d_res_tmp.p, bytes, h->d_res_counts.p, h->d_res_prefix.p, (int)len, h->stream));
         LAUNCHED();
-        k_pf_residual_find<<<1, 1, 0, h->stream>>>(h->d_res_prefix.p, len, M - fill, h->d_res.p);
+        k_pf_residual_find<<<1, 1, 0, h->stream>>>(h->d_res_prefix.p, len, M - fill, &h->d_recs.p->res);
         LAUNCHED();
-        CU(cudaMemcpyAsync(h->h_res, h->d_res.p, sizeof(PfResidualState), cudaMemcpyDeviceToHost, h->stream));
-        CU(cudaStreamSynchronize(h->stream));
-        const uint64_t filled = h->h_res->filled, used = h->h_res->used;
+        RES(pf_fetch(h, h->h_recs->res));
+        const uint64_t filled = h->h_recs->res.filled, used = h->h_recs->res.used;
         const uint64_t lo = std::max<uint64_t>(fill, first), hi = std::min<uint64_t>(fill + filled, (uint64_t)first + n_local);
         if (lo < hi) {
             const uint32_t n_k = (uint32_t)(hi - lo);
@@ -2740,23 +2729,6 @@ extern "C" int b2_pf_resample_residual(b2_pf* h, const b2_transform* poses_dev, 
     return B2_OK;
 }
 
-// KLD-sampling (Fox 2003; rmcl/docs/RMCL.md:80-83): the residual's statistics pass, the integer weights and their scan, then the draws in
-// chunks of doubling size, each drawn into the hash set, flagged, scanned and searched for the first draw that meets the stop rule, with one
-// read-back per chunk; the slots a chunk filled are built right after it
-static int kld_stats(b2_pf* h, const b2_particle_attr* attrs_dev, uint32_t n)
-{
-    const uint32_t grid = std::min<uint32_t>((uint32_t)h->n_sm * 4u, (n + 255) / 256);
-    if (!h->d_res.p) {
-        RES(h->d_res_part.reserve((size_t)B2_RES_NV * 4 * (size_t)h->n_sm)); RES(h->d_res.reserve(1));
-        CU(cudaMemset(h->d_res.p, 0, sizeof(PfResidualState)));
-        CU(cudaMallocHost((void**)&h->h_res, sizeof(PfResidualState)));
-    }
-    k_pf_residual_stats<<<grid, 256, 0, h->stream>>>(attrs_dev, n, h->d_res_part.p, h->d_res.p);
-    LAUNCHED();
-    CU(cudaMemcpyAsync(h->h_res, h->d_res.p, sizeof(PfResidualState), cudaMemcpyDeviceToHost, h->stream));
-    CU(cudaStreamSynchronize(h->stream));
-    return B2_OK;
-}
 // K = ceil(2 pi / res_yaw) of the ratio shrunk by 2^-20: a float res_yaw is 2 pi / K rounded (10 deg in float is a hair under 10 deg), and
 // a plain ceil would then give K + 1 sectors; with the shrink every float within 2^-21 of 2 pi / K gives K (SURVEY G3)
 static const double kKldPi = 3.14159265358979323846;
@@ -2775,6 +2747,9 @@ static int kld_sector_table(b2_pf* h, uint32_t K)
     h->kld_K = K;
     return B2_OK;
 }
+// KLD-sampling (Fox 2003; rmcl/docs/RMCL.md:80-83): the weight statistics, the integer weights and their scan, then the draws in chunks of
+// doubling size, each drawn into the hash set, flagged, scanned and searched for the first draw that meets the stop rule, with one read-back
+// per chunk; the slots a chunk filled are built right after it
 extern "C" int b2_pf_resample_kld(b2_pf* h, const b2_transform* poses_dev, const b2_particle_attr* attrs_dev, uint32_t n, uint32_t n_max, uint32_t first,
                                   uint32_t n_local, b2_transform* poses_new_dev, b2_particle_attr* attrs_new_dev, const b2_gladiator_config* cfg,
                                   const b2_kld_config* kld, uint64_t seed, uint32_t step, b2_kld_result* out_host)
@@ -2782,13 +2757,7 @@ extern "C" int b2_pf_resample_kld(b2_pf* h, const b2_transform* poses_dev, const
     NOTNULL(h); NOTNULL(poses_dev); NOTNULL(attrs_dev); NOTNULL(poses_new_dev); NOTNULL(attrs_new_dev); NOTNULL(cfg); NOTNULL(kld); NOTNULL(out_host);
     if (n == 0 || n_max == 0) return fail(B2_ERR_INVALID, "resample kld: %u particles into %u slots (both must be > 0)", n, n_max);
     if (kld->n_min == 0 || kld->n_min > n_max) return fail(B2_ERR_INVALID, "resample kld: n_min = %u must lie in [1, n_max = %u]", kld->n_min, n_max);
-    if ((uint64_t)first + n_local > n_max) return fail(B2_ERR_INVALID, "resample kld: slots %u+%u exceed the %u output slots", first, n_local, n_max);
-    const size_t in_p = sizeof(b2_transform) * (size_t)n, in_a = sizeof(b2_particle_attr) * (size_t)n;
-    const size_t out_p = sizeof(b2_transform) * (size_t)n_local, out_a = sizeof(b2_particle_attr) * (size_t)n_local;
-    if (ranges_overlap(poses_new_dev, out_p, poses_dev, in_p) || ranges_overlap(poses_new_dev, out_p, attrs_dev, in_a) ||
-        ranges_overlap(attrs_new_dev, out_a, poses_dev, in_p) || ranges_overlap(attrs_new_dev, out_a, attrs_dev, in_a) ||
-        ranges_overlap(poses_new_dev, out_p, attrs_new_dev, out_a))
-        return fail(B2_ERR_INVALID, "resample kld: an output range overlaps an input range or the other output (the node double-buffers)");
+    RES(check_resample_outputs("resample kld", poses_dev, attrs_dev, n, n_max, first, n_local, poses_new_dev, attrs_new_dev));
     if (!(std::isfinite(kld->res_xy) && kld->res_xy > 0.0f) || !(std::isfinite(kld->epsilon) && kld->epsilon > 0.0))
         return fail(B2_ERR_INVALID, "resample kld: res_xy = %g and epsilon = %g must be finite and > 0", (double)kld->res_xy, kld->epsilon);
     if (!(std::isfinite(kld->res_z) && kld->res_z >= 0.0f)) return fail(B2_ERR_INVALID, "resample kld: res_z = %g must be finite and >= 0", (double)kld->res_z);
@@ -2798,10 +2767,11 @@ extern "C" int b2_pf_resample_kld(b2_pf* h, const b2_transform* poses_dev, const
         return fail(B2_ERR_INVALID, "resample kld: res_yaw = %g gives %g yaw sectors (1 .. %u)", (double)kld->res_yaw, Kd, B2_KLD_MAX_SECTORS);
     const uint32_t K = (uint32_t)Kd;
     CU(cudaSetDevice(h->map->device));
-    RES(kld_stats(h, attrs_dev, n));
-    const double S = h->h_res->S, L_min = h->h_res->L_min, L_max = h->h_res->L_max;
+    bool usable = false;
+    RES(pf_weight_stats(h, attrs_dev, n, true, &usable));
+    const double S = h->h_recs->res.S, L_max = h->h_recs->res.L_max;
     b2_kld_result res = {0, 0, S, L_max};
-    if (!(std::isfinite(S) && S > 0.0 && L_min >= 0.0)) { *out_host = res; return B2_OK; }       // as residual (SURVEY D31)
+    if (!usable) { *out_host = res; return B2_OK; }
     // the chunk schedule: sizes double from max(n_min, 2^16) up to n_max draws in all; 2^30 keeps a chunk within the scan's int item count
     const uint64_t c0 = std::min<uint64_t>(std::max<uint64_t>(kld->n_min, 1ull << 16), n_max);
     uint64_t max_len = 0;
@@ -2815,7 +2785,6 @@ extern "C" int b2_pf_resample_kld(b2_pf* h, const b2_transform* poses_dev, const
     RES(h->d_kld_w.reserve(n)); RES(h->d_kld_W.reserve(n)); RES(h->d_kld_keys.reserve(T)); RES(h->d_kld_first.reserve(T));
     RES(h->d_kld_parents.reserve(max_len)); RES(h->d_kld_slots.reserve(max_len)); RES(h->d_kld_flags.reserve(max_len)); RES(h->d_kld_cum.reserve(max_len));
     RES(h->d_kld_tmp.reserve(std::max<size_t>(std::max(scan_w, scan_f), 16)));
-    if (!h->d_kld.p) { RES(h->d_kld.reserve(1)); CU(cudaMallocHost((void**)&h->h_kld, sizeof(PfKldState))); }
     RES(kld_sector_table(h, K));
     // the hash set is cleared by memset on the stream: at 12 B per slot it costs less than one chunk's draws, and unlike epoch tags it keeps
     // every stored key a plain 64-bit word that one atomicCAS claims
@@ -2828,24 +2797,24 @@ extern "C" int b2_pf_resample_kld(b2_pf* h, const b2_transform* poses_dev, const
     LAUNCHED();
     const KldBins bins{kld->res_xy, kld->res_z, K, h->d_kld_tab.p};
     uint64_t d0 = 0, n_bins = 0, chunk = c0;
+    PfKldState* st = &h->d_recs.p->kld;
     bool done = false;
     while (!done && d0 < n_max) {
         const uint32_t len = (uint32_t)std::min<uint64_t>(chunk, n_max - d0), grid = (len + 255) / 256;
         k_pf_kld_draw<<<grid, 256, 0, h->stream>>>(h->d_kld_W.p, n, poses_dev, bins, seed, step, d0, len, h->d_kld_keys.p, h->d_kld_first.p, T - 1,
-                                                   h->d_kld_parents.p, h->d_kld_slots.p, h->d_kld.p);
+                                                   h->d_kld_parents.p, h->d_kld_slots.p, st);
         LAUNCHED();
         k_pf_kld_flags<<<grid, 256, 0, h->stream>>>(h->d_kld_first.p, h->d_kld_slots.p, d0, len, h->d_kld_flags.p);
         LAUNCHED();
         bytes = h->d_kld_tmp.cap;
         CU(cub::DeviceScan::InclusiveSum(h->d_kld_tmp.p, bytes, h->d_kld_flags.p, h->d_kld_cum.p, (int)len, h->stream));
         LAUNCHED();
-        k_pf_kld_stop<<<grid, 256, 0, h->stream>>>(h->d_kld_cum.p, d0, len, n_bins, kld->n_min, n_max, kld->epsilon, kld->z, h->d_kld.p);
+        k_pf_kld_stop<<<grid, 256, 0, h->stream>>>(h->d_kld_cum.p, d0, len, n_bins, kld->n_min, n_max, kld->epsilon, kld->z, st);
         LAUNCHED();
-        CU(cudaMemcpyAsync(h->h_kld, h->d_kld.p, sizeof(PfKldState), cudaMemcpyDeviceToHost, h->stream));
-        CU(cudaStreamSynchronize(h->stream));
-        const unsigned long long stop = h->h_kld->stop;
+        RES(pf_fetch(h, h->h_recs->kld));
+        const unsigned long long stop = h->h_recs->kld.stop;
         done = stop != ~0ull;
-        const uint64_t used = done ? (stop >> 32) + 1 : len, chunk_bins = done ? (stop & 0xffffffffull) : h->h_kld->bins;
+        const uint64_t used = done ? (stop >> 32) + 1 : len, chunk_bins = done ? (stop & 0xffffffffull) : h->h_recs->kld.bins;
         const uint64_t lo = std::max<uint64_t>(d0, first), hi = std::min<uint64_t>(d0 + used, (uint64_t)first + n_local);
         if (lo < hi) {
             const uint32_t n_k = (uint32_t)(hi - lo);
@@ -2879,10 +2848,11 @@ extern "C" int b2_pf_cluster_stats(b2_pf* h, const b2_transform* poses_dev, cons
         return fail(B2_ERR_INVALID, "cluster stats: max_records = %u must lie in [1, %u]", cfg->max_records, B2_CLUSTER_MAX_RECORDS);
     const uint32_t K = (uint32_t)Kd;
     CU(cudaSetDevice(h->map->device));
-    RES(kld_stats(h, attrs_dev, n));
-    const double S = h->h_res->S, L_min = h->h_res->L_min, L_max = h->h_res->L_max;
+    bool usable = false;
+    RES(pf_weight_stats(h, attrs_dev, n, true, &usable));
+    const double S = h->h_recs->res.S, L_max = h->h_recs->res.L_max;
     b2_cluster_result res = {0, 0, 0, 0, 0, 0, S, L_max};
-    if (!(std::isfinite(S) && S > 0.0 && L_min >= 0.0)) { *out_host = res; return B2_OK; }       // as KLD (SURVEY G1)
+    if (!usable) { *out_host = res; return B2_OK; }       // as KLD (SURVEY G1)
     uint64_t T = 1;                                      // the hash set: a power of two >= 2 n slots (load <= 1/2)
     while (T < 2 * (uint64_t)n) T <<= 1;
     size_t sort_c = 0, sort_p = 0;
@@ -2891,23 +2861,17 @@ extern "C" int b2_pf_cluster_stats(b2_pf* h, const b2_transform* poses_dev, cons
     RES(h->d_kld_keys.reserve(T)); RES(h->d_kld_first.reserve(T)); RES(h->d_cl_w.reserve(T)); RES(h->d_cl_cnt.reserve(T)); RES(h->d_cl_aux.reserve(T));
     RES(h->d_kld_w.reserve(n)); RES(h->d_kld_W.reserve(n)); RES(h->d_cl_slot.reserve(n)); RES(h->d_cl_key.reserve(n)); RES(h->d_cl_key2.reserve(n));
     RES(h->d_cl_idx.reserve(n)); RES(h->d_cl_idx2.reserve(n)); RES(h->d_kld_tmp.reserve(std::max<size_t>(std::max(sort_c, sort_p), 16)));
-    const size_t off_heads = sizeof(PfClusterState), off_recs = off_heads + sizeof(PfClusterHead) * B2_CLUSTER_MAX_RECORDS;
-    if (!h->d_cl.p) {
-        RES(h->d_cl.reserve(1)); RES(h->d_cl_heads.reserve(B2_CLUSTER_MAX_RECORDS)); RES(h->d_cl_recs.reserve(B2_CLUSTER_MAX_RECORDS));
-        CU(cudaMallocHost((void**)&h->h_cl, off_recs + sizeof(b2_particle_stats) * B2_CLUSTER_MAX_RECORDS));
-    }
-    const PfClusterState* st = reinterpret_cast<const PfClusterState*>(h->h_cl);
-    const PfClusterHead* heads = reinterpret_cast<const PfClusterHead*>(h->h_cl + off_heads);
-    const b2_particle_stats* recs = reinterpret_cast<const b2_particle_stats*>(h->h_cl + off_recs);
+    PfRecords* d = h->d_recs.p;
+    const PfRecords& hr = *h->h_recs;
     RES(kld_sector_table(h, K));
     CU(cudaMemsetAsync(h->d_kld_keys.p, 0, sizeof(unsigned long long) * T, h->stream));
     CU(cudaMemsetAsync(h->d_cl_w.p, 0, sizeof(unsigned long long) * T, h->stream));
     CU(cudaMemsetAsync(h->d_cl_cnt.p, 0, sizeof(unsigned int) * T, h->stream));
-    CU(cudaMemsetAsync(h->d_cl.p, 0, sizeof(PfClusterState), h->stream));
+    CU(cudaMemsetAsync(&d->cl, 0, sizeof(PfClusterState), h->stream));
     const KldBins bins{cfg->res_xy, cfg->res_z, K, h->d_kld_tab.p};
     const uint32_t grid_n = (n + 255) / 256, grid_T = (uint32_t)((T + 255) / 256);
     k_pf_cluster_insert<<<grid_n, 256, 0, h->stream>>>(poses_dev, attrs_dev, n, L_max, bins, h->d_kld_keys.p, T - 1, h->d_kld_first.p, h->d_cl_w.p, h->d_cl_cnt.p,
-                                                       h->d_cl_slot.p, h->d_cl.p);
+                                                       h->d_cl_slot.p, &d->cl);
     LAUNCHED();
     // A round joins every pair of touching bins and ends in the fixed point unless one of its bounded loops ran out, which the bounds (the
     // table's size, above any path or retry count) do not allow; the cap keeps the call finite even so.
@@ -2915,19 +2879,18 @@ extern "C" int b2_pf_cluster_stats(b2_pf* h, const b2_transform* poses_dev, cons
     for (;;) {
         if (rounds == B2_CLUSTER_MAX_ROUNDS) return fail(B2_ERR_CUDA, "cluster stats: the labelling did not settle within %u rounds", B2_CLUSTER_MAX_ROUNDS);
         rounds++;
-        CU(cudaMemsetAsync(&h->d_cl.p->retry, 0, sizeof(unsigned int), h->stream));
-        k_pf_cluster_hook<<<grid_T, 256, 0, h->stream>>>(h->d_kld_keys.p, T - 1, K, cfg->res_z > 0.0f ? 1 : 0, h->d_kld_first.p, h->d_cl_aux.p, h->d_cl.p);
+        CU(cudaMemsetAsync(&d->cl.retry, 0, sizeof(unsigned int), h->stream));
+        k_pf_cluster_hook<<<grid_T, 256, 0, h->stream>>>(h->d_kld_keys.p, T - 1, K, cfg->res_z > 0.0f ? 1 : 0, h->d_kld_first.p, h->d_cl_aux.p, &d->cl);
         LAUNCHED();
         k_pf_cluster_flatten<<<grid_T, 256, 0, h->stream>>>(h->d_kld_keys.p, T - 1, h->d_kld_first.p, h->d_cl_w.p, h->d_cl_cnt.p, h->d_cl_aux.p, h->d_cl_idx.p,
-                                                            h->d_kld_w.p, h->d_cl.p);
+                                                            h->d_kld_w.p, &d->cl);
         LAUNCHED();
-        CU(cudaMemcpyAsync(h->h_cl, h->d_cl.p, sizeof(PfClusterState), cudaMemcpyDeviceToHost, h->stream));
-        CU(cudaStreamSynchronize(h->stream));
-        if (st->fault) return fail(B2_ERR_CUDA, "cluster stats: the hash set of %llu slots had no room for %u particles", (unsigned long long)T, n);
-        if (!st->retry) break;
+        RES(pf_fetch(h, hr.cl));
+        if (hr.cl.fault) return fail(B2_ERR_CUDA, "cluster stats: the hash set of %llu slots had no room for %u particles", (unsigned long long)T, n);
+        if (!hr.cl.retry) break;
     }
-    const uint32_t m = st->n_clusters, n_records = std::min<uint32_t>(m, cfg->max_records);
-    res.n_clusters = m; res.n_records = n_records; res.bins = st->bins; res.n_clustered = st->n_clustered; res.weight_total = st->weight_total; res.rounds = rounds;
+    const uint32_t m = hr.cl.n_clusters, n_records = std::min<uint32_t>(m, cfg->max_records);
+    res.n_clusters = m; res.n_records = n_records; res.bins = hr.cl.bins; res.n_clustered = hr.cl.n_clustered; res.weight_total = hr.cl.weight_total; res.rounds = rounds;
     if (m == 0) {                                        // weights > 0, but no finite pose among them
         if (labels_dev) CU(cudaMemsetAsync(labels_dev, 0xff, sizeof(uint32_t) * (size_t)n, h->stream));
         CU(cudaStreamSynchronize(h->stream));
@@ -2945,9 +2908,8 @@ extern "C" int b2_pf_cluster_stats(b2_pf* h, const b2_transform* poses_dev, cons
         CU(cub::DeviceRadixSort::SortPairs(h->d_kld_tmp.p, bytes, h->d_kld_w.p, h->d_kld_W.p, h->d_cl_idx2.p, h->d_cl_idx.p, (int)m, 0, 64, h->stream));
         LAUNCHED();
     }
-    k_pf_cluster_rank<<<(m + 255) / 256, 256, 0, h->stream>>>(h->d_cl_idx.p, m, n_records, h->d_kld_keys.p, h->d_cl_w.p, h->d_cl_cnt.p, h->d_cl_aux.p, h->d_cl_heads.p);
+    k_pf_cluster_rank<<<(m + 255) / 256, 256, 0, h->stream>>>(h->d_cl_idx.p, m, n_records, h->d_kld_keys.p, h->d_cl_w.p, h->d_cl_cnt.p, h->d_cl_aux.p, d->heads);
     LAUNCHED();
-    CU(cudaMemcpyAsync(h->h_cl + off_heads, h->d_cl_heads.p, sizeof(PfClusterHead) * n_records, cudaMemcpyDeviceToHost, h->stream));
     k_pf_cluster_labels<<<grid_n, 256, 0, h->stream>>>(h->d_cl_slot.p, n, h->d_kld_first.p, h->d_cl_aux.p, n_records, labels_dev, h->d_cl_key.p, h->d_cl_idx.p);
     LAUNCHED();
     int bits = 1;                                        // sort keys 0 .. n_records
@@ -2955,26 +2917,26 @@ extern "C" int b2_pf_cluster_stats(b2_pf* h, const b2_transform* poses_dev, cons
     bytes = h->d_kld_tmp.cap;
     CU(cub::DeviceRadixSort::SortPairs(h->d_kld_tmp.p, bytes, h->d_cl_key.p, h->d_cl_key2.p, h->d_cl_idx.p, h->d_cl_idx2.p, (int)n, 0, bits, h->stream));
     LAUNCHED();
-    CU(cudaStreamSynchronize(h->stream));
+    RES(pf_fetch(h, hr.heads[0], n_records));
     uint64_t total = 0;
-    for (uint32_t r = 0; r < n_records; r++) total += heads[r].members;
+    for (uint32_t r = 0; r < n_records; r++) total += hr.heads[r].members;
     RES(h->d_cl_poses.reserve(total)); RES(h->d_cl_attrs.reserve(total));
     k_pf_cluster_gather<<<(uint32_t)((total + 255) / 256), 256, 0, h->stream>>>(h->d_cl_idx2.p, (uint32_t)total, poses_dev, attrs_dev, h->d_cl_poses.p, h->d_cl_attrs.p);
     LAUNCHED();
     uint64_t at = 0;
     for (uint32_t r = 0; r < n_records; r++) {
-        RES(estimate_launch(h, h->d_cl_poses.p + at, h->d_cl_attrs.p + at, heads[r].members));
-        CU(cudaMemcpyAsync(h->d_cl_recs.p + r, &h->d_est.p->rec, sizeof(b2_particle_stats), cudaMemcpyDeviceToDevice, h->stream));
-        at += heads[r].members;
+        RES(estimate_launch(h, h->d_cl_poses.p + at, h->d_cl_attrs.p + at, hr.heads[r].members));
+        CU(cudaMemcpyAsync(&d->recs[r], &d->est.rec, sizeof(b2_particle_stats), cudaMemcpyDeviceToDevice, h->stream));
+        at += hr.heads[r].members;
     }
-    CU(cudaMemcpyAsync(h->h_cl + off_recs, h->d_cl_recs.p, sizeof(b2_particle_stats) * n_records, cudaMemcpyDeviceToHost, h->stream));
-    CU(cudaStreamSynchronize(h->stream));
+    RES(pf_fetch(h, hr.recs[0], n_records));
     for (uint32_t r = 0; r < n_records; r++) {
+        const PfClusterHead& hd = hr.heads[r];
         b2_cluster_record& o = records_host[r];
         memset(&o, 0, sizeof(o));
-        o.stats = recs[r];
-        o.weight = (double)heads[r].weight_int / (double)res.weight_total;
-        o.weight_int = heads[r].weight_int; o.bins = heads[r].bins; o.key = heads[r].key;
+        o.stats = hr.recs[r];
+        o.weight = (double)hd.weight_int / (double)res.weight_total;
+        o.weight_int = hd.weight_int; o.bins = hd.bins; o.key = hd.key;
     }
     *out_host = res;
     return B2_OK;

@@ -1681,46 +1681,6 @@ __global__ void __launch_bounds__(256) k_pf_gladiator_p2p(PfPeers peers, b2_tran
 }
 #endif
 
-// compute_stats (rmcl_ros/src/rmcl/resampling.cu:41-92) over all SMs: FP64 block sums + max, the last block combines in block order
-__global__ void __launch_bounds__(256) k_pf_stats(const b2_particle_attr* __restrict__ attrs, uint32_t n, double* __restrict__ partials, unsigned int* __restrict__ ticket,
-                                                  float* __restrict__ out /* [sum, max] */)
-{
-    __shared__ double s_sum[8]; __shared__ float s_max[8]; __shared__ bool is_last;
-    double sum = 0.0; float mx = 0.0f;                                                     // max starts at 0 like the reference (:54)
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) { const float L = attrs[i].likelihood.mean; sum += (double)L; mx = fmaxf(mx, L); }
-    sum = warp_sum(sum);
-    #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    if ((threadIdx.x & 31) == 0) { s_sum[threadIdx.x >> 5] = sum; s_max[threadIdx.x >> 5] = mx; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double a = 0.0; float m = 0.0f;
-        for (int w = 0; w < 8; w++) { a += s_sum[w]; m = fmaxf(m, s_max[w]); }
-        partials[2 * blockIdx.x] = a; partials[2 * blockIdx.x + 1] = (double)m;
-        __threadfence();
-        is_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
-    }
-    __syncthreads();
-    if (!is_last) return;
-    __threadfence();
-    // the last block combines the block partials with all its threads in a fixed order (a serial loop over ~600 partials on one thread
-    // was 20 of this kernel's 29 us: one L2 round trip per iteration)
-    double a = 0.0; float m = 0.0f;
-    for (uint32_t b = threadIdx.x; b < gridDim.x; b += blockDim.x) { a += __ldcg(partials + 2 * b); m = fmaxf(m, (float)__ldcg(partials + 2 * b + 1)); }
-    a = warp_sum(a);
-    #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) { s_sum[threadIdx.x >> 5] = a; s_max[threadIdx.x >> 5] = m; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double t = 0.0; float tm = 0.0f;
-        for (int w = 0; w < 8; w++) { t += s_sum[w]; tm = fmaxf(tm, s_max[w]); }
-        out[0] = (float)t; out[1] = tm;
-        *ticket = 0u;
-    }
-}
-
 // ---------------------------------------------------------------------------------------------------------------------
 // Pose estimate of the particle set: RmclNode::estimateStats (rmcl_ros/src/nodes/rmcl_localization.cpp:642-731) in two read passes.
 // Pass 1 (k_pf_estimate_moments): likelihood sums, min / max, translation AABB, sum L t and sum L q q^T; its last block forms the weighted
@@ -2040,7 +2000,9 @@ struct PfResidualState {
     unsigned int ticket, pad;
 };
 #ifdef __CUDACC__
-// 4 B read per particle; grid, block and grid-stride order of k_pf_estimate_moments, so S is bit-equal to its L_sum for the same n
+// The set's weight statistics S, L_min and L_max (api.cu pf_weight_stats), for likelihoodStats (compute_stats, rmcl_ros/src/rmcl/
+// resampling.cu:41-92), the residual and KLD resamplers, the clusters and the recovery.  4 B read per particle; grid, block and grid-stride
+// order of k_pf_estimate_moments, so S is bit-equal to its L_sum for the same n
 __global__ void __launch_bounds__(256) k_pf_residual_stats(const b2_particle_attr* __restrict__ attrs, uint32_t n, double* __restrict__ partials, PfResidualState* __restrict__ st)
 {
     __shared__ double s_w[8 * B2_RES_NV], tot[B2_RES_NV];

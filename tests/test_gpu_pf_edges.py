@@ -1,4 +1,4 @@
-"""The particle filter's sensor update (k_pf_update<CORR, MAP>) and its likelihood statistics (k_pf_stats) at the edges of their launch
+"""The particle filter's sensor update (k_pf_update<CORR, MAP>) and its likelihood statistics (k_pf_residual_stats) at the edges of their launch
 geometry, against a float64 restatement of the same operations.
 
 The oracle restates the device's FP32 arithmetic op for op, so a mistake shared by both in the Gaussian evaluation stays invisible to it, and
@@ -717,7 +717,7 @@ def test_pf_beam_order(po, corr, ng_mode):
 
 @pytest.mark.gpu
 def test_pf_likelihood_stats_edges():
-    """likelihoodStats (k_pf_stats) on each side of one block, of a last-block combine that strides (more blocks than its 256 threads), of the
+    """likelihoodStats (k_pf_residual_stats) on each side of one block, of a last-block combine that strides (more blocks than a warp has lanes), of the
     grid cap 4 n_sm and far beyond it (grid-stride): float64 sum within 2e-6 relative, max exact; back-to-back calls of different sizes on
     one handle (the ticket is reset by each call's last block)."""
     import torch
@@ -740,3 +740,57 @@ def test_pf_likelihood_stats_edges():
     A2["likelihood"]["mean"][-1] = 0.5
     _, Ad2 = to_dev(scan_particles(1), A2)
     assert up.likelihoodStats(Ad2)[1] == np.float32(0.5)
+
+
+def scratch_call(up, op, Pd, Ad):
+    """one particle-filter call of test_pf_shared_scratch_calls -> what it returned and wrote, as numpy arrays"""
+    import torch
+    import rmcl_b200
+    n = Pd.shape[0]
+    if op == "stats":
+        return [np.array(up.likelihoodStats(Ad), np.float32)]
+    if op == "estimate":
+        return [up.estimateStats(Pd, Ad, max_induction_particles=n)]
+    if op == "recovery":
+        up.recoveryReset()
+        return [up.recoveryObserve(Ad, want_state=True)]
+    if op == "clusters":
+        labels = torch.zeros(n, dtype=torch.int32, device=Pd.device)
+        res, recs = up.estimateClusters(Pd, Ad, labels=labels)
+        return [res, recs, labels.cpu().numpy()]
+    Pn, An = torch.zeros_like(Pd), torch.zeros_like(Ad)
+    if op == "residual":
+        res = up.resampleResidual(Pd, Ad, Pn, An, seed=5, step=1)
+    else:
+        kld = rmcl_b200.KLDConfig.defaults()
+        kld.n_min = min(kld.n_min, n)                                      # n_min <= n_max = n
+        res = up.resampleKLD(Pd, Ad, Pn, An, kld, seed=5, step=2)
+    return [res, Pn.cpu().numpy(), An.cpu().numpy()]
+
+
+@pytest.mark.gpu
+def test_pf_shared_scratch_calls():
+    """likelihoodStats, estimateStats, resampleResidual, resampleKLD, estimateClusters and recoveryReset + recoveryObserve share one handle's
+    block partials, tickets and records: on one handle, in a seeded shuffled order at 1, 257, 4 n_sm 256 + 1 and 1 000 003 particles, each
+    call equals byte for byte the same call on a fresh handle.  likelihoodStats is the float32 of resampleResidual's weight_sum and weight_max
+    on the same set: every caller reads one pass of the set's weight statistics."""
+    import torch
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    rng = np.random.default_rng(17)
+    ops = ["stats", "estimate", "residual", "kld", "clusters", "recovery"]
+    shared = updater()
+    for n in (1, 257, 4 * sms * 256 + 1, 1_000_003):
+        P = scan_particles(n, n % 1000, 0.5, 0.3)
+        A = attrs(n)
+        A["likelihood"]["mean"] = rng.uniform(0, 0.2, n).astype(np.float32)
+        A["likelihood"]["mean"][rng.integers(0, n, max(1, n // 100))] = 0.0
+        A["likelihood"]["mean"][0] = 0.1
+        Pd, Ad = to_dev(P, A)
+        got = {}
+        for op in (ops[i] for i in rng.permutation(len(ops))):
+            got[op] = scratch_call(shared, op, Pd, Ad)
+            want = scratch_call(updater(), op, Pd, Ad)
+            assert [a.tobytes() for a in got[op]] == [b.tobytes() for b in want], (n, op)
+        r = got["residual"][0]
+        assert got["stats"][0].tobytes() == np.array([r["weight_sum"], r["weight_max"]], np.float32).tobytes(), (n, got["stats"][0], r)
+        assert r["n_particles"] > 0 and got["clusters"][0]["n_records"] >= 1, n
