@@ -610,6 +610,56 @@ B2_API int b2_pf_recovery_inject(b2_pf* h, b2_transform* poses_dev, b2_particle_
                                  const double bb_max[6], const b2_surface_config* surface /* nullable */, uint32_t max_tries, uint64_t seed, uint32_t step,
                                  b2_recovery_result* out_host /* nullable */);
 
+/* ---------------------------------------------------------------- distance field ----------------------------- */
+/* Truncated distance field of the map and the particle filter's sensor update from it (no reference counterpart; AMCL's
+ * laser_model_type likelihood_field; SURVEY appendix K).  The closest-point update (correspondence_type 1) walks the BVH once per
+ * (particle, beam); the field is built once per map and each beam then costs one interpolated lookup, whatever the depth of the tree.
+ *
+ * Definition (origin, h, dims, trunc).  Node (i, j, k) sits at x = origin.x + (float)i * h (likewise y, z; each op rounded) and holds
+ * min(d, trunc), d the closest-point distance of b2_rcc's closest-point correspondences at that position (a bounded query: same value).
+ * Storage: a dense uint32 index over bricks of 8^3 cells (0xFFFFFFFF: not allocated) and, per allocated brick, its 9^3 nodes (z, y, x; x
+ * fastest; the far face is shared with the next brick).  A brick is allocated iff the distance from its centre node is < trunc + 8h; every
+ * node of an unallocated brick has value trunc.  Memory: 4 B per brick of the box plus 2916 B per allocated brick.
+ * Lookup at p: g = (p - origin) * (1 / h) per axis; inside iff 0 <= g <= dims - 1; cell = min(floor(g), dims - 2); trilinear in the order
+ * x, y, z.  Unallocated brick or finite point outside the box: trunc.  Non-finite point: +inf.  No texture filtering.
+ * Accuracy: |field(p) - min(d_exact(p), trunc)| <= (sqrt(3) / 2) h plus float rounding.  Choose h from this bound.
+ *
+ * b2_dfield_create: builds the field on the map's device (classify bricks, scan, fill nodes) and synchronises.  params.bb_min / bb_max
+ *  (both or neither, 3 floats each) give the box; NULL: the map's AABB grown by `truncation`.  The field keeps a reference to the map,
+ *  which may be destroyed first.  It is a snapshot: after b2_mesh_refit it still describes the map as it was -- destroy and recreate it.
+ *  Refused (B2_ERR_INVALID, nothing built, *out = NULL): null arguments, one of bb_min / bb_max null, resolution or truncation not finite
+ *  and > 0, non-finite bounds, bb_min >= bb_max on an axis, more than 2^24 nodes on an axis (8 x bricks + 1, so that (float)i is exact),
+ *  more than 2^32 - 2 bricks.  An empty map: B2_ERR_NO_MAP; allocation failure: B2_ERR_OOM.
+ * b2_dfield_get_info: the grid, counts, bytes resident and the build's wall time.
+ * b2_dfield_download: the raw layout (bricks_total uint32 index words, bricks_allocated x 729 floats), either pointer may be NULL.
+ * b2_dfield_query: lookups of n points (xyz), synchronous.  src_is_device != 0: points and dist_out are device addresses on the field's
+ *  device; otherwise host arrays.
+ * b2_pf_sensor_update_field: b2_pf_sensor_update's contract (DEVICE poses / attrs, HOST beams, merge per particle in beam order with the
+ *  MAX_N_MEAS clamp, attrs read-modified-written once, enqueued on the handle's stream) with the error e = field(orig + dir * range), the
+ *  closest-point branch's point; params.correspondence_type is ignored.  Where e equals the closest-point distance the evaluation is bit-equal
+ *  to correspondence_type 1.  Elsewhere each beam's likelihood differs from it by at most exp(-1/2) / (dist_sigma * denom) * (sqrt(3)/2) h
+ *  while d < trunc - (sqrt(3)/2) h, denom = sqrt(2 pi dist_sigma^2); beyond trunc the clamp moves an evaluation by at most
+ *  exp(-trunc^2 / (2 dist_sigma^2)) / denom (exp(-4.5) / denom for trunc = 3 dist_sigma).  Refused (B2_ERR_INVALID, no launch): null h,
+ *  f, Tsb or params, null buffers with n > 0 or n_beams > 0, a field on another device than the handle. */
+typedef struct b2_dfield b2_dfield;
+typedef struct { float resolution, truncation; const float* bb_min; const float* bb_max; } b2_dfield_params;               /* 24 B */
+typedef char b2_dfield_params_is_24_bytes[sizeof(b2_dfield_params) == 24 ? 1 : -1];
+typedef struct {
+    uint32_t dims[3], brick_dims[3];          /* nodes / bricks per axis */
+    float origin[3], resolution, inv_resolution, truncation;
+    uint64_t bricks_total, bricks_allocated, bytes;
+    float build_ms;                           /* wall time of b2_dfield_create */
+    int device;
+} b2_dfield_info;                                                                                                         /* 80 B */
+typedef char b2_dfield_info_is_80_bytes[sizeof(b2_dfield_info) == 80 ? 1 : -1];
+B2_API int b2_dfield_create(b2_mesh* map, const b2_dfield_params* params, b2_dfield** out);
+B2_API int b2_dfield_destroy(b2_dfield* f);
+B2_API int b2_dfield_get_info(const b2_dfield* f, b2_dfield_info* info);
+B2_API int b2_dfield_download(const b2_dfield* f, uint32_t* index_host, float* bricks_host);
+B2_API int b2_dfield_query(b2_dfield* f, const float* points_xyz, uint32_t n, float* dist_out, int src_is_device);
+B2_API int b2_pf_sensor_update_field(b2_pf* h, const b2_dfield* f, const b2_transform* poses_dev, b2_particle_attr* attrs_dev, uint32_t n_particles,
+                                     const b2_transform* Tsb, const b2_range_meas* beams_host, uint32_t n_beams, const b2_pf_params* params);
+
 /* ---------------------------------------------------------------- introspection ------------------------------ */
 /* CUDA-event timing of the kernels inside b2_rcc_correct_once*(): when enabled, events are recorded on the handle's stream around the
  * find kernel and around the reduction/Umeyama kernels; b2_rcc_last_timing returns the two durations of the most recent call (ms). */

@@ -64,6 +64,27 @@ private:
 };
 using B200MapPtr = std::shared_ptr<B200Map>;
 
+// truncated distance field of a map (b2_dfield_*; AMCL's likelihood field, no reference counterpart): built once on the map's device, a
+// snapshot of the map (rebuild after B200Map::refit).  bb_min / bb_max null: the map's box grown by truncation.
+class B200DistanceField {
+public:
+    B200DistanceField(B200MapPtr map, float resolution, float truncation, const float* bb_min = nullptr, const float* bb_max = nullptr) : map_(std::move(map))
+    {
+        if (!map_) throw std::runtime_error("NO MAP");
+        const b2_dfield_params p{resolution, truncation, bb_min, bb_max};
+        b2_check(b2_dfield_create(map_->handle(), &p, &f_), "B200DistanceField");
+    }
+    ~B200DistanceField() { b2_dfield_destroy(f_); }
+    B200DistanceField(const B200DistanceField&) = delete; B200DistanceField& operator=(const B200DistanceField&) = delete;
+    b2_dfield* handle() const { return f_; }
+    b2_dfield_info info() const { b2_dfield_info i; b2_check(b2_dfield_get_info(f_, &i), "B200DistanceField::info"); return i; }
+    // lookups of n points (xyz), synchronous; on_device: both arrays are device addresses
+    void query(const float* points_xyz, uint32_t n, float* dist_out, bool on_device = false) { b2_check(b2_dfield_query(f_, points_xyz, n, dist_out, on_device ? 1 : 0), "B200DistanceField::query"); }
+private:
+    B200MapPtr map_;
+    b2_dfield* f_ = nullptr;
+};
+
 // device-resident point cloud views (rm::PointCloudView_<VRAM_CUDA>)
 struct PointCloudViewB200 { rm::MemoryView<rm::Vector3f, rm::VRAM_CUDA> points; rm::MemoryView<uint8_t, rm::VRAM_CUDA> mask; rm::MemoryView<rm::Vector3f, rm::VRAM_CUDA> normals; };
 
@@ -388,9 +409,13 @@ public:
     void setBeams(const std::vector<RangeMeasurement>& beams) { beams_ = beams; input_ = CloudInput{}; }
     // how rays are mapped to lanes (a schedule, results identical): 0 beams of one particle, 1 particles, 2 particles sorted by pose, 3 (default) by timing
     void setMapping(int mode) { b2_check(b2_pf_set_mapping(h_, mode), "setMapping"); }
+    // likelihood field: while a field is set, the VRAM update() evaluates each beam from it (b2_pf_sensor_update_field) instead of tracing the
+    // map, and the RAM update() throws.  The updater keeps the field alive; nullptr returns to the map.
+    void setDistanceField(std::shared_ptr<B200DistanceField> field) { field_ = std::move(field); }
     // ParticleUpdater<RAM>::update
     ParticleUpdateResults update(rm::MemoryView<rm::Transform, rm::RAM> poses, rm::MemoryView<ParticleAttributes, rm::RAM> attrs, const ParticleUpdateConfig& = {})
     {
+        if (field_) throw std::runtime_error("update: a distance field is set; the field update takes device particles only");
         sample_input();
         b2_check(b2_pf_sensor_update_host(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(),
                                           reinterpret_cast<const b2_transform*>(&Tsb_), reinterpret_cast<const b2_range_meas*>(beams_.data()), (uint32_t)beams_.size(), &config), "update");
@@ -400,6 +425,12 @@ public:
     ParticleUpdateResults update(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs, const ParticleUpdateConfig& = {}) B2_PF_OVERRIDE
     {
         sample_input();
+        if (field_) {
+            b2_check(b2_pf_sensor_update_field(h_, field_->handle(), reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()),
+                                               (uint32_t)poses.size(), reinterpret_cast<const b2_transform*>(&Tsb_), reinterpret_cast<const b2_range_meas*>(beams_.data()),
+                                               (uint32_t)beams_.size(), &config), "update");
+            return {};
+        }
         b2_check(b2_pf_sensor_update(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(),
                                      reinterpret_cast<const b2_transform*>(&Tsb_), reinterpret_cast<const b2_range_meas*>(beams_.data()), (uint32_t)beams_.size(), &config), "update");
         return {};
@@ -558,6 +589,7 @@ private:
     }
     B200MapPtr map_;
     b2_pf* h_ = nullptr;
+    std::shared_ptr<B200DistanceField> field_;
     rm::Transform Tsb_ = rm::Transform::Identity();
     std::vector<RangeMeasurement> beams_;
     CloudInput input_;

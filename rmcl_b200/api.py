@@ -169,7 +169,8 @@ EXPORTS = [
     "b2_micp_correct", "b2_pf_init_uniform", "b2_pf_init_gaussian", "b2_pf_estimate_stats", "b2_rcc_set_cloud_o1dn",
     "b2_rcc_set_cloud_spherical", "b2_pf_sample_cloud", "b2_pf_resample_residual", "b2_pf_project_to_surface",
     "b2_pf_resample_kld", "b2_pf_cluster_stats", "b2_micp_pose_covariance", "b2_pf_recovery_reset", "b2_pf_recovery_observe",
-    "b2_pf_recovery_inject",
+    "b2_pf_recovery_inject", "b2_dfield_create", "b2_dfield_destroy", "b2_dfield_get_info", "b2_dfield_download", "b2_dfield_query",
+    "b2_pf_sensor_update_field",
 ]
 
 
@@ -715,6 +716,75 @@ def umeyama_transform(stats, device=0):
     return out
 
 
+class _DfieldParams(C.Structure):
+    _fields_ = [("resolution", C.c_float), ("truncation", C.c_float), ("bb_min", C.c_void_p), ("bb_max", C.c_void_p)]
+
+
+class _DfieldInfo(C.Structure):
+    _fields_ = [("dims", C.c_uint32 * 3), ("brick_dims", C.c_uint32 * 3), ("origin", C.c_float * 3), ("resolution", C.c_float), ("inv_resolution", C.c_float),
+                ("truncation", C.c_float), ("bricks_total", C.c_uint64), ("bricks_allocated", C.c_uint64), ("bytes", C.c_uint64), ("build_ms", C.c_float),
+                ("device", C.c_int)]
+
+
+class DistanceField:
+    """Truncated distance field of a map (b2_dfield_*; AMCL's likelihood field): nodes every `resolution` m over [bb_min, bb_max] (default:
+    the map's box grown by `truncation`) holding min(distance to the surface, truncation), stored as sparse 8^3-cell bricks.  Lookups are
+    trilinear, within (sqrt(3)/2) * resolution of the clamped distance.  A snapshot of the map: rebuild it after Map.refit."""
+
+    def __init__(self, map_: Map, resolution, truncation, bb_min=None, bb_max=None):
+        self.map = map_                 # the library keeps its own reference too
+        lo = None if bb_min is None else _f32(bb_min).reshape(3)
+        hi = None if bb_max is None else _f32(bb_max).reshape(3)
+        prm = _DfieldParams(float(resolution), float(truncation), None if lo is None else lo.ctypes.data, None if hi is None else hi.ctypes.data)
+        h = C.c_void_p()
+        _chk(load_library().b2_dfield_create(map_._h, C.byref(prm), C.byref(h)))
+        self._h = h
+
+    def close(self):
+        if getattr(self, "_h", None):
+            load_library().b2_dfield_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def info(self):
+        inf = _DfieldInfo()
+        _chk(load_library().b2_dfield_get_info(self._h, C.byref(inf)))
+        out = {k: getattr(inf, k) for k, _ in _DfieldInfo._fields_}
+        for k in ("dims", "brick_dims", "origin"):
+            out[k] = tuple(out[k])
+        return out
+
+    def download(self):
+        """-> (index uint32 (bz, by, bx): brick slot or 0xFFFFFFFF, bricks float32 (n_allocated, 9, 9, 9) indexed [z, y, x])"""
+        inf = self.info()
+        bx, by, bz = inf["brick_dims"]
+        index = np.empty((bz, by, bx), np.uint32)
+        bricks = np.empty((inf["bricks_allocated"], 9, 9, 9), np.float32)
+        _chk(load_library().b2_dfield_download(self._h, _p(index), _p(bricks) if bricks.size else None))
+        return index, bricks
+
+    def query(self, points):
+        """Lookups of (n, 3) points: numpy in, numpy out; a float32 CUDA tensor in, a CUDA tensor out (read in place)."""
+        lib = load_library()
+        if hasattr(points, "data_ptr"):
+            import torch
+            pts = points.reshape(-1, 3)
+            out = torch.empty(pts.shape[0], dtype=torch.float32, device=pts.device)
+            if pts.dtype != torch.float32:
+                raise TypeError("expected a float32 tensor")
+            _chk(lib.b2_dfield_query(self._h, _devptr(pts), C.c_uint32(pts.shape[0]), _devptr(out), C.c_int(1)))
+            return out
+        pts = _f32(points).reshape(-1, 3)
+        out = np.empty(len(pts), np.float32)
+        _chk(lib.b2_dfield_query(self._h, _p(pts), C.c_uint32(len(pts)), _p(out), C.c_int(0)))
+        return out
+
+
 class PCDSensorUpdaterB200:
     """Particle-filter sensor update: ParticleUpdater<MemT>::update (rmcl_ros/include/rmcl_ros/rmcl/ParticleUpdater.hpp:39-43) with the
     hot loop of PCDSensorUpdaterEmbree::update (PCDSensorUpdaterEmbree.cpp:290-342).  Its beams are drawn from the cloud of setInput
@@ -730,6 +800,7 @@ class PCDSensorUpdaterB200:
         self.seed = 0                   # the same on every rank of a sharded particle set
         self.step = 0                   # advanced by every update() that samples the input
         self._input = None
+        self._field = None
 
     def close(self):
         if getattr(self, "_h", None):
@@ -774,11 +845,20 @@ class PCDSensorUpdaterB200:
         The reference is kept; the data is read when update() runs."""
         self._input = cloud
 
+    def setDistanceField(self, field):
+        """While a DistanceField is set, update() on CUDA tensors evaluates each beam from it (b2_pf_sensor_update_field) instead of tracing
+        the map; update() on numpy arrays raises B2Error.  None returns to the map."""
+        if field is not None and not isinstance(field, DistanceField):
+            raise TypeError("expected a DistanceField or None")
+        self._field = field
+
     def update(self, particle_poses, particle_attrs, Tsb, beams=None, params: PFParams | None = None, inplace=False):
         """RAM variant: numpy arrays in, updated attrs array out (inplace=True: the caller's attrs array is updated itself, as the reference's
         update(MemoryView) does -- no staging copy; pin the arrays and the transfers overlap the kernel).  VRAM variant: torch CUDA tensors, attrs
         updated in place.  beams=None: `samples` beams are drawn from the setInput cloud with (seed, step), then step advances by one."""
         prm = params or self.config
+        if self._field is not None and not hasattr(particle_poses, "data_ptr"):
+            raise B2Error(-1, "update: a distance field is set; the field update takes CUDA tensors only")
         if beams is None:
             if self._input is None:
                 raise B2Error(-1, "update: no beams and no input cloud (setInput first)")
@@ -790,6 +870,10 @@ class PCDSensorUpdaterB200:
         lib = load_library()
         if hasattr(particle_poses, "data_ptr"):
             n = particle_poses.numel() * particle_poses.element_size() // 32
+            if self._field is not None:
+                _chk(lib.b2_pf_sensor_update_field(self._h, self._field._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(n), _p(Tsb),
+                                                   _p(beams), C.c_uint32(len(beams)), C.byref(prm)))
+                return particle_attrs
             _chk(lib.b2_pf_sensor_update(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(n), _p(Tsb), _p(beams),
                                          C.c_uint32(len(beams)), C.byref(prm)))
             return particle_attrs

@@ -2000,6 +2000,7 @@ static int pf_init(b2_pf* h)
     CU(cudaFuncSetAttribute(k_pf_update<1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
     CU(cudaFuncSetAttribute(k_pf_update<0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
     CU(cudaFuncSetAttribute(k_pf_update<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
+    CU(cudaFuncSetAttribute(k_pf_update_field, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
     CU(cudaEventCreate(&h->ev_m0)); CU(cudaEventCreate(&h->ev_m1));
     { const char* e = getenv("B2_PF_MAP"); if (e) h->map_mode = std::min(3, std::max(0, atoi(e))); }
     return B2_OK;
@@ -2264,6 +2265,174 @@ extern "C" int b2_pf_sensor_update_host(b2_pf* h, const b2_transform* poses, b2_
     }
     if (n_chunks > 1) { CU(cudaEventRecord(h->ev_side, h->side)); CU(cudaStreamWaitEvent(h->stream, h->ev_side, 0)); }
     CU(cudaStreamSynchronize(h->stream));
+    return B2_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// truncated distance field (kernels.cuh: FIELD, LAYOUT, LOOKUP).  A snapshot of the map at creation: it keeps a reference to the map, and a
+// b2_mesh_refit afterwards leaves it as built.
+// ---------------------------------------------------------------------------------------------------------------------
+struct b2_dfield {
+    b2_mesh* map = nullptr;
+    DfieldView v{};
+    uint64_t n_bricks = 0, n_alloc = 0;
+    float build_ms = 0.f;
+    DevBuf<uint32_t> d_index; DevBuf<float> d_bricks;
+    DevBuf<float> d_qin, d_qout;                      // staging of host queries
+};
+
+extern "C" int b2_dfield_destroy(b2_dfield* f)
+{
+    if (!f) return B2_OK;
+    cudaSetDevice(f->map->device);
+    cudaDeviceSynchronize();
+    f->d_index.release(); f->d_bricks.release(); f->d_qin.release(); f->d_qout.release();
+    b2_mesh* map = f->map;
+    delete f;
+    (void)cudaGetLastError();
+    mesh_unref(map);
+    return B2_OK;
+}
+
+// grid-stride launches over up to 2^32 x 729 items: blocks of 256, at most 64 per SM
+static unsigned dfield_grid(int n_sm, uint64_t n) { return (unsigned)std::max<uint64_t>(1u, std::min<uint64_t>((n + 255u) / 256u, (uint64_t)n_sm * 64u)); }
+
+static int dfield_build(b2_dfield* f)
+{
+    b2_mesh* map = f->map;
+    int n_sm = 0; CU(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, map->device));
+    const BvhView bvh = map->view();
+    float ta, ta2, trunc2; df_limits(f->v, ta, ta2, trunc2);
+    const uint64_t nb = f->n_bricks;
+    RES(f->d_index.reserve(nb));
+    DevBuf<uint32_t> offs, list; DevBuf<unsigned char> tmp;
+    int rc = offs.reserve(nb);
+    if (rc == B2_OK) {
+        k_dfield_classify<<<dfield_grid(n_sm, nb), 256>>>(bvh, f->v, nb, ta, ta2, f->d_index.p);
+        g_launches.fetch_add(1);
+        size_t tmp_bytes = 0;
+        cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, f->d_index.p, offs.p, (int64_t)nb);
+        if (e == cudaSuccess) rc = tmp.reserve(std::max<size_t>(tmp_bytes, 1));
+        if (e == cudaSuccess && rc == B2_OK) e = cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, f->d_index.p, offs.p, (int64_t)nb);
+        uint32_t last[2] = {0u, 0u};
+        if (e == cudaSuccess && rc == B2_OK) e = cudaMemcpy(&last[0], offs.p + (nb - 1), sizeof(uint32_t), cudaMemcpyDeviceToHost);
+        if (e == cudaSuccess && rc == B2_OK) e = cudaMemcpy(&last[1], f->d_index.p + (nb - 1), sizeof(uint32_t), cudaMemcpyDeviceToHost);
+        if (e != cudaSuccess) rc = fail(B2_ERR_CUDA, "distance field classification failed: %s", cudaGetErrorString(e));
+        f->n_alloc = (uint64_t)last[0] + last[1];
+        tmp.release();
+        if (rc == B2_OK && f->n_alloc) rc = list.reserve(f->n_alloc);
+        if (rc == B2_OK && f->n_alloc) rc = f->d_bricks.reserve(f->n_alloc * B2_DF_NODES);
+        if (rc == B2_OK) {
+            k_dfield_index<<<dfield_grid(n_sm, nb), 256>>>(nb, offs.p, f->d_index.p, f->n_alloc ? list.p : nullptr);
+            g_launches.fetch_add(1);
+            if (f->n_alloc) {
+                f->v.index = f->d_index.p; f->v.bricks = f->d_bricks.p;
+                k_dfield_fill<<<dfield_grid(n_sm, f->n_alloc * B2_DF_NODES), 256>>>(bvh, f->v, list.p, f->n_alloc * B2_DF_NODES, trunc2, f->d_bricks.p);
+                g_launches.fetch_add(1);
+            }
+            e = cudaDeviceSynchronize();
+            if (e == cudaSuccess) e = cudaGetLastError();
+            if (e != cudaSuccess) rc = fail(B2_ERR_CUDA, "distance field build failed: %s", cudaGetErrorString(e));
+        }
+    }
+    offs.release(); list.release();
+    f->v.index = f->d_index.p; f->v.bricks = f->d_bricks.p;
+    return rc;
+}
+
+extern "C" int b2_dfield_create(b2_mesh* map, const b2_dfield_params* prm, b2_dfield** out)
+{
+    NOTNULL(out); *out = nullptr;
+    NOTNULL(map); NOTNULL(prm);
+    if ((prm->bb_min == nullptr) != (prm->bb_max == nullptr)) return fail(B2_ERR_INVALID, "dfield_create: give both bb_min and bb_max or neither");
+    const float h = prm->resolution, trunc = prm->truncation;
+    if (!(std::isfinite(h) && h > 0.0f && std::isfinite(trunc) && trunc > 0.0f))
+        return fail(B2_ERR_INVALID, "dfield_create: resolution %g and truncation %g must be finite and > 0", (double)h, (double)trunc);
+    if (map->n_faces == 0) return fail(B2_ERR_NO_MAP, "EMPTY MAP");
+    float lo[3], hi[3];
+    CU(cudaSetDevice(map->device));
+    if (prm->bb_min) { for (int k = 0; k < 3; k++) { lo[k] = prm->bb_min[k]; hi[k] = prm->bb_max[k]; } }
+    else {
+        // the map's AABB: the union of the root's child boxes (exact float AABBs of the triangles; empty slots are +inf / -inf), grown by trunc
+        B2Node8 root;
+        CU(cudaMemcpy(&root, map->d_nodes, sizeof(B2Node8), cudaMemcpyDeviceToHost));
+        for (int k = 0; k < 3; k++) {
+            float a = INFINITY, b = -INFINITY;
+            for (int s = 0; s < 8; s++) { a = std::min(a, root.lo[k][s]); b = std::max(b, root.hi[k][s]); }
+            lo[k] = a - trunc; hi[k] = b + trunc;
+        }
+    }
+    DfieldView v; uint64_t nb = 0;
+    if (const char* why = df_grid(lo, hi, h, trunc, &v, &nb)) return fail(B2_ERR_INVALID, "dfield_create: %s", why);
+    b2_dfield* f = new (std::nothrow) b2_dfield();
+    if (!f) return fail(B2_ERR_OOM, "out of host memory");
+    f->map = map; f->v = v; f->n_bricks = nb;
+    map->refs.fetch_add(1);             // released in b2_dfield_destroy
+    const auto t0 = std::chrono::steady_clock::now();
+    const int rc = dfield_build(f);
+    if (rc != B2_OK) { b2_dfield_destroy(f); return rc; }
+    f->build_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    *out = f;
+    return B2_OK;
+}
+
+extern "C" int b2_dfield_get_info(const b2_dfield* f, b2_dfield_info* info)
+{
+    NOTNULL(f); NOTNULL(info);
+    b2_dfield_info r{};
+    r.dims[0] = f->v.dx; r.dims[1] = f->v.dy; r.dims[2] = f->v.dz;
+    r.brick_dims[0] = f->v.bx; r.brick_dims[1] = f->v.by; r.brick_dims[2] = f->v.bz;
+    r.origin[0] = f->v.ox; r.origin[1] = f->v.oy; r.origin[2] = f->v.oz;
+    r.resolution = f->v.h; r.inv_resolution = f->v.inv_h; r.truncation = f->v.trunc;
+    r.bricks_total = f->n_bricks; r.bricks_allocated = f->n_alloc;
+    r.bytes = sizeof(uint32_t) * f->n_bricks + sizeof(float) * B2_DF_NODES * f->n_alloc;
+    r.build_ms = f->build_ms; r.device = f->map->device;
+    *info = r;
+    return B2_OK;
+}
+
+extern "C" int b2_dfield_download(const b2_dfield* f, uint32_t* index_host, float* bricks_host)
+{
+    NOTNULL(f);
+    CU(cudaSetDevice(f->map->device));
+    if (index_host) CU(cudaMemcpy(index_host, f->d_index.p, sizeof(uint32_t) * f->n_bricks, cudaMemcpyDeviceToHost));
+    if (bricks_host && f->n_alloc) CU(cudaMemcpy(bricks_host, f->d_bricks.p, sizeof(float) * B2_DF_NODES * f->n_alloc, cudaMemcpyDeviceToHost));
+    return B2_OK;
+}
+
+extern "C" int b2_dfield_query(b2_dfield* f, const float* points_xyz, uint32_t n, float* dist_out, int src_is_device)
+{
+    NOTNULL(f);
+    if (n == 0) return B2_OK;
+    NOTNULL(points_xyz); NOTNULL(dist_out);
+    CU(cudaSetDevice(f->map->device));
+    const float* pin = points_xyz; float* pout = dist_out;
+    if (!src_is_device) {
+        RES(f->d_qin.reserve(3 * (size_t)n)); RES(f->d_qout.reserve(n));
+        CU(cudaMemcpy(f->d_qin.p, points_xyz, sizeof(float) * 3 * (size_t)n, cudaMemcpyHostToDevice));
+        pin = f->d_qin.p; pout = f->d_qout.p;
+    }
+    k_dfield_query<<<(n + 255) / 256, 256>>>(f->v, pin, n, pout);
+    LAUNCHED();
+    if (!src_is_device) CU(cudaMemcpy(dist_out, pout, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
+    else CU(cudaDeviceSynchronize());
+    return B2_OK;
+}
+
+extern "C" int b2_pf_sensor_update_field(b2_pf* h, const b2_dfield* f, const b2_transform* poses_dev, b2_particle_attr* attrs_dev, uint32_t n,
+                                         const b2_transform* Tsb, const b2_range_meas* beams, uint32_t n_beams, const b2_pf_params* prm)
+{
+    NOTNULL(h); NOTNULL(f); NOTNULL(Tsb); NOTNULL(prm);
+    if (n) { NOTNULL(poses_dev); NOTNULL(attrs_dev); }
+    if (n_beams) NOTNULL(beams);
+    if (f->map->device != h->map->device) return fail(B2_ERR_INVALID, "pf_sensor_update_field: the field is on device %d, the handle on device %d", f->map->device, h->map->device);
+    CU(cudaSetDevice(h->map->device));
+    if (n == 0 || n_beams == 0) return B2_OK;
+    uint32_t ppb = 1;
+    RES(pf_prepare_beams(h, beams, n_beams, &ppb));
+    const uint32_t grid = (n + ppb - 1) / ppb;
+    k_pf_update_field<<<grid, B2_PF_BLOCK, sizeof(float) * (size_t)n_beams * ppb, h->stream>>>(f->v, poses_dev, attrs_dev, n, *Tsb, h->d_beams.p, n_beams, *prm, ppb);
+    LAUNCHED();
     return B2_OK;
 }
 

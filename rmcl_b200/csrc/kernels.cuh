@@ -1181,6 +1181,180 @@ __global__ void __launch_bounds__(B2_PF_BLOCK, 7) k_pf_update(BvhView bvh, const
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Truncated distance field of the map (b2_dfield_*; no reference counterpart, SURVEY appendix K) and the particle filter's sensor update
+// from it (b2_pf_sensor_update_field).
+// FIELD (origin, h, dims, trunc): node (i, j, k) sits at x = add(origin.x, mul((float)i, h)) (likewise y, z) and holds
+//   v = min(sqrtf(d2), trunc), d2 the closest point's result (trace.cuh) at that position; no face within trunc gives trunc.  Every stored
+//   value equals orc_closest_point's d_out clamped at trunc, whatever the BVH and builder: the bounded query (trace.cuh) returns the same
+//   clamped value as the unbounded one.
+// LAYOUT: sparse bricks of 8^3 cells.  A dense uint32 index over bdims = ceil((dims - 1) / 8) bricks per axis (z-major, x fastest) holds each
+//   brick's slot or B2_NOBRICK; an allocated brick stores its 9^3 nodes 8b .. 8b + 8 per axis (z, y, x; x fastest), so the 8 corners of a
+//   cell always sit in one brick.  A brick is allocated iff the distance from its centre node 8b + 4 is < trunc + 8h (bounded query at that
+//   limit: strict, so that the bounded and the unbounded query decide alike).  Its nodes lie within 4 sqrt(3) h < 8h of the centre and the
+//   distance is 1-Lipschitz, so every node of an unallocated brick has value trunc (up to float rounding of the positions, far below h).
+// LOOKUP at p: g = mul(sub(p, origin), inv_h) per axis (inv_h = the float 1 / h).  Inside iff 0 <= g <= dims - 1 on every axis; the cell is
+//   min(floor(g), dims - 2), t = sub(g, cell); trilinear in the fixed order x, y, z, each lerp add(mul(a, sub(1, t)), mul(b, t)).  An
+//   unallocated brick or a finite point outside the box gives trunc; a non-finite point gives +inf (the closest-point update's miss).
+// ACCURACY: min(d, trunc) is 1-Lipschitz and the trilinear weights w_i of the corners c_i satisfy sum w_i |c_i - p|^2 = h^2 sum_k u_k (1 - u_k)
+//   <= 3h^2 / 4, so |field(p) - min(d_exact(p), trunc)| <= (sqrt(3) / 2) h, plus float rounding of the nodes and of the interpolation.
+// ---------------------------------------------------------------------------------------------------------------------
+#define B2_NOBRICK 0xFFFFFFFFu
+#define B2_DF_NODES 729u                 // 9^3 nodes per brick
+
+struct DfieldView {
+    const uint32_t* index;               // [bz][by][bx] -> brick slot or B2_NOBRICK
+    const float* bricks;                 // [slot][9][9][9]
+    float ox, oy, oz, h, inv_h, trunc;
+    uint32_t dx, dy, dz;                 // nodes per axis (>= 2)
+    uint32_t bx, by, bz;                 // bricks per axis
+};
+
+// grid of a field over the box [lo, hi] (host): cells per axis max(1, ceil((hi - lo) / h)) in float64, dims = cells + 1, bricks per axis
+// ceil(cells / 8).  Returns nullptr, or why the grid is refused: non-finite or empty box, h or trunc not finite and > 0, more than 2^24 nodes
+// on an axis counting the last brick's far face (node coordinates must be exact in float), more than 2^32 - 2 bricks (B2_NOBRICK stays free).
+inline const char* df_grid(const float lo[3], const float hi[3], float h, float trunc, DfieldView* f, uint64_t* n_bricks)
+{
+    if (!(std::isfinite(h) && h > 0.0f)) return "resolution must be finite and > 0";
+    if (!(std::isfinite(trunc) && trunc > 0.0f)) return "truncation must be finite and > 0";
+    uint64_t cells[3], bricks[3];
+    for (int k = 0; k < 3; k++) {
+        if (!(std::isfinite(lo[k]) && std::isfinite(hi[k]))) return "bounds must be finite";
+        if (!(lo[k] < hi[k])) return "bb_min must be below bb_max on every axis";
+        const double c = std::ceil(((double)hi[k] - (double)lo[k]) / (double)h);
+        if (!(c <= 16777216.0)) return "more than 2^24 nodes on an axis";
+        cells[k] = c < 1.0 ? 1u : (uint64_t)c;
+        bricks[k] = (cells[k] + 7u) / 8u;
+        if (8u * bricks[k] + 1u > 16777216u) return "more than 2^24 nodes on an axis";
+    }
+    const uint64_t total = bricks[0] * bricks[1] * bricks[2];
+    if (total > 0xFFFFFFFEull) return "more than 2^32 - 2 bricks";
+    f->index = nullptr; f->bricks = nullptr;
+    f->ox = lo[0]; f->oy = lo[1]; f->oz = lo[2]; f->h = h; f->inv_h = 1.0f / h; f->trunc = trunc;
+    f->dx = (uint32_t)cells[0] + 1u; f->dy = (uint32_t)cells[1] + 1u; f->dz = (uint32_t)cells[2] + 1u;
+    f->bx = (uint32_t)bricks[0]; f->by = (uint32_t)bricks[1]; f->bz = (uint32_t)bricks[2];
+    *n_bricks = total;
+    return nullptr;
+}
+
+B2_DEV float df_coord(float o, uint32_t i, float h) { return add(o, mul((float)i, h)); }
+// the build's limits: the allocation distance ta = add(trunc, mul(8, h)), its square and trunc2 = mul(trunc, trunc)
+B2_DEV void df_limits(const DfieldView& f, float& ta, float& ta2, float& trunc2) { ta = add(f.trunc, mul(8.0f, f.h)); ta2 = mul(ta, ta); trunc2 = mul(f.trunc, f.trunc); }
+
+// value of the node at global node coordinates (i, j, k); trunc2 = mul(trunc, trunc)
+B2_DEV float df_node_value(const BvhView& bvh, const DfieldView& f, uint32_t i, uint32_t j, uint32_t k, float trunc2)
+{
+    CpBest best; uint32_t nn = 0, nt = 0;
+    closest_point<false, true>(bvh, mk3(df_coord(f.ox, i, f.h), df_coord(f.oy, j, f.h), df_coord(f.oz, k, f.h)), best, nn, nt, trunc2);
+    return fminf(sqrtf(best.d2), f.trunc);
+}
+
+// allocation rule of brick (bi, bj, bk): ta = add(trunc, mul(8, h)), ta2 = mul(ta, ta)
+B2_DEV bool df_brick_alloc(const BvhView& bvh, const DfieldView& f, uint32_t bi, uint32_t bj, uint32_t bk, float ta, float ta2)
+{
+    CpBest best; uint32_t nn = 0, nt = 0;
+    closest_point<false, true>(bvh, mk3(df_coord(f.ox, 8u * bi + 4u, f.h), df_coord(f.oy, 8u * bj + 4u, f.h), df_coord(f.oz, 8u * bk + 4u, f.h)), best, nn, nt, ta2);
+    return sqrtf(best.d2) < ta;
+}
+
+// node l (0 .. 728) of the brick with linear index id -> global node coordinates
+B2_DEV void df_brick_node(const DfieldView& f, uint32_t id, uint32_t l, uint32_t& i, uint32_t& j, uint32_t& k)
+{
+    const uint32_t bi = id % f.bx, bj = (id / f.bx) % f.by, bk = id / f.bx / f.by;
+    i = 8u * bi + l % 9u; j = 8u * bj + (l / 9u) % 9u; k = 8u * bk + l / 81u;
+}
+
+B2_DEV float df_lerp(float a, float b, float t) { return add(mul(a, sub(1.0f, t)), mul(b, t)); }
+
+B2_DEV float df_lookup(const DfieldView& f, V3 p)
+{
+    const float inf = u2f(0x7f800000u);
+    if (!(fabsf(p.x) < inf && fabsf(p.y) < inf && fabsf(p.z) < inf)) return inf;
+    const float gx = mul(sub(p.x, f.ox), f.inv_h), gy = mul(sub(p.y, f.oy), f.inv_h), gz = mul(sub(p.z, f.oz), f.inv_h);
+    if (!(gx >= 0.0f && gy >= 0.0f && gz >= 0.0f && gx <= (float)(f.dx - 1u) && gy <= (float)(f.dy - 1u) && gz <= (float)(f.dz - 1u))) return f.trunc;
+    auto cell = [](float g, uint32_t d) { const uint32_t c = (uint32_t)floorf(g); return c < d - 2u ? c : d - 2u; };
+    const uint32_t cx = cell(gx, f.dx), cy = cell(gy, f.dy), cz = cell(gz, f.dz);
+    const float tx = sub(gx, (float)cx), ty = sub(gy, (float)cy), tz = sub(gz, (float)cz);
+    const uint32_t slot = ldg(f.index + ((size_t)(cz >> 3) * f.by + (cy >> 3)) * f.bx + (cx >> 3));
+    if (slot == B2_NOBRICK) return f.trunc;
+    const float* b = f.bricks + (size_t)slot * B2_DF_NODES + ((cz & 7u) * 9u + (cy & 7u)) * 9u + (cx & 7u);
+    const float c00 = df_lerp(ldg(b + 0), ldg(b + 1), tx), c10 = df_lerp(ldg(b + 9), ldg(b + 10), tx);
+    const float c01 = df_lerp(ldg(b + 81), ldg(b + 82), tx), c11 = df_lerp(ldg(b + 90), ldg(b + 91), tx);
+    return df_lerp(df_lerp(c00, c10, ty), df_lerp(c01, c11, ty), tz);
+}
+
+// Gaussian evaluation of one (particle, beam) pair from the field: the closest-point branch of pf_eval_one with e = field(q)
+B2_DEV float pf_eval_field(const DfieldView& f, Tf Tsm, const PfBeam& b, float sigma_quad, double denom)
+{
+    const V3 orig_m = tf_apply(Tsm, mk3(b.ox, b.oy, b.oz));
+    const V3 dir_m = q_rot(Tsm.R, mk3(b.dx, b.dy, b.dz));
+    const float error = df_lookup(f, v_add(orig_m, v_scale(dir_m, b.range)));
+    const float arg = dvd(dvd(-mul(error, error), sigma_quad), 2.0f);
+    return (float)(exp((double)arg) / denom);
+}
+
+#ifdef __CUDACC__
+// build: one thread per brick writes its allocation flag (0 / 1) into the index ...
+__global__ void k_dfield_classify(BvhView bvh, DfieldView f, uint64_t n_bricks, float ta, float ta2, uint32_t* __restrict__ flags)
+{
+    for (uint64_t id = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; id < n_bricks; id += (uint64_t)gridDim.x * blockDim.x) {
+        const uint32_t bi = (uint32_t)(id % f.bx), bj = (uint32_t)(id / f.bx % f.by), bk = (uint32_t)(id / f.bx / f.by);
+        flags[id] = df_brick_alloc(bvh, f, bi, bj, bk, ta, ta2) ? 1u : 0u;
+    }
+}
+// ... an exclusive scan gives the slots; the index becomes slot / B2_NOBRICK in place, and the slot -> brick list is written
+__global__ void k_dfield_index(uint64_t n_bricks, const uint32_t* __restrict__ offs, uint32_t* __restrict__ index, uint32_t* __restrict__ list)
+{
+    for (uint64_t id = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; id < n_bricks; id += (uint64_t)gridDim.x * blockDim.x) {
+        const bool a = index[id] != 0u;
+        index[id] = a ? offs[id] : B2_NOBRICK;
+        if (a && list) list[offs[id]] = (uint32_t)id;
+    }
+}
+// one thread per node of each allocated brick
+__global__ void k_dfield_fill(BvhView bvh, DfieldView f, const uint32_t* __restrict__ list, uint64_t n_nodes, float trunc2, float* __restrict__ bricks)
+{
+    for (uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; t < n_nodes; t += (uint64_t)gridDim.x * blockDim.x) {
+        uint32_t i, j, k;
+        df_brick_node(f, list[t / B2_DF_NODES], (uint32_t)(t % B2_DF_NODES), i, j, k);
+        bricks[t] = df_node_value(bvh, f, i, j, k, trunc2);
+    }
+}
+__global__ void k_dfield_query(DfieldView f, const float* __restrict__ pts, uint32_t n, float* __restrict__ out)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    out[i] = df_lookup(f, mk3(pts[3 * (size_t)i], pts[3 * (size_t)i + 1], pts[3 * (size_t)i + 2]));
+}
+// The sensor update from the field: k_pf_update's contract (block of ppb particles x all beams, evaluations in shared memory, merge in beam
+// order, attrs read-modified-written once) with e = field(q).  Lanes = consecutive beams of one particle: the beams are sorted by direction
+// (pf_prepare_beams), so a warp's lookups land in neighbouring cells of the field.
+__global__ void __launch_bounds__(B2_PF_BLOCK) k_pf_update_field(DfieldView f, const b2_transform* __restrict__ poses, b2_particle_attr* __restrict__ attrs,
+                                                              uint32_t n_particles, b2_transform Tsb_val, const PfBeam* __restrict__ beams, uint32_t n_beams,
+                                                              b2_pf_params prm, uint32_t ppb)
+{
+    extern __shared__ float s_eval[];            // [ppb][n_beams]
+    const uint32_t p0 = blockIdx.x * ppb;
+    const uint32_t np = min(ppb, n_particles - p0);
+    float sigma_quad; double denom; pf_constants(prm, sigma_quad, denom);
+    const Tf Tsb = tf_from_pod(Tsb_val);
+    const uint32_t total = np * n_beams;
+    for (uint32_t w = threadIdx.x; w < total; w += blockDim.x) {
+        const uint32_t pl = w / n_beams, bi = w % n_beams;
+        const Tf Tsm = tf_mul(tf_load(poses + p0 + pl), Tsb);
+        const PfBeam b = beams[bi];
+        s_eval[pl * n_beams + b.slot] = pf_eval_field(f, Tsm, b, sigma_quad, denom);
+    }
+    __syncthreads();
+    if (threadIdx.x < np) {
+        b2_particle_attr* ap = attrs + p0 + threadIdx.x;
+        b2_gaussian1d lk = ap->likelihood;
+        pf_merge(lk, s_eval + threadIdx.x * n_beams, n_beams);
+        ap->likelihood = lk;
+    }
+}
+#endif
+
 #ifdef __CUDACC__
 // sort key of a particle for MAP 1: 16 heading bins (yaw), then the Morton code of its (x, y) cell on a 1024 x 1024 lattice over the map
 __global__ void k_pf_sort_keys(const b2_transform* __restrict__ poses, uint32_t n, float bx, float by, uint32_t* __restrict__ keys, uint32_t* __restrict__ idx)

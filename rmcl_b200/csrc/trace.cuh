@@ -389,13 +389,23 @@ B2_DEV void cp_tri_test(const BvhView& bvh, V3 q, float delta, uint32_t tri_idx,
 
 B2_DEV float cp_delta(V3 q) { return mul(1.52587890625e-05f, add(1.0f, fmaxf(fmaxf(fabsf(q.x), fabsf(q.y)), fabsf(q.z)))); }
 
-template <bool STATS>
-B2_DEV void closest_point(const BvhView& bvh, V3 q, CpBest& best, uint32_t& n_nodes, uint32_t& n_tris)
+// BOUNDED QUERY (BOUNDED = true, trunc2 = fl(trunc * trunc) with trunc > 0): the walk starts with best.lim = lim(trunc2) instead of +inf;
+//   best.d2 still starts at +inf and the candidate rule is unchanged.  Let (d2*, f*) be the unbounded result.
+//   (a) d2* < trunc2: the winner and every candidate tying with it have b2(triangle AABB) <= lim(d2*) <= lim(trunc2) (lim is monotone), and
+//       lim(best d2) >= lim(d2*) at every later point of the walk, so each such candidate's leaf is visited as in the unbounded walk and
+//       tested against the same rule: the bounded result is (d2*, f*), bit for bit.
+//   (b) d2* >= trunc2 (or no candidate): the bounded result is a counting candidate or none, so its d2 >= d2* >= trunc2 or +inf, and
+//       sqrtf(d2) >= sqrtf(fl(trunc^2)) = trunc (a correctly rounded square root of a correctly rounded square returns |trunc|).
+//   Hence min(sqrtf(d2), trunc) is the same for both forms of the query.  The unbounded form (BOUNDED = false, the default) compiles to the
+//   code it always had.
+template <bool STATS, bool BOUNDED = false>
+B2_DEV void closest_point(const BvhView& bvh, V3 q, CpBest& best, uint32_t& n_nodes, uint32_t& n_tris, float trunc2 = 0.0f)
 {
     best.d2 = u2f(0x7f800000u); best.lim = u2f(0x7f800000u); best.face = B2_NOFACE; best.tri = 0u; best.p = mk3(0.f, 0.f, 0.f);
     // a non-finite query has no counting candidate (every comparison fails); do not walk the tree for it
     if (!(fabsf(q.x) < u2f(0x7f800000u) && fabsf(q.y) < u2f(0x7f800000u) && fabsf(q.z) < u2f(0x7f800000u))) return;
     const float delta = cp_delta(q);
+    if (BOUNDED) best.lim = cp_lim(trunc2, delta);
     uint2 stack[B2_TRAVERSAL_STACK];
     int sp = 0;
     uint32_t next = 0u; float next_b2 = 0.0f; bool have_next = true;        // node to visit once the pending leaves are done (root first)
