@@ -652,7 +652,7 @@ static void svd3(double A[3][3], double U[3][3], double w[3], double V[3][3])
             double alpha = 0, beta = 0, gamma = 0;
             for (int i = 0; i < 3; i++) { alpha += B[i][p] * B[i][p]; beta += B[i][q] * B[i][q]; gamma += B[i][p] * B[i][q]; }
             if (gamma == 0.0) continue;
-            double lim = 1e-30 + 1e-16 * sqrt(alpha * beta);
+            double lim = 1e-16 * sqrt(alpha * beta);          /* relative only: an absolute floor stopped every rotation of a C below ~1e-15 */
             if (fabs(gamma) <= lim) continue;
             off += fabs(gamma);
             double zeta = (beta - alpha) / (2.0 * gamma);
@@ -957,7 +957,8 @@ static void cp_triangle(const float a[3], const float b[3], const float c[3], co
     const float d3 = dot_plain(ab, bp), d4 = dot_plain(ac, bp);
     if (d3 >= 0.0f && d4 <= d3) { for (int k = 0; k < 3; k++) out[k] = b[k]; return; }
     const float vc = d1 * d4 - d3 * d2;
-    if (vc <= 0.0f && d1 >= 0.0f && d3 <= 0.0f) { const float v = d1 / (d1 - d3); for (int k = 0; k < 3; k++) out[k] = a[k] + ab[k] * v; return; }
+    /* d1 != d3: a == b (a segment a-c) gives d1 = d3 = 0, whose 0/0 made the candidate NaN; the ac region below takes it instead */
+    if (vc <= 0.0f && d1 >= 0.0f && d3 <= 0.0f && d1 != d3) { const float v = d1 / (d1 - d3); for (int k = 0; k < 3; k++) out[k] = a[k] + ab[k] * v; return; }
     for (int k = 0; k < 3; k++) cp[k] = p[k] - c[k];
     const float d5 = dot_plain(ab, cp), d6 = dot_plain(ac, cp);
     if (d6 >= 0.0f && d5 <= d6) { for (int k = 0; k < 3; k++) out[k] = c[k]; return; }

@@ -86,7 +86,7 @@ __host__ __device__ __noinline__ void svd3_dev(const double A[3][3], double U[3]
             double alpha = 0, beta = 0, gamma = 0;
             for (int i = 0; i < 3; i++) { alpha += B[i][p] * B[i][p]; beta += B[i][q] * B[i][q]; gamma += B[i][p] * B[i][q]; }
             if (gamma == 0.0) continue;
-            const double lim = 1e-30 + 1e-16 * sqrt(alpha * beta);
+            const double lim = 1e-16 * sqrt(alpha * beta);        // relative only: an absolute floor stopped every rotation of a C below ~1e-15
             if (fabs(gamma) <= lim) continue;
             off += fabs(gamma);
             const double zeta = (beta - alpha) / (2.0 * gamma);

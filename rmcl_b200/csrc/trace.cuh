@@ -351,7 +351,8 @@ B2_DEV V3 cp_triangle(V3 a, V3 b, V3 c, V3 p)
     const float d3 = dot_plain(ab, bp), d4 = dot_plain(ac, bp);
     if (d3 >= 0.0f && d4 <= d3) return b;
     const float vc = sub(mul(d1, d4), mul(d3, d2));
-    if (vc <= 0.0f && d1 >= 0.0f && d3 <= 0.0f) { const float v = dvd(d1, sub(d1, d3)); return mk3(add(a.x, mul(ab.x, v)), add(a.y, mul(ab.y, v)), add(a.z, mul(ab.z, v))); }
+    // d1 != d3: a == b (a segment a-c) gives d1 = d3 = 0, whose 0/0 made the candidate NaN; the ac region below takes it instead
+    if (vc <= 0.0f && d1 >= 0.0f && d3 <= 0.0f && d1 != d3) { const float v = dvd(d1, sub(d1, d3)); return mk3(add(a.x, mul(ab.x, v)), add(a.y, mul(ab.y, v)), add(a.z, mul(ab.z, v))); }
     const V3 cp = v_sub(p, c);
     const float d5 = dot_plain(ab, cp), d6 = dot_plain(ac, cp);
     if (d6 >= 0.0f && d5 <= d6) return c;

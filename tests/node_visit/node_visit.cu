@@ -10,6 +10,9 @@
 //   * node_test<true> when ray_setup flagged the ray B2_RAY_INTBOX;
 // and, for flagged rays, that no near plane value is NaN and no far plane value is NaN or -0 (the premise of the integer test).
 // Prints "cases <n> intbox <n flagged> mismatch <n> premise <n>".
+//
+//   node_visit flags BX BY BZ  reads rays "ox oy oz dx dy dz" (strtof syntax, hex floats exact) from stdin, one per line, and prints
+//                              ray_setup's B2_RAY_INTBOX flag (0 / 1) for each against a map whose max |vertex coordinate| per axis is BX BY BZ
 #include "../../rmcl_b200/csrc/trace.cuh"
 
 #include <cstdio>
@@ -107,6 +110,18 @@ int main(int argc, char** argv)
     BvhView bvh; bvh.nodes = reinterpret_cast<const float4*>(node); bvh.tris = nullptr;
     uint32_t* hdr = reinterpret_cast<uint32_t*>(node + 48);
     hdr[0] = 0; hdr[1] = 0; hdr[2] = 0xffu; hdr[3] = 0;              // every slot inner: the hit bits come back in `inner`
+    if (argc >= 5 && std::string_view(argv[1]) == "flags") {
+        bvh.bx = strtof(argv[2], nullptr); bvh.by = strtof(argv[3], nullptr); bvh.bz = strtof(argv[4], nullptr);
+        char line[512];
+        while (fgets(line, sizeof line, stdin)) {
+            float v[6];
+            char* p = line;
+            for (int k = 0; k < 6; k++) { char* e; v[k] = strtof(p, &e); if (e == p) return 2; p = e; }
+            const RaySetup r = ray_setup(mk3(v[0], v[1], v[2]), mk3(v[3], v[4], v[5]), bvh);
+            printf("%d\n", (r.noff & B2_RAY_INTBOX) ? 1 : 0);
+        }
+        return 0;
+    }
     Counts c;
     const bool corner = argc >= 2 && std::string_view(argv[1]) == "corner";
     if (corner) {
