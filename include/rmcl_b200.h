@@ -660,6 +660,28 @@ B2_API int b2_dfield_query(b2_dfield* f, const float* points_xyz, uint32_t n, fl
 B2_API int b2_pf_sensor_update_field(b2_pf* h, const b2_dfield* f, const b2_transform* poses_dev, b2_particle_attr* attrs_dev, uint32_t n_particles,
                                      const b2_transform* Tsb, const b2_range_meas* beams_host, uint32_t n_beams, const b2_pf_params* params);
 
+/* b2_pf_stein_update: `iterations` Stein variational gradient descent steps (SVGD, Liu & Wang 2016; the MegaParticles TODO of the reference's
+ * docs/RMCL.md) that move the n particles toward the beams' likelihood over the field, in place, on the handle's stream, with no host round
+ * trip between iterations (SURVEY appendix L states every operation).  Chart c = (x, y, psi), psi the ZYX yaw; a step moves x, y and turns
+ * the pose about the world z axis through the body origin; z, roll and pitch stay (call b2_pf_project_to_surface after it on maps with
+ * ramps).  Target: sum over beams of log((1 - w_rand) exp(-e^2 / (2 dist_sigma^2)) + w_rand), e = the field at the point
+ * b2_pf_sensor_update_field looks up.  Each iteration scores a reference set J of m particles (all n in index order when n_ref == 0 or
+ * n_ref >= n; else n_ref draws with replacement keyed by (seed, step, iteration)), sets the kernel bandwidth from the spread of the set, moves
+ * every particle by the RMSProp-scaled kernel-weighted mean over J of score plus repulsion, and keeps a particle's pose for that iteration
+ * where the motion update's wall check (a ray from the old to the new position) hits the map.  Attributes are not touched.
+ * The result record (nullable out_host: one 32-byte copy and a synchronise): the last iteration's bandwidth (x, y, psi) and RMS step over
+ * the finite particles (m, rad), m, and the blocked steps summed over all iterations.  n == 0 or iterations == 0: B2_OK, nothing launched
+ * (out_host zeroed).  n_beams == 0: the score is 0, the particles only repel each other.  Refused (B2_ERR_INVALID, no launch):
+ * b2_pf_sensor_update_field's checks, null cfg, a step or bandwidth floor not finite and > 0, w_rand outside [0, 1), dist_sigma not
+ * finite and > 0.  Non-finite particles keep their pose and take no part in J's sums or the bandwidth. */
+typedef struct { uint32_t iterations, n_ref; float step_t, step_r, min_bandwidth_t, min_bandwidth_r, w_rand, pad; } b2_stein_config;       /* 32 B */
+typedef struct { float bandwidth[3]; uint32_t n_ref, n_blocked; float rms_step_t, rms_step_r, pad; } b2_stein_result;                      /* 32 B */
+typedef char b2_stein_config_is_32_bytes[sizeof(b2_stein_config) == 32 ? 1 : -1];
+typedef char b2_stein_result_is_32_bytes[sizeof(b2_stein_result) == 32 ? 1 : -1];
+B2_API int b2_pf_stein_update(b2_pf* h, const b2_dfield* f, b2_transform* poses_dev, uint32_t n, const b2_transform* Tsb,
+                              const b2_range_meas* beams_host, uint32_t n_beams, const b2_pf_params* params,
+                              const b2_stein_config* cfg, uint64_t seed, uint32_t step, b2_stein_result* out_host /* nullable */);
+
 /* ---------------------------------------------------------------- introspection ------------------------------ */
 /* CUDA-event timing of the kernels inside b2_rcc_correct_once*(): when enabled, events are recorded on the handle's stream around the
  * find kernel and around the reduction/Umeyama kernels; b2_rcc_last_timing returns the two durations of the most recent call (ms). */

@@ -453,6 +453,19 @@ public:
         b2_check(b2_pf_project_to_surface(h_, reinterpret_cast<b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(), &cfg),
                  "projectToSurface");
     }
+    // Stein variational steps toward the beams' likelihood over the field of setDistanceField (b2_pf_stein_update; SURVEY appendix L): in
+    // place on the device poses, on the handle's stream; x, y and yaw move, z, roll, pitch and the attributes stay.  Throws without a field.
+    // Returns the result record (a 32-byte read-back and a synchronise).  stein_config() gives the suggested values.
+    static b2_stein_config stein_config() { return b2_stein_config{10u, 4096u, 0.02f, 0.01f, 0.05f, 0.02f, 0.05f, 0.0f}; }
+    b2_stein_result steinUpdate(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses, const b2_range_meas* beams, uint32_t n_beams,
+                                const b2_stein_config& cfg = stein_config(), uint64_t seed = 0, uint32_t step = 0)
+    {
+        if (!field_) throw std::runtime_error("steinUpdate: no distance field (setDistanceField first)");
+        b2_stein_result r{};
+        b2_check(b2_pf_stein_update(h_, field_->handle(), reinterpret_cast<b2_transform*>(poses.raw()), (uint32_t)poses.size(),
+                                    reinterpret_cast<const b2_transform*>(&Tsb_), beams, n_beams, &config, &cfg, seed, step, &r), "steinUpdate");
+        return r;
+    }
     // Recovery from a kidnapping (Augmented MCL, b2_pf_recovery_*): recoveryObserve after each update keeps a slow and a fast average of the
     // set's mean likelihood at recovery_config's rates (AMCL's recovery_alpha_slow / _fast); recoveryInject after resampling replaces a
     // fraction p_inject = max(0, 1 - w_fast / w_slow) of the particles with random poses of the box (on the map's ground when `surface` is

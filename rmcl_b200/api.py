@@ -104,6 +104,23 @@ class RecoveryConfig(C.Structure):
         return RecoveryConfig(0.001, 0.1)
 
 
+class SteinConfig(C.Structure):
+    """b2_stein_config: the Stein variational steps of steinUpdate: iterations per call, the reference set's size n_ref (0: every particle),
+    the RMSProp step sizes step_t (m) and step_r (rad), the kernel bandwidth's floors min_bandwidth_t (m) and min_bandwidth_r (rad), and
+    the likelihood's uniform share w_rand in [0, 1).  defaults() are the suggested values (SURVEY appendix L says why)."""
+    _fields_ = [("iterations", C.c_uint32), ("n_ref", C.c_uint32), ("step_t", C.c_float), ("step_r", C.c_float), ("min_bandwidth_t", C.c_float),
+                ("min_bandwidth_r", C.c_float), ("w_rand", C.c_float), ("pad", C.c_float)]
+
+    @staticmethod
+    def defaults():
+        return SteinConfig(10, 4096, 0.02, 0.01, 0.05, 0.02, 0.05, 0.0)
+
+
+class _SteinResult(C.Structure):
+    _fields_ = [("bandwidth", C.c_float * 3), ("n_ref", C.c_uint32), ("n_blocked", C.c_uint32), ("rms_step_t", C.c_float), ("rms_step_r", C.c_float),
+                ("pad", C.c_float)]
+
+
 class _CloudLayout(C.Structure):
     _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("point_step", C.c_uint32), ("row_step", C.c_uint32), ("offset_x", C.c_uint32),
                 ("offset_y", C.c_uint32), ("offset_z", C.c_uint32), ("datatype", C.c_uint8), ("is_bigendian", C.c_uint8), ("pad", C.c_uint8 * 2)]
@@ -170,7 +187,7 @@ EXPORTS = [
     "b2_rcc_set_cloud_spherical", "b2_pf_sample_cloud", "b2_pf_resample_residual", "b2_pf_project_to_surface",
     "b2_pf_resample_kld", "b2_pf_cluster_stats", "b2_micp_pose_covariance", "b2_pf_recovery_reset", "b2_pf_recovery_observe",
     "b2_pf_recovery_inject", "b2_dfield_create", "b2_dfield_destroy", "b2_dfield_get_info", "b2_dfield_download", "b2_dfield_query",
-    "b2_pf_sensor_update_field",
+    "b2_pf_sensor_update_field", "b2_pf_stein_update",
 ]
 
 
@@ -886,6 +903,27 @@ class PCDSensorUpdaterB200:
         assert attrs.dtype.itemsize == 36
         _chk(lib.b2_pf_sensor_update_host(self._h, _p(poses), _p(attrs), C.c_uint32(len(poses)), _p(Tsb), _p(beams), C.c_uint32(len(beams)), C.byref(prm)))
         return attrs
+
+    def steinUpdate(self, particle_poses, Tsb, beams, config=None, params: PFParams | None = None, seed=None, step=0):
+        """Stein variational steps toward the beams' likelihood over the distance field of setDistanceField (b2_pf_stein_update; SURVEY
+        appendix L): in place on the (n, 8) float32 CUDA tensor of poses, on the handle's stream.  Each of config.iterations steps moves every
+        particle in x, y and yaw along the kernel-weighted score of a reference set plus the kernel's repulsion; a step the map's walls block
+        is not taken.  z, roll, pitch and the attributes stay: the next update() scores the moved particles.  `config`: a SteinConfig
+        (default defaults()); `params`: the sensor model's dist_sigma (default self.config); `seed` (default self.seed) and `step` key the
+        reference draws.  -> dict(bandwidth, n_ref, n_blocked, rms_step_t, rms_step_r), read back with a synchronise."""
+        if self._field is None:
+            raise B2Error(-1, "steinUpdate: no distance field (setDistanceField first)")
+        cfg = config or SteinConfig.defaults()
+        prm = params or self.config
+        beams = np.ascontiguousarray(beams)
+        assert beams.dtype.itemsize == 64
+        n = particle_poses.numel() * particle_poses.element_size() // 32
+        out = _SteinResult()
+        _chk(load_library().b2_pf_stein_update(self._h, self._field._h, _devptr(particle_poses), C.c_uint32(n), _p(_tf(Tsb)),
+                                               _p(beams) if len(beams) else None, C.c_uint32(len(beams)), C.byref(prm), C.byref(cfg),
+                                               C.c_uint64(self.seed if seed is None else int(seed)), C.c_uint32(int(step)), C.byref(out)))
+        return {"bandwidth": tuple(out.bandwidth), "n_ref": out.n_ref, "n_blocked": out.n_blocked, "rms_step_t": out.rms_step_t,
+                "rms_step_r": out.rms_step_r}
 
     def motionUpdate(self, particle_poses, particle_attrs, T_bnew_bold, forget_rate, check_collision=False):
         """TFMotionUpdaterGPU (rmcl_ros/src/rmcl/particle_motion.cu:11-46): in place on torch CUDA tensors.  check_collision adds the CPU

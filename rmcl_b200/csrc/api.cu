@@ -1944,6 +1944,7 @@ struct PfRecords {
     b2_recovery_state rec;                              // the recovery's {w_avg, w_slow, w_fast, p_inject}
     b2_recovery_result rec_res;                         // the result of an injection
     unsigned long long traffic;                         // remote bytes read by the p2p Gladiator kernel
+    PfSteinState stein;                                 // the Stein step's result record and reduction tickets
 };
 
 // The scratch below (partials, records, the resamplers' and the clusters' buffers) is shared by the entry points: a handle serves one call at
@@ -1983,6 +1984,9 @@ struct b2_pf {
     // sort (the index buffers also list the roots); and the gathered members
     DevBuf<unsigned long long> d_cl_w; DevBuf<unsigned int> d_cl_cnt, d_cl_aux; DevBuf<uint32_t> d_cl_slot, d_cl_key, d_cl_key2, d_cl_idx, d_cl_idx2;
     DevBuf<b2_transform> d_cl_poses; DevBuf<b2_particle_attr> d_cl_attrs;
+    // Stein steps (b2_pf_stein_update), grown at its calls: J's snapshot, the RMSProp state of a call (3 floats per particle) and the block
+    // partials of its two grid reductions (one block per 256 particles)
+    DevBuf<SteinRef> d_stein_snap; DevBuf<float> d_stein_v; DevBuf<double> d_stein_part;
 };
 
 extern "C" int b2_pf_destroy(b2_pf* h);
@@ -2001,6 +2005,7 @@ static int pf_init(b2_pf* h)
     CU(cudaFuncSetAttribute(k_pf_update<0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
     CU(cudaFuncSetAttribute(k_pf_update<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
     CU(cudaFuncSetAttribute(k_pf_update_field, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
+    CU(cudaFuncSetAttribute(k_pf_stein_score, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
     CU(cudaEventCreate(&h->ev_m0)); CU(cudaEventCreate(&h->ev_m1));
     { const char* e = getenv("B2_PF_MAP"); if (e) h->map_mode = std::min(3, std::max(0, atoi(e))); }
     return B2_OK;
@@ -2047,6 +2052,7 @@ extern "C" int b2_pf_destroy(b2_pf* h)
     h->d_kld_flags.release(); h->d_kld_cum.release(); h->d_kld_tmp.release(); h->d_kld_tab.release();
     h->d_cl_w.release(); h->d_cl_cnt.release(); h->d_cl_aux.release(); h->d_cl_slot.release(); h->d_cl_key.release(); h->d_cl_key2.release(); h->d_cl_idx.release();
     h->d_cl_idx2.release(); h->d_cl_poses.release(); h->d_cl_attrs.release();
+    h->d_stein_snap.release(); h->d_stein_v.release(); h->d_stein_part.release();
     b2_mesh* map = h->map;
     delete h;
     (void)cudaGetLastError();
@@ -2433,6 +2439,56 @@ extern "C" int b2_pf_sensor_update_field(b2_pf* h, const b2_dfield* f, const b2_
     const uint32_t grid = (n + ppb - 1) / ppb;
     k_pf_update_field<<<grid, B2_PF_BLOCK, sizeof(float) * (size_t)n_beams * ppb, h->stream>>>(f->v, poses_dev, attrs_dev, n, *Tsb, h->d_beams.p, n_beams, *prm, ppb);
     LAUNCHED();
+    return B2_OK;
+}
+
+// Stein variational steps (kernels.cuh, SURVEY appendix L): per iteration the score of J, the bandwidth and the move, all on h->stream
+extern "C" int b2_pf_stein_update(b2_pf* h, const b2_dfield* f, b2_transform* poses_dev, uint32_t n, const b2_transform* Tsb, const b2_range_meas* beams,
+                                  uint32_t n_beams, const b2_pf_params* prm, const b2_stein_config* cfg, uint64_t seed, uint32_t step, b2_stein_result* out_host)
+{
+    NOTNULL(h); NOTNULL(f); NOTNULL(Tsb); NOTNULL(prm); NOTNULL(cfg);
+    if (n) NOTNULL(poses_dev);
+    if (n_beams) NOTNULL(beams);
+    if (f->map->device != h->map->device) return fail(B2_ERR_INVALID, "pf_stein_update: the field is on device %d, the handle on device %d", f->map->device, h->map->device);
+    const b2_stein_config c = *cfg;
+    auto pos = [](float v) { return std::isfinite(v) && v > 0.0f; };
+    if (!(pos(c.step_t) && pos(c.step_r) && pos(c.min_bandwidth_t) && pos(c.min_bandwidth_r)))
+        return fail(B2_ERR_INVALID, "pf_stein_update: steps (%g, %g) and bandwidth floors (%g, %g) must be finite and > 0", (double)c.step_t, (double)c.step_r,
+                    (double)c.min_bandwidth_t, (double)c.min_bandwidth_r);
+    if (!(c.w_rand >= 0.0f && c.w_rand < 1.0f)) return fail(B2_ERR_INVALID, "pf_stein_update: w_rand = %g outside [0, 1)", (double)c.w_rand);
+    if (!pos(prm->dist_sigma)) return fail(B2_ERR_INVALID, "pf_stein_update: dist_sigma = %g must be finite and > 0", (double)prm->dist_sigma);
+    if (out_host) memset(out_host, 0, sizeof(*out_host));
+    CU(cudaSetDevice(h->map->device));
+    if (n == 0 || c.iterations == 0) return B2_OK;
+    const uint32_t m = (c.n_ref == 0 || c.n_ref >= n) ? n : c.n_ref;
+    uint32_t ppb = B2_PF_BLOCK;
+    if (n_beams) {
+        if (sizeof(float) * 3 * (size_t)n_beams > (size_t)h->smem_optin) return fail(B2_ERR_UNSUPPORTED, "pf_stein_update: too many beams (%u)", n_beams);
+        RES(pf_prepare_beams(h, beams, n_beams, &ppb));
+        ppb = std::max<uint32_t>(1u, std::min<uint32_t>(ppb, (uint32_t)((size_t)h->smem_optin / (sizeof(float) * 3 * (size_t)n_beams))));
+    }
+    const uint32_t grid = (n + B2_STEIN_BLOCK - 1) / B2_STEIN_BLOCK;
+    RES(h->d_stein_snap.reserve(m)); RES(h->d_stein_v.reserve(3 * (size_t)n));
+    RES(h->d_stein_part.reserve((size_t)std::max(B2_STEIN_NBW, B2_STEIN_NMV) * grid));
+    PfSteinState* st = &h->d_recs.p->stein;
+    CU(cudaMemsetAsync(&st->rec, 0, sizeof(b2_stein_result), h->stream));
+    CU(cudaMemsetAsync(h->d_stein_v.p, 0, sizeof(float) * 3 * (size_t)n, h->stream));
+    const BvhView bvh = h->map->view();
+    const double fac = std::pow((double)m, -1.0 / 7.0);                    // Scott's rule in 3 dimensions
+    const float sigma2 = prm->dist_sigma * prm->dist_sigma;
+    for (uint32_t it = 0; it < c.iterations; it++) {
+        k_pf_stein_score<<<(m + ppb - 1) / ppb, B2_PF_BLOCK, sizeof(float) * 3 * (size_t)n_beams * ppb, h->stream>>>(f->v, poses_dev, n, m, c.n_ref, seed, step, it, *Tsb,
+                                                                                                                 h->d_beams.p, n_beams, sigma2, c.w_rand, ppb, h->d_stein_snap.p);
+        LAUNCHED();
+        k_pf_stein_bandwidth<<<grid, B2_STEIN_BLOCK, 0, h->stream>>>(poses_dev, n, m, fac, c.min_bandwidth_t, c.min_bandwidth_r, h->d_stein_part.p, st);
+        LAUNCHED();
+        k_pf_stein_move<<<grid, B2_STEIN_BLOCK, 0, h->stream>>>(bvh, poses_dev, n, h->d_stein_snap.p, m, it, c.step_t, c.step_r, h->d_stein_v.p, h->d_stein_part.p, st);
+        LAUNCHED();
+    }
+    if (out_host) {
+        RES(pf_fetch(h, h->h_recs->stein.rec));
+        *out_host = h->h_recs->stein.rec;
+    }
     return B2_OK;
 }
 

@@ -82,6 +82,46 @@ B2_DEV double add_d(double a, double b) { return a + b; }
 B2_DEV double sqrt_d(double a) { return std::sqrt(a); }
 B2_DEV double atan2_d(double y, double x) { return std::atan2(y, x); }
 #endif
+// FP64 library sine and cosine (CUDA's on the device, libm's on the host), for the Stein step's half-angle
+#if B2_ON_DEVICE
+B2_DEV double sin_d(double a) { return ::sin(a); }
+B2_DEV double cos_d(double a) { return ::cos(a); }
+#else
+B2_DEV double sin_d(double a) { return std::sin(a); }
+B2_DEV double cos_d(double a) { return std::cos(a); }
+#endif
+B2_DEV float rint_f(float a)
+{
+#if B2_ON_DEVICE
+    return rintf(a);
+#else
+    return std::nearbyint(a);                // round half to even, like rintf on the device
+#endif
+}
+
+// exp in FP32, every operation individually rounded and the FMAs explicit, so the device and the host compute the same bits.  Cody-Waite
+// reduction x = j ln2 + r (j = rint(x log2 e), ln2 split in a 16-bit-mantissa head and a tail, |r| <= 0.3466), Taylor polynomial of degree 7
+// in Horner form (truncation below 6e-9 relative), then two exact power-of-two scalings 2^(j/2) 2^(j - j/2), the second one rounding into the
+// subnormal range where the result lies there.  Within 2 ulp of exp(x) in float64 for x < 88.72 (tests/test_pf_stein.py); NaN gives NaN, x >=
+// 88.7228394 gives +inf, x < -103.972084 gives 0.
+B2_DEV float exp_f(float x)
+{
+    if (!(x < 88.7228394f)) return x != x ? x : u2f(0x7f800000u);
+    if (x < -103.972084f) return 0.0f;
+    const float j = rint_f(mul(x, 1.44269502f));
+    float r = fma_rn(j, -0.693145752f, x);                 // j * head is exact for |j| <= 151
+    r = fma_rn(j, -1.42860677e-06f, r);
+    float p = 1.98412701e-04f;                             // 1 / 7!
+    p = fma_rn(p, r, 1.38888892e-03f);
+    p = fma_rn(p, r, 8.33333377e-03f);
+    p = fma_rn(p, r, 4.16666679e-02f);
+    p = fma_rn(p, r, 1.66666672e-01f);
+    p = fma_rn(p, r, 0.5f);
+    p = fma_rn(p, r, 1.0f);
+    p = fma_rn(p, r, 1.0f);
+    const int e = (int)j, e1 = e / 2, e2 = e - e1;         // |e1|, |e2| <= 76: both powers are normal floats
+    return mul(mul(p, u2f((uint32_t)(e1 + 127) << 23)), u2f((uint32_t)(e2 + 127) << 23));
+}
 
 B2_DEV V3 mk3(float x, float y, float z) { V3 r; r.x = x; r.y = y; r.z = z; return r; }
 B2_DEV V3 v_add(V3 a, V3 b) { return mk3(add(a.x, b.x), add(a.y, b.y), add(a.z, b.z)); }

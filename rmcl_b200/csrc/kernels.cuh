@@ -1283,6 +1283,32 @@ B2_DEV float df_lookup(const DfieldView& f, V3 p)
     return df_lerp(df_lerp(c00, c10, ty), df_lerp(c01, c11, ty), tz);
 }
 
+// df_lookup's value, bit for bit, and the gradient of the same trilinear interpolant in the cell the lookup chose (one-sided at cell faces):
+// inv_h times the corner differences along an axis, lerped over the other two axes in df_lookup's order.  The gradient is 0 where the
+// value is not interpolated: outside the box, in an unallocated brick, at a non-finite point.
+B2_DEV float df_lookup_grad(const DfieldView& f, V3 p, V3& grad)
+{
+    const float inf = u2f(0x7f800000u);
+    grad = mk3(0.0f, 0.0f, 0.0f);
+    if (!(fabsf(p.x) < inf && fabsf(p.y) < inf && fabsf(p.z) < inf)) return inf;
+    const float gx = mul(sub(p.x, f.ox), f.inv_h), gy = mul(sub(p.y, f.oy), f.inv_h), gz = mul(sub(p.z, f.oz), f.inv_h);
+    if (!(gx >= 0.0f && gy >= 0.0f && gz >= 0.0f && gx <= (float)(f.dx - 1u) && gy <= (float)(f.dy - 1u) && gz <= (float)(f.dz - 1u))) return f.trunc;
+    auto cell = [](float g, uint32_t d) { const uint32_t c = (uint32_t)floorf(g); return c < d - 2u ? c : d - 2u; };
+    const uint32_t cx = cell(gx, f.dx), cy = cell(gy, f.dy), cz = cell(gz, f.dz);
+    const float tx = sub(gx, (float)cx), ty = sub(gy, (float)cy), tz = sub(gz, (float)cz);
+    const uint32_t slot = ldg(f.index + ((size_t)(cz >> 3) * f.by + (cy >> 3)) * f.bx + (cx >> 3));
+    if (slot == B2_NOBRICK) return f.trunc;
+    const float* b = f.bricks + (size_t)slot * B2_DF_NODES + ((cz & 7u) * 9u + (cy & 7u)) * 9u + (cx & 7u);
+    const float n000 = ldg(b + 0), n100 = ldg(b + 1), n010 = ldg(b + 9), n110 = ldg(b + 10);
+    const float n001 = ldg(b + 81), n101 = ldg(b + 82), n011 = ldg(b + 90), n111 = ldg(b + 91);
+    const float c00 = df_lerp(n000, n100, tx), c10 = df_lerp(n010, n110, tx), c01 = df_lerp(n001, n101, tx), c11 = df_lerp(n011, n111, tx);
+    const float c0 = df_lerp(c00, c10, ty), c1 = df_lerp(c01, c11, ty);
+    const float dx = df_lerp(df_lerp(sub(n100, n000), sub(n110, n010), ty), df_lerp(sub(n101, n001), sub(n111, n011), ty), tz);
+    const float dy = df_lerp(sub(c10, c00), sub(c11, c01), tz);
+    grad = mk3(mul(dx, f.inv_h), mul(dy, f.inv_h), mul(sub(c1, c0), f.inv_h));
+    return df_lerp(c0, c1, tz);
+}
+
 // Gaussian evaluation of one (particle, beam) pair from the field: the closest-point branch of pf_eval_one with e = field(q)
 B2_DEV float pf_eval_field(const DfieldView& f, Tf Tsm, const PfBeam& b, float sigma_quad, double denom)
 {
@@ -1377,6 +1403,19 @@ __global__ void k_pf_sort_keys(const b2_transform* __restrict__ poses, uint32_t 
 // particle_move_and_forget_kernel (rmcl_ros/src/rmcl/particle_motion.cu:11-34): HBM stream, 2 x (32 + 36) B per particle
 // With COLLIDE the wall check of the CPU updater (TFMotionUpdaterCPU.cpp:17-50,205-216) rides along: one ray from the old to the new
 // position, tfar = their distance; a hit pins the likelihood to {0, 0, MAX_N_MEAS}.
+// The same wall check on its own, for the Stein step: true iff a face lies on the segment from `from` to `to` (none below 1e-5 m of travel).
+// pf_motion_one keeps its inline copy: calling this from it changes k_pf_motion<true>'s machine code.
+B2_DEV bool pf_wall_hit(const BvhView& bvh, V3 from, V3 to)
+{
+    const V3 vec = v_sub(to, from);
+    const float length = v_l2norm(vec);
+    if (length < 0.00001f) return false;
+    const RaySetup r = ray_setup(from, mk3(dvd(vec.x, length), dvd(vec.y, length), dvd(vec.z, length)), bvh);
+    HitRec h = trace_init(length);
+    uint32_t nn = 0, nt = 0;
+    trace_closest<false>(bvh, r, h, nn, nt);
+    return h.face != B2_NOFACE;
+}
 B2_DEV void pf_motion_one(const BvhView* bvh, b2_transform* pose_io, b2_particle_attr* attr_io, Tf T, double forget_rate)
 {
     const Tf pose_old = tf_load(pose_io);
@@ -2817,6 +2856,224 @@ __global__ void __launch_bounds__(B2_COV_BLOCK) k_micp_information(const __grid_
         micp_cov_finalize(&s_sum[0][0], w, L.n_sensors, L.tau, L.degenerate_variance, out);
         *ticket = 0u;
     }
+}
+#endif
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Stein variational steps of the particle set over the distance field (b2_pf_stein_update; SURVEY appendix L; the MegaParticles TODO of
+// the reference's docs/RMCL.md).  Per iteration: k_pf_stein_score writes J's snapshot (chart and score of each reference), then
+// k_pf_stein_bandwidth the kernel bandwidth h, then k_pf_stein_move moves every particle from the snapshot.  The move reads J from the
+// snapshot only, so it can write the poses in place.  Every operation below is individually rounded (FMAs explicit; exp_f, atan2_d,
+// sin_d, cos_d of b2_math.cuh), so the host-compiled functions reproduce the device's bits.
+// ---------------------------------------------------------------------------------------------------------------------
+#define B2_PF_STEIN_TAG 8u
+#define B2_STEIN_BLOCK 256               // bandwidth and move: one particle per thread, est_grid_reduce's 8 warps
+#define B2_STEIN_NBW 7                   // bandwidth sums: count, x, y, x^2, y^2, cos psi, sin psi
+#define B2_STEIN_NMV 3                   // step sums: count, dx^2 + dy^2, dpsi^2
+struct SteinRef { float x, y, p, gx, gy, gp; };       // one reference: chart and score; x = NaN marks one that contributes nothing
+struct PfSteinState { b2_stein_result rec; unsigned int ticket[2]; };
+
+B2_DEV bool stein_finite3(const float c[3])
+{
+    const float inf = u2f(0x7f800000u);
+    return fabsf(c[0]) < inf && fabsf(c[1]) < inf && fabsf(c[2]) < inf;
+}
+// chart (x, y, psi) of a pose: psi = atan2(2 (wz + xy), 1 - 2 (y^2 + z^2)), the arguments in float ops, atan2 in FP64 rounded to float;
+// psi is NaN for a non-finite quaternion (atan2 of two infinities is finite)
+B2_DEV void stein_chart(const Tf& T, float c[3])
+{
+    const Q4 q = T.R;
+    const float inf = u2f(0x7f800000u);
+    const float b = mul(2.0f, add(mul(q.w, q.z), mul(q.x, q.y))), a = sub(1.0f, mul(2.0f, add(mul(q.y, q.y), mul(q.z, q.z))));
+    const bool qf = fabsf(q.x) < inf && fabsf(q.y) < inf && fabsf(q.z) < inf && fabsf(q.w) < inf;
+    c[0] = T.t.x; c[1] = T.t.y; c[2] = qf ? (float)atan2_d((double)b, (double)a) : u2f(0x7fc00000u);
+}
+// wrap(a) = a - 2 pi rint(a / 2 pi), as fma(rint(a * (1 / 2 pi)), -2 pi, a) with both constants in float
+B2_DEV float stein_wrap(float a) { return fma_rn(rint_f(mul(a, 0.159154937f)), -6.28318548f, a); }
+
+// index of reference r of iteration k: r itself when J is the whole set, else word 0 of Philox4x32-10 with counter (r, B2_PF_STEIN_TAG,
+// step, k) and key seed, modulo n
+B2_DEV uint32_t stein_ref_index(uint32_t r, uint32_t n, uint32_t n_ref, uint64_t seed, uint32_t step, uint32_t k)
+{
+    if (n_ref == 0u || n_ref >= n) return r;
+    uint32_t w[4];
+    philox4x32_10(r, B2_PF_STEIN_TAG, step, k, (uint32_t)seed, (uint32_t)(seed >> 32), w);
+    return w[0] % n;
+}
+
+// one beam's term of the score of the particle with map pose T (Tsm = T Tsb): a (grad_x, grad_y, (q_x - t_x) grad_y - (q_y - t_y) grad_x),
+// q the point k_pf_update_field looks up, a = -(e / sigma2) (1 - w) G / ((1 - w) G + w), G = exp(-e^2 / (2 sigma2)) (0 when (1 - w) G is 0);
+// zero for a non-finite point
+B2_DEV void stein_beam_term(const DfieldView& f, const Tf& Tsm, V3 t, const PfBeam& b, float sigma2, float w, float out[3])
+{
+    const V3 orig_m = tf_apply(Tsm, mk3(b.ox, b.oy, b.oz));
+    const V3 dir_m = q_rot(Tsm.R, mk3(b.dx, b.dy, b.dz));
+    const V3 q = v_add(orig_m, v_scale(dir_m, b.range));
+    V3 g;
+    const float e = df_lookup_grad(f, q, g);
+    out[0] = out[1] = out[2] = 0.0f;
+    if (!(fabsf(e) < u2f(0x7f800000u))) return;
+    const float G = exp_f(dvd(dvd(-mul(e, e), sigma2), 2.0f));
+    const float num = mul(sub(1.0f, w), G);
+    const float a = -mul(dvd(e, sigma2), num > 0.0f ? dvd(num, add(num, w)) : 0.0f);
+    out[0] = mul(a, g.x); out[1] = mul(a, g.y);
+    out[2] = mul(a, sub(mul(sub(q.x, t.x), g.y), mul(sub(q.y, t.y), g.x)));
+}
+// a reference's snapshot entry: the score sums its n_beams terms ([slot][3]) in slot order; a non-finite chart or score gives all NaN
+B2_DEV SteinRef stein_ref_entry(const Tf& T, const float* terms, uint32_t n_beams)
+{
+    float g[3] = {0.0f, 0.0f, 0.0f}, c[3];
+    for (uint32_t b = 0; b < n_beams; b++) { g[0] = add(g[0], terms[3 * b]); g[1] = add(g[1], terms[3 * b + 1]); g[2] = add(g[2], terms[3 * b + 2]); }
+    stein_chart(T, c);
+    SteinRef s;
+    if (stein_finite3(c) && stein_finite3(g)) { s.x = c[0]; s.y = c[1]; s.p = c[2]; s.gx = g[0]; s.gy = g[1]; s.gp = g[2]; }
+    else s.x = s.y = s.p = s.gx = s.gy = s.gp = u2f(0x7fc00000u);
+    return s;
+}
+
+// one particle's bandwidth terms (FP64): 1, x, y, x^2, y^2 and the unit yaw vector (a, b) / |(a, b)| of psi's arguments (0 when |(a, b)| is 0);
+// all zero for a particle with a non-finite chart
+B2_DEV void stein_bw_terms(const Tf& T, double acc[B2_STEIN_NBW])
+{
+    float c[3];
+    stein_chart(T, c);
+    if (!stein_finite3(c)) return;
+    const double x = (double)c[0], y = (double)c[1];
+    const double qx = T.R.x, qy = T.R.y, qz = T.R.z, qw = T.R.w;
+    const double a = 1.0 - 2.0 * (qy * qy + qz * qz), b = 2.0 * (qw * qz + qx * qy), r = sqrt_d(a * a + b * b);
+    acc[0] = 1.0; acc[1] = x; acc[2] = y; acc[3] = x * x; acc[4] = y * y;
+    acc[5] = r > 0.0 ? a / r : 0.0; acc[6] = r > 0.0 ? b / r : 0.0;
+}
+// h_d = max(s_d * fac, floor_d), fac = m^(-1/7) (host, double): s_x, s_y the standard deviations, s_psi = sqrt(2 (1 - R)), R the mean
+// resultant length; the product rounded to float; no finite particle gives the floors
+B2_DEV void stein_bandwidth(const double tot[B2_STEIN_NBW], double fac, float floor_t, float floor_r, float h[3])
+{
+    const double N = tot[0], mx = tot[1] / N, my = tot[2] / N, vx = tot[3] / N - mx * mx, vy = tot[4] / N - my * my;
+    const double C = tot[5] / N, S = tot[6] / N, one_m_R = 1.0 - sqrt_d(C * C + S * S);
+    const double s[3] = {sqrt_d(vx > 0.0 ? vx : 0.0), sqrt_d(vy > 0.0 ? vy : 0.0), sqrt_d(2.0 * (one_m_R > 0.0 ? one_m_R : 0.0))};
+    const float fl[3] = {floor_t, floor_t, floor_r};
+    for (int d = 0; d < 3; d++) { const float v = (float)(s[d] * fac); h[d] = v > fl[d] ? v : fl[d]; }
+}
+
+// one pair (i, j): acc += k_ij (g_j + Delta_ij / h^2), k_ij = exp(-1/2 sum_d Delta_d^2 / h_d^2); ih2 = 1 / h^2 per dimension (float)
+B2_DEV void stein_pair(const float ci[3], const SteinRef& r, const float ih2[3], float acc[3])
+{
+    const float dx = sub(ci[0], r.x), dy = sub(ci[1], r.y), dp = stein_wrap(sub(ci[2], r.p));
+    const float ux = mul(dx, ih2[0]), uy = mul(dy, ih2[1]), up = mul(dp, ih2[2]);
+    const float k = exp_f(mul(-0.5f, fma_rn(up, dp, fma_rn(uy, dy, mul(ux, dx)))));
+    acc[0] = fma_rn(k, add(r.gx, ux), acc[0]);
+    acc[1] = fma_rn(k, add(r.gy, uy), acc[1]);
+    acc[2] = fma_rn(k, add(r.gp, up), acc[2]);
+}
+B2_DEV void stein_inv_h2(const float h[3], float ih2[3]) { for (int d = 0; d < 3; d++) ih2[d] = dvd(1.0f, mul(h[d], h[d])); }
+
+// the step of particle i (pose T at pose_io, RMSProp state v_io) from its pair sum acc over m references, iteration it.  phi = acc / m;
+// v = phi^2 (it 0) or 0.9 v + 0.1 phi^2; delta = eps phi / (sqrt(v) + 1e-6).  A non-finite delta leaves pose and v.  Otherwise v is stored,
+// sums gets (1, dx^2 + dy^2, dpsi^2) of the proposed step, and the pose moves (x, y and R' = normalize(q_z(dpsi) R)) unless the wall check
+// from the old to the new position hits; returns 1 for a blocked step.
+B2_DEV uint32_t stein_move_one(const BvhView& bvh, b2_transform* pose_io, const Tf& T, float* v_io, const float acc[3], uint32_t m, uint32_t it,
+                               float step_t, float step_r, double sums[B2_STEIN_NMV])
+{
+    const float eps[3] = {step_t, step_t, step_r};
+    float v[3], d[3];
+    for (int k = 0; k < 3; k++) {
+        const float phi = dvd(acc[k], (float)m), p2 = mul(phi, phi);
+        v[k] = it == 0u ? p2 : add(mul(0.9f, v_io[k]), mul(0.1f, p2));
+        d[k] = dvd(mul(eps[k], phi), add(sqrt_rn(v[k]), 1e-6f));
+    }
+    if (!stein_finite3(d)) return 0u;
+    v_io[0] = v[0]; v_io[1] = v[1]; v_io[2] = v[2];
+    sums[0] = 1.0; sums[1] = (double)d[0] * (double)d[0] + (double)d[1] * (double)d[1]; sums[2] = (double)d[2] * (double)d[2];
+    const V3 t = mk3(add(T.t.x, d[0]), add(T.t.y, d[1]), T.t.z);
+    const float hh = mul(d[2], 0.5f);
+    Q4 qz; qz.x = 0.0f; qz.y = 0.0f; qz.z = (float)sin_d((double)hh); qz.w = (float)cos_d((double)hh);
+    const Q4 R = q_normalize(q_mul(qz, T.R));
+    if (pf_wall_hit(bvh, T.t, t)) return 1u;
+    pose_io->R.x = R.x; pose_io->R.y = R.y; pose_io->R.z = R.z; pose_io->R.w = R.w;          // the stamp stays
+    pose_io->t.x = t.x; pose_io->t.y = t.y;
+    return 0u;
+}
+
+#ifdef __CUDACC__
+// J x beams in k_pf_update_field's layout: a block of ppb references, lanes over beams, each term in shared memory at its beam's slot, one
+// thread per reference summing in slot order into the snapshot
+__global__ void __launch_bounds__(B2_PF_BLOCK) k_pf_stein_score(DfieldView f, const b2_transform* __restrict__ poses, uint32_t n, uint32_t m, uint32_t n_ref,
+                                                             uint64_t seed, uint32_t step, uint32_t it, b2_transform Tsb_val, const PfBeam* __restrict__ beams,
+                                                             uint32_t n_beams, float sigma2, float w_rand, uint32_t ppb, SteinRef* __restrict__ snap)
+{
+    extern __shared__ float s_term[];            // [ppb][n_beams][3]
+    __shared__ uint32_t s_idx[B2_PF_BLOCK];
+    const uint32_t r0 = blockIdx.x * ppb, nr = min(ppb, m - r0);
+    if (threadIdx.x < nr) s_idx[threadIdx.x] = stein_ref_index(r0 + threadIdx.x, n, n_ref, seed, step, it);
+    __syncthreads();
+    const Tf Tsb = tf_from_pod(Tsb_val);
+    const uint32_t total = nr * n_beams;
+    for (uint32_t t = threadIdx.x; t < total; t += blockDim.x) {
+        const uint32_t rl = t / n_beams, bi = t % n_beams;
+        const Tf T = tf_load(poses + s_idx[rl]);
+        const PfBeam b = beams[bi];
+        stein_beam_term(f, tf_mul(T, Tsb), T.t, b, sigma2, w_rand, s_term + 3 * ((size_t)rl * n_beams + b.slot));
+    }
+    __syncthreads();
+    if (threadIdx.x < nr) snap[r0 + threadIdx.x] = stein_ref_entry(tf_load(poses + s_idx[threadIdx.x]), s_term + 3 * (size_t)threadIdx.x * n_beams, n_beams);
+}
+// the bandwidth over all n particles: one per thread, est_grid_reduce's fixed order, the last block writes h and m into the record
+__global__ void __launch_bounds__(B2_STEIN_BLOCK) k_pf_stein_bandwidth(const b2_transform* __restrict__ poses, uint32_t n, uint32_t m, double fac, float floor_t,
+                                                                    float floor_r, double* __restrict__ partials, PfSteinState* __restrict__ st)
+{
+    __shared__ double s_w[8 * B2_STEIN_NBW], tot[B2_STEIN_NBW];
+    __shared__ bool is_last;
+    double acc[B2_STEIN_NBW];
+    #pragma unroll
+    for (int j = 0; j < B2_STEIN_NBW; j++) acc[j] = 0.0;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) stein_bw_terms(tf_load(poses + i), acc);
+    if (!est_grid_reduce<B2_STEIN_NBW, EstSlots2>(acc, partials, &st->ticket[0], s_w, tot, is_last)) return;
+    if (threadIdx.x != 0) return;
+    stein_bandwidth(tot, fac, floor_t, floor_r, st->rec.bandwidth);
+    st->rec.n_ref = m;
+    st->ticket[0] = 0u;
+}
+// One thread per particle i: the pair sum over J in tiles of B2_STEIN_BLOCK references (shared memory, N-body style), then the step.  The
+// blocked count goes to the record by integer atomics; the step sums by est_grid_reduce, whose last block writes the RMS steps.
+__global__ void __launch_bounds__(B2_STEIN_BLOCK) k_pf_stein_move(BvhView bvh, b2_transform* __restrict__ poses, uint32_t n, const SteinRef* __restrict__ snap,
+                                                               uint32_t m, uint32_t it, float step_t, float step_r, float* __restrict__ vstate,
+                                                               double* __restrict__ partials, PfSteinState* __restrict__ st)
+{
+    __shared__ SteinRef s_ref[B2_STEIN_BLOCK];
+    __shared__ double s_w[8 * B2_STEIN_NMV], tot[B2_STEIN_NMV];
+    __shared__ bool is_last;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    Tf T = tf_identity();
+    float ci[3] = {0.0f, 0.0f, 0.0f};
+    bool live = false;
+    if (i < n) { T = tf_load(poses + i); stein_chart(T, ci); live = stein_finite3(ci); }
+    float ih2[3];
+    { const float h[3] = {st->rec.bandwidth[0], st->rec.bandwidth[1], st->rec.bandwidth[2]}; stein_inv_h2(h, ih2); }
+    float acc[3] = {0.0f, 0.0f, 0.0f};
+    for (uint32_t j0 = 0; j0 < m; j0 += B2_STEIN_BLOCK) {
+        const uint32_t nt = min((uint32_t)B2_STEIN_BLOCK, m - j0);
+        __syncthreads();
+        if (threadIdx.x < nt) s_ref[threadIdx.x] = snap[j0 + threadIdx.x];
+        __syncthreads();
+        if (live) {
+            #pragma unroll 4
+            for (uint32_t j = 0; j < nt; j++) {
+                const SteinRef r = s_ref[j];
+                if (r.x == r.x) stein_pair(ci, r, ih2, acc);
+            }
+        }
+    }
+    double sums[B2_STEIN_NMV] = {0.0, 0.0, 0.0};
+    uint32_t blocked = 0u;
+    if (live) blocked = stein_move_one(bvh, poses + i, T, vstate + 3 * (size_t)i, acc, m, it, step_t, step_r, sums);
+    blocked = warp_sum_u32(blocked);
+    if ((threadIdx.x & 31) == 0 && blocked) atomicAdd(&st->rec.n_blocked, blocked);
+    if (!est_grid_reduce<B2_STEIN_NMV, EstSlots2>(sums, partials, &st->ticket[1], s_w, tot, is_last)) return;
+    if (threadIdx.x != 0) return;
+    st->rec.rms_step_t = tot[0] > 0.0 ? (float)sqrt(tot[1] / tot[0]) : 0.0f;
+    st->rec.rms_step_r = tot[0] > 0.0 ? (float)sqrt(tot[2] / tot[0]) : 0.0f;
+    st->ticket[1] = 0u;
 }
 #endif
 
