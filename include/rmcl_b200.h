@@ -86,7 +86,10 @@ B2_API int         b2_device_count(int* n);
 
 /* ---------------------------------------------------------------- map ---------------------------------------- */
 /* replaces rm::import_embree_map + Embree scene commit (rmcl_ros/src/nodes/micp_localization.cpp:188,
- * rmcl_ros/src/rmcl/PCDSensorUpdaterEmbree.cpp:158): vertices/faces in HOST memory -> BVH resident in HBM of `device`. */
+ * rmcl_ros/src/rmcl/PCDSensorUpdaterEmbree.cpp:158): vertices/faces in HOST memory -> BVH resident in HBM of `device`.
+ * Every vertex coordinate must be finite and at most 2^62 in magnitude (B2_ERR_INVALID otherwise): box extents then stay below 2^63, so the
+ * builders' box half-areas (<= 3 * 2^126 < FLT_MAX), box centres and octant slot costs are finite.  Beyond that they overflow to inf / NaN,
+ * and the tree would lose or misfile triangles; metric maps are many orders of magnitude smaller. */
 B2_API int b2_mesh_create(const float* verts_xyz, uint32_t n_vertices, const uint32_t* faces_ijk, uint32_t n_faces,
                           int device, int build_mode, b2_mesh** out);
 /* rm::import_embree_map(file) (rmcl_ros/src/nodes/micp_localization.cpp:188, rmcl_ros/src/rmcl/PCDSensorUpdaterEmbree.cpp:158): mesh file ->
@@ -98,7 +101,8 @@ B2_API int b2_mesh_file_load(const char* path, float** verts_xyz, uint32_t* nv, 
 B2_API void b2_mesh_file_free(float* verts_xyz, uint32_t* faces_ijk);
 /* Dynamic maps (SURVEY.md 8f1): the vertices moved, faces unchanged -> refit the resident BVH instead of rebuilding it (the reference
  * re-commits its Embree scene and flags dependants `outdated`, Correspondences.hpp:26-31).  Maps built with B2_BUILD_DEVICE_LBVH only; the call
- * synchronises the device first, so no handle may be tracing concurrently from another thread.  Results afterwards equal a fresh build's. */
+ * synchronises the device first, so no handle may be tracing concurrently from another thread.  Results afterwards equal a fresh build's.
+ * Host vertices obey b2_mesh_create's bound (finite, |coordinate| <= 2^62); device vertices are not inspected. */
 B2_API int b2_mesh_refit(b2_mesh* m, const float* verts_xyz, uint32_t nv, int src_is_device);
 /* BVH blob (SURVEY.md 8b): the built map as one host buffer (header + nodes + leaf triangle records), so that a map is built once and
  * shipped to the other ranks (broadcast) or cached on disk; b2_mesh_create_from_blob validates the header and every index before uploading. */

@@ -78,7 +78,7 @@ extern "C" int b2_mesh_create(const float* verts, uint32_t nv, const uint32_t* f
     CU(cudaSetDevice(device));
     if (build_mode == B2_BUILD_DEVICE_LBVH) {
         for (size_t i = 0; i < 3 * (size_t)nf; i++) if (faces[i] >= nv) return fail(B2_ERR_INVALID, "BVH build failed: face index out of range");
-        for (size_t i = 0; i < 3 * (size_t)nv; i++) if (!std::isfinite(verts[i])) return fail(B2_ERR_INVALID, "BVH build failed: non-finite vertex");
+        if (!b2_vertices_ok(verts, 3 * (size_t)nv)) return fail(B2_ERR_INVALID, "BVH build failed: a vertex coordinate is not finite or exceeds 2^62 in magnitude");
         const auto t0 = std::chrono::steady_clock::now();
         float* d_v = nullptr; uint32_t* d_f = nullptr;
         cudaError_t e = cudaMalloc((void**)&d_v, sizeof(float) * 3 * (size_t)nv);
@@ -156,7 +156,7 @@ extern "C" int b2_mesh_refit(b2_mesh* m, const float* verts, uint32_t nv, int sr
     if (nv != m->n_verts) return fail(B2_ERR_INVALID, "refit keeps the topology: %u vertices given, the map has %u", nv, m->n_verts);
     CU(cudaSetDevice(m->device));
     const auto t0 = std::chrono::steady_clock::now();
-    if (!src_is_device) for (size_t i = 0; i < 3 * (size_t)nv; i++) if (!std::isfinite(verts[i])) return fail(B2_ERR_INVALID, "refit: non-finite vertex");
+    if (!src_is_device && !b2_vertices_ok(verts, 3 * (size_t)nv)) return fail(B2_ERR_INVALID, "refit: a vertex coordinate is not finite or exceeds 2^62 in magnitude");
     DevBuf<float> d_v; DevBuf<unsigned int> d_bits;
     const float* vp = verts;
     if (!src_is_device) {
@@ -185,15 +185,7 @@ extern "C" int b2_mesh_refit(b2_mesh* m, const float* verts, uint32_t nv, int sr
     return rc;
 }
 
-// ---- BVH blob: build once, ship to the other ranks / to disk (SURVEY.md 8b: b2_mesh_bvh_blob for broadcast) ---------------------------
-struct B2BlobHeader {
-    char     magic[8];                 // "B2BVH8F\0"
-    uint32_t version, node_bytes, tri_bytes, n_nodes, n_tris, n_faces, n_verts, max_depth;
-    int32_t  build_mode;
-    float    abs_max[3], sah;
-    uint32_t pad;                      // 64 bytes: the node array that follows stays 16-byte aligned inside an aligned buffer
-};
-static_assert(sizeof(B2BlobHeader) == 64, "blob header must be 64 bytes");
+// ---- BVH blob: build once, ship to the other ranks / to disk (SURVEY.md 8b: b2_mesh_bvh_blob for broadcast); layout in bvh8.h --------
 static const char kBlobMagic[8] = {'B', '2', 'B', 'V', 'H', '8', 'F', 0};
 
 extern "C" int b2_mesh_blob_size(const b2_mesh* m, uint64_t* bytes)

@@ -26,6 +26,7 @@
 // Leaf triangle record (48 B = 3 x 16 B): (v0.xyz, face_id as bits), (v1.xyz, 0), (v2.xyz, 0); records of one node are contiguous,
 // in slot order; at most 3 triangles per leaf child, at most 24 per node.
 #pragma once
+#include <stddef.h>
 #include <stdint.h>
 
 struct alignas(16) B2Node8 {
@@ -70,6 +71,27 @@ static_assert(sizeof(B2Tri) == 48, "triangle record must be 48 bytes");
 
 #define B2_TRAVERSAL_STACK 40          // uint2 entries per ray; builder refuses trees deeper than B2_TRAVERSAL_STACK - 4
 #define B2_MAX_LEAF_TRIS 3
+
+// Largest |vertex coordinate| a map accepts: 2^62.  Box extents then stay below 2^63, so every box half-area the builders form
+// (dx dy + dy dz + dz dx <= 3 * 2^126 < FLT_MAX), every box centre 0.5 (lo + hi) and every slot cost (a sum of three centre differences)
+// is finite; larger coordinates would turn them into inf / NaN and the SAH and octant decisions with them.
+#define B2_MAX_ABS_COORD 4611686018427387904.0f
+// vertices a map can be built or refitted from: finite and within B2_MAX_ABS_COORD
+inline bool b2_vertices_ok(const float* v, size_t n_floats)
+{
+    for (size_t i = 0; i < n_floats; i++) if (!(v[i] >= -B2_MAX_ABS_COORD && v[i] <= B2_MAX_ABS_COORD)) return false;
+    return true;
+}
+
+// BVH blob (b2_mesh_export_blob / b2_mesh_create_from_blob): this header, then n_nodes B2Node8, then n_tris B2Tri
+struct B2BlobHeader {
+    char     magic[8];                 // "B2BVH8F\0"
+    uint32_t version, node_bytes, tri_bytes, n_nodes, n_tris, n_faces, n_verts, max_depth;
+    int32_t  build_mode;
+    float    abs_max[3], sah;
+    uint32_t pad;                      // 64 bytes: the node array that follows stays 16-byte aligned inside an aligned buffer
+};
+static_assert(sizeof(B2BlobHeader) == 64, "blob header must be 64 bytes");
 
 // host-side result of a build
 struct B2BvhHost {

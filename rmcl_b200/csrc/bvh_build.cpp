@@ -36,7 +36,7 @@ struct Prim { Box box; float c[3]; };
 constexpr int   kBins = 32;
 constexpr float kCNode = 1.0f;      // cost of visiting one wide node
 static float kCPrim = 0.35f;        // cost of testing one triangle relative to visiting one wide node (B2_SAH_CPRIM overrides)
-constexpr float kInf = 1e30f;
+constexpr float kInf = INFINITY;    // "no candidate yet": every finite cost beats it
 
 struct Builder {
     const Prim* prims;
@@ -152,14 +152,14 @@ int b2_build_bvh8_host(const float* verts, uint32_t nv, const uint32_t* faces, u
 {
     static const char* e_empty = "empty mesh";
     static const char* e_index = "face index out of range";
-    static const char* e_nan = "non-finite vertex";
+    static const char* e_nan = "a vertex coordinate is not finite or exceeds 2^62 in magnitude";
     static const char* e_depth = "BVH too deep for the traversal stack";
     static const char* e_oom = "out of host memory";
     *out = B2BvhHost();
     if (const char* e = getenv("B2_SAH_CPRIM")) kCPrim = (float)atof(e);
     if (nf == 0 || nv == 0) { *err = e_empty; return -3; }
     for (uint32_t i = 0; i < 3 * nf; i++) if (faces[i] >= nv) { *err = e_index; return -1; }
-    for (size_t i = 0; i < 3 * (size_t)nv; i++) if (!std::isfinite(verts[i])) { *err = e_nan; return -1; }
+    if (!b2_vertices_ok(verts, 3 * (size_t)nv)) { *err = e_nan; return -1; }
 
     std::vector<Prim> prims(nf);
     std::vector<uint32_t> order(nf);
@@ -203,9 +203,10 @@ int b2_build_bvh8_host(const float* verts, uint32_t nv, const uint32_t* faces, u
             }
             cd[j] = best; d.dist[j] = (uint8_t)bk;
         }
-        const float c_leaf = nd.count <= B2_MAX_LEAF_TRIS ? A * (float)nd.count * kCPrim : kInf;
+        // a sub-tree with more triangles than a leaf child holds is an inner node whatever the costs say (they may be inf)
+        const float c_leaf = A * (float)nd.count * kCPrim;
         const float c_inner = cd[8] + A * kCNode;
-        if (c_leaf <= c_inner) { d.c[1] = c_leaf; d.kind1 = 0; } else { d.c[1] = c_inner; d.kind1 = 1; }
+        if (nd.count <= B2_MAX_LEAF_TRIS && c_leaf <= c_inner) { d.c[1] = c_leaf; d.kind1 = 0; } else { d.c[1] = c_inner; d.kind1 = 1; }
         for (int i = 2; i <= 7; i++) {
             if (cd[i] < d.c[i - 1]) { d.c[i] = cd[i]; d.use_dist[i] = 1; } else { d.c[i] = d.c[i - 1]; d.use_dist[i] = 0; }
         }
@@ -250,6 +251,10 @@ int b2_build_bvh8_host(const float* verts, uint32_t nv, const uint32_t* faces, u
             float bv = -kInf; int bc = -1, bs = -1;
             for (int c = 0; c < nc; c++) if (slot_of[c] < 0)
                 for (int s = 0; s < 8; s++) if (child_in_slot[s] < 0 && cost[c][s] > bv) { bv = cost[c][s]; bc = c; bs = s; }
+            if (bc < 0) {                                 // every remaining cost is NaN or -inf: first free child into the first free slot
+                for (bc = 0; slot_of[bc] >= 0; bc++) {}
+                for (bs = 0; child_in_slot[bs] >= 0; bs++) {}
+            }
             slot_of[bc] = bs; child_in_slot[bs] = bc;
         }
 

@@ -13,17 +13,31 @@ extern "C" {
 
 struct EmulScene { B2BvhHost bvh; };
 
-__attribute__((visibility("default"))) void* emul_scene_create(const float* verts, uint32_t nv, const uint32_t* faces, uint32_t nf)
+__attribute__((visibility("default"))) void* emul_scene_create(const float* verts, uint32_t nv, const uint32_t* faces, uint32_t nf, const char** err)
 {
     EmulScene* s = new EmulScene();
-    const char* err = "";
-    if (b2_build_bvh8_host(verts, nv, faces, nf, &s->bvh, &err) != 0) { delete s; return nullptr; }
+    *err = "";
+    if (b2_build_bvh8_host(verts, nv, faces, nf, &s->bvh, err) != 0) { delete s; return nullptr; }
     return s;
 }
 __attribute__((visibility("default"))) void emul_scene_destroy(void* p) { if (p) { b2_free_bvh8_host(&((EmulScene*)p)->bvh); delete (EmulScene*)p; } }
 __attribute__((visibility("default"))) void emul_scene_info(void* p, uint32_t* n_nodes, uint32_t* n_tris, uint32_t* depth, float* sah)
 {
     EmulScene* s = (EmulScene*)p; *n_nodes = s->bvh.n_nodes; *n_tris = s->bvh.n_tris; *depth = s->bvh.max_depth; *sah = s->bvh.sah_cost;
+}
+// the host-built tree in the layout of b2_mesh_export_blob (header as b2_mesh_create leaves it for a host build: build mode 0, n_verts nv),
+// so that one checker reads both; dst holds sizeof(B2BlobHeader) + n_nodes * 224 + n_tris * 48 bytes
+__attribute__((visibility("default"))) void emul_export(void* p, uint32_t n_faces, uint32_t n_verts, uint8_t* dst)
+{
+    const B2BvhHost& b = ((EmulScene*)p)->bvh;
+    B2BlobHeader hd; memset(&hd, 0, sizeof(hd));
+    memcpy(hd.magic, "B2BVH8F", 8);
+    hd.version = 2; hd.node_bytes = sizeof(B2Node8); hd.tri_bytes = sizeof(B2Tri); hd.n_nodes = b.n_nodes; hd.n_tris = b.n_tris; hd.n_faces = n_faces;
+    hd.n_verts = n_verts; hd.max_depth = b.max_depth; hd.build_mode = 0; hd.sah = b.sah_cost;
+    for (int k = 0; k < 3; k++) hd.abs_max[k] = b.abs_max[k];
+    memcpy(dst, &hd, sizeof(hd));
+    memcpy(dst + sizeof(hd), b.nodes, sizeof(B2Node8) * (size_t)b.n_nodes);
+    memcpy(dst + sizeof(hd) + sizeof(B2Node8) * (size_t)b.n_nodes, b.tris, sizeof(B2Tri) * (size_t)b.n_tris);
 }
 static BvhView view(void* p)
 {

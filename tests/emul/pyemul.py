@@ -60,9 +60,10 @@ class Scene:
     def __init__(self, verts, faces):
         self.verts = _f32(verts).reshape(-1, 3)
         self.faces = np.ascontiguousarray(faces, np.uint32).reshape(-1, 3)
-        h = lib().emul_scene_create(_p(self.verts), C.c_uint32(len(self.verts)), _p(self.faces), C.c_uint32(len(self.faces)))
+        err = C.c_char_p()
+        h = lib().emul_scene_create(_p(self.verts), C.c_uint32(len(self.verts)), _p(self.faces), C.c_uint32(len(self.faces)), C.byref(err))
         if not h:
-            raise RuntimeError("emul BVH build failed")
+            raise RuntimeError("emul BVH build failed: " + err.value.decode())
         self._h = C.c_void_p(h)
 
     def __del__(self):
@@ -75,6 +76,13 @@ class Scene:
         a, b, c, d = C.c_uint32(), C.c_uint32(), C.c_uint32(), C.c_float()
         lib().emul_scene_info(self._h, C.byref(a), C.byref(b), C.byref(c), C.byref(d))
         return dict(n_nodes=a.value, n_tris=b.value, max_depth=c.value, sah=d.value)
+
+    def export_blob(self):
+        """the host-built tree as Map.export_blob lays it out (numpy uint8)"""
+        inf = self.info()
+        buf = np.zeros(64 + 224 * inf["n_nodes"] + 48 * inf["n_tris"], np.uint8)
+        lib().emul_export(self._h, C.c_uint32(len(self.faces)), C.c_uint32(len(self.verts)), _p(buf))
+        return buf
 
     def intersect(self, origs, dirs, tfar=np.inf, per_ray=False):
         origs, dirs = _f32(origs).reshape(-1, 3), _f32(dirs).reshape(-1, 3)

@@ -141,10 +141,11 @@ def mesh(name):
 
 
 class Scene64:
-    """float64 view of a float32 mesh, with a grouping of the faces for culling large scenes"""
+    """float64 view of a float32 mesh (the named scene's, or V, F given), with a grouping of the faces for culling large scenes"""
 
-    def __init__(self, name):
-        V, F = mesh(name)
+    def __init__(self, name, V=None, F=None):
+        if V is None:
+            V, F = mesh(name)
         self.name, self.V, self.F = name, V, F
         v = V.astype(np.float64)
         self.v0, self.v1, self.v2 = v[F[:, 0]], v[F[:, 1]], v[F[:, 2]]
