@@ -102,9 +102,11 @@ def node_points(g, ids):
 
 
 def brick_centres(g):
-    """float32 centre node (8b + 4) of every brick, in linear order"""
-    ids = np.arange(g.n_bricks)
-    return node_points(g, ids)[:, 4, 4, 4, :]
+    """float32 centre node (8b + 4) of every brick, in linear order: node_points(g, ids)[:, 4, 4, 4] without its other 728 nodes"""
+    ids = np.arange(g.n_bricks, dtype=np.int64)
+    bx, by, _ = g.bdims
+    b = np.stack([ids % bx, ids // bx % by, ids // bx // by], 1)
+    return g.lo + (8 * b + 4).astype(np.float32) * np.float32(g.h)
 
 
 def lookup64(g, index, bricks, pts):
@@ -264,3 +266,32 @@ class RefField:
         out = np.empty(len(pts), np.float32)
         _ref_lib().orc_df_dist(C.c_void_p(self._s), _p(pts), C.c_uint32(len(pts)), C.c_int(int(brute)), _p(out))
         return out
+
+    def lower_bound(self, pts, depth=2):
+        """float64 lower bound of the distance from each point to the mesh: the distance to the nearest of 2^depth boxes that together hold
+        every face (faces split at the median centroid along the longest axis of their box, depth times)"""
+        T = self.V[self.F].astype(np.float64)
+        groups = [np.arange(len(T))]
+        for _ in range(depth):
+            nxt = []
+            for g in groups:
+                if len(g) < 2:
+                    nxt.append(g)
+                    continue
+                c = T[g].mean(1)
+                ax = int(np.argmax(c.max(0) - c.min(0)))
+                o = g[np.argsort(c[:, ax], kind="stable")]
+                nxt += [o[: len(o) // 2], o[len(o) // 2:]]
+            groups = nxt
+        lo = np.array([T[g].min((0, 1)) for g in groups])
+        hi = np.array([T[g].max((0, 1)) for g in groups])
+        pts = np.asarray(pts, np.float64).reshape(-1, 3)
+        out = np.full(len(pts), np.inf)
+        for l, h in zip(lo, hi):
+            d2 = np.zeros(len(pts))
+            for k in range(3):
+                e = np.maximum(l[k] - pts[:, k], pts[:, k] - h[k])
+                np.maximum(e, 0.0, out=e)
+                d2 += e * e
+            np.minimum(out, d2, out=out)
+        return np.sqrt(out)
