@@ -4,42 +4,17 @@
   the chain of correct() (:847-854) as a loop over the oracle's multi-sensor correctOnce (oracle/: orc_micp_correct_once_multi) fed with it.
 * product_progress / product_gate: the product's own update (rmcl_b200/csrc/icp_loop.cuh) compiled for the CPU (chain_ref/progress_emul.cu).
 * progress_np: a numpy restatement of the same update.
-
-The two small libraries are compiled on first use into a per-user directory under the system temporary directory (keyed by the sources'
-hash), never into the tree."""
+"""
 import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRC = os.path.join(_HERE, "chain_ref")
-_CSRC = os.path.join(os.path.dirname(_HERE), "rmcl_b200", "csrc")
+import native
+from rmcl_b200.synth import CROSS_STATS_DTYPE as CROSS_STATS, TRANSFORM_DTYPE as TRANSFORM
 
-TRANSFORM = np.dtype([("R", np.float32, 4), ("t", np.float32, 3), ("stamp", np.uint32)])
-CROSS_STATS = np.dtype([("dataset_mean", np.float32, 3), ("model_mean", np.float32, 3), ("covariance", np.float32, 9), ("n_meas", np.uint32)])
 # one b2_micp_step record (include/rmcl_b200.h)
 MICP_STEP = np.dtype([("Tom_new", TRANSFORM), ("T_onew_oold", TRANSFORM), ("Cmerged_o", CROSS_STATS), ("convergence_progress", np.float64),
                       ("valid_measurements", np.uint32), ("total_measurements", np.uint32)])
-
-
-def _build(name, sources, cmd):
-    h = hashlib.sha1()
-    for s in sources:
-        with open(s, "rb") as f:
-            h.update(f.read())
-    h.update(" ".join(cmd).encode())
-    d = os.path.join(tempfile.gettempdir(), f"b2_chain_ref_{os.getuid()}")
-    os.makedirs(d, exist_ok=True)
-    out = os.path.join(d, f"{name}_{h.hexdigest()[:16]}.so")
-    if not os.path.exists(out):
-        tmp = f"{out}.{os.getpid()}.tmp"
-        subprocess.check_call(cmd + ["-o", tmp])
-        os.replace(tmp, out)
-    return C.CDLL(out)
 
 
 _ref = None
@@ -49,9 +24,7 @@ _emul = None
 def _ref_lib():
     global _ref
     if _ref is None:
-        src = os.path.join(_SRC, "progress_ref.c")
-        cc = "/usr/bin/gcc" if os.access("/usr/bin/gcc", os.X_OK) else "gcc"
-        _ref = _build("progress_ref", [src], [cc, "-O2", "-ffp-contract=off", "-mavx2", "-mfma", "-fPIC", "-std=gnu11", "-shared", src, "-lm"])
+        _ref = native.restatement("chain_ref/progress_ref.c")
         _ref.ref_micp_progress.restype = C.c_double
         _ref.ref_micp_progress.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_int]
     return _ref
@@ -60,12 +33,7 @@ def _ref_lib():
 def _emul_lib():
     global _emul
     if _emul is None:
-        src = os.path.join(_SRC, "progress_emul.cu")
-        deps = [src] + [os.path.join(_CSRC, f) for f in ("kernels.cuh", "icp_loop.cuh", "trace.cuh", "b2_math.cuh", "bvh8.h")] + \
-               [os.path.join(os.path.dirname(_HERE), "include", "rmcl_b200.h")]
-        nvcc = os.environ.get("NVCC", "nvcc")
-        _emul = _build("progress_emul", deps, [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17", "-fmad=false",
-                                               "-Xcompiler", "-fPIC,-ffp-contract=off,-mavx2,-mfma,-fvisibility=hidden", "-shared", src])
+        _emul = native.emulator()
         _emul.emul_micp_progress.restype = C.c_double
         _emul.emul_micp_progress.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_int]
         _emul.emul_adaptive_max_dist.restype = C.c_float

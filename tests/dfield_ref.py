@@ -5,17 +5,14 @@
 * RefField: a node's value restated over the oracle's closest point (dfield_ref/dfield_ref.c), brute force or through the oracle's BVH.
 * node_points / lookup64 / update64: numpy restatements -- the nodes' positions in float32 ops, the trilinear lookup in float64 over the
   stored nodes, the sensor update in float64.
-Both libraries are built on first use into the per-user temporary directory of chain_ref."""
+Both libraries are built on first use by native.py."""
 import ctypes as C
-import os
 
 import numpy as np
 
-from chain_ref import _build
+import native
+import pyemul
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ROOT = os.path.dirname(_HERE)
-_CSRC = os.path.join(_ROOT, "rmcl_b200", "csrc")
 NOBRICK = 0xFFFFFFFF
 _ref = None
 _emul = None
@@ -24,10 +21,7 @@ _emul = None
 def _ref_lib():
     global _ref
     if _ref is None:
-        src = os.path.join(_HERE, "dfield_ref", "dfield_ref.c")
-        cc = "/usr/bin/gcc" if os.access("/usr/bin/gcc", os.X_OK) else "gcc"
-        deps = [src, os.path.join(_ROOT, "oracle", "oracle.c"), os.path.join(_ROOT, "oracle", "oracle.h")]
-        _ref = _build("dfield_ref", deps, [cc, "-O2", "-fopenmp", "-ffp-contract=off", "-mavx2", "-mfma", "-fPIC", "-std=gnu11", "-shared", src, "-lm"])
+        _ref = native.restatement("dfield_ref/dfield_ref.c")
         _ref.orc_scene_create.restype = C.c_void_p
         _ref.orc_scene_destroy.argtypes = [C.c_void_p]
     return _ref
@@ -36,15 +30,7 @@ def _ref_lib():
 def _emul_lib():
     global _emul
     if _emul is None:
-        src = os.path.join(_HERE, "dfield_ref", "dfield_emul.cu")
-        deps = [src] + [os.path.join(_CSRC, f) for f in ("kernels.cuh", "icp_loop.cuh", "trace.cuh", "b2_math.cuh", "bvh8.h", "bvh_build.cpp")] + \
-               [os.path.join(_ROOT, "include", "rmcl_b200.h")]
-        nvcc = os.environ.get("NVCC", "nvcc")
-        _emul = _build("dfield_emul", deps, [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17", "-fmad=false",
-                                             "-Xcompiler", "-fPIC,-fopenmp,-ffp-contract=off,-mavx2,-mfma,-fvisibility=hidden", "-shared", src,
-                                             os.path.join(_CSRC, "bvh_build.cpp"), "-lgomp"])
-        _emul.emul_df_scene.restype = C.c_void_p
-        _emul.emul_df_scene_free.argtypes = [C.c_void_p]
+        _emul = native.emulator()
         _emul.emul_df_build.restype = C.c_int64
         _emul.emul_df_grid.restype = C.c_int
     return _emul
@@ -191,17 +177,8 @@ def evaluate64(err, dist_sigma):
     return np.exp(-(err * err) / sq / 2.0) / np.sqrt(2.0 * sq * np.pi)
 
 
-class ProductField:
+class ProductField(pyemul.Scene):
     """the product's distance-field functions on the CPU"""
-
-    def __init__(self, V, F):
-        self.V, self.F = _mesh(V, F)
-        self._s = _emul_lib().emul_df_scene(_p(self.V), C.c_uint32(len(self.V)), _p(self.F), C.c_uint32(len(self.F)))
-        assert self._s
-
-    def __del__(self):
-        if getattr(self, "_s", None):
-            _emul_lib().emul_df_scene_free(self._s)
 
     def build(self, g):
         """-> (index uint32 (bz, by, bx), bricks float32 (n, 9, 9, 9))"""
@@ -209,7 +186,7 @@ class ProductField:
         index = np.empty((bz, by, bx), np.uint32)
         cap = g.n_bricks
         bricks = np.empty((cap, 9, 9, 9), np.float32)
-        n = _emul_lib().emul_df_build(C.c_void_p(self._s), *g.args(), _p(index), _p(bricks), C.c_uint64(cap))
+        n = _emul_lib().emul_df_build(self._h, *g.args(), _p(index), _p(bricks), C.c_uint64(cap))
         assert n >= 0
         return index, bricks[:n].copy()
 
@@ -218,7 +195,7 @@ class ProductField:
         pts = np.ascontiguousarray(pts, np.float32).reshape(-1, 3)
         d2, face = np.empty(len(pts), np.float32), np.empty(len(pts), np.uint32)
         t = np.float32(trunc)
-        _emul_lib().emul_df_closest(C.c_void_p(self._s), _p(pts), C.c_uint32(len(pts)), C.c_int(int(bounded)), C.c_float(float(t * t)), _p(d2), _p(face))
+        _emul_lib().emul_df_closest(self._h, _p(pts), C.c_uint32(len(pts)), C.c_int(int(bounded)), C.c_float(float(t * t)), _p(d2), _p(face))
         return d2, face
 
 

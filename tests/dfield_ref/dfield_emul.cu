@@ -1,34 +1,7 @@
 // dfield_emul.cu -- TEST HARNESS ONLY: the product's distance-field functions (rmcl_b200/csrc/kernels.cuh: df_grid, df_limits,
 // df_brick_alloc, df_node_value, df_brick_node, df_lookup, pf_eval_field, pf_merge; trace.cuh: closest_point) compiled for the CPU over the
 // product's host-built BVH.  The build runs the three device steps as host loops: every brick classified, slots handed out in brick order
-// (the exclusive scan), every node of every allocated brick filled.  Built by tests/dfield_ref.py with the flags of tests/chain_ref (host
-// code with -ffp-contract=off: plain ops rounded like __fmul_rn etc.).
-#include "../../rmcl_b200/csrc/kernels.cuh"
-
-#include <cstdio>
-#include <vector>
-
-#define EMUL_API extern "C" __attribute__((visibility("default")))
-
-static BvhView view_of(const void* p)
-{
-    const B2BvhHost* b = (const B2BvhHost*)p;
-    BvhView v; v.nodes = (const float4*)b->nodes; v.tris = (const float4*)b->tris;
-    v.bx = b->abs_max[0]; v.by = b->abs_max[1]; v.bz = b->abs_max[2];
-    return v;
-}
-
-EMUL_API void* emul_df_scene(const float* verts, uint32_t nv, const uint32_t* faces, uint32_t nf)
-{
-    B2BvhHost* b = new B2BvhHost();
-    const char* err = "";
-    if (b2_build_bvh8_host(verts, nv, faces, nf, b, &err) != 0) { delete b; return nullptr; }
-    return b;
-}
-EMUL_API void emul_df_scene_free(void* p)
-{
-    if (p) { b2_free_bvh8_host((B2BvhHost*)p); delete (B2BvhHost*)p; }
-}
+// (the exclusive scan), every node of every allocated brick filled.  Included into the emulator library (tests/emul/emul.cu).
 
 // grid of the box: dims_out[0..2] nodes, dims_out[3..5] bricks, origin / inv_h; returns 0, or 1 when df_grid refuses (reason in why)
 EMUL_API int emul_df_grid(const float* lo, const float* hi, float h, float trunc, uint32_t* dims_out, float* inv_h, uint64_t* n_bricks, char* why, int why_cap)
@@ -64,14 +37,6 @@ EMUL_API int64_t emul_df_build(void* p, const float* lo, const float* hi, float 
         bricks[t] = df_node_value(bvh, f, i, j, k, trunc2);
     }
     return (int64_t)list.size();
-}
-
-static DfieldView field_of(const float* lo, const float* hi, float h, float trunc, const uint32_t* index, const float* bricks)
-{
-    DfieldView f; uint64_t nb = 0;
-    df_grid(lo, hi, h, trunc, &f, &nb);
-    f.index = index; f.bricks = bricks;
-    return f;
 }
 
 EMUL_API void emul_df_lookup(const float* lo, const float* hi, float h, float trunc, const uint32_t* index, const float* bricks, const float* pts, uint32_t n, float* out)

@@ -1,35 +1,56 @@
 // emul.cu -- TEST HARNESS ONLY: runs the product's host+device traversal / math functions (rmcl_b200/csrc/*.cuh) on the CPU so
 // that the BVH builder, the traversal logic and the op-for-op parity with the oracle can be checked in a container without a GPU.
-// Not part of librmcl_b200.so and never shipped; built into tests/emul/_build/libb2emul.so by tests/emul/Makefile.
+// Not part of librmcl_b200.so and never shipped.  One translation unit with every feature's *_emul.cu (included at the end), built
+// with the host BVH build into one library by tests/native.py (emulator).
 // Host code is compiled with -ffp-contract=off -mfma, so plain float ops are individually rounded exactly like the device's
 // __fmul_rn/__fadd_rn and fmaf() is a true FMA.
 #include "../../rmcl_b200/csrc/kernels.cuh"
 
+#include <algorithm>
+#include <cmath>
+#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <vector>
 
+#define EMUL_API extern "C" __attribute__((visibility("default")))
+
+// the product's host-built BVH of a mesh: the scene handle of every emul_* function that takes one
+EMUL_API void* emul_scene_create(const float* verts, uint32_t nv, const uint32_t* faces, uint32_t nf, const char** err)
+{
+    B2BvhHost* b = new B2BvhHost();
+    *err = "";
+    if (b2_build_bvh8_host(verts, nv, faces, nf, b, err) != 0) { delete b; return nullptr; }
+    return b;
+}
+EMUL_API void emul_scene_destroy(void* p) { if (p) { b2_free_bvh8_host((B2BvhHost*)p); delete (B2BvhHost*)p; } }
+static BvhView view_of(const void* p)
+{
+    const B2BvhHost* b = (const B2BvhHost*)p;
+    BvhView v; v.nodes = (const float4*)b->nodes; v.tris = (const float4*)b->tris;
+    v.bx = b->abs_max[0]; v.by = b->abs_max[1]; v.bz = b->abs_max[2];
+    return v;
+}
+// a distance field's view over host arrays, its grid as df_grid makes it
+static DfieldView field_of(const float* lo, const float* hi, float h, float trunc, const uint32_t* index, const float* bricks)
+{
+    DfieldView f; uint64_t nb = 0;
+    df_grid(lo, hi, h, trunc, &f, &nb);
+    f.index = index; f.bricks = bricks;
+    return f;
+}
+
 extern "C" {
 
-struct EmulScene { B2BvhHost bvh; };
-
-__attribute__((visibility("default"))) void* emul_scene_create(const float* verts, uint32_t nv, const uint32_t* faces, uint32_t nf, const char** err)
-{
-    EmulScene* s = new EmulScene();
-    *err = "";
-    if (b2_build_bvh8_host(verts, nv, faces, nf, &s->bvh, err) != 0) { delete s; return nullptr; }
-    return s;
-}
-__attribute__((visibility("default"))) void emul_scene_destroy(void* p) { if (p) { b2_free_bvh8_host(&((EmulScene*)p)->bvh); delete (EmulScene*)p; } }
 __attribute__((visibility("default"))) void emul_scene_info(void* p, uint32_t* n_nodes, uint32_t* n_tris, uint32_t* depth, float* sah)
 {
-    EmulScene* s = (EmulScene*)p; *n_nodes = s->bvh.n_nodes; *n_tris = s->bvh.n_tris; *depth = s->bvh.max_depth; *sah = s->bvh.sah_cost;
+    const B2BvhHost* b = (const B2BvhHost*)p; *n_nodes = b->n_nodes; *n_tris = b->n_tris; *depth = b->max_depth; *sah = b->sah_cost;
 }
 // the host-built tree in the layout of b2_mesh_export_blob (header as b2_mesh_create leaves it for a host build: build mode 0, n_verts nv),
 // so that one checker reads both; dst holds sizeof(B2BlobHeader) + n_nodes * 224 + n_tris * 48 bytes
 __attribute__((visibility("default"))) void emul_export(void* p, uint32_t n_faces, uint32_t n_verts, uint8_t* dst)
 {
-    const B2BvhHost& b = ((EmulScene*)p)->bvh;
+    const B2BvhHost& b = *(const B2BvhHost*)p;
     B2BlobHeader hd; memset(&hd, 0, sizeof(hd));
     memcpy(hd.magic, "B2BVH8F", 8);
     hd.version = 2; hd.node_bytes = sizeof(B2Node8); hd.tri_bytes = sizeof(B2Tri); hd.n_nodes = b.n_nodes; hd.n_tris = b.n_tris; hd.n_faces = n_faces;
@@ -39,16 +60,11 @@ __attribute__((visibility("default"))) void emul_export(void* p, uint32_t n_face
     memcpy(dst + sizeof(hd), b.nodes, sizeof(B2Node8) * (size_t)b.n_nodes);
     memcpy(dst + sizeof(hd) + sizeof(B2Node8) * (size_t)b.n_nodes, b.tris, sizeof(B2Tri) * (size_t)b.n_tris);
 }
-static BvhView view(void* p)
-{
-    EmulScene* s = (EmulScene*)p; BvhView v; v.nodes = (const float4*)s->bvh.nodes; v.tris = (const float4*)s->bvh.tris;
-    v.bx = s->bvh.abs_max[0]; v.by = s->bvh.abs_max[1]; v.bz = s->bvh.abs_max[2]; return v;
-}
 
 __attribute__((visibility("default"))) void emul_intersect(void* sc, const float* origs, const float* dirs, uint32_t n, float tfar,
                                                            float* t_out, uint32_t* face_out, float* ng_out, uint8_t* hit_out, double* mean_nodes, double* mean_tris, uint32_t* per_ray_nodes, uint32_t* per_ray_tris)
 {
-    const BvhView bvh = view(sc);
+    const BvhView bvh = view_of(sc);
     unsigned long long tn = 0, tt = 0;
     #pragma omp parallel for schedule(dynamic, 256) reduction(+ : tn, tt)
     for (int64_t i = 0; i < (int64_t)n; i++) {
@@ -79,7 +95,7 @@ __attribute__((visibility("default"))) void emul_find(void* sc, const b2_transfo
 __attribute__((visibility("default"))) void emul_find_opt(void* sc, const b2_transform* Tbm, const b2_transform* Tsb, uint32_t n, const float* origs, uint32_t n_origs,
                                                           const float* dirs, float range_min, float range_max, uint32_t sim_opts, float* pts, float* nrm, uint8_t* hits, uint32_t* faces, float* ranges)
 {
-    const BvhView bvh = view(sc);
+    const BvhView bvh = view_of(sc);
     RayModel m; m.dirs = dirs; m.origs = origs; m.n_origs = n_origs; m.n = n; m.range_min = range_min; m.range_max = range_max; m.sim_opts = sim_opts;
     ModelBuffers out; out.pts = pts; out.nrm = nrm; out.hits = hits; out.faces = faces; out.ranges = ranges;
     const Tf Tsm = tf_mul(tf_from_pod(*Tbm), tf_from_pod(*Tsb));
@@ -90,7 +106,7 @@ __attribute__((visibility("default"))) void emul_find_opt(void* sc, const b2_tra
 __attribute__((visibility("default"))) void emul_cpc_find(void* sc, const b2_transform* Tbm, const b2_transform* Tsb, uint32_t n, const float* dpts, float max_dist,
                                                           float* pts, float* nrm, uint8_t* hits, uint32_t* faces, float* dists, double* mean_nodes, double* mean_tris, uint32_t* per_nodes, uint32_t* per_tris)
 {
-    const BvhView bvh = view(sc);
+    const BvhView bvh = view_of(sc);
     ModelBuffers out; out.pts = pts; out.nrm = nrm; out.hits = hits; out.faces = faces; out.ranges = dists;
     const Tf Tsm = tf_mul(tf_from_pod(*Tbm), tf_from_pod(*Tsb));
     const Tf Tms = tf_inv(Tsm);
@@ -142,7 +158,7 @@ __attribute__((visibility("default"))) void emul_segment(uint32_t n, const float
 
 __attribute__((visibility("default"))) void emul_pf_motion(void* sc, uint32_t n, b2_transform* poses, b2_particle_attr* attrs, const b2_transform* T, double forget_rate, int collide)
 {
-    const BvhView bvh = view(sc);
+    const BvhView bvh = view_of(sc);
     for (uint32_t i = 0; i < n; i++) pf_motion_one(collide ? &bvh : nullptr, poses + i, attrs + i, tf_from_pod(*T), forget_rate);
 }
 
@@ -150,10 +166,10 @@ __attribute__((visibility("default"))) void emul_pf_motion(void* sc, uint32_t n,
 // larger indices in both builders' layouts; returns -1 if that does not hold)
 __attribute__((visibility("default"))) int emul_refit(void* p, const float* verts, uint32_t nv, const uint32_t* faces)
 {
-    EmulScene* s = (EmulScene*)p;
-    for (uint32_t t = 0; t < s->bvh.n_nodes; t++) if (s->bvh.nodes[t].imask() && s->bvh.nodes[t].child_base <= t) return -1;
-    for (uint32_t t = s->bvh.n_nodes; t-- > 0;) bvh8_refit_node(t, s->bvh.nodes, s->bvh.tris, verts, faces);
-    for (int k = 0; k < 3; k++) { float m = 0.f; for (uint32_t i = 0; i < nv; i++) m = fmaxf(m, fabsf(verts[3 * (size_t)i + k])); s->bvh.abs_max[k] = m; }
+    B2BvhHost& b = *(B2BvhHost*)p;
+    for (uint32_t t = 0; t < b.n_nodes; t++) if (b.nodes[t].imask() && b.nodes[t].child_base <= t) return -1;
+    for (uint32_t t = b.n_nodes; t-- > 0;) bvh8_refit_node(t, b.nodes, b.tris, verts, faces);
+    for (int k = 0; k < 3; k++) { float m = 0.f; for (uint32_t i = 0; i < nv; i++) m = fmaxf(m, fabsf(verts[3 * (size_t)i + k])); b.abs_max[k] = m; }
     return 0;
 }
 
@@ -252,7 +268,7 @@ __attribute__((visibility("default"))) void emul_correct_once(void* sc, uint32_t
 __attribute__((visibility("default"))) void emul_pf_update(void* sc, uint32_t n_particles, const b2_transform* poses, b2_particle_attr* attrs, const b2_transform* Tsb,
                                                            uint32_t n_beams, const b2_range_meas* beams, const b2_pf_params* prm)
 {
-    const BvhView bvh = view(sc);
+    const BvhView bvh = view_of(sc);
     float sigma_quad; double denom; pf_constants(*prm, sigma_quad, denom);
     std::vector<PfBeam> pb(n_beams);
     for (uint32_t j = 0; j < n_beams; j++) {
@@ -271,3 +287,18 @@ __attribute__((visibility("default"))) void emul_pf_update(void* sc, uint32_t n_
 }
 
 }  // extern "C"
+
+// the features' functions
+#include "../chain_ref/progress_emul.cu"
+#include "../dfield_ref/dfield_emul.cu"
+#include "../micp_cov_ref/cov_emul.cu"
+#include "../pc2_ref/pc2_emul.cu"
+#include "../pc2_scan_ref/scan_emul.cu"
+#include "../pf_cloud_ref/cloud_emul.cu"
+#include "../pf_cluster_ref/cluster_emul.cu"
+#include "../pf_estimate_ref/estimate_emul.cu"
+#include "../pf_kld_ref/kld_emul.cu"
+#include "../pf_recovery_ref/recovery_emul.cu"
+#include "../pf_residual_ref/residual_emul.cu"
+#include "../pf_stein_ref/stein_emul.cu"
+#include "../pf_surface_ref/surface_emul.cu"

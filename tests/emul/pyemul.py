@@ -1,17 +1,13 @@
-"""ctypes binding of tests/emul/libb2emul.so -- TEST HARNESS ONLY (CPU run of the product's host+device traversal code)."""
+"""ctypes binding of the emulator library (tests/emul/emul.cu, built by tests/native.py) -- TEST HARNESS ONLY (CPU run of the product's
+host+device traversal code)."""
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = os.path.join(_HERE, "_build", "libb2emul.so")
-
-TRANSFORM = np.dtype([("R", np.float32, 4), ("t", np.float32, 3), ("stamp", np.uint32)])
-CROSS_STATS = np.dtype([("dataset_mean", np.float32, 3), ("model_mean", np.float32, 3), ("covariance", np.float32, 9), ("n_meas", np.uint32)])
+import native
+from rmcl_b200.synth import CROSS_STATS_DTYPE as CROSS_STATS, TRANSFORM_DTYPE as TRANSFORM
 
 
 class _EmulTf(C.Structure):
@@ -30,20 +26,13 @@ class PFParams(C.Structure):
                 ("correspondence_type", C.c_int)]
 
 
-def build(force=False):
-    subprocess.check_call(["make", "-C", _HERE, "-s"] + (["-B"] if force else []))
-    return _LIB
-
-
 _lib = None
 
 
 def lib():
     global _lib
     if _lib is None:
-        if not os.path.exists(_LIB):
-            build()
-        _lib = C.CDLL(_LIB)
+        _lib = native.emulator()
         _lib.emul_scene_create.restype = C.c_void_p
     return _lib
 
@@ -57,6 +46,8 @@ def _f32(a):
 
 
 class Scene:
+    """the product's host-built BVH of a mesh"""
+
     def __init__(self, verts, faces):
         self.verts = _f32(verts).reshape(-1, 3)
         self.faces = np.ascontiguousarray(faces, np.uint32).reshape(-1, 3)

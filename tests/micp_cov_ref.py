@@ -4,19 +4,14 @@
 * frames / information_np: the Jacobian rows J = (n, q x n) of the accepted pairs in the reference body frame and their sums, in float64 from
   the float buffers.
 * product_finalize / product_pretransform / product_gate: the product's own micp_cov_finalize, pre-transform and P2L gate
-  (rmcl_b200/csrc/kernels.cuh) compiled for the CPU (micp_cov_ref/cov_emul.cu), built on first use into the per-user temporary directory of
-  chain_ref."""
+  (rmcl_b200/csrc/kernels.cuh) compiled for the CPU (micp_cov_ref/cov_emul.cu), built on first use by native.py."""
 import ctypes as C
-import os
 
 import numpy as np
 
-from chain_ref import _build
+import native
+from rmcl_b200.synth import TRANSFORM_DTYPE as TRANSFORM
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ROOT = os.path.dirname(_HERE)
-_CSRC = os.path.join(_ROOT, "rmcl_b200", "csrc")
-TRANSFORM = np.dtype([("R", np.float32, 4), ("t", np.float32, 3), ("stamp", np.uint32)])
 # b2_micp_covariance (include/rmcl_b200.h)
 COVARIANCE = np.dtype([("information", np.float64, 36), ("covariance", np.float64, 36), ("eigenvalues", np.float64, 6),
                        ("eigenvectors", np.float64, 36), ("sigma2", np.float64), ("residual_sq_sum", np.float64), ("weight_sum", np.float64),
@@ -30,12 +25,7 @@ _emul = None
 def _emul_lib():
     global _emul
     if _emul is None:
-        src = os.path.join(_HERE, "micp_cov_ref", "cov_emul.cu")
-        deps = [src] + [os.path.join(_CSRC, f) for f in ("kernels.cuh", "icp_loop.cuh", "trace.cuh", "b2_math.cuh", "bvh8.h")] + \
-               [os.path.join(_ROOT, "include", "rmcl_b200.h")]
-        nvcc = os.environ.get("NVCC", "nvcc")
-        _emul = _build("micp_cov_emul", deps, [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17", "-fmad=false",
-                                               "-Xcompiler", "-fPIC,-ffp-contract=off,-mavx2,-mfma,-fvisibility=hidden", "-shared", src])
+        _emul = native.emulator()
         for f in ("emul_micp_cov_finalize", "emul_micp_cov_pretransform", "emul_micp_cov_gate"):
             getattr(_emul, f).restype = None
     return _emul

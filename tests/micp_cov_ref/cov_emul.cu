@@ -1,9 +1,6 @@
 // cov_emul.cu -- TEST HARNESS ONLY: the product's pieces of b2_micp_pose_covariance (rmcl_b200/csrc/kernels.cuh: micp_cov_finalize, the
 // pre-transform and the P2L gate the kernel applies) compiled for the CPU, so that they can be compared with numpy in a container without a GPU.
-// Built by tests/micp_cov_ref.py with the flags of tests/chain_ref (host code with -ffp-contract=off: plain float ops rounded like __fmul_rn).
-#include "../../rmcl_b200/csrc/kernels.cuh"
-
-#define EMUL_API extern "C" __attribute__((visibility("default")))
+// Included into the emulator library (tests/emul/emul.cu).
 
 EMUL_API void emul_micp_cov_finalize(const double* sums, const double* weights, uint32_t n_sensors, double tau, double degenerate_variance,
                                      b2_micp_covariance* out)

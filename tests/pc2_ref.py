@@ -5,16 +5,13 @@
   dataset of MICPO1DnSensorCUDA::unpackMessage (MICPO1DnSensorCUDA.cpp:171-230).  reference_mask=True also applies the reference's use of a
   field named `mask` as the range (conversions.cpp:1014-1017), which the product deliberately does not (SURVEY Appendix D).
 * product_np: the product's own per-ray function (rmcl_b200/csrc/kernels.cuh) compiled for the CPU (pc2_ref/pc2_emul.cu), built on first
-  use into the per-user temporary directory of chain_ref."""
+  use by native.py."""
 import ctypes as C
-import os
 
 import numpy as np
 
-from chain_ref import _build
+import native
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_CSRC = os.path.join(os.path.dirname(_HERE), "rmcl_b200", "csrc")
 _emul = None
 
 
@@ -63,12 +60,7 @@ def convert_np(cloud, flt, reference_mask=False):
 def _emul_lib():
     global _emul
     if _emul is None:
-        src = os.path.join(_HERE, "pc2_ref", "pc2_emul.cu")
-        deps = [src] + [os.path.join(_CSRC, f) for f in ("kernels.cuh", "icp_loop.cuh", "trace.cuh", "b2_math.cuh", "bvh8.h")] + \
-               [os.path.join(os.path.dirname(_HERE), "include", "rmcl_b200.h")]
-        nvcc = os.environ.get("NVCC", "nvcc")
-        _emul = _build("pc2_emul", deps, [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17", "-fmad=false",
-                                          "-Xcompiler", "-fPIC,-ffp-contract=off,-mavx2,-mfma,-fvisibility=hidden", "-shared", src])
+        _emul = native.emulator()
         _emul.emul_o1dn_from_cloud.restype = None
     return _emul
 

@@ -1,7 +1,6 @@
 // pc2_emul.cu -- TEST HARNESS ONLY: the product's per-ray function of b2_rcc_set_cloud_o1dn (rmcl_b200/csrc/kernels.cuh: o1dn_cloud_entry, with
 // cloud_coord, o1dn_from_point and dataset_entry inlined) compiled for the CPU, one call per output ray as the kernel's threads make them.
-// Built by tests/pc2_ref.py with the flags of tests/chain_ref (host code with -ffp-contract=off: plain float ops rounded like __fmul_rn etc.).
-#include "../../rmcl_b200/csrc/kernels.cuh"
+// Included into the emulator library (tests/emul/emul.cu).
 
 extern "C" __attribute__((visibility("default"))) void emul_o1dn_from_cloud(const uint8_t* cloud, uint32_t w_out, uint32_t h_out, uint64_t row_step,
                                                                            uint32_t point_step, const uint32_t* off, uint32_t f64, const uint32_t* h_skip_inc,

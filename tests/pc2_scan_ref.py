@@ -4,19 +4,15 @@
   compiles the oracle's source in for the Transform product), with the elevation rule and the atan2 precision as test-only arguments.
 * product: the product's own per-point and per-cell functions (rmcl_b200/csrc/kernels.cuh) compiled for the CPU (pc2_scan_ref/scan_emul.cu),
   the points visited in any order.
-Both libraries are built on first use into the per-user temporary directory of chain_ref."""
+Both libraries are built on first use by native.py."""
 import ctypes as C
-import os
 
 import numpy as np
 
-from chain_ref import _build
+import native
 from rmcl_b200.api import _SphericalModel
 from rmcl_b200.synth import TRANSFORM_DTYPE, make_transform
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ROOT = os.path.dirname(_HERE)
-_CSRC = os.path.join(_ROOT, "rmcl_b200", "csrc")
 _ref = None
 _emul = None
 
@@ -27,10 +23,7 @@ ATAN2F = 2          # float atan2f instead of FP64 atan2 rounded to float
 def _ref_lib():
     global _ref
     if _ref is None:
-        src = os.path.join(_HERE, "pc2_scan_ref", "pc2_scan_ref.c")
-        cc = "/usr/bin/gcc" if os.access("/usr/bin/gcc", os.X_OK) else "gcc"
-        deps = [src, os.path.join(_ROOT, "oracle", "oracle.c"), os.path.join(_ROOT, "oracle", "oracle.h")]
-        _ref = _build("pc2_scan_ref", deps, [cc, "-O2", "-fopenmp", "-ffp-contract=off", "-mavx2", "-mfma", "-fPIC", "-std=gnu11", "-shared", src, "-lm"])
+        _ref = native.restatement("pc2_scan_ref/pc2_scan_ref.c")
         _ref.ref_pc2_to_scan.restype = None
         _ref.ref_spherical_dirs.restype = None
     return _ref
@@ -39,12 +32,7 @@ def _ref_lib():
 def _emul_lib():
     global _emul
     if _emul is None:
-        src = os.path.join(_HERE, "pc2_scan_ref", "scan_emul.cu")
-        deps = [src] + [os.path.join(_CSRC, f) for f in ("kernels.cuh", "icp_loop.cuh", "trace.cuh", "b2_math.cuh", "bvh8.h")] + \
-               [os.path.join(_ROOT, "include", "rmcl_b200.h")]
-        nvcc = os.environ.get("NVCC", "nvcc")
-        _emul = _build("scan_emul", deps, [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17", "-fmad=false",
-                                           "-Xcompiler", "-fPIC,-ffp-contract=off,-mavx2,-mfma,-fvisibility=hidden", "-shared", src])
+        _emul = native.emulator()
         _emul.emul_scan_from_cloud.restype = None
     return _emul
 

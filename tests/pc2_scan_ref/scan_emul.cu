@@ -1,11 +1,7 @@
 // scan_emul.cu -- TEST HARNESS ONLY: the product's per-point and per-cell functions of b2_rcc_set_cloud_spherical (rmcl_b200/csrc/kernels.cuh:
 // scan_cloud_key and scan_cell_entry, with scan_point_key, scan_bin and dataset_entry inlined) compiled for the CPU.  Points are visited in
 // the caller's order and each cell keeps the larger key, as k_scan_bin_cloud's atomicMax does; then one scan_cell_entry per cell.
-// Built by tests/pc2_scan_ref.py with the flags of tests/chain_ref (host code with -ffp-contract=off: plain ops rounded like __fmul_rn etc.).
-#include <algorithm>
-#include <vector>
-
-#include "../../rmcl_b200/csrc/kernels.cuh"
+// Included into the emulator library (tests/emul/emul.cu).
 
 extern "C" __attribute__((visibility("default"))) void emul_scan_from_cloud(const uint8_t* cloud, uint32_t width, uint32_t height, uint64_t row_step,
                                                                            uint32_t point_step, const uint32_t* off, uint32_t f64, const b2_transform* T,

@@ -4,18 +4,14 @@
   which compiles the oracle's source in for Philox4x32-10).
 * product_samples: the product's per-sample function (rmcl_b200/csrc/kernels.cuh: pf_sample_beam) compiled for the CPU
   (pf_cloud_ref/cloud_emul.cu), every sample's flag and beam; product = those under the give-up rule.
-Both libraries are built on first use into the per-user temporary directory of chain_ref."""
+Both libraries are built on first use by native.py."""
 import ctypes as C
-import os
 
 import numpy as np
 
-from chain_ref import _build
+import native
 from rmcl_b200.synth import RANGE_MEAS_DTYPE
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ROOT = os.path.dirname(_HERE)
-_CSRC = os.path.join(_ROOT, "rmcl_b200", "csrc")
 _ref = None
 _emul = None
 MAX_INVALIDS = 10
@@ -24,10 +20,7 @@ MAX_INVALIDS = 10
 def _ref_lib():
     global _ref
     if _ref is None:
-        src = os.path.join(_HERE, "pf_cloud_ref", "pf_cloud_ref.c")
-        cc = "/usr/bin/gcc" if os.access("/usr/bin/gcc", os.X_OK) else "gcc"
-        deps = [src, os.path.join(_ROOT, "oracle", "oracle.c"), os.path.join(_ROOT, "oracle", "oracle.h")]
-        _ref = _build("pf_cloud_ref", deps, [cc, "-O2", "-fopenmp", "-ffp-contract=off", "-mavx2", "-mfma", "-fPIC", "-std=gnu11", "-shared", src, "-lm"])
+        _ref = native.restatement("pf_cloud_ref/pf_cloud_ref.c")
         _ref.ref_pf_sample_cloud.restype = C.c_uint32
         _ref.ref_pf_sample_one.restype = C.c_int
     return _ref
@@ -36,12 +29,7 @@ def _ref_lib():
 def _emul_lib():
     global _emul
     if _emul is None:
-        src = os.path.join(_HERE, "pf_cloud_ref", "cloud_emul.cu")
-        deps = [src] + [os.path.join(_CSRC, f) for f in ("kernels.cuh", "icp_loop.cuh", "trace.cuh", "b2_math.cuh", "bvh8.h")] + \
-               [os.path.join(_ROOT, "include", "rmcl_b200.h")]
-        nvcc = os.environ.get("NVCC", "nvcc")
-        _emul = _build("pf_cloud_emul", deps, [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17", "-fmad=false",
-                                               "-Xcompiler", "-fPIC,-ffp-contract=off,-mavx2,-mfma,-fvisibility=hidden", "-shared", src])
+        _emul = native.emulator()
         _emul.emul_pf_samples.restype = None
     return _emul
 

@@ -1,8 +1,6 @@
 // cloud_emul.cu -- TEST HARNESS ONLY: the product's per-sample function of b2_pf_sample_cloud (rmcl_b200/csrc/kernels.cuh: pf_sample_beam,
 // with philox4x32_10 and cloud_coord inlined) compiled for the CPU, run for samples 0 .. n_samples-1 as k_pf_sample_cloud runs them: each
-// writes its valid flag and its beam (all zero when invalid).  Built by tests/pf_cloud_ref.py with the flags of tests/chain_ref (host code
-// with -ffp-contract=off: plain ops rounded like __fmul_rn etc.).
-#include "../../rmcl_b200/csrc/kernels.cuh"
+// writes its valid flag and its beam (all zero when invalid).  Included into the emulator library (tests/emul/emul.cu).
 
 extern "C" __attribute__((visibility("default"))) void emul_pf_samples(const uint8_t* cloud, uint32_t width, uint32_t height, uint64_t row_step,
                                                                       uint32_t point_step, const uint32_t* off, uint32_t f64, uint64_t seed, uint32_t step,

@@ -4,18 +4,14 @@
   fed the bin keys and integer weights of the KLD restatement (pf_kld_ref).
 * product_neighbours / product_offsets: the product's kld_key_neighbour / kld_key_offset (rmcl_b200/csrc/kernels.cuh) compiled for the CPU
   (pf_cluster_ref/cluster_emul.cu).
-Both libraries are built on first use into the per-user temporary directory of chain_ref."""
+Both libraries are built on first use by native.py."""
 import ctypes as C
-import os
 
 import numpy as np
 
+import native
 import pf_kld_ref
-from chain_ref import _build
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ROOT = os.path.dirname(_HERE)
-_CSRC = os.path.join(_ROOT, "rmcl_b200", "csrc")
 NONE_KEY = np.uint64(0xFFFFFFFFFFFFFFFF)
 NONE = np.uint32(0xFFFFFFFF)
 _ref = None
@@ -25,9 +21,7 @@ _emul = None
 def _ref_lib():
     global _ref
     if _ref is None:
-        src = os.path.join(_HERE, "pf_cluster_ref", "pf_cluster_ref.c")
-        cc = "/usr/bin/gcc" if os.access("/usr/bin/gcc", os.X_OK) else "gcc"
-        _ref = _build("pf_cluster_ref", [src], [cc, "-O2", "-fPIC", "-std=gnu11", "-shared", src])
+        _ref = native.restatement("pf_cluster_ref/pf_cluster_ref.c")
         _ref.orc_cluster_neighbours.restype = None
         _ref.orc_pf_cluster.restype = None
     return _ref
@@ -36,12 +30,7 @@ def _ref_lib():
 def _emul_lib():
     global _emul
     if _emul is None:
-        src = os.path.join(_HERE, "pf_cluster_ref", "cluster_emul.cu")
-        deps = [src] + [os.path.join(_CSRC, f) for f in ("kernels.cuh", "icp_loop.cuh", "trace.cuh", "b2_math.cuh", "bvh8.h")] + \
-               [os.path.join(_ROOT, "include", "rmcl_b200.h")]
-        nvcc = os.environ.get("NVCC", "nvcc")
-        _emul = _build("pf_cluster_emul", deps, [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17", "-fmad=false",
-                                                 "-Xcompiler", "-fPIC,-ffp-contract=off,-mavx2,-mfma,-fvisibility=hidden", "-shared", src])
+        _emul = native.emulator()
         _emul.emul_cluster_neighbours.restype = None
         _emul.emul_cluster_offsets.restype = None
     return _emul

@@ -1,9 +1,6 @@
 // cluster_emul.cu -- TEST HARNESS ONLY: the product's bin-neighbour functions of b2_pf_cluster_stats (rmcl_b200/csrc/kernels.cuh:
 // kld_key_neighbour, kld_key_offset) compiled for the CPU, so that they can be compared with the C restatement in a container without a GPU.
-// Built by tests/pf_cluster_ref.py with the flags of tests/pf_kld_ref.
-#include "../../rmcl_b200/csrc/kernels.cuh"
-
-#define EMUL_API extern "C" __attribute__((visibility("default")))
+// Included into the emulator library (tests/emul/emul.cu).
 
 EMUL_API void emul_cluster_neighbours(const uint64_t* keys, uint64_t count, int dx, int dy, int dz, int ds, uint32_t K, int has_z, uint64_t* out)
 {

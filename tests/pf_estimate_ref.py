@@ -5,17 +5,14 @@ rmcl_ros/src/nodes/rmcl_localization.cpp:642-731).
   AABB, the weighted Markley mean (numpy.linalg.eigh of sum w q q^T) rounded to a float Transform, and the covariance of (~Tbm * pose) about
   that Tbm.  Pass 2 can be fed another Tbm (the device's), so that a comparison isolates the float deviation arithmetic.
 * product_eigvec / product_deviation: the product's own B2_DEV functions (rmcl_b200/csrc/kernels.cuh) compiled for the CPU
-  (pf_estimate_ref/estimate_emul.cu), built on first use into the per-user temporary directory of chain_ref."""
+  (pf_estimate_ref/estimate_emul.cu), built on first use by native.py."""
 import ctypes as C
-import os
 
 import numpy as np
 
-from chain_ref import _build
+import native
 from rmcl_b200.synth import PARTICLE_STATS_DTYPE, TRANSFORM_DTYPE
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_CSRC = os.path.join(os.path.dirname(_HERE), "rmcl_b200", "csrc")
 DBL_MAX = float(np.finfo(np.float64).max)
 FLT_MAX = float(np.finfo(np.float32).max)
 _emul = None
@@ -24,12 +21,7 @@ _emul = None
 def _emul_lib():
     global _emul
     if _emul is None:
-        src = os.path.join(_HERE, "pf_estimate_ref", "estimate_emul.cu")
-        deps = [src] + [os.path.join(_CSRC, f) for f in ("kernels.cuh", "icp_loop.cuh", "trace.cuh", "b2_math.cuh", "bvh8.h")] + \
-               [os.path.join(os.path.dirname(_HERE), "include", "rmcl_b200.h")]
-        nvcc = os.environ.get("NVCC", "nvcc")
-        _emul = _build("estimate_emul", deps, [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17", "-fmad=false",
-                                               "-Xcompiler", "-fPIC,-ffp-contract=off,-mavx2,-mfma,-fvisibility=hidden", "-shared", src])
+        _emul = native.emulator()
         _emul.emul_sym4_top_eigvec.restype = None
         _emul.emul_pf_deviation.restype = None
     return _emul

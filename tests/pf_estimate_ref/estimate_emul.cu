@@ -1,8 +1,6 @@
 // estimate_emul.cu -- TEST HARNESS ONLY: the product's building blocks of the pose estimate (rmcl_b200/csrc/kernels.cuh: sym4_top_eigvec, the
 // Markley mean's 4x4 eigen solver, and pf_deviation, the 6-vector of a particle about the mean) compiled for the CPU, so that they can be
-// compared with numpy in a container without a GPU.  Built by tests/pf_estimate_ref.py with the flags of tests/chain_ref (host code with
-// -ffp-contract=off: plain float ops rounded like __fmul_rn / __fadd_rn).
-#include "../../rmcl_b200/csrc/kernels.cuh"
+// compared with numpy in a container without a GPU.  Included into the emulator library (tests/emul/emul.cu).
 
 extern "C" {
 __attribute__((visibility("default"))) void emul_sym4_top_eigvec(const double* A16, double* v4, double* lambda) { sym4_top_eigvec(A16, v4, lambda); }

@@ -1,26 +1,20 @@
 """TEST INFRASTRUCTURE ONLY: reference for the particle set initialisers (b2_pf_init_uniform / b2_pf_init_gaussian), a thin ctypes layer
 over pf_init_ref/pf_init_ref.c.  That file compiles the oracle's source (oracle/oracle.c) in, so Philox4x32-10, euler_to_quat and the
-Transform product are the oracle's own.  The library is compiled on first use into the per-user temporary directory of chain_ref."""
+Transform product are the oracle's own.  The library is compiled on first use by native.py."""
 import ctypes as C
-import os
 
 import numpy as np
 
-from chain_ref import _build
+import native
 from rmcl_b200.synth import PARTICLE_ATTR_DTYPE, TRANSFORM_DTYPE
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ORACLE = os.path.join(os.path.dirname(_HERE), "oracle")
 _lib = None
 
 
 def lib():
     global _lib
     if _lib is None:
-        src = os.path.join(_HERE, "pf_init_ref", "pf_init_ref.c")
-        cc = "/usr/bin/gcc" if os.access("/usr/bin/gcc", os.X_OK) else "gcc"
-        deps = [src, os.path.join(_ORACLE, "oracle.c"), os.path.join(_ORACLE, "oracle.h")]
-        _lib = _build("pf_init_ref", deps, [cc, "-O2", "-fopenmp", "-ffp-contract=off", "-mavx2", "-mfma", "-fPIC", "-std=gnu11", "-shared", src, "-lm"])
+        _lib = native.restatement("pf_init_ref/pf_init_ref.c")
         _lib.orc_pf_chol6.restype = C.c_int
     return _lib
 

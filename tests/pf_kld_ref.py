@@ -4,19 +4,15 @@
   and through it the oracle's source in for Philox4x32-10, the normals and the copy).
 * product_*: the product's per-element functions (rmcl_b200/csrc/kernels.cuh: kld_weight, kld_parent, kld_key, kld_bound, kld_stop)
   compiled for the CPU (pf_kld_ref/kld_emul.cu).
-Both libraries are built on first use into the per-user temporary directory of chain_ref."""
+Both libraries are built on first use by native.py."""
 import ctypes as C
-import os
 
 import numpy as np
 
-from chain_ref import _build
+import native
 from rmcl_b200.api import GladiatorConfig, KLDConfig
 from rmcl_b200.synth import PARTICLE_ATTR_DTYPE, TRANSFORM_DTYPE
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ROOT = os.path.dirname(_HERE)
-_CSRC = os.path.join(_ROOT, "rmcl_b200", "csrc")
 _ref = None
 _emul = None
 
@@ -24,11 +20,7 @@ _emul = None
 def _ref_lib():
     global _ref
     if _ref is None:
-        src = os.path.join(_HERE, "pf_kld_ref", "pf_kld_ref.c")
-        cc = "/usr/bin/gcc" if os.access("/usr/bin/gcc", os.X_OK) else "gcc"
-        deps = [src, os.path.join(_HERE, "pf_residual_ref", "pf_residual_ref.c"), os.path.join(_ROOT, "oracle", "oracle.c"),
-                os.path.join(_ROOT, "oracle", "oracle.h")]
-        _ref = _build("pf_kld_ref", deps, [cc, "-O2", "-fopenmp", "-ffp-contract=off", "-mavx2", "-mfma", "-fPIC", "-std=gnu11", "-shared", src, "-lm"])
+        _ref = native.restatement("pf_kld_ref/pf_kld_ref.c")
         for f in ("orc_kld_table", "orc_kld_keys", "orc_kld_bounds", "orc_kld_prefix", "orc_kld_parents", "orc_pf_resample_kld"):
             getattr(_ref, f).restype = None
         _ref.orc_kld_sectors.restype = C.c_uint32
@@ -39,12 +31,7 @@ def _ref_lib():
 def _emul_lib():
     global _emul
     if _emul is None:
-        src = os.path.join(_HERE, "pf_kld_ref", "kld_emul.cu")
-        deps = [src] + [os.path.join(_CSRC, f) for f in ("kernels.cuh", "icp_loop.cuh", "trace.cuh", "b2_math.cuh", "bvh8.h")] + \
-               [os.path.join(_ROOT, "include", "rmcl_b200.h")]
-        nvcc = os.environ.get("NVCC", "nvcc")
-        _emul = _build("pf_kld_emul", deps, [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17", "-fmad=false",
-                                             "-Xcompiler", "-fPIC,-ffp-contract=off,-mavx2,-mfma,-fvisibility=hidden", "-shared", src])
+        _emul = native.emulator()
         for f in ("emul_kld_prefix", "emul_kld_parents", "emul_kld_keys", "emul_kld_bounds", "emul_kld_stop"):
             getattr(_emul, f).restype = None
     return _emul

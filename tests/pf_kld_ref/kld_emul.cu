@@ -1,10 +1,6 @@
 // kld_emul.cu -- TEST HARNESS ONLY: the product's per-element functions of KLD-sampling (rmcl_b200/csrc/kernels.cuh: kld_weight,
 // kld_parent, kld_key, kld_bound, kld_stop) compiled for the CPU, so that they can be compared with the C restatement in a container without
-// a GPU.  Built by tests/pf_kld_ref.py with the flags of tests/chain_ref (host code with -ffp-contract=off: plain float and double ops rounded
-// like __fmul_rn / __dmul_rn and friends).
-#include "../../rmcl_b200/csrc/kernels.cuh"
-
-#define EMUL_API extern "C" __attribute__((visibility("default")))
+// a GPU.  Included into the emulator library (tests/emul/emul.cu).
 
 // the inclusive prefix of the integer weights of L[0 .. n-1]
 EMUL_API void emul_kld_prefix(const float* L, uint32_t n, double L_max, unsigned long long* W)

@@ -5,19 +5,16 @@
 * ProductRecovery.inject / product_filter: the product's pf_recovery_one and pf_recovery_filter (rmcl_b200/csrc/kernels.cuh) compiled for
   the CPU over the product's host-built BVH (pf_recovery_ref/recovery_emul.cu).
 * filter64: the record's recurrence transcribed in float64 Python.
-Both libraries are built on first use into the per-user temporary directory of chain_ref."""
+Both libraries are built on first use by native.py."""
 import ctypes as C
 import math
-import os
 
 import numpy as np
 
-from chain_ref import _build
+import native
+import pyemul
 from rmcl_b200.synth import RECOVERY_STATE_DTYPE
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ROOT = os.path.dirname(_HERE)
-_CSRC = os.path.join(_ROOT, "rmcl_b200", "csrc")
 _ref = None
 _emul = None
 
@@ -25,10 +22,7 @@ _emul = None
 def _ref_lib():
     global _ref
     if _ref is None:
-        src = os.path.join(_HERE, "pf_recovery_ref", "pf_recovery_ref.c")
-        cc = "/usr/bin/gcc" if os.access("/usr/bin/gcc", os.X_OK) else "gcc"
-        deps = [src, os.path.join(_HERE, "pf_surface_ref", "pf_surface_ref.c"), os.path.join(_ROOT, "oracle", "oracle.c"), os.path.join(_ROOT, "oracle", "oracle.h")]
-        _ref = _build("pf_recovery_ref", deps, [cc, "-O2", "-fopenmp", "-ffp-contract=off", "-mavx2", "-mfma", "-fPIC", "-std=gnu11", "-shared", src, "-lm"])
+        _ref = native.restatement("pf_recovery_ref/pf_recovery_ref.c")
         _ref.orc_scene_create.restype = C.c_void_p
         _ref.orc_scene_destroy.argtypes = [C.c_void_p]
         _ref.orc_pf_recovery.restype = None
@@ -38,15 +32,7 @@ def _ref_lib():
 def _emul_lib():
     global _emul
     if _emul is None:
-        src = os.path.join(_HERE, "pf_recovery_ref", "recovery_emul.cu")
-        deps = [src] + [os.path.join(_CSRC, f) for f in ("kernels.cuh", "icp_loop.cuh", "trace.cuh", "b2_math.cuh", "bvh8.h", "bvh_build.cpp")] + \
-               [os.path.join(_ROOT, "include", "rmcl_b200.h")]
-        nvcc = os.environ.get("NVCC", "nvcc")
-        _emul = _build("pf_recovery_emul", deps, [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17", "-fmad=false",
-                                                  "-Xcompiler", "-fPIC,-fopenmp,-ffp-contract=off,-mavx2,-mfma,-fvisibility=hidden", "-shared", src,
-                                                  os.path.join(_CSRC, "bvh_build.cpp"), "-lgomp"])
-        _emul.emul_recovery_scene.restype = C.c_void_p
-        _emul.emul_recovery_scene_free.argtypes = [C.c_void_p]
+        _emul = native.emulator()
         _emul.emul_pf_recovery.restype = None
         _emul.emul_recovery_filter.restype = None
     return _emul
@@ -91,20 +77,11 @@ class RefRecovery(_Scene):
                                    C.c_uint32(n), C.c_double(p), _p(lo), _p(hi), C.c_uint32(max_tries), C.c_uint64(seed), C.c_uint32(step), _p(P), _p(A), _p(counts))
 
 
-class ProductRecovery(_Scene):
+class ProductRecovery(_Scene, pyemul.Scene):
     """the product's pf_recovery_one on the CPU"""
 
-    def __init__(self, V, F):
-        self.V, self.F = _mesh(V, F)
-        self._s = _emul_lib().emul_recovery_scene(_p(self.V), C.c_uint32(len(self.V)), _p(self.F), C.c_uint32(len(self.F)))
-        assert self._s
-
-    def __del__(self):
-        if getattr(self, "_s", None):
-            _emul_lib().emul_recovery_scene_free(self._s)
-
     def _run(self, surface, first, n, p, lo, hi, max_tries, seed, step, P, A, counts):
-        _emul_lib().emul_pf_recovery(C.c_void_p(self._s), C.byref(surface) if surface is not None else None, C.c_uint32(first), C.c_uint32(n), C.c_double(p),
+        _emul_lib().emul_pf_recovery(self._h, C.byref(surface) if surface is not None else None, C.c_uint32(first), C.c_uint32(n), C.c_double(p),
                                      _p(lo), _p(hi), C.c_uint32(max_tries), C.c_uint64(seed), C.c_uint32(step), _p(P), _p(A), _p(counts))
 
 

@@ -5,19 +5,15 @@ rmcl_ros/src/rmcl/ResidualResamplerCPU.cpp:55-202).
   the oracle's source in for Philox4x32-10, the Euler conversions and the Transform product).
 * product_*: the product's per-element functions (rmcl_b200/csrc/kernels.cuh: residual_parent, residual_count, residual_normals,
   residual_copy) compiled for the CPU (pf_residual_ref/residual_emul.cu).
-Both libraries are built on first use into the per-user temporary directory of chain_ref."""
+Both libraries are built on first use by native.py."""
 import ctypes as C
-import os
 
 import numpy as np
 
-from chain_ref import _build
+import native
 from rmcl_b200.api import GladiatorConfig
 from rmcl_b200.synth import PARTICLE_ATTR_DTYPE, TRANSFORM_DTYPE
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ROOT = os.path.dirname(_HERE)
-_CSRC = os.path.join(_ROOT, "rmcl_b200", "csrc")
 _ref = None
 _emul = None
 
@@ -25,10 +21,7 @@ _emul = None
 def _ref_lib():
     global _ref
     if _ref is None:
-        src = os.path.join(_HERE, "pf_residual_ref", "pf_residual_ref.c")
-        cc = "/usr/bin/gcc" if os.access("/usr/bin/gcc", os.X_OK) else "gcc"
-        deps = [src, os.path.join(_ROOT, "oracle", "oracle.c"), os.path.join(_ROOT, "oracle", "oracle.h")]
-        _ref = _build("pf_residual_ref", deps, [cc, "-O2", "-fopenmp", "-ffp-contract=off", "-mavx2", "-mfma", "-fPIC", "-std=gnu11", "-shared", src, "-lm"])
+        _ref = native.restatement("pf_residual_ref/pf_residual_ref.c")
         for f in ("orc_residual_parents", "orc_residual_normals", "orc_residual_stats", "orc_pf_resample_residual"):
             getattr(_ref, f).restype = None
     return _ref
@@ -37,12 +30,7 @@ def _ref_lib():
 def _emul_lib():
     global _emul
     if _emul is None:
-        src = os.path.join(_HERE, "pf_residual_ref", "residual_emul.cu")
-        deps = [src] + [os.path.join(_CSRC, f) for f in ("kernels.cuh", "icp_loop.cuh", "trace.cuh", "b2_math.cuh", "bvh8.h")] + \
-               [os.path.join(_ROOT, "include", "rmcl_b200.h")]
-        nvcc = os.environ.get("NVCC", "nvcc")
-        _emul = _build("pf_residual_emul", deps, [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17", "-fmad=false",
-                                                  "-Xcompiler", "-fPIC,-ffp-contract=off,-mavx2,-mfma,-fvisibility=hidden", "-shared", src])
+        _emul = native.emulator()
         for f in ("emul_residual_parents", "emul_residual_counts", "emul_residual_normals", "emul_residual_copies"):
             getattr(_emul, f).restype = None
     return _emul

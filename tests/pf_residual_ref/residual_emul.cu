@@ -1,10 +1,6 @@
 // residual_emul.cu -- TEST HARNESS ONLY: the product's per-element functions of residual resampling (rmcl_b200/csrc/kernels.cuh:
 // residual_parent, residual_count, residual_normals, residual_copy) compiled for the CPU, so that they can be compared with the C
-// restatement in a container without a GPU.  Built by tests/pf_residual_ref.py with the flags of tests/chain_ref (host code with
-// -ffp-contract=off: plain float ops rounded like __fmul_rn / __fadd_rn).
-#include "../../rmcl_b200/csrc/kernels.cuh"
-
-#define EMUL_API extern "C" __attribute__((visibility("default")))
+// restatement in a container without a GPU.  Included into the emulator library (tests/emul/emul.cu).
 
 EMUL_API void emul_residual_parents(uint64_t seed, uint32_t step, uint64_t d0, uint64_t count, uint32_t n, uint32_t* out)
 {

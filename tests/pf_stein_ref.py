@@ -4,18 +4,15 @@
   forms, df_lookup_grad, the draws of J, the score, the bandwidth, the pair sums, the move and the whole call, in the device's order.
 * float64 numpy restatements of SURVEY appendix L: philox (Random123's Philox4x32-10), the draws of J, the chart, the score from a field
   given as (index, bricks), the bandwidth and the pair sums.
-The library is built on first use into the per-user temporary directory of chain_ref."""
+The library is built on first use by native.py."""
 import ctypes as C
-import os
 
 import numpy as np
 
+import native
+import pyemul
 import dfield_ref as DR
-from chain_ref import _build
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ROOT = os.path.dirname(_HERE)
-_CSRC = os.path.join(_ROOT, "rmcl_b200", "csrc")
 TAG = 8
 _emul = None
 
@@ -23,15 +20,7 @@ _emul = None
 def lib():
     global _emul
     if _emul is None:
-        src = os.path.join(_HERE, "pf_stein_ref", "stein_emul.cu")
-        deps = [src] + [os.path.join(_CSRC, f) for f in ("kernels.cuh", "icp_loop.cuh", "trace.cuh", "b2_math.cuh", "bvh8.h", "bvh_build.cpp")] + \
-               [os.path.join(_ROOT, "include", "rmcl_b200.h")]
-        nvcc = os.environ.get("NVCC", "nvcc")
-        _emul = _build("stein_emul", deps, [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17", "-fmad=false",
-                                            "-Xcompiler", "-fPIC,-fopenmp,-ffp-contract=off,-mavx2,-mfma,-fvisibility=hidden", "-shared", src,
-                                            os.path.join(_CSRC, "bvh_build.cpp"), "-lgomp"])
-        _emul.emul_stein_scene.restype = C.c_void_p
-        _emul.emul_stein_scene_free.argtypes = [C.c_void_p]
+        _emul = native.emulator()
     return _emul
 
 
@@ -120,23 +109,14 @@ def pairs(ci, snap, h):
     return acc
 
 
-class Scene:
+class Scene(pyemul.Scene):
     """the product's host-built BVH of a mesh (the walls of the move)"""
-
-    def __init__(self, V, F):
-        self.V, self.F = DR._mesh(V, F)
-        self._s = lib().emul_stein_scene(_p(self.V), C.c_uint32(len(self.V)), _p(self.F), C.c_uint32(len(self.F)))
-        assert self._s
-
-    def __del__(self):
-        if getattr(self, "_s", None):
-            lib().emul_stein_scene_free(self._s)
 
     def move(self, poses, snap, it, step_t, step_r, v, h, rec):
         """the product's k_pf_stein_move: poses and v (n, 3) float32 in place, rec (SteinResult) updated"""
         snap = np.ascontiguousarray(snap, np.float32)
         h = np.ascontiguousarray(h, np.float32)
-        lib().emul_stein_move(C.c_void_p(self._s), _p(poses), C.c_uint32(len(poses)), _p(snap), C.c_uint32(len(snap)), C.c_uint32(it), C.c_float(step_t),
+        lib().emul_stein_move(self._h, _p(poses), C.c_uint32(len(poses)), _p(snap), C.c_uint32(len(snap)), C.c_uint32(it), C.c_float(step_t),
                               C.c_float(step_r), _p(v), _p(h), C.byref(rec))
 
     def update(self, g, index, bricks, poses, Tsb, beams, dist_sigma, cfg, seed, step):
@@ -145,7 +125,7 @@ class Scene:
         B, T = np.ascontiguousarray(beams), np.ascontiguousarray(Tsb)
         bricks = np.ascontiguousarray(bricks, np.float32)
         rec = SteinResult()
-        lib().emul_stein_update(C.c_void_p(self._s), *g.args(), _p(np.ascontiguousarray(index)), _p(bricks) if bricks.size else None, _p(P),
+        lib().emul_stein_update(self._h, *g.args(), _p(np.ascontiguousarray(index)), _p(bricks) if bricks.size else None, _p(P),
                                 C.c_uint32(len(P)), _p(T), _p(B) if len(B) else None, C.c_uint32(len(B)), C.c_float(dist_sigma), C.byref(cfg),
                                 C.c_uint64(seed), C.c_uint32(step), C.byref(rec))
         return P, rec

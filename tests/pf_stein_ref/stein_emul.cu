@@ -2,39 +2,8 @@
 // stein_beam_term, stein_ref_entry, stein_bw_terms, stein_bandwidth, stein_pair, stein_move_one; b2_math.cuh: exp_f, atan2_d, sin_d, cos_d)
 // compiled for the CPU over the product's host-built BVH.  The three kernels of an iteration run as host loops; the two grid reductions
 // are restated in est_grid_reduce's order (one value per thread, blocks of 256: warp butterflies, the block's 8 warps in order, then in the
-// last block lane l adds the partials of blocks l, l + 32, ... and a butterfly), so the results are the device's bits.  Built by
-// tests/pf_stein_ref.py with the flags of tests/chain_ref (host code with -ffp-contract=off: plain ops rounded like __fmul_rn etc.).
-#include "../../rmcl_b200/csrc/kernels.cuh"
-
-#include <vector>
-
-#define EMUL_API extern "C" __attribute__((visibility("default")))
-
-static BvhView view_of(const void* p)
-{
-    const B2BvhHost* b = (const B2BvhHost*)p;
-    BvhView v; v.nodes = (const float4*)b->nodes; v.tris = (const float4*)b->tris;
-    v.bx = b->abs_max[0]; v.by = b->abs_max[1]; v.bz = b->abs_max[2];
-    return v;
-}
-EMUL_API void* emul_stein_scene(const float* verts, uint32_t nv, const uint32_t* faces, uint32_t nf)
-{
-    B2BvhHost* b = new B2BvhHost();
-    const char* err = "";
-    if (b2_build_bvh8_host(verts, nv, faces, nf, b, &err) != 0) { delete b; return nullptr; }
-    return b;
-}
-EMUL_API void emul_stein_scene_free(void* p)
-{
-    if (p) { b2_free_bvh8_host((B2BvhHost*)p); delete (B2BvhHost*)p; }
-}
-static DfieldView field_of(const float* lo, const float* hi, float h, float trunc, const uint32_t* index, const float* bricks)
-{
-    DfieldView f; uint64_t nb = 0;
-    df_grid(lo, hi, h, trunc, &f, &nb);
-    f.index = index; f.bricks = bricks;
-    return f;
-}
+// last block lane l adds the partials of blocks l, l + 32, ... and a butterfly), so the results are the device's bits.
+// Included into the emulator library (tests/emul/emul.cu).
 
 EMUL_API void emul_exp_f(const float* x, uint64_t n, float* out)
 {

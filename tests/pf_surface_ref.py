@@ -4,18 +4,15 @@
 * ProductScene.project: the product's pf_surface_one (rmcl_b200/csrc/kernels.cuh) compiled for the CPU over the product's host-built BVH
   (pf_surface_ref/surface_emul.cu).
 * quat_rotate64 / quat_mul64: float64 quaternion helpers for the geometric checks.
-Both libraries are built on first use into the per-user temporary directory of chain_ref."""
+Both libraries are built on first use by native.py."""
 import ctypes as C
-import os
 
 import numpy as np
 
-from chain_ref import _build
+import native
+import pyemul
 from rmcl_b200.api import SurfaceConfig
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ROOT = os.path.dirname(_HERE)
-_CSRC = os.path.join(_ROOT, "rmcl_b200", "csrc")
 _ref = None
 _emul = None
 
@@ -23,10 +20,7 @@ _emul = None
 def _ref_lib():
     global _ref
     if _ref is None:
-        src = os.path.join(_HERE, "pf_surface_ref", "pf_surface_ref.c")
-        cc = "/usr/bin/gcc" if os.access("/usr/bin/gcc", os.X_OK) else "gcc"
-        deps = [src, os.path.join(_ROOT, "oracle", "oracle.c"), os.path.join(_ROOT, "oracle", "oracle.h")]
-        _ref = _build("pf_surface_ref", deps, [cc, "-O2", "-fopenmp", "-ffp-contract=off", "-mavx2", "-mfma", "-fPIC", "-std=gnu11", "-shared", src, "-lm"])
+        _ref = native.restatement("pf_surface_ref/pf_surface_ref.c")
         _ref.orc_scene_create.restype = C.c_void_p
         _ref.orc_scene_destroy.argtypes = [C.c_void_p]
         _ref.orc_pf_surface.restype = None
@@ -36,15 +30,7 @@ def _ref_lib():
 def _emul_lib():
     global _emul
     if _emul is None:
-        src = os.path.join(_HERE, "pf_surface_ref", "surface_emul.cu")
-        deps = [src] + [os.path.join(_CSRC, f) for f in ("kernels.cuh", "icp_loop.cuh", "trace.cuh", "b2_math.cuh", "bvh8.h", "bvh_build.cpp")] + \
-               [os.path.join(_ROOT, "include", "rmcl_b200.h")]
-        nvcc = os.environ.get("NVCC", "nvcc")
-        _emul = _build("pf_surface_emul", deps, [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17", "-fmad=false",
-                                                 "-Xcompiler", "-fPIC,-fopenmp,-ffp-contract=off,-mavx2,-mfma,-fvisibility=hidden", "-shared", src,
-                                                 os.path.join(_CSRC, "bvh_build.cpp"), "-lgomp"])
-        _emul.emul_surface_scene.restype = C.c_void_p
-        _emul.emul_surface_scene_free.argtypes = [C.c_void_p]
+        _emul = native.emulator()
         _emul.emul_pf_surface.restype = None
     return _emul
 
@@ -78,21 +64,12 @@ class RefScene:
         return P, A
 
 
-class ProductScene:
+class ProductScene(pyemul.Scene):
     """the product's pf_surface_one on the CPU"""
-
-    def __init__(self, V, F):
-        self.V, self.F = _mesh(V, F)
-        self._s = _emul_lib().emul_surface_scene(_p(self.V), C.c_uint32(len(self.V)), _p(self.F), C.c_uint32(len(self.F)))
-        assert self._s
-
-    def __del__(self):
-        if getattr(self, "_s", None):
-            _emul_lib().emul_surface_scene_free(self._s)
 
     def project(self, P, A, cfg=None):
         P, A = np.array(P, copy=True), np.array(A, copy=True)
-        _emul_lib().emul_pf_surface(C.c_void_p(self._s), _p(P), _p(A), C.c_uint32(len(P)), C.byref(cfg or SurfaceConfig.defaults()))
+        _emul_lib().emul_pf_surface(self._h, _p(P), _p(A), C.c_uint32(len(P)), C.byref(cfg or SurfaceConfig.defaults()))
         return P, A
 
 

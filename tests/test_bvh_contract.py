@@ -15,7 +15,7 @@ from conftest import mesh
 @pytest.fixture(scope="module")
 def pe():
     import pyemul
-    pyemul.build()
+    pyemul.lib()
     return pyemul
 
 

@@ -20,7 +20,7 @@ def emul_scene(name):
 @pytest.fixture(scope="module")
 def pe():
     import pyemul
-    pyemul.build()
+    pyemul.lib()
     return pyemul
 
 

@@ -3,15 +3,15 @@ the downloaded buffers, sensors adding up, closed-form degeneracies of simple sc
 repeatability, refusals and the C++ mirror (SURVEY appendix I)."""
 import ctypes as C
 import math
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
-from conftest import ROOT, gpu_map
+from conftest import gpu_map
 import chain_ref
 import micp_cov_ref as ref
+import native
 import pf_estimate_ref
 
 pytestmark = pytest.mark.gpu
@@ -315,12 +315,7 @@ def test_cpp_mirror_matches_python(synth, tmp_path):
     """tests/micp_cov_cpp/micp_cov_cpp.cpp, compiled here against include/rmcl_b200/rcc_b200.hpp: rmcl::micp_correct then
     rmcl::micp_pose_covariance give the same bytes as the Python path"""
     import rmcl_b200
-    cuda = os.environ.get("CUDA_HOME", "/usr/local/cuda")
-    exe = str(tmp_path / "micp_cov_cpp")
-    lib_dir = os.path.dirname(rmcl_b200.lib_path())
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(cuda, "include"), "-o", exe,
-                           os.path.join(ROOT, "tests", "micp_cov_cpp", "micp_cov_cpp.cpp"), "-L" + lib_dir, "-lrmcl_b200",
-                           "-L" + os.path.join(cuda, "lib64"), "-lcudart", "-Wl,-rpath," + lib_dir])
+    exe = native.adapter("micp_cov_cpp")
     V, F = _scene("box")
     m = synth.c1_sensor()
     Tsb = synth.make_transform((0.1, 0.0, 0.3))

@@ -4,12 +4,12 @@ b2_pf_sensor_update fed the restated beams bit for bit (both correspondence type
 with the oracle; sharded halves equal the whole; step advances per update; refusals change nothing and launch nothing; the C++ adapter
 matches the Python path."""
 import ctypes as C
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
+import native
 import pf_cloud_ref as ref
 import rmcl_b200
 import test_gpu_pf_edges as E
@@ -17,7 +17,6 @@ from rmcl_b200 import synth
 from rmcl_b200.api import B2_CLOUD_NO_FIELD, cloud_layout
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SEED = 0x5EED0123456789AB
 
 
@@ -170,12 +169,7 @@ def test_refusals_change_nothing():
 def test_cpp_adapter_matches_python(tmp_path):
     """tests/pf_cloud_cpp: rmcl::b200::setInput over a PointCloud2-shaped struct, then two device updates and one host update of
     PCDSensorUpdaterB200 -- byte for byte the Python path"""
-    cuda = os.environ.get("CUDA_HOME", "/usr/local/cuda")
-    exe = str(tmp_path / "pf_cloud_cpp")
-    lib_dir = os.path.dirname(rmcl_b200.lib_path())
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(cuda, "include"), "-o", exe,
-                           os.path.join(ROOT, "tests", "pf_cloud_cpp", "pf_cloud_cpp.cpp"), "-L" + lib_dir, "-lrmcl_b200",
-                           "-L" + os.path.join(cuda, "lib64"), "-lcudart", "-Wl,-rpath," + lib_dir])
+    exe = native.adapter("pf_cloud_cpp")
     V, F = E.scene_mesh()
     c = scan_cloud(12, dtype=np.float64, point_step=48, offsets=(3, 17, 29), row_pad=6, extra={"intensity": 44})
     P, A = E.scan_particles(700, 13, 0.5, 0.3), E.attrs(700, n_meas=2, mean=0.8)

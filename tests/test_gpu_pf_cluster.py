@@ -4,12 +4,12 @@ kernels per recorded cluster) against the C restatement of tests/pf_cluster_ref,
 
 Counts, weights, keys and every label are exact; each record's stats equals, byte for byte, estimateStats of that cluster's members alone."""
 import math
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
+import native
 import pf_cluster_ref as ref
 from conftest import gpu_map
 from test_gpu_pf_residual import _dev, _np, _out
@@ -17,7 +17,6 @@ from test_pf_cluster import RES_Z, attrs_of, blob, cfg, poses_in_bins, snake
 from test_pf_residual import CFG, particles
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 NONE = 0xFFFFFFFF
 _up = None
 
@@ -299,12 +298,7 @@ def test_cpp_classes_match_python(tmp_path):
     """tests/pf_cluster_cpp/pf_cluster_cpp.cpp, compiled here against include/rmcl_b200/rcc_b200.hpp, clusters device particles through
     PCDSensorUpdaterB200::estimateClusters with its cluster_config: byte for byte what the Python path gives"""
     import rmcl_b200
-    cuda = os.environ.get("CUDA_HOME", "/usr/local/cuda")
-    exe = str(tmp_path / "pf_cluster_cpp")
-    lib_dir = os.path.dirname(rmcl_b200.lib_path())
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(cuda, "include"), "-o", exe,
-                           os.path.join(ROOT, "tests", "pf_cluster_cpp", "pf_cluster_cpp.cpp"), "-L" + lib_dir, "-lrmcl_b200",
-                           "-L" + os.path.join(cuda, "lib64"), "-lcudart", "-Wl,-rpath," + lib_dir])
+    exe = native.adapter("pf_cluster_cpp")
     P, A = _case(20_000, 12, "uniform")
     inp, out = tmp_path / "in.bin", tmp_path / "out.bin"
     with open(inp, "wb") as f:

@@ -13,18 +13,17 @@ Tolerances.
     and |dangle| <= 8e-6 per particle (tests/test_pf_estimate.py bounds the product's deviation function so), each entry is within
     sum w (da |v_b| + |v_a| db + da db), plus FP64 reordering."""
 import ctypes as C
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
+import native
 import pf_estimate_ref as er
 from conftest import gpu_map
 from test_pf_init import RVIZ_COV, _gauss_case
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EPS32 = float(np.finfo(np.float32).eps)
 EPS64 = float(np.finfo(np.float64).eps)
 
@@ -286,13 +285,7 @@ def test_round_trip_on_the_device(cov):
 def test_cpp_classes_match_python(tmp_path):
     """tests/pf_estimate_cpp: PCDSensorUpdaterB200::estimateStats + fillParticleStats into a message-shaped struct, byte for byte the Python
     path's record"""
-    import rmcl_b200
-    cuda = os.environ.get("CUDA_HOME", "/usr/local/cuda")
-    exe = str(tmp_path / "pf_estimate_cpp")
-    lib_dir = os.path.dirname(rmcl_b200.lib_path())
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(cuda, "include"), "-o", exe,
-                           os.path.join(ROOT, "tests", "pf_estimate_cpp", "pf_estimate_cpp.cpp"), "-L" + lib_dir, "-lrmcl_b200",
-                           "-L" + os.path.join(cuda, "lib64"), "-lcudart", "-Wl,-rpath," + lib_dir])
+    exe = native.adapter("pf_estimate_cpp")
     P, A = _random_set(60_000, seed=33)
     src = str(tmp_path / "particles.bin")
     with open(src, "wb") as f:

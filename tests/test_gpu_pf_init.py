@@ -12,19 +12,18 @@ asserts this bound for the same Box-Muller code).  With e = 4e-6 and s = the lar
     and the addition, a few ulp of |t|max;
   * each quaternion component is a sum of products of cos and sin of half angles, so it moves by at most 3 * dx/2 through the angles,
     plus the 2e-6 of the device functions, plus the pose product's rounding (a few ulp of 1)."""
-import os
 import subprocess
 import tempfile
 
 import numpy as np
 import pytest
 
+import native
 import pf_init_ref as ref
 from conftest import gpu_map
 from test_pf_init import BOX_MAX, BOX_MIN, RVIZ_COV, _gauss_case
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EPS = float(np.finfo(np.float32).eps)
 
 
@@ -203,14 +202,8 @@ def test_refusals_leave_outputs_untouched():
 def test_cpp_classes_match_python(tmp_path):
     """tests/pf_init_cpp/pf_init_cpp.cpp, compiled here against include/rmcl_b200/rcc_b200.hpp, fills device memory through
     PCDSensorUpdaterB200::initSamplesUniform / initSamples: byte for byte what the Python path gives"""
-    import rmcl_b200
     from rmcl_b200 import synth
-    cuda = os.environ.get("CUDA_HOME", "/usr/local/cuda")
-    exe = str(tmp_path / "pf_init_cpp")
-    lib_dir = os.path.dirname(rmcl_b200.lib_path())
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(cuda, "include"), "-o", exe,
-                           os.path.join(ROOT, "tests", "pf_init_cpp", "pf_init_cpp.cpp"), "-L" + lib_dir, "-lrmcl_b200",
-                           "-L" + os.path.join(cuda, "lib64"), "-lcudart", "-Wl,-rpath," + lib_dir])
+    exe = native.adapter("pf_init_cpp")
     n, first, seed = 5000, 123, 2024
     out = str(tmp_path / "particles.bin")
     r = subprocess.run([exe, out, str(n), str(first), str(seed)], capture_output=True, text=True, timeout=120)

@@ -5,19 +5,18 @@ weight_sum and weight_max.  Every stamp is its particle's index, so the parentag
 n_particles, bins, the parents and everything copied from the parent are exact; t, R and n_meas are within the tolerances of
 test_gpu_pf_residual (the copy is residual's, whose normals go through device logf / sinf / cosf)."""
 import math
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
+import native
 import pf_kld_ref as ref
 from conftest import gpu_map
 from test_gpu_pf_residual import _check, _dev, _np, _out
 from test_pf_residual import CFG, particles
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 N_MIN = 100
 _up = None
 
@@ -252,12 +251,7 @@ def test_cpp_classes_match_python(tmp_path):
     """tests/pf_kld_cpp/pf_kld_cpp.cpp, compiled here against include/rmcl_b200/rcc_b200.hpp, resamples device particles through
     PCDSensorUpdaterB200::resampleKLD with its kld_config: byte for byte what the Python path gives, record included"""
     import rmcl_b200
-    cuda = os.environ.get("CUDA_HOME", "/usr/local/cuda")
-    exe = str(tmp_path / "pf_kld_cpp")
-    lib_dir = os.path.dirname(rmcl_b200.lib_path())
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(cuda, "include"), "-o", exe,
-                           os.path.join(ROOT, "tests", "pf_kld_cpp", "pf_kld_cpp.cpp"), "-L" + lib_dir, "-lrmcl_b200",
-                           "-L" + os.path.join(cuda, "lib64"), "-lcudart", "-Wl,-rpath," + lib_dir])
+    exe = native.adapter("pf_kld_cpp")
     P, A = _case(20_000, 12, spread=1.5)                           # about 1 300 bins: fewer particles than slots
     n_max = 150_000
     inp, out = tmp_path / "in.bin", tmp_path / "out.bin"

@@ -12,18 +12,17 @@
   particle comes near it."""
 import ctypes as C
 import math
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
 from conftest import gpu_map, mesh
+import native
 from pf_recovery_ref import ProductRecovery, filter64
 from test_pf_recovery import TERRAIN_TRIS, particles, replaced_mask
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 R_TOL = 4e-6
 _MAPS = {}
 
@@ -269,12 +268,7 @@ def test_cpp_classes_match_python(tmp_path):
     """tests/pf_recovery_cpp/pf_recovery_cpp.cpp, compiled here against include/rmcl_b200/rcc_b200.hpp, runs reset, two observes and an
     injection through PCDSensorUpdaterB200: byte for byte what the Python path gives, records included"""
     import rmcl_b200
-    cuda = os.environ.get("CUDA_HOME", "/usr/local/cuda")
-    exe = str(tmp_path / "pf_recovery_cpp")
-    lib_dir = os.path.dirname(rmcl_b200.lib_path())
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(cuda, "include"), "-o", exe,
-                           os.path.join(ROOT, "tests", "pf_recovery_cpp", "pf_recovery_cpp.cpp"), "-L" + lib_dir, "-lrmcl_b200",
-                           "-L" + os.path.join(cuda, "lib64"), "-lcudart", "-Wl,-rpath," + lib_dir])
+    exe = native.adapter("pf_recovery_cpp")
     gm, _, (V, F) = _map("terrain")
     P, A = particles(20_000, seed=31)
     lo, hi = _box("terrain")

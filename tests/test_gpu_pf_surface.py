@@ -8,19 +8,18 @@
   -> estimateStats cycle tracks the true z and pitch."""
 import ctypes as C
 import math
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
 from conftest import gpu_map, mesh
+import native
 from pf_surface_ref import ProductScene
 from test_pf_surface import (CFG_IDS, CONFIGS, PLANE_BOUND, TERRAIN_TRIS, _cfg, _lattice_cases, _marked, _mezzanine_cases, _on_plane,
                              _plane, _random_cases, _special_cases, _stairs_cases)
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 RAMP_SLOPE = math.atan2(3.0, 17.0)
 
 _MAPS = {}
@@ -279,12 +278,7 @@ def test_cpp_classes_match_python(tmp_path):
     """tests/pf_surface_cpp/pf_surface_cpp.cpp, compiled here against include/rmcl_b200/rcc_b200.hpp, projects device particles through
     PCDSensorUpdaterB200::projectToSurface: byte for byte what the Python path gives"""
     import rmcl_b200
-    cuda = os.environ.get("CUDA_HOME", "/usr/local/cuda")
-    exe = str(tmp_path / "pf_surface_cpp")
-    lib_dir = os.path.dirname(rmcl_b200.lib_path())
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(cuda, "include"), "-o", exe,
-                           os.path.join(ROOT, "tests", "pf_surface_cpp", "pf_surface_cpp.cpp"), "-L" + lib_dir, "-lrmcl_b200",
-                           "-L" + os.path.join(cuda, "lib64"), "-lcudart", "-Wl,-rpath," + lib_dir])
+    exe = native.adapter("pf_surface_cpp")
     _, _, (V, F) = _map("terrain")
     P, A = _random_cases(31)
     inp, out = tmp_path / "in.bin", tmp_path / "out.bin"

@@ -2,19 +2,18 @@
 tests/pc2_ref bit for bit; corrections after it equal those after set_model_o1dn + set_ranges fed with the restated tables; the find's tile
 schedule is kept across clouds of one layout and reset otherwise; refusals change nothing; the C++ adapter matches the Python path."""
 import ctypes as C
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
+import native
 import pc2_ref as ref
 import rmcl_b200
 from conftest import gpu_map
 from rmcl_b200 import O1DnCloudFilter, synth
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MAP = "cube29"
 TGT = synth.make_transform((0.7, -0.4, 0.3), (0.02, -0.03, 0.4))
 
@@ -212,12 +211,7 @@ def test_refusals_change_nothing():
 
 def test_cpp_adapter_matches_python(tmp_path):
     """tests/pointcloud_cpp: unpackPointCloud over PointCloud2-shaped structs, then correctOnce -- byte for byte the Python path"""
-    cuda = os.environ.get("CUDA_HOME", "/usr/local/cuda")
-    exe = str(tmp_path / "pointcloud_cpp")
-    lib_dir = os.path.dirname(rmcl_b200.lib_path())
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(cuda, "include"), "-o", exe,
-                           os.path.join(ROOT, "tests", "pointcloud_cpp", "pointcloud_cpp.cpp"), "-L" + lib_dir, "-lrmcl_b200",
-                           "-L" + os.path.join(cuda, "lib64"), "-lcudart", "-Wl,-rpath," + lib_dir])
+    exe = native.adapter("pointcloud_cpp")
     from conftest import mesh
     V, F = mesh(MAP)
     with open(tmp_path / "map.bin", "wb") as f:

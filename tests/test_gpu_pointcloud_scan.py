@@ -4,12 +4,12 @@ restated ranges; the find's tile schedule survives a cloud; the key buffer reset
 the Python path."""
 import ctypes as C
 import math
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
+import native
 import pc2_scan_ref as ref
 import rmcl_b200
 from pc2_ref import same_bits
@@ -18,7 +18,6 @@ from rmcl_b200 import synth
 from rmcl_b200.api import B2_CLOUD_NO_FIELD, cloud_layout
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MAP = "cube29"
 TGT = synth.make_transform((0.7, -0.4, 0.3), (0.02, -0.03, 0.4))
 T_SC = synth.make_transform((0.05, -0.02, 0.1), (0.0, 0.02, -0.6))          # a cloud frame rotated and offset against the sensor
@@ -264,12 +263,7 @@ def test_refusals_change_nothing():
 def test_cpp_adapter_matches_python(tmp_path):
     """tests/pointcloud_scan_cpp: unpackPointCloud into an RCCB200Spherical over PointCloud2-shaped structs, then correctOnce -- byte for
     byte the Python path"""
-    cuda = os.environ.get("CUDA_HOME", "/usr/local/cuda")
-    exe = str(tmp_path / "pointcloud_scan_cpp")
-    lib_dir = os.path.dirname(rmcl_b200.lib_path())
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(cuda, "include"), "-o", exe,
-                           os.path.join(ROOT, "tests", "pointcloud_scan_cpp", "pointcloud_scan_cpp.cpp"), "-L" + lib_dir, "-lrmcl_b200",
-                           "-L" + os.path.join(cuda, "lib64"), "-lcudart", "-Wl,-rpath," + lib_dir])
+    exe = native.adapter("pointcloud_scan_cpp")
     from conftest import mesh
     V, F = mesh(MAP)
     with open(tmp_path / "map.bin", "wb") as f:

@@ -53,12 +53,13 @@ Printed per case: rays redrawn, inadmissible rays kept, the largest error as a f
 crossing a face within the edge margin missed it and every face behind the edge: evidence for a watertightness issue.
 """
 import ctypes as C
-import os
 import subprocess
 import time
 
 import numpy as np
 import pytest
+
+import native
 
 U = 2.0 ** -24
 K_T = 32.0
@@ -71,7 +72,6 @@ KEEP = 0.5                     # crossings kept by the model: signed edge distan
 NOFACE = 0xFFFFFFFF
 FIND_BLOCK = 64                # threads per k_rcc_find / k_cpc_find block
 PERM_MAX_TILES = 11520         # the find's tile schedule covers at most this many tiles
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 _T0 = time.time()
 
 
@@ -711,20 +711,10 @@ def check_umeyama(out, cases, what=""):
 # =====================================================================================================================================
 # the host harness: ray_setup's B2_RAY_INTBOX flag
 # =====================================================================================================================================
-_HARNESS = {}
-
-
 def intbox_flags(o, d, bmax):
-    if "exe" not in _HARNESS:
-        import tempfile
-        exe = os.path.join(tempfile.mkdtemp(prefix="node_visit_"), "node_visit")
-        nvcc = os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "nvcc")
-        subprocess.run([nvcc if os.path.exists(nvcc) else "nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17", "-fmad=false",
-                        "-Xcompiler", "-ffp-contract=off,-mfma", "-o", exe, os.path.join(ROOT, "tests", "node_visit", "node_visit.cu")], check=True, timeout=600)
-        _HARNESS["exe"] = exe
     lines = "".join(" ".join(float(x).hex() for x in np.concatenate([a, b])) + "\n" for a, b in zip(o.astype(np.float32), d.astype(np.float32)))
-    r = subprocess.run([_HARNESS["exe"], "flags"] + [float(x).hex() for x in np.asarray(bmax, np.float32)], input=lines, capture_output=True, text=True,
-                       timeout=600, check=True)
+    r = subprocess.run([native.nvcc_program("node_visit/node_visit.cu"), "flags"] + [float(x).hex() for x in np.asarray(bmax, np.float32)], input=lines,
+                       capture_output=True, text=True, timeout=600, check=True)
     return np.array([int(x) for x in r.stdout.split()], np.int64)
 
 

@@ -1,23 +1,17 @@
 """CPU tests of the box test's integer reduction (trace.cuh, INTEGER BOX TEST): for every ray ray_setup flags B2_RAY_INTBOX, the hit bits of
 node_test<true> equal the float reduction's, on special values (-0, +-inf, NaN, denormals, huge coordinates, tfar of -0 / NaN) and on
 random rays, nodes and tbest; rays outside the integer domain take node_test<false>, which must equal the float reduction too."""
-import os
 import re
 import subprocess
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "node_visit", "node_visit.cu")
+import native
 
 
 @pytest.fixture(scope="module")
-def harness(tmp_path_factory):
-    exe = str(tmp_path_factory.mktemp("node_visit") / "node_visit")
-    nvcc = os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "nvcc")
-    subprocess.run([nvcc if os.path.exists(nvcc) else "nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17", "-fmad=false", "-Xcompiler", "-ffp-contract=off,-mfma",
-                    "-o", exe, SRC], check=True, timeout=600)
-    return exe
+def harness():
+    return native.nvcc_program("node_visit/node_visit.cu")
 
 
 def run(exe, *args):
