@@ -686,6 +686,37 @@ B2_API int b2_pf_stein_update(b2_pf* h, const b2_dfield* f, b2_transform* poses_
                               const b2_range_meas* beams_host, uint32_t n_beams, const b2_pf_params* params,
                               const b2_stein_config* cfg, uint64_t seed, uint32_t step, b2_stein_result* out_host /* nullable */);
 
+/* b2_pf_stein_slice_*: the same steps on a particle set sharded over GPUs, one session per rank and handle (SURVEY L14).  The ranks'
+ * slices, concatenated in rank order after the last move, equal b2_pf_stein_update of the whole set byte for byte; b2_pf_stein_update is
+ * the one-rank case of this code.  The caller exchanges between the calls, over its own communicator, per iteration k:
+ *   1. every rank holds poses_all_dev, all n_all poses in rank order (an all-gather of the slices, 32 B per particle);
+ *   2. b2_pf_stein_slice_score(k) scores J's references [j_first, j_first + j_count) into snap_dev (j_count entries);
+ *   3. the caller all-gathers the snapshots in J's order into snap_all_dev (m entries, 24 B each);
+ *   4. b2_pf_stein_slice_move(k) computes the bandwidth over poses_all_dev (same bits on every rank), then moves poses first + i,
+ *      i < n_local, against all m entries into poses_out_dev[i] (n_local poses: poses_all_dev + first, in place, or a buffer that does
+ *      not overlap poses_all_dev).
+ * m = n_all when n_ref is 0 or >= n_all, else n_ref.  begin runs b2_pf_stein_update's checks plus first + n_local <= n_all and
+ * j_first + j_count <= m, uploads the beams (a synchronise), sizes the scratch and zeroes the RMSProp state and the record.  Score and move
+ * only launch kernels on the handle's stream (score 1 unless j_count is 0, move 2: the bandwidth always, the move unless n_local is 0); no
+ * synchronise, no allocation.  Sequence: iteration k's score follows begin (k = 0) or iteration k - 1's move, its move follows its score,
+ * and k < cfg->iterations; a call out of sequence is refused (B2_ERR_INVALID) with nothing launched and the session unchanged.  A refused
+ * begin leaves the previous session as it was.  n_all == 0: B2_OK everywhere, nothing launched.  The field, the poses and the snapshot
+ * buffers are read at the launches: they must live until the last move has run on the stream.
+ * b2_pf_stein_slice_result (one 40-byte copy and a synchronise): the last bandwidth (the same on every rank), m, the steps this rank's
+ * slice had blocked over all iterations, and the count and FP64 sums of squared proposed steps of its slice's last iteration.  Summed over
+ * ranks, rms_step_t = (float) sqrt(sum_step_t2 / n_steps) and rms_step_r likewise give b2_stein_result's RMS steps. */
+typedef struct { float x, y, psi, gx, gy, gpsi; } b2_stein_ref;          /* J's snapshot entry: chart and score; x = NaN contributes nothing */
+typedef struct { float bandwidth[3]; uint32_t n_ref, n_blocked, n_steps; double sum_step_t2, sum_step_r2; } b2_stein_slice_result;      /* 40 B */
+typedef char b2_stein_ref_is_24_bytes[sizeof(b2_stein_ref) == 24 ? 1 : -1];
+typedef char b2_stein_slice_result_is_40_bytes[sizeof(b2_stein_slice_result) == 40 ? 1 : -1];
+B2_API int b2_pf_stein_slice_begin(b2_pf* h, const b2_dfield* f, uint32_t n_all, uint32_t first, uint32_t n_local, uint32_t j_first, uint32_t j_count,
+                                   const b2_transform* Tsb, const b2_range_meas* beams_host, uint32_t n_beams, const b2_pf_params* params,
+                                   const b2_stein_config* cfg, uint64_t seed, uint32_t step);
+B2_API int b2_pf_stein_slice_score(b2_pf* h, const b2_transform* poses_all_dev, uint32_t iteration, b2_stein_ref* snap_dev /* j_count */);
+B2_API int b2_pf_stein_slice_move(b2_pf* h, const b2_transform* poses_all_dev, const b2_stein_ref* snap_all_dev /* m */, uint32_t iteration,
+                                  b2_transform* poses_out_dev /* n_local */);
+B2_API int b2_pf_stein_slice_result(b2_pf* h, b2_stein_slice_result* out_host);
+
 /* ---------------------------------------------------------------- introspection ------------------------------ */
 /* CUDA-event timing of the kernels inside b2_rcc_correct_once*(): when enabled, events are recorded on the handle's stream around the
  * find kernel and around the reduction/Umeyama kernels; b2_rcc_last_timing returns the two durations of the most recent call (ms). */

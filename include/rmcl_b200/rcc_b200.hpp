@@ -466,6 +466,35 @@ public:
                                     reinterpret_cast<const b2_transform*>(&Tsb_), beams, n_beams, &config, &cfg, seed, step, &r), "steinUpdate");
         return r;
     }
+    // The same steps on a particle set sharded over GPUs (b2_pf_stein_slice_*; SURVEY L14), for a node with its own communicator: steinBegin
+    // opens this rank's session (its slice [first, first + n_local) of n_all, its range [j_first, j_first + j_count) of J's m references;
+    // uploads the beams, a synchronise).  Per iteration k the caller all-gathers the poses into poses_all, calls steinScore(poses_all, k,
+    // snap) (j_count entries), all-gathers the snapshots in J's order into snap_all (m entries), then steinMove(poses_all, snap_all, k,
+    // out) (n_local poses; out may be poses_all + first).  Both only launch on the handle's stream.  steinResult reads the record (a
+    // synchronise).  The slices concatenated equal steinUpdate of the whole set byte for byte.  Throws on a call out of sequence.
+    void steinBegin(uint32_t n_all, uint32_t first, uint32_t n_local, uint32_t j_first, uint32_t j_count, const b2_range_meas* beams, uint32_t n_beams,
+                    const b2_stein_config& cfg = stein_config(), uint64_t seed = 0, uint32_t step = 0)
+    {
+        if (!field_) throw std::runtime_error("steinBegin: no distance field (setDistanceField first)");
+        b2_check(b2_pf_stein_slice_begin(h_, field_->handle(), n_all, first, n_local, j_first, j_count, reinterpret_cast<const b2_transform*>(&Tsb_), beams,
+                                         n_beams, &config, &cfg, seed, step), "steinBegin");
+    }
+    void steinScore(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses_all, uint32_t iteration, b2_stein_ref* snap_dev)
+    {
+        b2_check(b2_pf_stein_slice_score(h_, reinterpret_cast<const b2_transform*>(poses_all.raw()), iteration, snap_dev), "steinScore");
+    }
+    void steinMove(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses_all, const b2_stein_ref* snap_all_dev, uint32_t iteration,
+                   rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses_out)
+    {
+        b2_check(b2_pf_stein_slice_move(h_, reinterpret_cast<const b2_transform*>(poses_all.raw()), snap_all_dev, iteration,
+                                        reinterpret_cast<b2_transform*>(poses_out.raw())), "steinMove");
+    }
+    b2_stein_slice_result steinResult()
+    {
+        b2_stein_slice_result r{};
+        b2_check(b2_pf_stein_slice_result(h_, &r), "steinResult");
+        return r;
+    }
     // Recovery from a kidnapping (Augmented MCL, b2_pf_recovery_*): recoveryObserve after each update keeps a slow and a fast average of the
     // set's mean likelihood at recovery_config's rates (AMCL's recovery_alpha_slow / _fast); recoveryInject after resampling replaces a
     // fraction p_inject = max(0, 1 - w_fast / w_slow) of the particles with random poses of the box (on the map's ground when `surface` is

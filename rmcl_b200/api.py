@@ -121,6 +121,11 @@ class _SteinResult(C.Structure):
                 ("pad", C.c_float)]
 
 
+class _SteinSliceResult(C.Structure):
+    _fields_ = [("bandwidth", C.c_float * 3), ("n_ref", C.c_uint32), ("n_blocked", C.c_uint32), ("n_steps", C.c_uint32), ("sum_step_t2", C.c_double),
+                ("sum_step_r2", C.c_double)]
+
+
 class _CloudLayout(C.Structure):
     _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("point_step", C.c_uint32), ("row_step", C.c_uint32), ("offset_x", C.c_uint32),
                 ("offset_y", C.c_uint32), ("offset_z", C.c_uint32), ("datatype", C.c_uint8), ("is_bigendian", C.c_uint8), ("pad", C.c_uint8 * 2)]
@@ -187,7 +192,8 @@ EXPORTS = [
     "b2_rcc_set_cloud_spherical", "b2_pf_sample_cloud", "b2_pf_resample_residual", "b2_pf_project_to_surface",
     "b2_pf_resample_kld", "b2_pf_cluster_stats", "b2_micp_pose_covariance", "b2_pf_recovery_reset", "b2_pf_recovery_observe",
     "b2_pf_recovery_inject", "b2_dfield_create", "b2_dfield_destroy", "b2_dfield_get_info", "b2_dfield_download", "b2_dfield_query",
-    "b2_pf_sensor_update_field", "b2_pf_stein_update",
+    "b2_pf_sensor_update_field", "b2_pf_stein_update", "b2_pf_stein_slice_begin", "b2_pf_stein_slice_score", "b2_pf_stein_slice_move",
+    "b2_pf_stein_slice_result",
 ]
 
 
@@ -818,6 +824,7 @@ class PCDSensorUpdaterB200:
         self.step = 0                   # advanced by every update() that samples the input
         self._input = None
         self._field = None
+        self._stream = 0                # the handle's stream, as setStream last set it
 
     def close(self):
         if getattr(self, "_h", None):
@@ -832,6 +839,7 @@ class PCDSensorUpdaterB200:
 
     def setStream(self, cuda_stream):
         _chk(load_library().b2_pf_set_stream(self._h, C.c_void_p(int(cuda_stream))))
+        self._stream = int(cuda_stream)
 
     def setMapping(self, mode):
         """0 lanes = beams of one particle, 1 lanes = particles, 2 lanes = particles sorted by pose, 3 (default) auto by timing; results identical."""
@@ -924,6 +932,57 @@ class PCDSensorUpdaterB200:
                                                C.c_uint64(self.seed if seed is None else int(seed)), C.c_uint32(int(step)), C.byref(out)))
         return {"bandwidth": tuple(out.bandwidth), "n_ref": out.n_ref, "n_blocked": out.n_blocked, "rms_step_t": out.rms_step_t,
                 "rms_step_r": out.rms_step_r}
+
+    def steinBegin(self, n_all, first, n_local, j_first, j_count, Tsb, beams, config=None, params: PFParams | None = None, seed=None, step=0):
+        """Open a session of Stein steps on a slice of a set sharded over GPUs (b2_pf_stein_slice_begin; SURVEY L14): this rank moves the
+        particles [first, first + n_local) of n_all and scores J's references [j_first, j_first + j_count).  Arguments as steinUpdate's.
+        Uploads the beams (a synchronise); steinScore and steinMove then only launch kernels on the handle's stream."""
+        if self._field is None:
+            raise B2Error(-1, "steinBegin: no distance field (setDistanceField first)")
+        cfg = config or SteinConfig.defaults()
+        prm = params or self.config
+        beams = np.ascontiguousarray(beams)
+        assert beams.dtype.itemsize == 64
+        _chk(load_library().b2_pf_stein_slice_begin(self._h, self._field._h, C.c_uint32(n_all), C.c_uint32(first), C.c_uint32(n_local), C.c_uint32(j_first),
+                                                    C.c_uint32(j_count), _p(_tf(Tsb)), _p(beams) if len(beams) else None, C.c_uint32(len(beams)),
+                                                    C.byref(prm), C.byref(cfg), C.c_uint64(self.seed if seed is None else int(seed)), C.c_uint32(int(step))))
+
+    def steinScore(self, poses_all, iteration, snap):
+        """Iteration `iteration`'s score of the session's J range (b2_pf_stein_slice_score): poses_all the (n_all, 8) float32 CUDA tensor of
+        the whole set, snap a float32 CUDA tensor whose first j_count rows of 6 (x, y, psi, gx, gy, gpsi) are written."""
+        _chk(load_library().b2_pf_stein_slice_score(self._h, _devptr(poses_all), C.c_uint32(int(iteration)), _devptr(snap)))
+
+    def steinMove(self, poses_all, snap_all, iteration, poses_out):
+        """Iteration `iteration`'s bandwidth over poses_all and move of the session's slice against J's whole snapshot snap_all (m rows of 6)
+        into poses_out (n_local rows of 8; may be poses_all[first:first + n_local]) (b2_pf_stein_slice_move)."""
+        _chk(load_library().b2_pf_stein_slice_move(self._h, _devptr(poses_all), _devptr(snap_all), C.c_uint32(int(iteration)), _devptr(poses_out)))
+
+    def steinResult(self):
+        """The session's record (b2_pf_stein_slice_result, a synchronise): -> dict(bandwidth, n_ref, n_blocked, n_steps, sum_step_t2,
+        sum_step_r2); n_blocked counts this slice over all iterations, the step count and sums cover its last iteration."""
+        r = _SteinSliceResult()
+        _chk(load_library().b2_pf_stein_slice_result(self._h, C.byref(r)))
+        return {"bandwidth": tuple(r.bandwidth), "n_ref": r.n_ref, "n_blocked": r.n_blocked, "n_steps": r.n_steps, "sum_step_t2": r.sum_step_t2,
+                "sum_step_r2": r.sum_step_r2}
+
+    def steinUpdateSharded(self, poses_local, Tsb, beams, dist, config=None, params: PFParams | None = None, seed=None, step=0):
+        """steinUpdate on a particle set sharded over ranks in equal contiguous slices (rank order = global order): poses_local, this rank's
+        (n, 8) float32 CUDA tensor, moves in place.  Per iteration the poses (32 B per particle) and J's snapshot (24 B per reference) are
+        all-gathered over `dist` (torch.distributed, nccl); the slices then equal steinUpdate of the whole set byte for byte.  `seed`
+        (default self.seed) must be the same on every rank.  For the call the handle runs on torch's current stream, where the collectives
+        run, so the iterations need no host synchronise; the handle's stream is restored afterwards.  -> steinUpdate's dict for the whole
+        set: bandwidth and n_ref, n_blocked summed over ranks, the RMS steps from the summed squares."""
+        import torch
+        from .shard import stein_update_sharded
+        cfg = config or SteinConfig.defaults()
+        prev = self._stream
+        self.setStream(torch.cuda.current_stream(poses_local.device).cuda_stream)
+        try:
+            return stein_update_sharded(
+                lambda n_all, first, n_local, j_first, j_count: self.steinBegin(n_all, first, n_local, j_first, j_count, Tsb, beams, cfg, params, seed, step),
+                self.steinScore, self.steinMove, self.steinResult, poses_local, dist, cfg.iterations, cfg.n_ref)
+        finally:
+            self.setStream(prev)
 
     def motionUpdate(self, particle_poses, particle_attrs, T_bnew_bold, forget_rate, check_collision=False):
         """TFMotionUpdaterGPU (rmcl_ros/src/rmcl/particle_motion.cu:11-46): in place on torch CUDA tensors.  check_collision adds the CPU

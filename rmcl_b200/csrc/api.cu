@@ -1924,6 +1924,21 @@ extern "C" int b2_debug_read_bandwidth(int device, uint64_t bytes, int iters, do
 // ---------------------------------------------------------------------------------------------------------------------
 // particle filter
 // ---------------------------------------------------------------------------------------------------------------------
+// A Stein session (b2_pf_stein_slice_*): begin's arguments and the launch shape, and where the sequence stands.  open: begin succeeded;
+// next: the iteration the next score or move belongs to; scored: that iteration's score ran.
+struct PfSteinSession {
+    bool open = false, scored = false;
+    uint32_t next = 0;
+    DfieldView f{};
+    b2_transform Tsb{};
+    b2_stein_config cfg{};
+    uint32_t n_all = 0, first = 0, n_local = 0, j_first = 0, j_count = 0, m = 0, n_beams = 0, ppb = 0;
+    uint64_t seed = 0;
+    uint32_t step = 0;
+    float sigma2 = 0.0f;
+    double fac = 0.0;
+};
+
 // the fixed-size device records of the particle-filter entry points: one device block, zeroed at the handle's creation, and one pinned
 // host mirror of the same layout that pf_fetch reads members back into
 struct PfRecords {
@@ -1976,9 +1991,11 @@ struct b2_pf {
     // sort (the index buffers also list the roots); and the gathered members
     DevBuf<unsigned long long> d_cl_w; DevBuf<unsigned int> d_cl_cnt, d_cl_aux; DevBuf<uint32_t> d_cl_slot, d_cl_key, d_cl_key2, d_cl_idx, d_cl_idx2;
     DevBuf<b2_transform> d_cl_poses; DevBuf<b2_particle_attr> d_cl_attrs;
-    // Stein steps (b2_pf_stein_update), grown at its calls: J's snapshot, the RMSProp state of a call (3 floats per particle) and the block
-    // partials of its two grid reductions (one block per 256 particles)
-    DevBuf<SteinRef> d_stein_snap; DevBuf<float> d_stein_v; DevBuf<double> d_stein_part;
+    // Stein steps (b2_pf_stein_update, b2_pf_stein_slice_*), grown at a session's begin: J's snapshot (b2_pf_stein_update's), the session's
+    // beam table (its own, so that another call's beams between its score and move do not reach it), the RMSProp state of the slice (3
+    // floats per particle) and the block partials of the two grid reductions (one block per 256 particles of the whole set); the session
+    DevBuf<SteinRef> d_stein_snap; DevBuf<PfBeam> d_stein_beams; DevBuf<float> d_stein_v; DevBuf<double> d_stein_part;
+    PfSteinSession stein;
 };
 
 extern "C" int b2_pf_destroy(b2_pf* h);
@@ -2044,7 +2061,7 @@ extern "C" int b2_pf_destroy(b2_pf* h)
     h->d_kld_flags.release(); h->d_kld_cum.release(); h->d_kld_tmp.release(); h->d_kld_tab.release();
     h->d_cl_w.release(); h->d_cl_cnt.release(); h->d_cl_aux.release(); h->d_cl_slot.release(); h->d_cl_key.release(); h->d_cl_key2.release(); h->d_cl_idx.release();
     h->d_cl_idx2.release(); h->d_cl_poses.release(); h->d_cl_attrs.release();
-    h->d_stein_snap.release(); h->d_stein_v.release(); h->d_stein_part.release();
+    h->d_stein_snap.release(); h->d_stein_beams.release(); h->d_stein_v.release(); h->d_stein_part.release();
     b2_mesh* map = h->map;
     delete h;
     (void)cudaGetLastError();
@@ -2434,52 +2451,136 @@ extern "C" int b2_pf_sensor_update_field(b2_pf* h, const b2_dfield* f, const b2_
     return B2_OK;
 }
 
-// Stein variational steps (kernels.cuh, SURVEY appendix L): per iteration the score of J, the bandwidth and the move, all on h->stream
-extern "C" int b2_pf_stein_update(b2_pf* h, const b2_dfield* f, b2_transform* poses_dev, uint32_t n, const b2_transform* Tsb, const b2_range_meas* beams,
-                                  uint32_t n_beams, const b2_pf_params* prm, const b2_stein_config* cfg, uint64_t seed, uint32_t step, b2_stein_result* out_host)
+// Stein variational steps (kernels.cuh, SURVEY appendix L, L14): a session per rank, per iteration the score of a range of J, then the
+// bandwidth over the whole set and the move of the rank's slice, all on h->stream.  b2_pf_stein_update is the session of one rank.
+static_assert(sizeof(SteinRef) == sizeof(b2_stein_ref), "b2_stein_ref is SteinRef");
+extern "C" int b2_pf_stein_slice_begin(b2_pf* h, const b2_dfield* f, uint32_t n_all, uint32_t first, uint32_t n_local, uint32_t j_first, uint32_t j_count,
+                                       const b2_transform* Tsb, const b2_range_meas* beams, uint32_t n_beams, const b2_pf_params* prm, const b2_stein_config* cfg,
+                                       uint64_t seed, uint32_t step)
 {
     NOTNULL(h); NOTNULL(f); NOTNULL(Tsb); NOTNULL(prm); NOTNULL(cfg);
-    if (n) NOTNULL(poses_dev);
     if (n_beams) NOTNULL(beams);
-    if (f->map->device != h->map->device) return fail(B2_ERR_INVALID, "pf_stein_update: the field is on device %d, the handle on device %d", f->map->device, h->map->device);
+    if (f->map->device != h->map->device) return fail(B2_ERR_INVALID, "pf_stein: the field is on device %d, the handle on device %d", f->map->device, h->map->device);
     const b2_stein_config c = *cfg;
     auto pos = [](float v) { return std::isfinite(v) && v > 0.0f; };
     if (!(pos(c.step_t) && pos(c.step_r) && pos(c.min_bandwidth_t) && pos(c.min_bandwidth_r)))
-        return fail(B2_ERR_INVALID, "pf_stein_update: steps (%g, %g) and bandwidth floors (%g, %g) must be finite and > 0", (double)c.step_t, (double)c.step_r,
+        return fail(B2_ERR_INVALID, "pf_stein: steps (%g, %g) and bandwidth floors (%g, %g) must be finite and > 0", (double)c.step_t, (double)c.step_r,
                     (double)c.min_bandwidth_t, (double)c.min_bandwidth_r);
-    if (!(c.w_rand >= 0.0f && c.w_rand < 1.0f)) return fail(B2_ERR_INVALID, "pf_stein_update: w_rand = %g outside [0, 1)", (double)c.w_rand);
-    if (!pos(prm->dist_sigma)) return fail(B2_ERR_INVALID, "pf_stein_update: dist_sigma = %g must be finite and > 0", (double)prm->dist_sigma);
-    if (out_host) memset(out_host, 0, sizeof(*out_host));
+    if (!(c.w_rand >= 0.0f && c.w_rand < 1.0f)) return fail(B2_ERR_INVALID, "pf_stein: w_rand = %g outside [0, 1)", (double)c.w_rand);
+    if (!pos(prm->dist_sigma)) return fail(B2_ERR_INVALID, "pf_stein: dist_sigma = %g must be finite and > 0", (double)prm->dist_sigma);
+    const uint32_t m = (c.n_ref == 0 || c.n_ref >= n_all) ? n_all : c.n_ref;
+    if ((uint64_t)first + n_local > n_all) return fail(B2_ERR_INVALID, "pf_stein: slice [%u, %u + %u) beyond the %u particles", first, first, n_local, n_all);
+    if ((uint64_t)j_first + j_count > m) return fail(B2_ERR_INVALID, "pf_stein: references [%u, %u + %u) beyond J's %u", j_first, j_first, j_count, m);
+    if (n_all && n_beams && sizeof(float) * 3 * (size_t)n_beams > (size_t)h->smem_optin) return fail(B2_ERR_UNSUPPORTED, "pf_stein: too many beams (%u)", n_beams);
     CU(cudaSetDevice(h->map->device));
-    if (n == 0 || c.iterations == 0) return B2_OK;
-    const uint32_t m = (c.n_ref == 0 || c.n_ref >= n) ? n : c.n_ref;
+    PfSteinSession& ss = h->stein;
+    ss = PfSteinSession{};
+    ss.f = f->v; ss.Tsb = *Tsb; ss.cfg = c; ss.n_all = n_all; ss.first = first; ss.n_local = n_local; ss.j_first = j_first; ss.j_count = j_count; ss.m = m;
+    ss.n_beams = n_beams; ss.seed = seed; ss.step = step; ss.sigma2 = prm->dist_sigma * prm->dist_sigma;
+    ss.fac = std::pow((double)m, -1.0 / 7.0);                               // Scott's rule in 3 dimensions
+    if (n_all == 0) { ss.open = true; return B2_OK; }
     uint32_t ppb = B2_PF_BLOCK;
     if (n_beams) {
-        if (sizeof(float) * 3 * (size_t)n_beams > (size_t)h->smem_optin) return fail(B2_ERR_UNSUPPORTED, "pf_stein_update: too many beams (%u)", n_beams);
         RES(pf_prepare_beams(h, beams, n_beams, &ppb));
         ppb = std::max<uint32_t>(1u, std::min<uint32_t>(ppb, (uint32_t)((size_t)h->smem_optin / (sizeof(float) * 3 * (size_t)n_beams))));
+        RES(h->d_stein_beams.reserve(n_beams));
+        CU(cudaMemcpyAsync(h->d_stein_beams.p, h->d_beams.p, sizeof(PfBeam) * (size_t)n_beams, cudaMemcpyDeviceToDevice, h->stream));
     }
-    const uint32_t grid = (n + B2_STEIN_BLOCK - 1) / B2_STEIN_BLOCK;
-    RES(h->d_stein_snap.reserve(m)); RES(h->d_stein_v.reserve(3 * (size_t)n));
+    ss.ppb = ppb;
+    const uint32_t grid = (n_all + B2_STEIN_BLOCK - 1) / B2_STEIN_BLOCK;
+    RES(h->d_stein_v.reserve(3 * (size_t)n_local));
     RES(h->d_stein_part.reserve((size_t)std::max(B2_STEIN_NBW, B2_STEIN_NMV) * grid));
+    CU(cudaMemsetAsync(&h->d_recs.p->stein.rec, 0, sizeof(b2_stein_slice_result), h->stream));
+    if (n_local) CU(cudaMemsetAsync(h->d_stein_v.p, 0, sizeof(float) * 3 * (size_t)n_local, h->stream));
+    ss.open = true;
+    return B2_OK;
+}
+// the sequence of a session's calls (b2_pf_stein_slice_*); 1 where n_all is 0 (nothing to launch)
+static int pf_stein_in_sequence(const PfSteinSession& ss, uint32_t it, bool move, const char* fn)
+{
+    if (!ss.open) return fail(B2_ERR_INVALID, "%s: no session (b2_pf_stein_slice_begin first)", fn);
+    if (ss.n_all == 0) return 1;
+    if (it >= ss.cfg.iterations) return fail(B2_ERR_INVALID, "%s: iteration %u of %u", fn, it, ss.cfg.iterations);
+    if (it != ss.next || ss.scored != move)
+        return fail(B2_ERR_INVALID, "%s: iteration %u out of sequence (next: the %s of iteration %u)", fn, it, ss.scored ? "move" : "score", ss.next);
+    return B2_OK;
+}
+extern "C" int b2_pf_stein_slice_score(b2_pf* h, const b2_transform* poses_all, uint32_t it, b2_stein_ref* snap)
+{
+    NOTNULL(h);
+    PfSteinSession& ss = h->stein;
+    const int seq = pf_stein_in_sequence(ss, it, false, __func__);
+    if (seq != B2_OK) return seq == 1 ? B2_OK : seq;
+    NOTNULL(poses_all);
+    if (ss.j_count) NOTNULL(snap);
+    CU(cudaSetDevice(h->map->device));
+    if (ss.j_count) {
+        k_pf_stein_score<<<(ss.j_count + ss.ppb - 1) / ss.ppb, B2_PF_BLOCK, sizeof(float) * 3 * (size_t)ss.n_beams * ss.ppb, h->stream>>>(
+            ss.f, poses_all, ss.n_all, ss.j_first, ss.j_count, ss.cfg.n_ref, ss.seed, ss.step, it, ss.Tsb, h->d_stein_beams.p, ss.n_beams, ss.sigma2,
+            ss.cfg.w_rand, ss.ppb, reinterpret_cast<SteinRef*>(snap));
+        LAUNCHED();
+    }
+    ss.scored = true;
+    return B2_OK;
+}
+extern "C" int b2_pf_stein_slice_move(b2_pf* h, const b2_transform* poses_all, const b2_stein_ref* snap_all, uint32_t it, b2_transform* poses_out)
+{
+    NOTNULL(h);
+    PfSteinSession& ss = h->stein;
+    const int seq = pf_stein_in_sequence(ss, it, true, __func__);
+    if (seq != B2_OK) return seq == 1 ? B2_OK : seq;
+    NOTNULL(poses_all); NOTNULL(snap_all);
+    if (ss.n_local) NOTNULL(poses_out);
+    if (poses_out != poses_all + ss.first && poses_out + ss.n_local > poses_all && poses_out < poses_all + ss.n_all)
+        return fail(B2_ERR_INVALID, "%s: poses_out overlaps poses_all other than at the slice", __func__);
+    CU(cudaSetDevice(h->map->device));
     PfSteinState* st = &h->d_recs.p->stein;
-    CU(cudaMemsetAsync(&st->rec, 0, sizeof(b2_stein_result), h->stream));
-    CU(cudaMemsetAsync(h->d_stein_v.p, 0, sizeof(float) * 3 * (size_t)n, h->stream));
-    const BvhView bvh = h->map->view();
-    const double fac = std::pow((double)m, -1.0 / 7.0);                    // Scott's rule in 3 dimensions
-    const float sigma2 = prm->dist_sigma * prm->dist_sigma;
-    for (uint32_t it = 0; it < c.iterations; it++) {
-        k_pf_stein_score<<<(m + ppb - 1) / ppb, B2_PF_BLOCK, sizeof(float) * 3 * (size_t)n_beams * ppb, h->stream>>>(f->v, poses_dev, n, m, c.n_ref, seed, step, it, *Tsb,
-                                                                                                                 h->d_beams.p, n_beams, sigma2, c.w_rand, ppb, h->d_stein_snap.p);
+    const uint32_t grid = (ss.n_all + B2_STEIN_BLOCK - 1) / B2_STEIN_BLOCK;
+    k_pf_stein_bandwidth<<<grid, B2_STEIN_BLOCK, 0, h->stream>>>(poses_all, ss.n_all, ss.m, ss.fac, ss.cfg.min_bandwidth_t, ss.cfg.min_bandwidth_r, h->d_stein_part.p, st);
+    LAUNCHED();
+    if (ss.n_local) {
+        k_pf_stein_move<<<(ss.n_local + B2_STEIN_BLOCK - 1) / B2_STEIN_BLOCK, B2_STEIN_BLOCK, 0, h->stream>>>(
+            h->map->view(), poses_all, ss.first, ss.n_local, poses_out, reinterpret_cast<const SteinRef*>(snap_all), ss.m, it, ss.cfg.step_t, ss.cfg.step_r,
+            h->d_stein_v.p, h->d_stein_part.p, st);
         LAUNCHED();
-        k_pf_stein_bandwidth<<<grid, B2_STEIN_BLOCK, 0, h->stream>>>(poses_dev, n, m, fac, c.min_bandwidth_t, c.min_bandwidth_r, h->d_stein_part.p, st);
-        LAUNCHED();
-        k_pf_stein_move<<<grid, B2_STEIN_BLOCK, 0, h->stream>>>(bvh, poses_dev, n, h->d_stein_snap.p, m, it, c.step_t, c.step_r, h->d_stein_v.p, h->d_stein_part.p, st);
-        LAUNCHED();
+    }
+    ss.scored = false;
+    ss.next = it + 1;
+    return B2_OK;
+}
+extern "C" int b2_pf_stein_slice_result(b2_pf* h, b2_stein_slice_result* out_host)
+{
+    NOTNULL(h); NOTNULL(out_host);
+    if (!h->stein.open) return fail(B2_ERR_INVALID, "%s: no session (b2_pf_stein_slice_begin first)", __func__);
+    if (h->stein.n_all == 0) { memset(out_host, 0, sizeof(*out_host)); return B2_OK; }
+    CU(cudaSetDevice(h->map->device));
+    RES(pf_fetch(h, h->h_recs->stein.rec));
+    *out_host = h->h_recs->stein.rec;
+    return B2_OK;
+}
+extern "C" int b2_pf_stein_update(b2_pf* h, const b2_dfield* f, b2_transform* poses_dev, uint32_t n, const b2_transform* Tsb, const b2_range_meas* beams,
+                                  uint32_t n_beams, const b2_pf_params* prm, const b2_stein_config* cfg, uint64_t seed, uint32_t step, b2_stein_result* out_host)
+{
+    NOTNULL(h); NOTNULL(cfg);
+    if (n) NOTNULL(poses_dev);
+    const uint32_t iterations = n ? cfg->iterations : 0u;
+    const uint32_t m = (cfg->n_ref == 0 || cfg->n_ref >= n) ? n : cfg->n_ref;
+    RES(b2_pf_stein_slice_begin(h, f, iterations ? n : 0u, 0, iterations ? n : 0u, 0, iterations ? m : 0u, Tsb, beams, n_beams, prm, cfg, seed, step));
+    if (out_host) memset(out_host, 0, sizeof(*out_host));
+    if (iterations == 0) return B2_OK;
+    RES(h->d_stein_snap.reserve(m));
+    b2_stein_ref* snap = reinterpret_cast<b2_stein_ref*>(h->d_stein_snap.p);
+    for (uint32_t it = 0; it < iterations; it++) {
+        RES(b2_pf_stein_slice_score(h, poses_dev, it, snap));
+        RES(b2_pf_stein_slice_move(h, poses_dev, snap, it, poses_dev));
     }
     if (out_host) {
-        RES(pf_fetch(h, h->h_recs->stein.rec));
-        *out_host = h->h_recs->stein.rec;
+        b2_stein_slice_result r;
+        RES(b2_pf_stein_slice_result(h, &r));
+        out_host->bandwidth[0] = r.bandwidth[0]; out_host->bandwidth[1] = r.bandwidth[1]; out_host->bandwidth[2] = r.bandwidth[2];
+        out_host->n_ref = r.n_ref; out_host->n_blocked = r.n_blocked;
+        out_host->rms_step_t = r.n_steps ? (float)std::sqrt(r.sum_step_t2 / (double)r.n_steps) : 0.0f;
+        out_host->rms_step_r = r.n_steps ? (float)std::sqrt(r.sum_step_r2 / (double)r.n_steps) : 0.0f;
     }
     return B2_OK;
 }

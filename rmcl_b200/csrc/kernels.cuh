@@ -2860,10 +2860,10 @@ __global__ void __launch_bounds__(B2_COV_BLOCK) k_micp_information(const __grid_
 #endif
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Stein variational steps of the particle set over the distance field (b2_pf_stein_update; SURVEY appendix L; the MegaParticles TODO of
-// the reference's docs/RMCL.md).  Per iteration: k_pf_stein_score writes J's snapshot (chart and score of each reference), then
-// k_pf_stein_bandwidth the kernel bandwidth h, then k_pf_stein_move moves every particle from the snapshot.  The move reads J from the
-// snapshot only, so it can write the poses in place.  Every operation below is individually rounded (FMAs explicit; exp_f, atan2_d,
+// Stein variational steps of the particle set over the distance field (b2_pf_stein_update, b2_pf_stein_slice_*; SURVEY appendix L; the
+// MegaParticles TODO of the reference's docs/RMCL.md).  Per iteration: k_pf_stein_score writes J's snapshot (chart and score of each
+// reference of a range of J), then k_pf_stein_bandwidth the kernel bandwidth h over the whole set, then k_pf_stein_move moves a slice of
+// the set from the whole snapshot.  The move reads J from the snapshot only, so it can write the poses in place.  Every operation below is individually rounded (FMAs explicit; exp_f, atan2_d,
 // sin_d, cos_d of b2_math.cuh), so the host-compiled functions reproduce the device's bits.
 // ---------------------------------------------------------------------------------------------------------------------
 #define B2_PF_STEIN_TAG 8u
@@ -2871,7 +2871,7 @@ __global__ void __launch_bounds__(B2_COV_BLOCK) k_micp_information(const __grid_
 #define B2_STEIN_NBW 7                   // bandwidth sums: count, x, y, x^2, y^2, cos psi, sin psi
 #define B2_STEIN_NMV 3                   // step sums: count, dx^2 + dy^2, dpsi^2
 struct SteinRef { float x, y, p, gx, gy, gp; };       // one reference: chart and score; x = NaN marks one that contributes nothing
-struct PfSteinState { b2_stein_result rec; unsigned int ticket[2]; };
+struct PfSteinState { b2_stein_slice_result rec; unsigned int ticket[2]; };
 
 B2_DEV bool stein_finite3(const float c[3])
 {
@@ -2995,16 +2995,17 @@ B2_DEV uint32_t stein_move_one(const BvhView& bvh, b2_transform* pose_io, const 
 }
 
 #ifdef __CUDACC__
-// J x beams in k_pf_update_field's layout: a block of ppb references, lanes over beams, each term in shared memory at its beam's slot, one
-// thread per reference summing in slot order into the snapshot
-__global__ void __launch_bounds__(B2_PF_BLOCK) k_pf_stein_score(DfieldView f, const b2_transform* __restrict__ poses, uint32_t n, uint32_t m, uint32_t n_ref,
-                                                             uint64_t seed, uint32_t step, uint32_t it, b2_transform Tsb_val, const PfBeam* __restrict__ beams,
-                                                             uint32_t n_beams, float sigma2, float w_rand, uint32_t ppb, SteinRef* __restrict__ snap)
+// J's references [j_first, j_first + j_count) x beams in k_pf_update_field's layout: a block of ppb references, lanes over beams, each term
+// in shared memory at its beam's slot, one thread per reference summing in slot order into snap[r - j_first]
+__global__ void __launch_bounds__(B2_PF_BLOCK) k_pf_stein_score(DfieldView f, const b2_transform* __restrict__ poses, uint32_t n, uint32_t j_first, uint32_t j_count,
+                                                             uint32_t n_ref, uint64_t seed, uint32_t step, uint32_t it, b2_transform Tsb_val,
+                                                             const PfBeam* __restrict__ beams, uint32_t n_beams, float sigma2, float w_rand, uint32_t ppb,
+                                                             SteinRef* __restrict__ snap)
 {
     extern __shared__ float s_term[];            // [ppb][n_beams][3]
     __shared__ uint32_t s_idx[B2_PF_BLOCK];
-    const uint32_t r0 = blockIdx.x * ppb, nr = min(ppb, m - r0);
-    if (threadIdx.x < nr) s_idx[threadIdx.x] = stein_ref_index(r0 + threadIdx.x, n, n_ref, seed, step, it);
+    const uint32_t r0 = blockIdx.x * ppb, nr = min(ppb, j_count - r0);
+    if (threadIdx.x < nr) s_idx[threadIdx.x] = stein_ref_index(j_first + r0 + threadIdx.x, n, n_ref, seed, step, it);
     __syncthreads();
     const Tf Tsb = tf_from_pod(Tsb_val);
     const uint32_t total = nr * n_beams;
@@ -3034,11 +3035,12 @@ __global__ void __launch_bounds__(B2_STEIN_BLOCK) k_pf_stein_bandwidth(const b2_
     st->rec.n_ref = m;
     st->ticket[0] = 0u;
 }
-// One thread per particle i: the pair sum over J in tiles of B2_STEIN_BLOCK references (shared memory, N-body style), then the step.  The
-// blocked count goes to the record by integer atomics; the step sums by est_grid_reduce, whose last block writes the RMS steps.
-__global__ void __launch_bounds__(B2_STEIN_BLOCK) k_pf_stein_move(BvhView bvh, b2_transform* __restrict__ poses, uint32_t n, const SteinRef* __restrict__ snap,
-                                                               uint32_t m, uint32_t it, float step_t, float step_r, float* __restrict__ vstate,
-                                                               double* __restrict__ partials, PfSteinState* __restrict__ st)
+// One thread per particle i of the slice: pose first + i of `poses`, written to out[i] (out == poses + first: in place; else out must not
+// overlap `poses`).  The pair sum over J in tiles of B2_STEIN_BLOCK references (shared memory, N-body style), then the step.  The blocked
+// count goes to the record by integer atomics; the step sums by est_grid_reduce, whose last block writes them into the record.
+__global__ void __launch_bounds__(B2_STEIN_BLOCK) k_pf_stein_move(BvhView bvh, const b2_transform* poses, uint32_t first, uint32_t n, b2_transform* out,
+                                                               const SteinRef* __restrict__ snap, uint32_t m, uint32_t it, float step_t, float step_r,
+                                                               float* __restrict__ vstate, double* __restrict__ partials, PfSteinState* __restrict__ st)
 {
     __shared__ SteinRef s_ref[B2_STEIN_BLOCK];
     __shared__ double s_w[8 * B2_STEIN_NMV], tot[B2_STEIN_NMV];
@@ -3047,7 +3049,11 @@ __global__ void __launch_bounds__(B2_STEIN_BLOCK) k_pf_stein_move(BvhView bvh, b
     Tf T = tf_identity();
     float ci[3] = {0.0f, 0.0f, 0.0f};
     bool live = false;
-    if (i < n) { T = tf_load(poses + i); stein_chart(T, ci); live = stein_finite3(ci); }
+    if (i < n) {
+        const b2_transform* src = poses + first + i;
+        T = tf_load(src); stein_chart(T, ci); live = stein_finite3(ci);
+        if (out + i != src) out[i] = *src;              // a step not taken leaves the pose as it was
+    }
     float ih2[3];
     { const float h[3] = {st->rec.bandwidth[0], st->rec.bandwidth[1], st->rec.bandwidth[2]}; stein_inv_h2(h, ih2); }
     float acc[3] = {0.0f, 0.0f, 0.0f};
@@ -3066,13 +3072,14 @@ __global__ void __launch_bounds__(B2_STEIN_BLOCK) k_pf_stein_move(BvhView bvh, b
     }
     double sums[B2_STEIN_NMV] = {0.0, 0.0, 0.0};
     uint32_t blocked = 0u;
-    if (live) blocked = stein_move_one(bvh, poses + i, T, vstate + 3 * (size_t)i, acc, m, it, step_t, step_r, sums);
+    if (live) blocked = stein_move_one(bvh, out + i, T, vstate + 3 * (size_t)i, acc, m, it, step_t, step_r, sums);
     blocked = warp_sum_u32(blocked);
     if ((threadIdx.x & 31) == 0 && blocked) atomicAdd(&st->rec.n_blocked, blocked);
     if (!est_grid_reduce<B2_STEIN_NMV, EstSlots2>(sums, partials, &st->ticket[1], s_w, tot, is_last)) return;
     if (threadIdx.x != 0) return;
-    st->rec.rms_step_t = tot[0] > 0.0 ? (float)sqrt(tot[1] / tot[0]) : 0.0f;
-    st->rec.rms_step_r = tot[0] > 0.0 ? (float)sqrt(tot[2] / tot[0]) : 0.0f;
+    st->rec.n_steps = (uint32_t)tot[0];
+    st->rec.sum_step_t2 = tot[1];
+    st->rec.sum_step_r2 = tot[2];
     st->ticket[1] = 0u;
 }
 #endif

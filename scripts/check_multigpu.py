@@ -7,7 +7,9 @@ Checks, with particles sharded contiguously over the ranks and the map replicate
   2. Gladiator resampling: all-gather variant == peer-memory (CUDA IPC over NVLink) variant on every rank, and their concatenation ==
      rank 0's single-GPU resampling of the gathered set; exchanged bytes of both variants;
   3. particle set initialisation (uniform and Gaussian): each rank's shard (first = rank * n) gathered == rank 0's initialisation of the
-     whole set, byte for byte.
+     whole set, byte for byte;
+  4. Stein steps: steinUpdateSharded over NCCL (3 iterations, n_ref 4096) gathered == rank 0's steinUpdate of the gathered set, byte for
+     byte, with the same bandwidth, n_ref and n_blocked.
 Prints one JSON line on rank 0; exit code 1 on any mismatch."""
 import json
 import os
@@ -95,8 +97,28 @@ def main():
             up.initSamples(Pi, Ai, Tgt, cov, seed=17, first=rank * n_per)
         dist.all_gather_into_tensor(Pi_all, Pi); dist.all_gather_into_tensor(Ai_all, Ai)
         gathered[kind] = (Pi_all.clone(), Ai_all.clone())
+    # 4. Stein steps on the sharded set: all-gathers of the poses and of J's snapshot per iteration, each rank moving its own shard
+    us = rmcl_b200.PCDSensorUpdaterB200(gmap)
+    us.setDistanceField(rmcl_b200.DistanceField(gmap, 0.05, 1.0))
+    scfg = rmcl_b200.SteinConfig.defaults()
+    scfg.iterations = 3
+    sprm = rmcl_b200.PFParams.defaults()
+    sprm.dist_sigma = 0.2
+    Ps = Pd.clone()
+    torch.cuda.synchronize(); dist.barrier()
+    t0 = time.perf_counter()
+    sres = us.steinUpdateSharded(Ps, Tsb, beams, dist, scfg, sprm, seed=5, step=2)
+    torch.cuda.synchronize(); dist.barrier()
+    t_stein = time.perf_counter() - t0
+    Ps_all = torch.empty_like(P_all)
+    dist.all_gather_into_tensor(Ps_all, Ps)
     rc = 0
     if rank == 0:
+        Pw = P_all.clone()
+        wres = us.steinUpdate(Pw, Tsb, beams, scfg, sprm, seed=5, step=2)
+        torch.cuda.synchronize()
+        ok_stein = (bool(torch.equal(Pw.view(torch.int32), Ps_all.view(torch.int32))) and wres["bandwidth"] == sres["bandwidth"]
+                    and (wres["n_ref"], wres["n_blocked"]) == (sres["n_ref"], sres["n_blocked"]) and not torch.equal(Pw, P_all))
         ok_init = True
         for kind, (Pg_i, Ag_i) in gathered.items():
             Pw, Aw = torch.empty_like(P_all), torch.empty_like(A_all)
@@ -112,13 +134,13 @@ def main():
         ok_resample = bool(torch.equal(Pr, Pn_all) and torch.equal(Ar, An_all))
         changed = float((Ar[:, 0] != A_all[:, 0]).float().mean())
         line = {"world": world, "particles_per_rank": n_per, "sensor_update_shards_equal_whole": ok_update, "resample_sharded_equals_single_gpu": ok_resample,
-                "init_shards_equal_whole": ok_init,
+                "init_shards_equal_whole": ok_init, "stein_sharded_equals_single_gpu": ok_stein, "stein_sharded_wall_ms": t_stein * 1e3,
                 "p2p_equals_allgather_on_every_rank": [bool(int(f[0])) for f in allf] if p2p_err is None else None, "p2p_error": p2p_err,
                 "fraction_of_slots_replaced": changed, "checksum": hex(int(torch.from_numpy(Pn_all.cpu().numpy().view(np.uint32).astype(np.uint64)).sum().item()) & 0xffffffffffff),
                 "exchange_bytes": {"allgather_received_per_rank": (world - 1) * n_per * 68, "p2p_read_per_rank": [int(f[1]) for f in allf]},
                 "wall_ms": {"allgather_variant": t_allgather * 1e3, "p2p_variant": None if t_p2p is None else t_p2p * 1e3}}
         print(json.dumps(line))
-        if not (ok_update and ok_resample and ok_init and (p2p_err is not None or all(int(f[0]) for f in allf))):
+        if not (ok_update and ok_resample and ok_init and ok_stein and (p2p_err is not None or all(int(f[0]) for f in allf))):
             rc = 1
     dist.barrier()
     dist.destroy_process_group()
