@@ -416,22 +416,24 @@ public:
     ParticleUpdateResults update(rm::MemoryView<rm::Transform, rm::RAM> poses, rm::MemoryView<ParticleAttributes, rm::RAM> attrs, const ParticleUpdateConfig& = {})
     {
         if (field_) throw std::runtime_error("update: a distance field is set; the field update takes device particles only");
+        const uint32_t n = particle_count("update", poses, attrs);
         sample_input();
-        b2_check(b2_pf_sensor_update_host(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(),
+        b2_check(b2_pf_sensor_update_host(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), n,
                                           reinterpret_cast<const b2_transform*>(&Tsb_), reinterpret_cast<const b2_range_meas*>(beams_.data()), (uint32_t)beams_.size(), &config), "update");
         return {};
     }
     // ParticleUpdater<VRAM_CUDA>::update (ParticleUpdater.hpp:39-43)
     ParticleUpdateResults update(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs, const ParticleUpdateConfig& = {}) B2_PF_OVERRIDE
     {
+        const uint32_t n = particle_count("update", poses, attrs);
         sample_input();
         if (field_) {
             b2_check(b2_pf_sensor_update_field(h_, field_->handle(), reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()),
-                                               (uint32_t)poses.size(), reinterpret_cast<const b2_transform*>(&Tsb_), reinterpret_cast<const b2_range_meas*>(beams_.data()),
+                                               n, reinterpret_cast<const b2_transform*>(&Tsb_), reinterpret_cast<const b2_range_meas*>(beams_.data()),
                                                (uint32_t)beams_.size(), &config), "update");
             return {};
         }
-        b2_check(b2_pf_sensor_update(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(),
+        b2_check(b2_pf_sensor_update(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), n,
                                      reinterpret_cast<const b2_transform*>(&Tsb_), reinterpret_cast<const b2_range_meas*>(beams_.data()), (uint32_t)beams_.size(), &config), "update");
         return {};
     }
@@ -439,7 +441,7 @@ public:
     void motionUpdate(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs, const rm::Transform& T_bnew_bold, double forget_rate,
                       bool check_collision = false)       // true: the wall check of TFMotionUpdaterCPU (TFMotionUpdaterCPU.cpp:205-216)
     {
-        b2_check(b2_pf_motion_update(h_, reinterpret_cast<b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(),
+        b2_check(b2_pf_motion_update(h_, reinterpret_cast<b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), particle_count("motionUpdate", poses, attrs),
                                      reinterpret_cast<const b2_transform*>(&T_bnew_bold), forget_rate, check_collision ? 1 : 0), "motionUpdate");
     }
     // The surface-constrained motion update of docs/RMCL.md:72 (b2_pf_project_to_surface): each particle is put on the walkable surface
@@ -449,8 +451,8 @@ public:
     void projectToSurface(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs,
                           const b2_surface_config& cfg = surface_config())
     {
-        if (poses.size() != attrs.size()) throw std::invalid_argument("projectToSurface: poses and attrs differ in size");
-        b2_check(b2_pf_project_to_surface(h_, reinterpret_cast<b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(), &cfg),
+        b2_check(b2_pf_project_to_surface(h_, reinterpret_cast<b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()),
+                                          particle_count("projectToSurface", poses, attrs), &cfg),
                  "projectToSurface");
     }
     // Stein variational steps toward the beams' likelihood over the field of setDistanceField (b2_pf_stein_update; SURVEY appendix L): in
@@ -513,8 +515,8 @@ public:
                         const std::array<double, 6>& bb_min, const std::array<double, 6>& bb_max, const b2_surface_config* surface = nullptr,
                         uint32_t max_tries = 16, uint64_t seed = 1234, uint32_t step = 0, uint32_t first = 0, bool want_result = false)
     {
-        if (poses.size() != attrs.size()) throw std::invalid_argument("recoveryInject: poses and attrs differ in size");
-        b2_check(b2_pf_recovery_inject(h_, reinterpret_cast<b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), first, (uint32_t)poses.size(),
+        b2_check(b2_pf_recovery_inject(h_, reinterpret_cast<b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), first,
+                                       particle_count("recoveryInject", poses, attrs),
                                        bb_min.data(), bb_max.data(), surface, max_tries, seed, step, want_result ? &last_recovery : nullptr), "recoveryInject");
     }
     struct SimpleLikelihoodStats { float sum = 0.0f; float max = -1.0f; };                       // resampling.cuh:26-30
@@ -531,8 +533,9 @@ public:
                   rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses_new, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs_new,
                   uint64_t seed = 1234, uint32_t step = 0, uint32_t first = 0)
     {
-        b2_check(b2_pf_resample_gladiator(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<const b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(),
-                                          first, (uint32_t)poses_new.size(), reinterpret_cast<b2_transform*>(poses_new.raw()), reinterpret_cast<b2_particle_attr*>(attrs_new.raw()),
+        const uint32_t n_all = particle_count("resample", poses, attrs), n_local = particle_count("resample", poses_new, attrs_new);
+        b2_check(b2_pf_resample_gladiator(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<const b2_particle_attr*>(attrs.raw()), n_all,
+                                          first, n_local, reinterpret_cast<b2_transform*>(poses_new.raw()), reinterpret_cast<b2_particle_attr*>(attrs_new.raw()),
                                           &resampler_config, seed, step, nullptr, nullptr), "resample");
     }
     // ResidualResamplerCPU::update (ResidualResamplerCPU.cpp:55-202; config and defaults :35-47) on the device: all of `poses/attrs` resampled
@@ -544,10 +547,10 @@ public:
                                                   rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses_new, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs_new,
                                                   uint64_t seed = 1234, uint32_t step = 0, uint32_t first = 0, uint32_t n_new = 0)
     {
-        if (poses.size() != attrs.size() || poses_new.size() != attrs_new.size()) throw std::invalid_argument("resampleResidual: poses and attrs differ in size");
-        if (n_new == 0) n_new = first + (uint32_t)poses_new.size();
-        b2_check(b2_pf_resample_residual(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<const b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(),
-                                         n_new, first, (uint32_t)poses_new.size(), reinterpret_cast<b2_transform*>(poses_new.raw()),
+        const uint32_t n = particle_count("resampleResidual", poses, attrs), n_local = particle_count("resampleResidual", poses_new, attrs_new);
+        if (n_new == 0) n_new = first + n_local;
+        b2_check(b2_pf_resample_residual(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<const b2_particle_attr*>(attrs.raw()), n,
+                                         n_new, first, n_local, reinterpret_cast<b2_transform*>(poses_new.raw()),
                                          reinterpret_cast<b2_particle_attr*>(attrs_new.raw()), &residual_config, seed, step, &last_residual), "resampleResidual");
         ParticleUpdateDynamicResults res;
         res.n_particles = (uint32_t)last_residual.n_particles;
@@ -563,10 +566,10 @@ public:
                                              rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses_new, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs_new,
                                              uint64_t seed = 1234, uint32_t step = 0, uint32_t first = 0, uint32_t n_max = 0)
     {
-        if (poses.size() != attrs.size() || poses_new.size() != attrs_new.size()) throw std::invalid_argument("resampleKLD: poses and attrs differ in size");
-        if (n_max == 0) n_max = first + (uint32_t)poses_new.size();
-        b2_check(b2_pf_resample_kld(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<const b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(),
-                                    n_max, first, (uint32_t)poses_new.size(), reinterpret_cast<b2_transform*>(poses_new.raw()),
+        const uint32_t n = particle_count("resampleKLD", poses, attrs), n_local = particle_count("resampleKLD", poses_new, attrs_new);
+        if (n_max == 0) n_max = first + n_local;
+        b2_check(b2_pf_resample_kld(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<const b2_particle_attr*>(attrs.raw()), n,
+                                    n_max, first, n_local, reinterpret_cast<b2_transform*>(poses_new.raw()),
                                     reinterpret_cast<b2_particle_attr*>(attrs_new.raw()), &resampler_config, &kld_config, seed, step, &last_kld), "resampleKLD");
         ParticleUpdateDynamicResults res;
         res.n_particles = (uint32_t)last_kld.n_particles;
@@ -577,8 +580,8 @@ public:
     void initSamplesUniform(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs,
                             const std::array<double, 6>& bb_min, const std::array<double, 6>& bb_max, uint64_t seed, uint32_t first = 0)
     {
-        if (poses.size() != attrs.size()) throw std::invalid_argument("initSamplesUniform: poses and attrs differ in size");
-        b2_check(b2_pf_init_uniform(h_, reinterpret_cast<b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), first, (uint32_t)poses.size(),
+        b2_check(b2_pf_init_uniform(h_, reinterpret_cast<b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), first,
+                                    particle_count("initSamplesUniform", poses, attrs),
                                     bb_min.data(), bb_max.data(), seed), "initSamplesUniform");
     }
     // RmclNode::initSamples(PoseWithCovarianceStamped) (rmcl_localization.cpp:165-275) on the device: `pose` and the 36 row-major covariance
@@ -586,8 +589,8 @@ public:
     void initSamples(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs,
                      const rm::Transform& pose, const std::array<double, 36>& covariance, uint64_t seed, uint32_t first = 0)
     {
-        if (poses.size() != attrs.size()) throw std::invalid_argument("initSamples: poses and attrs differ in size");
-        b2_check(b2_pf_init_gaussian(h_, reinterpret_cast<b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), first, (uint32_t)poses.size(),
+        b2_check(b2_pf_init_gaussian(h_, reinterpret_cast<b2_transform*>(poses.raw()), reinterpret_cast<b2_particle_attr*>(attrs.raw()), first,
+                                     particle_count("initSamples", poses, attrs),
                                      reinterpret_cast<const b2_transform*>(&pose), covariance.data(), seed), "initSamples");
     }
     // RmclNode::estimateStats (rmcl_localization.cpp:642-731) on the device over the induction slice the caller passes, as the node passes
@@ -595,10 +598,9 @@ public:
     // (rmcl::b200::fillParticleStats in rmcl_msgs_adapters.hpp copies them into the message).
     b2_particle_stats estimateStats(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs)
     {
-        if (poses.size() != attrs.size()) throw std::invalid_argument("estimateStats: poses and attrs differ in size");
         b2_particle_stats s;
-        b2_check(b2_pf_estimate_stats(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<const b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(), &s),
-                 "estimateStats");
+        b2_check(b2_pf_estimate_stats(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<const b2_particle_attr*>(attrs.raw()),
+                                      particle_count("estimateStats", poses, attrs), &s), "estimateStats");
         return s;
     }
     // The filter's pose hypotheses (b2_pf_cluster_stats; AMCL's cluster statistics): the clusters of the set, heaviest first, at most
@@ -609,14 +611,20 @@ public:
     std::vector<b2_cluster_record> estimateClusters(rm::MemoryView<rm::Transform, rm::VRAM_CUDA> poses, rm::MemoryView<ParticleAttributes, rm::VRAM_CUDA> attrs,
                                                     uint32_t* labels = nullptr)
     {
-        if (poses.size() != attrs.size()) throw std::invalid_argument("estimateClusters: poses and attrs differ in size");
+        const uint32_t n = particle_count("estimateClusters", poses, attrs);
         std::vector<b2_cluster_record> recs(16);                                // max_records is at most 16
-        b2_check(b2_pf_cluster_stats(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<const b2_particle_attr*>(attrs.raw()), (uint32_t)poses.size(),
+        b2_check(b2_pf_cluster_stats(h_, reinterpret_cast<const b2_transform*>(poses.raw()), reinterpret_cast<const b2_particle_attr*>(attrs.raw()), n,
                                      &cluster_config, recs.data(), labels, &last_clusters), "estimateClusters");
         recs.resize(last_clusters.n_records);
         return recs;
     }
 private:
+    // The C ABI takes one count for a call's poses and attributes: views that differ in size are refused before anything runs
+    template <typename P, typename A> static uint32_t particle_count(const char* method, const P& poses, const A& attrs)
+    {
+        if (poses.size() != attrs.size()) throw std::invalid_argument(std::string(method) + ": poses and attrs differ in size");
+        return (uint32_t)poses.size();
+    }
     struct CloudInput { bool set = false; const void* data = nullptr; uint64_t bytes = 0; b2_cloud_layout layout{}; bool on_device = false; std::shared_ptr<const void> keep_alive; };
     // with an input cloud: this update's beams, `samples` drawn with (seed, step), then step advances
     void sample_input()

@@ -166,12 +166,14 @@ def _cloud_buffer(cloud):
     """(address, bytes, on device) of a PointCloud2-shaped object's data: a torch tensor, CUDA (read in place) or host, pinned or pageable
     (uploaded), or a numpy / bytes buffer (uploaded)"""
     data = cloud.data
-    if hasattr(data, "data_ptr"):
-        if not data.is_contiguous():
-            raise TypeError("setPointCloud: cloud.data must be contiguous")
-        return C.c_void_p(data.data_ptr()), data.numel() * data.element_size(), int(data.is_cuda)
-    data = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.ascontiguousarray(data).view(np.uint8).reshape(-1)
-    return C.c_void_p(data.ctypes.data) if data.size else None, data.size, 0
+    if hasattr(data, "data_ptr") and not data.is_contiguous():
+        raise TypeError("setPointCloud: cloud.data must be contiguous")
+    if getattr(data, "is_cuda", False):
+        return (*_records(data, 1), 1)
+    if isinstance(data, (bytes, bytearray, memoryview)):
+        data = np.frombuffer(data, np.uint8)
+    ptr, nbytes = _records(data, 1, lambda d: np.ascontiguousarray(d).view(np.uint8).reshape(-1))
+    return ptr if nbytes else None, nbytes, 0
 
 
 class _MeshInfo(C.Structure):
@@ -242,6 +244,10 @@ def _f32(a):
     return np.ascontiguousarray(a, np.float32)
 
 
+def _u8(a):
+    return np.ascontiguousarray(a, np.uint8)
+
+
 def _tf(a):
     a = np.ascontiguousarray(a)
     if a.dtype.itemsize != 32:
@@ -260,6 +266,40 @@ def _devptr(x):
             raise TypeError("expected a contiguous CUDA tensor")
         return C.c_void_p(x.data_ptr())
     raise TypeError(type(x))
+
+
+def _records(x, size, host=None):
+    """(address, count) of an array of `size`-byte records.  host None: a contiguous CUDA tensor, read in place.  Otherwise a host array,
+    made a contiguous numpy array by the conversion `host`; the address keeps that array alive.  A wrong kind of array, or a byte size that
+    is not a whole number of records, raises TypeError."""
+    if host is None:
+        if not hasattr(x, "data_ptr") or not x.is_cuda or not x.is_contiguous():
+            raise TypeError("expected a contiguous CUDA tensor")
+        addr, nbytes = C.c_void_p(x.data_ptr()), x.numel() * x.element_size()
+    else:
+        a = host(x)
+        addr, nbytes = a.ctypes.data_as(C.c_void_p), a.nbytes
+    if nbytes % size:
+        raise TypeError(f"expected {size}-byte records, got {nbytes} bytes")
+    return addr, nbytes // size
+
+
+def _agree(what, **arrays):
+    """The C ABI takes one count for all arrays of a call, so the binding checks their lengths: each keyword is (array, record size[, host
+    conversion]) as _records takes it, None passes as a null address.  -> (address of each array in keyword order..., the first array's
+    count).  A count that differs from the first raises ValueError."""
+    out, n, first = [], None, None
+    for name, (x, *spec) in arrays.items():
+        if x is None:
+            out.append(None)
+            continue
+        addr, k = _records(x, *spec)
+        if n is None:
+            n, first = k, name
+        elif k != n:
+            raise ValueError(f"{what}: {n} {first} but {k} {name}")
+        out.append(addr)
+    return (*out, n)
 
 
 def read_mesh_file(path):
@@ -341,16 +381,15 @@ class Map:
 
     def intersect(self, origs, dirs, tfar=np.inf):
         """Closest hit for arbitrary rays (replaces rtcIntersect1, PCDSensorUpdaterEmbree.cpp:30-47)."""
-        origs, dirs = _f32(origs).reshape(-1, 3), _f32(dirs).reshape(-1, 3)
-        n = len(origs)
+        o, d, n = _agree("intersect", origs=(origs, 12, _f32), dirs=(dirs, 12, _f32))
         t, f, ng, h = np.empty(n, np.float32), np.empty(n, np.uint32), np.empty((n, 3), np.float32), np.empty(n, np.uint8)
-        _chk(load_library().b2_mesh_intersect(self._h, _p(origs), _p(dirs), C.c_uint32(n), C.c_float(tfar), _p(t), _p(f), _p(ng), _p(h)))
+        _chk(load_library().b2_mesh_intersect(self._h, o, d, C.c_uint32(n), C.c_float(tfar), _p(t), _p(f), _p(ng), _p(h)))
         return t, f, ng, h
 
     def traversal_stats(self, origs, dirs, tfar=np.inf):
-        origs, dirs = _f32(origs).reshape(-1, 3), _f32(dirs).reshape(-1, 3)
+        o, d, n = _agree("traversal_stats", origs=(origs, 12, _f32), dirs=(dirs, 12, _f32))
         a, b = C.c_double(), C.c_double()
-        _chk(load_library().b2_mesh_intersect_stats(self._h, _p(origs), _p(dirs), C.c_uint32(len(origs)), C.c_float(tfar), C.byref(a), C.byref(b)))
+        _chk(load_library().b2_mesh_intersect_stats(self._h, o, d, C.c_uint32(n), C.c_float(tfar), C.byref(a), C.byref(b)))
         return a.value, b.value
 
 
@@ -419,13 +458,9 @@ class RCCB200:
         self.n = m.size
 
     def setDataset(self, points, mask=None):       # public field `dataset`, Correspondences.hpp:24
-        if hasattr(points, "data_ptr"):
-            n = points.numel() // 3
-            _chk(load_library().b2_rcc_set_dataset(self._h, _devptr(points), _devptr(mask), C.c_uint32(n), C.c_int(1)))
-        else:
-            points = _f32(points).reshape(-1, 3)
-            mask = None if mask is None else np.ascontiguousarray(mask, np.uint8)
-            _chk(load_library().b2_rcc_set_dataset(self._h, _p(points), _p(mask), C.c_uint32(len(points)), C.c_int(0)))
+        dev = hasattr(points, "data_ptr")
+        p, m, n = _agree("setDataset", points=(points, 12, None if dev else _f32), mask=(mask, 1, None if dev else _u8))
+        _chk(load_library().b2_rcc_set_dataset(self._h, p, m, C.c_uint32(n), C.c_int(int(dev))))
         self.outdated = True
 
     def setRanges(self, ranges):                   # MICP..Sensor..::unpackMessage / v1 setInputData
@@ -519,8 +554,8 @@ class RCCB200:
 
     def bindDataset(self, points, mask):
         """use caller-owned CUDA tensors as the dataset (no copy): the reference's public `dataset` member in VRAM (Correspondences.hpp:24)"""
-        n = points.numel() // 3
-        _chk(load_library().b2_rcc_bind_dataset(self._h, _devptr(points), _devptr(mask), C.c_uint32(n)))
+        p, m, n = _agree("bindDataset", points=(points, 12), mask=(mask, 1))
+        _chk(load_library().b2_rcc_bind_dataset(self._h, p, m, C.c_uint32(n)))
         self._bound = (points, mask)
         self.outdated = True
 
@@ -530,7 +565,8 @@ class RCCB200:
             _chk(load_library().b2_rcc_bind_model_buffers(self._h, None, None, None, C.c_uint32(0)))
             self._bound_model = None
             return
-        _chk(load_library().b2_rcc_bind_model_buffers(self._h, _devptr(points), _devptr(normals), _devptr(hits), C.c_uint32(hits.numel())))
+        h, p, nr, n = _agree("bindModelBuffers", hits=(hits, 1), points=(points, 12), normals=(normals, 12))
+        _chk(load_library().b2_rcc_bind_model_buffers(self._h, p, nr, h, C.c_uint32(n)))
         self._bound_model = (points, normals, hits)
 
     def setSimOptions(self, tfar_mode=0, min_mode=0, miss_fill=0):
@@ -572,16 +608,15 @@ class RCCB200:
         lib = load_library()
         if hasattr(Tbm, "data_ptr"):
             import torch
-            n = Tbm.numel() * Tbm.element_size() // 32
+            pT, n = _records(Tbm, 32)
             Td = torch.empty((n, 8), dtype=torch.float32, device=Tbm.device)
             nc = torch.empty((n,), dtype=torch.int32, device=Tbm.device)
             st = torch.empty((n, 16), dtype=torch.float32, device=Tbm.device)
-            _chk(lib.b2_rcc_correct_batch(self._h, _devptr(Tbm), C.c_uint32(n), C.c_int(1), _devptr(Td), _devptr(nc), _devptr(st), C.c_int(1)))
+            _chk(lib.b2_rcc_correct_batch(self._h, pT, C.c_uint32(n), C.c_int(1), _devptr(Td), _devptr(nc), _devptr(st), C.c_int(1)))
             return Td, nc, st
-        Tbm = _tf(Tbm).reshape(-1)
-        n = len(Tbm)
+        pT, n = _records(Tbm, 32, _tf)
         Td, nc, st = np.zeros(n, TRANSFORM_DTYPE), np.zeros(n, np.uint32), np.zeros(n, CROSS_STATS_DTYPE)
-        _chk(lib.b2_rcc_correct_batch(self._h, _p(Tbm), C.c_uint32(n), C.c_int(0), _p(Td), _p(nc), _p(st), C.c_int(0)))
+        _chk(lib.b2_rcc_correct_batch(self._h, pT, C.c_uint32(n), C.c_int(0), _p(Td), _p(nc), _p(st), C.c_int(0)))
         return Td, nc, st
 
 
@@ -733,9 +768,9 @@ def micp_pose_covariance(sensors, Tbo, T_onew_oold, convergence_progress=0.0, me
 
 def umeyama_transform(stats, device=0):
     """rm::umeyama_transform for an array of CrossStatistics (micp_localization.cpp:952-953)."""
-    stats = np.ascontiguousarray(stats).reshape(-1)
-    out = np.zeros(len(stats), TRANSFORM_DTYPE)
-    _chk(load_library().b2_umeyama_batch(_p(stats), C.c_uint32(len(stats)), _p(out), C.c_int(0), C.c_int(device), None))
+    ps, n = _records(stats, 64, np.ascontiguousarray)
+    out = np.zeros(n, TRANSFORM_DTYPE)
+    _chk(load_library().b2_umeyama_batch(ps, C.c_uint32(n), _p(out), C.c_int(0), C.c_int(device), None))
     return out
 
 
@@ -882,34 +917,27 @@ class PCDSensorUpdaterB200:
         update(MemoryView) does -- no staging copy; pin the arrays and the transfers overlap the kernel).  VRAM variant: torch CUDA tensors, attrs
         updated in place.  beams=None: `samples` beams are drawn from the setInput cloud with (seed, step), then step advances by one."""
         prm = params or self.config
-        if self._field is not None and not hasattr(particle_poses, "data_ptr"):
+        dev = hasattr(particle_poses, "data_ptr")
+        if self._field is not None and not dev:
             raise B2Error(-1, "update: a distance field is set; the field update takes CUDA tensors only")
+        if inplace and not dev:
+            assert isinstance(particle_attrs, np.ndarray) and particle_attrs.flags.c_contiguous and particle_attrs.flags.writeable
+        attrs = particle_attrs if dev or inplace else np.ascontiguousarray(particle_attrs).copy()
+        p, a, n = _agree("update", poses=(particle_poses, 32, None if dev else _tf), attrs=(attrs, 36, None if dev else np.ascontiguousarray))
         if beams is None:
             if self._input is None:
                 raise B2Error(-1, "update: no beams and no input cloud (setInput first)")
             beams = self.sampleBeams(self._input)
             self.step += 1
-        beams = np.ascontiguousarray(beams)
-        assert beams.dtype.itemsize == 64
+        pb, nb = _records(beams, 64, np.ascontiguousarray)
         Tsb = _tf(Tsb)
         lib = load_library()
-        if hasattr(particle_poses, "data_ptr"):
-            n = particle_poses.numel() * particle_poses.element_size() // 32
-            if self._field is not None:
-                _chk(lib.b2_pf_sensor_update_field(self._h, self._field._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(n), _p(Tsb),
-                                                   _p(beams), C.c_uint32(len(beams)), C.byref(prm)))
-                return particle_attrs
-            _chk(lib.b2_pf_sensor_update(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(n), _p(Tsb), _p(beams),
-                                         C.c_uint32(len(beams)), C.byref(prm)))
-            return particle_attrs
-        poses = _tf(particle_poses).reshape(-1)
-        if inplace:
-            attrs = particle_attrs
-            assert isinstance(attrs, np.ndarray) and attrs.flags.c_contiguous and attrs.flags.writeable
+        if not dev:
+            _chk(lib.b2_pf_sensor_update_host(self._h, p, a, C.c_uint32(n), _p(Tsb), pb, C.c_uint32(nb), C.byref(prm)))
+        elif self._field is not None:
+            _chk(lib.b2_pf_sensor_update_field(self._h, self._field._h, p, a, C.c_uint32(n), _p(Tsb), pb, C.c_uint32(nb), C.byref(prm)))
         else:
-            attrs = np.ascontiguousarray(particle_attrs).copy()
-        assert attrs.dtype.itemsize == 36
-        _chk(lib.b2_pf_sensor_update_host(self._h, _p(poses), _p(attrs), C.c_uint32(len(poses)), _p(Tsb), _p(beams), C.c_uint32(len(beams)), C.byref(prm)))
+            _chk(lib.b2_pf_sensor_update(self._h, p, a, C.c_uint32(n), _p(Tsb), pb, C.c_uint32(nb), C.byref(prm)))
         return attrs
 
     def steinUpdate(self, particle_poses, Tsb, beams, config=None, params: PFParams | None = None, seed=None, step=0):
@@ -923,13 +951,11 @@ class PCDSensorUpdaterB200:
             raise B2Error(-1, "steinUpdate: no distance field (setDistanceField first)")
         cfg = config or SteinConfig.defaults()
         prm = params or self.config
-        beams = np.ascontiguousarray(beams)
-        assert beams.dtype.itemsize == 64
-        n = particle_poses.numel() * particle_poses.element_size() // 32
+        pb, nb = _records(beams, 64, np.ascontiguousarray)
+        p, n = _records(particle_poses, 32)
         out = _SteinResult()
-        _chk(load_library().b2_pf_stein_update(self._h, self._field._h, _devptr(particle_poses), C.c_uint32(n), _p(_tf(Tsb)),
-                                               _p(beams) if len(beams) else None, C.c_uint32(len(beams)), C.byref(prm), C.byref(cfg),
-                                               C.c_uint64(self.seed if seed is None else int(seed)), C.c_uint32(int(step)), C.byref(out)))
+        _chk(load_library().b2_pf_stein_update(self._h, self._field._h, p, C.c_uint32(n), _p(_tf(Tsb)), pb if nb else None, C.c_uint32(nb), C.byref(prm),
+                                               C.byref(cfg), C.c_uint64(self.seed if seed is None else int(seed)), C.c_uint32(int(step)), C.byref(out)))
         return {"bandwidth": tuple(out.bandwidth), "n_ref": out.n_ref, "n_blocked": out.n_blocked, "rms_step_t": out.rms_step_t,
                 "rms_step_r": out.rms_step_r}
 
@@ -941,10 +967,9 @@ class PCDSensorUpdaterB200:
             raise B2Error(-1, "steinBegin: no distance field (setDistanceField first)")
         cfg = config or SteinConfig.defaults()
         prm = params or self.config
-        beams = np.ascontiguousarray(beams)
-        assert beams.dtype.itemsize == 64
+        pb, nb = _records(beams, 64, np.ascontiguousarray)
         _chk(load_library().b2_pf_stein_slice_begin(self._h, self._field._h, C.c_uint32(n_all), C.c_uint32(first), C.c_uint32(n_local), C.c_uint32(j_first),
-                                                    C.c_uint32(j_count), _p(_tf(Tsb)), _p(beams) if len(beams) else None, C.c_uint32(len(beams)),
+                                                    C.c_uint32(j_count), _p(_tf(Tsb)), pb if nb else None, C.c_uint32(nb),
                                                     C.byref(prm), C.byref(cfg), C.c_uint64(self.seed if seed is None else int(seed)), C.c_uint32(int(step))))
 
     def steinScore(self, poses_all, iteration, snap):
@@ -987,9 +1012,8 @@ class PCDSensorUpdaterB200:
     def motionUpdate(self, particle_poses, particle_attrs, T_bnew_bold, forget_rate, check_collision=False):
         """TFMotionUpdaterGPU (rmcl_ros/src/rmcl/particle_motion.cu:11-46): in place on torch CUDA tensors.  check_collision adds the CPU
         updater's wall check (TFMotionUpdaterCPU.cpp:17-50,205-216)."""
-        n = particle_poses.numel() * particle_poses.element_size() // 32
-        _chk(load_library().b2_pf_motion_update(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(n), _p(_tf(T_bnew_bold)), C.c_double(forget_rate),
-                                                C.c_int(int(check_collision))))
+        p, a, n = _agree("motionUpdate", poses=(particle_poses, 32), attrs=(particle_attrs, 36))
+        _chk(load_library().b2_pf_motion_update(self._h, p, a, C.c_uint32(n), _p(_tf(T_bnew_bold)), C.c_double(forget_rate), C.c_int(int(check_collision))))
 
     def projectToSurface(self, particle_poses, particle_attrs, config=None):
         """Keep the particles on the map's walkable surface (b2_pf_project_to_surface; the surface-constrained motion update of
@@ -997,17 +1021,15 @@ class PCDSensorUpdaterB200:
         within `config`'s probe window whose slope is at most max_slope (and tilted onto it with align 1); one found no such surface keeps
         its pose and gets the likelihood {0, 0, 10000}, so the next resampling replaces it.  `config`: a SurfaceConfig (default: defaults())."""
         cfg = config or SurfaceConfig.defaults()
-        n = particle_poses.numel() * particle_poses.element_size() // 32
-        if particle_attrs.numel() * particle_attrs.element_size() != 36 * n:
-            raise ValueError("projectToSurface: poses and attrs differ in length")
-        _chk(load_library().b2_pf_project_to_surface(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(n), C.byref(cfg)))
+        p, a, n = _agree("projectToSurface", poses=(particle_poses, 32), attrs=(particle_attrs, 36))
+        _chk(load_library().b2_pf_project_to_surface(self._h, p, a, C.c_uint32(n), C.byref(cfg)))
 
     def likelihoodStats(self, particle_attrs, dist=None):
         """compute_stats (rmcl_ros/src/rmcl/resampling.cu:41-92) of the local particles; with `dist` (torch.distributed, particles sharded
         across ranks) the 8 bytes are all-reduced (SUM / MAX) -- the only exchange step of the particle-filter cycle."""
-        n = particle_attrs.numel() * particle_attrs.element_size() // 36
+        a, n = _records(particle_attrs, 36)
         s, m = C.c_float(), C.c_float()
-        _chk(load_library().b2_pf_likelihood_stats(self._h, _devptr(particle_attrs), C.c_uint32(n), C.byref(s), C.byref(m)))
+        _chk(load_library().b2_pf_likelihood_stats(self._h, a, C.c_uint32(n), C.byref(s), C.byref(m)))
         s, m = s.value, m.value
         if dist is not None and dist.is_initialized() and dist.get_world_size() > 1:
             import torch
@@ -1019,21 +1041,12 @@ class PCDSensorUpdaterB200:
             s, m = float(ts[0]), float(tm[0])
         return s, m
 
-
-    @staticmethod
-    def _init_count(particle_poses, particle_attrs):
-        n = particle_poses.numel() * particle_poses.element_size() // 32
-        if particle_attrs.numel() * particle_attrs.element_size() != 36 * n:
-            raise ValueError(f"initSamples: {n} poses but {particle_attrs.numel() * particle_attrs.element_size() / 36:g} attrs")
-        return n
-
     def initSamplesUniform(self, particle_poses, particle_attrs, bb_min, bb_max, seed, first=0):
         """RmclNode::initSamplesUniform (rmcl_ros/src/nodes/rmcl_localization.cpp:277-342) on the device: fills the caller's (n, 8) / (n, 9)
         float32 CUDA tensors in place with particles first .. first+n-1 of a set drawn uniformly from the box (x, y, z, roll, pitch, yaw)."""
         lo, hi = np.ascontiguousarray(bb_min, np.float64).reshape(6), np.ascontiguousarray(bb_max, np.float64).reshape(6)
-        n = self._init_count(particle_poses, particle_attrs)
-        _chk(load_library().b2_pf_init_uniform(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(first), C.c_uint32(n), _p(lo), _p(hi),
-                                               C.c_uint64(seed)))
+        p, a, n = _agree("initSamplesUniform", poses=(particle_poses, 32), attrs=(particle_attrs, 36))
+        _chk(load_library().b2_pf_init_uniform(self._h, p, a, C.c_uint32(first), C.c_uint32(n), _p(lo), _p(hi), C.c_uint64(seed)))
         return particle_poses, particle_attrs
 
     def initSamples(self, particle_poses, particle_attrs, pose, cov, seed, first=0):
@@ -1041,21 +1054,18 @@ class PCDSensorUpdaterB200:
         Transform record), `cov` its 36 covariance entries (row-major); the noise acts in the pose frame.  Fills the tensors in place."""
         T = _tf(pose).reshape(())
         c = np.ascontiguousarray(cov, np.float64).reshape(36)
-        n = self._init_count(particle_poses, particle_attrs)
-        _chk(load_library().b2_pf_init_gaussian(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(first), C.c_uint32(n), _p(T), _p(c),
-                                                C.c_uint64(seed)))
+        p, a, n = _agree("initSamples", poses=(particle_poses, 32), attrs=(particle_attrs, 36))
+        _chk(load_library().b2_pf_init_gaussian(self._h, p, a, C.c_uint32(first), C.c_uint32(n), _p(T), _p(c), C.c_uint64(seed)))
         return particle_poses, particle_attrs
 
     def estimateStats(self, particle_poses, particle_attrs, max_induction_particles=50000):
         """RmclNode::estimateStats (rmcl_ros/src/nodes/rmcl_localization.cpp:642-731) on the device: the statistics of the first
         min(n, max_induction_particles) particles of the (n, 8) / (n, 9) float32 CUDA tensors, as a synth.PARTICLE_STATS_DTYPE record (the
         fields of rmcl_msgs/ParticleStats): likelihood statistics, translation bounds, the weighted Markley mean pose and its 6x6 covariance."""
-        n = particle_poses.numel() * particle_poses.element_size() // 32
-        if particle_attrs.numel() * particle_attrs.element_size() != 36 * n:
-            raise ValueError(f"estimateStats: {n} poses but {particle_attrs.numel() * particle_attrs.element_size() / 36:g} attrs")
+        p, a, n = _agree("estimateStats", poses=(particle_poses, 32), attrs=(particle_attrs, 36))
         k = max(0, min(n, int(max_induction_particles)))
         out = np.zeros((), PARTICLE_STATS_DTYPE)
-        _chk(load_library().b2_pf_estimate_stats(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(k), _p(out)))
+        _chk(load_library().b2_pf_estimate_stats(self._h, p, a, C.c_uint32(k), _p(out)))
         return out
 
     def estimateClusters(self, particle_poses, particle_attrs, config=None, labels=None):
@@ -1066,15 +1076,10 @@ class PCDSensorUpdaterB200:
         weight_total, rounds, weight_sum, weight_max) and the n_records heaviest clusters as synth.CLUSTER_RECORD_DTYPE, records[0] the
         best hypothesis: its share `weight` of the set, and in `stats` what estimateStats gives of its members alone."""
         cfg = config or ClusterConfig.defaults()
-        n = particle_poses.numel() * particle_poses.element_size() // 32
-        if particle_attrs.numel() * particle_attrs.element_size() != 36 * n:
-            raise ValueError(f"estimateClusters: {n} poses but {particle_attrs.numel() * particle_attrs.element_size() / 36:g} attrs")
-        if labels is not None and labels.numel() * labels.element_size() != 4 * n:
-            raise ValueError(f"estimateClusters: {n} particles but {labels.numel() * labels.element_size() / 4:g} labels")
+        p, a, lab, n = _agree("estimateClusters", poses=(particle_poses, 32), attrs=(particle_attrs, 36), labels=(labels, 4))
         out = np.zeros((), CLUSTER_RESULT_DTYPE)
         recs = np.zeros(max(1, min(int(cfg.max_records), 16)), CLUSTER_RECORD_DTYPE)
-        _chk(load_library().b2_pf_cluster_stats(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(n), C.byref(cfg), _p(recs),
-                                                None if labels is None else _devptr(labels), _p(out)))
+        _chk(load_library().b2_pf_cluster_stats(self._h, p, a, C.c_uint32(n), C.byref(cfg), _p(recs), lab, _p(out)))
         return out, recs[:int(out["n_records"])]
 
     def recoveryReset(self):
@@ -1089,9 +1094,9 @@ class PCDSensorUpdaterB200:
         recoveryInject.  want_state: -> a synth.RECOVERY_STATE_DTYPE record (w_avg, w_slow, w_fast, p_inject), read back with a
         synchronise; otherwise the call only enqueues and returns None."""
         c = cfg or RecoveryConfig.defaults()
-        n = particle_attrs.numel() * particle_attrs.element_size() // 36
+        a, n = _records(particle_attrs, 36)
         out = np.zeros((), RECOVERY_STATE_DTYPE) if want_state else None
-        _chk(load_library().b2_pf_recovery_observe(self._h, _devptr(particle_attrs), C.c_uint32(n), C.byref(c), _p(out)))
+        _chk(load_library().b2_pf_recovery_observe(self._h, a, C.c_uint32(n), C.byref(c), _p(out)))
         return out
 
     def recoveryInject(self, particle_poses, particle_attrs, bb_min, bb_max, surface=None, max_tries=16, seed=1234, step=0, first=0, want_result=False):
@@ -1103,13 +1108,10 @@ class PCDSensorUpdaterB200:
         want_result: -> a synth.RECOVERY_RESULT_DTYPE record (p_inject, n_replaced, n_failed), read back with a synchronise; otherwise the
         call only enqueues and returns None."""
         lo, hi = np.ascontiguousarray(bb_min, np.float64).reshape(6), np.ascontiguousarray(bb_max, np.float64).reshape(6)
-        n = particle_poses.numel() * particle_poses.element_size() // 32
-        if particle_attrs.numel() * particle_attrs.element_size() != 36 * n:
-            raise ValueError("recoveryInject: poses and attrs differ in length")
+        p, a, n = _agree("recoveryInject", poses=(particle_poses, 32), attrs=(particle_attrs, 36))
         out = np.zeros((), RECOVERY_RESULT_DTYPE) if want_result else None
-        _chk(load_library().b2_pf_recovery_inject(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(first), C.c_uint32(n), _p(lo), _p(hi),
-                                                  None if surface is None else C.byref(surface), C.c_uint32(max_tries), C.c_uint64(seed),
-                                                  C.c_uint32(step), _p(out)))
+        _chk(load_library().b2_pf_recovery_inject(self._h, p, a, C.c_uint32(first), C.c_uint32(n), _p(lo), _p(hi), None if surface is None else C.byref(surface),
+                                                  C.c_uint32(max_tries), C.c_uint64(seed), C.c_uint32(step), _p(out)))
         return out
 
     def gladiatorRandoms(self, seed, step, first, n, device=None):
@@ -1125,11 +1127,10 @@ class PCDSensorUpdaterB200:
         """GladiatorResamplerGPU::resample (rmcl_ros/src/rmcl/resampling.cu:108-221) on torch CUDA tensors.  `particle_poses/attrs` hold all
         particles opponents are drawn from; the outputs receive champions first .. first+len(out)-1 (single GPU: first = 0, same length)."""
         cfg = config or GladiatorConfig.defaults()
-        n_all = particle_poses.numel() * particle_poses.element_size() // 32
-        n_local = particle_poses_new.numel() * particle_poses_new.element_size() // 32
-        _chk(load_library().b2_pf_resample_gladiator(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(n_all), C.c_uint32(first), C.c_uint32(n_local),
-                                                     _devptr(particle_poses_new), _devptr(particle_attrs_new), C.byref(cfg), C.c_uint64(seed), C.c_uint32(step),
-                                                     _devptr(raw) if raw is not None else None, _devptr(normals) if normals is not None else None))
+        p, a, n_all = _agree("resample", poses=(particle_poses, 32), attrs=(particle_attrs, 36))
+        pn, an, r, nrm, n_local = _agree("resample", poses_new=(particle_poses_new, 32), attrs_new=(particle_attrs_new, 36), raw=(raw, 4), normals=(normals, 24))
+        _chk(load_library().b2_pf_resample_gladiator(self._h, p, a, C.c_uint32(n_all), C.c_uint32(first), C.c_uint32(n_local), pn, an, C.byref(cfg),
+                                                     C.c_uint64(seed), C.c_uint32(step), r, nrm))
         return particle_poses_new, particle_attrs_new
 
     def resampleResidual(self, particle_poses, particle_attrs, particle_poses_new, particle_attrs_new, config=None, seed=1234, step=0, first=0, n_new=None):
@@ -1138,15 +1139,12 @@ class PCDSensorUpdaterB200:
         receive slots first .. first+len(out)-1, and entries at or beyond the result's n_particles are left untouched.  `config` is a
         GladiatorConfig (the same fields and defaults).  -> a synth.RESIDUAL_RESULT_DTYPE record: n_particles, draws, weight_sum, weight_max."""
         cfg = config or GladiatorConfig.defaults()
-        n = particle_poses.numel() * particle_poses.element_size() // 32
-        n_local = particle_poses_new.numel() * particle_poses_new.element_size() // 32
-        if particle_attrs.numel() * particle_attrs.element_size() != 36 * n or particle_attrs_new.numel() * particle_attrs_new.element_size() != 36 * n_local:
-            raise ValueError("resampleResidual: poses and attrs differ in length")
+        p, a, n = _agree("resampleResidual", poses=(particle_poses, 32), attrs=(particle_attrs, 36))
+        pn, an, n_local = _agree("resampleResidual", poses_new=(particle_poses_new, 32), attrs_new=(particle_attrs_new, 36))
         n_new = first + n_local if n_new is None else int(n_new)
         out = np.zeros((), RESIDUAL_RESULT_DTYPE)
-        _chk(load_library().b2_pf_resample_residual(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(n), C.c_uint32(n_new), C.c_uint32(first),
-                                                    C.c_uint32(n_local), _devptr(particle_poses_new), _devptr(particle_attrs_new), C.byref(cfg), C.c_uint64(seed),
-                                                    C.c_uint32(step), _p(out)))
+        _chk(load_library().b2_pf_resample_residual(self._h, p, a, C.c_uint32(n), C.c_uint32(n_new), C.c_uint32(first), C.c_uint32(n_local), pn, an,
+                                                    C.byref(cfg), C.c_uint64(seed), C.c_uint32(step), _p(out)))
         return out
 
     def resampleKLD(self, particle_poses, particle_attrs, particle_poses_new, particle_attrs_new, kld=None, config=None, seed=1234, step=0, first=0, n_max=None):
@@ -1157,15 +1155,12 @@ class PCDSensorUpdaterB200:
         weight_sum, weight_max."""
         kcfg = kld or KLDConfig.defaults()
         cfg = config or GladiatorConfig.defaults()
-        n = particle_poses.numel() * particle_poses.element_size() // 32
-        n_local = particle_poses_new.numel() * particle_poses_new.element_size() // 32
-        if particle_attrs.numel() * particle_attrs.element_size() != 36 * n or particle_attrs_new.numel() * particle_attrs_new.element_size() != 36 * n_local:
-            raise ValueError("resampleKLD: poses and attrs differ in length")
+        p, a, n = _agree("resampleKLD", poses=(particle_poses, 32), attrs=(particle_attrs, 36))
+        pn, an, n_local = _agree("resampleKLD", poses_new=(particle_poses_new, 32), attrs_new=(particle_attrs_new, 36))
         n_max = first + n_local if n_max is None else int(n_max)
         out = np.zeros((), KLD_RESULT_DTYPE)
-        _chk(load_library().b2_pf_resample_kld(self._h, _devptr(particle_poses), _devptr(particle_attrs), C.c_uint32(n), C.c_uint32(n_max), C.c_uint32(first),
-                                               C.c_uint32(n_local), _devptr(particle_poses_new), _devptr(particle_attrs_new), C.byref(cfg), C.byref(kcfg),
-                                               C.c_uint64(seed), C.c_uint32(step), _p(out)))
+        _chk(load_library().b2_pf_resample_kld(self._h, p, a, C.c_uint32(n), C.c_uint32(n_max), C.c_uint32(first), C.c_uint32(n_local), pn, an,
+                                               C.byref(cfg), C.byref(kcfg), C.c_uint64(seed), C.c_uint32(step), _p(out)))
         return out
 
     def p2pConnect(self, dist, n_per_rank):
