@@ -717,6 +717,39 @@ B2_API int b2_pf_stein_slice_move(b2_pf* h, const b2_transform* poses_all_dev, c
                                   b2_transform* poses_out_dev /* n_local */);
 B2_API int b2_pf_stein_slice_result(b2_pf* h, b2_stein_slice_result* out_host);
 
+/* b2_pf_global_search: where on the map does this scan fit best?  An exhaustive correlative search (Olson 2009; Hess et al. 2016) over a
+ * grid of flat poses (x, y, yaw) scored against the distance field, returning its best separated peaks, best first (SURVEY appendix M).
+ * Deterministic: the same scan gives the same records.  Hand each record to b2_pf_init_gaussian to start the filter there.
+ *  - Candidate c = (k * ny + j) * nx + i (i < nx, j < ny, k < n_yaw = K): t = (x0 + (float)i * step, y0 + (float)j * step, z0), each op
+ *    rounded in float; R = (0, 0, (float)sin(psi_k / 2), (float)cos(psi_k / 2)) with psi_k = -pi + 2 pi k / K in double; stamp 0.
+ *  - surface (nullable): the candidate is what b2_pf_project_to_surface's rule makes of that pose; one it finds off surface is invalid.
+ *  - score: the likelihood.mean a particle at the candidate would get from one b2_pf_sensor_update_field call with the same Tsb, beams and
+ *    params, starting from {0, 0, 0}: bit for bit, finite and >= 0 (0 without beams).  An invalid candidate scores -1.
+ *  - peak: a valid candidate whose every valid neighbour n (i +- 1, j +- 1, k +- 1 modulo K; up to 26) has score_n < score_c, or the same
+ *    score and n > c.
+ *  - records: the peaks by score descending, ties by the smaller c; walking that order, a peak is kept unless a kept one lies both closer
+ *    than min_separation_xy (Euclidean distance of the grid positions) and closer than min_separation_yaw (the wrapped difference of the
+ *    psi_k, in double); 0 / 0 keeps every peak.  records_host[r], r < n_records = min(kept, max_records), is rank r: the candidate's pose
+ *    (surface applied), score and (i, j, k).
+ * Runs on the handle's stream and synchronises it; the particle set, the ray-mapping timers and the recovery record are untouched.
+ * scores_dev (nullable, DEVICE): receives the n_candidates scores in c order, the likelihood map.  Scratch: 4 B per candidate (in
+ * scores_dev when given), 32 B per (i, j) cell with surface, and 16 B per possible peak (at most ceil(nx/2) ceil(ny/2) ceil(K/2)) for the
+ * ranking.  Refused (B2_ERR_INVALID, no launch, nothing written): null h, f, Tsb, params, cfg, records_host or out_host; null beams with
+ * n_beams > 0; a field on another device than the handle; nx, ny or n_yaw 0, n_yaw > 32768, more than 2^30 candidates; step not finite
+ * and > 0, a non-finite x0, y0 or z0 or last grid position; max_records outside [1, 64]; a separation negative or not finite; dist_sigma
+ * not finite and > 0 or whose square is not (the scores would not be finite); b2_pf_project_to_surface's refusals for surface.
+ * Suggested values: step 0.25 m, n_yaw 72 (5 deg), max_records 8, separations 1 m and 30 deg. */
+typedef struct { float x0, y0, z0, step; uint32_t nx, ny, n_yaw, max_records; float min_separation_xy, min_separation_yaw; } b2_search_config;   /* 40 B */
+typedef char b2_search_config_is_40_bytes[sizeof(b2_search_config) == 40 ? 1 : -1];
+typedef struct { b2_transform pose; float score; uint32_t i, j, k; } b2_search_record;                                                       /* 48 B */
+typedef char b2_search_record_is_48_bytes[sizeof(b2_search_record) == 48 ? 1 : -1];
+typedef struct { uint64_t n_candidates, n_valid, n_peaks, n_records; } b2_search_result;                                                     /* 32 B */
+typedef char b2_search_result_is_32_bytes[sizeof(b2_search_result) == 32 ? 1 : -1];
+B2_API int b2_pf_global_search(b2_pf* h, const b2_dfield* f, const b2_transform* Tsb, const b2_range_meas* beams_host, uint32_t n_beams,
+                               const b2_pf_params* params, const b2_search_config* cfg, const b2_surface_config* surface /* nullable */,
+                               b2_search_record* records_host, float* scores_dev /* nullable: n_candidates floats in c order */,
+                               b2_search_result* out_host);
+
 /* ---------------------------------------------------------------- introspection ------------------------------ */
 /* CUDA-event timing of the kernels inside b2_rcc_correct_once*(): when enabled, events are recorded on the handle's stream around the
  * find kernel and around the reduction/Umeyama kernels; b2_rcc_last_timing returns the two durations of the most recent call (ms). */

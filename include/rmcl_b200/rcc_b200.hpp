@@ -455,6 +455,27 @@ public:
                                           particle_count("projectToSurface", poses, attrs), &cfg),
                  "projectToSurface");
     }
+    // Where on the map does the scan fit best (b2_pf_global_search; SURVEY appendix M): every pose of cfg's (x, y, yaw) grid scored from
+    // `field` as the field update scores a particle there from {0, 0, 0} (with this updater's Tsb and config), the local maxima of the
+    // scores ranked and separated.  surface (may be null) puts the candidates where projectToSurface would; scores_dev (may be null, n_candidates
+    // device floats) receives the likelihood map.  Returns the kept peaks, best first; result (may be null) receives the counts.  Synchronises.
+    // search_config(...) gives the suggested values over an (x, y) box.
+    static b2_search_config search_config(float x_min, float y_min, float x_max, float y_max, float z0, float step = 0.25f)
+    {
+        return b2_search_config{x_min, y_min, z0, step, (uint32_t)((x_max - x_min) / step) + 1u, (uint32_t)((y_max - y_min) / step) + 1u, 72u, 8u, 1.0f,
+                                0.52359878f};
+    }
+    std::vector<b2_search_record> globalSearch(const B200DistanceField& field, const b2_range_meas* beams, uint32_t n_beams, const b2_search_config& cfg,
+                                               const b2_surface_config* surface = nullptr, float* scores_dev = nullptr, b2_search_result* result = nullptr)
+    {
+        std::vector<b2_search_record> recs(cfg.max_records >= 1 && cfg.max_records <= 64 ? cfg.max_records : 1);
+        b2_search_result r{};
+        b2_check(b2_pf_global_search(h_, field.handle(), reinterpret_cast<const b2_transform*>(&Tsb_), beams, n_beams, &config, &cfg, surface, recs.data(),
+                                     scores_dev, &r), "globalSearch");
+        recs.resize(r.n_records);
+        if (result) *result = r;
+        return recs;
+    }
     // Stein variational steps toward the beams' likelihood over the field of setDistanceField (b2_pf_stein_update; SURVEY appendix L): in
     // place on the device poses, on the handle's stream; x, y and yaw move, z, roll, pitch and the attributes stay.  Throws without a field.
     // Returns the result record (a 32-byte read-back and a synchronise).  stein_config() gives the suggested values.

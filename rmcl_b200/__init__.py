@@ -6,10 +6,10 @@ v1 correct(), ParticleUpdater::update).  There is no CPU fallback: importing wor
 the CUDA library and a GPU and raises otherwise.
 """
 from .api import (B2Error, Map, RCCB200, RCCB200Spherical, RCCB200Pinhole, RCCB200O1Dn, RCCB200OnDn, CPCB200, SphereCorrectorB200, PinholeCorrectorB200, O1DnCloudFilter,
-                  O1DnCorrectorB200, OnDnCorrectorB200, PCDSensorUpdaterB200, DistanceField, PFParams, GladiatorConfig, SurfaceConfig, KLDConfig, ClusterConfig, RecoveryConfig, SteinConfig, umeyama_transform, micp_correct_once, micp_correct,
+                  O1DnCorrectorB200, OnDnCorrectorB200, PCDSensorUpdaterB200, DistanceField, PFParams, GladiatorConfig, SurfaceConfig, KLDConfig, ClusterConfig, RecoveryConfig, SteinConfig, SearchConfig, umeyama_transform, micp_correct_once, micp_correct,
                   micp_pose_covariance, MICP_STEP_DTYPE, MICP_COVARIANCE_DTYPE, read_mesh_file, kernel_launch_count, lib_path, load_library)
 from . import synth
 
 __all__ = ["B2Error", "Map", "RCCB200", "RCCB200Spherical", "RCCB200Pinhole", "RCCB200O1Dn", "RCCB200OnDn", "CPCB200", "SphereCorrectorB200",
-           "PinholeCorrectorB200", "O1DnCorrectorB200", "OnDnCorrectorB200", "PCDSensorUpdaterB200", "DistanceField", "PFParams", "GladiatorConfig", "SurfaceConfig", "KLDConfig", "ClusterConfig", "RecoveryConfig", "SteinConfig", "O1DnCloudFilter", "umeyama_transform", "micp_correct_once",
+           "PinholeCorrectorB200", "O1DnCorrectorB200", "OnDnCorrectorB200", "PCDSensorUpdaterB200", "DistanceField", "PFParams", "GladiatorConfig", "SurfaceConfig", "KLDConfig", "ClusterConfig", "RecoveryConfig", "SteinConfig", "SearchConfig", "O1DnCloudFilter", "umeyama_transform", "micp_correct_once",
            "micp_correct", "micp_pose_covariance", "MICP_STEP_DTYPE", "MICP_COVARIANCE_DTYPE", "read_mesh_file", "kernel_launch_count", "lib_path", "load_library", "synth"]

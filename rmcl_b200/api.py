@@ -11,7 +11,7 @@ import os
 import numpy as np
 
 from .synth import (CLUSTER_RECORD_DTYPE, CLUSTER_RESULT_DTYPE, CROSS_STATS_DTYPE, KLD_RESULT_DTYPE, PARTICLE_ATTR_DTYPE, PARTICLE_STATS_DTYPE, RANGE_MEAS_DTYPE,
-                    RECOVERY_RESULT_DTYPE, RECOVERY_STATE_DTYPE, RESIDUAL_RESULT_DTYPE, TRANSFORM_DTYPE)
+                    RECOVERY_RESULT_DTYPE, RECOVERY_STATE_DTYPE, RESIDUAL_RESULT_DTYPE, SEARCH_RECORD_DTYPE, TRANSFORM_DTYPE)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.environ.get("B2_LIB_PATH") or os.path.join(_HERE, "lib", "librmcl_b200.so")     # B2_LIB_PATH: experiment builds (scripts/)
@@ -116,6 +116,28 @@ class SteinConfig(C.Structure):
         return SteinConfig(10, 4096, 0.02, 0.01, 0.05, 0.02, 0.05, 0.0)
 
 
+class SearchConfig(C.Structure):
+    """b2_search_config: the grid of globalSearch, candidate (i, j, k) at (x0 + i * step, y0 + j * step, z0) with heading -pi + 2 pi k /
+    n_yaw (i < nx, j < ny), the number of records to return (1 .. 64) and the least distance (m) and heading difference (rad) a record
+    keeps from every better one unless it differs in the other.  defaults(bb_min, bb_max, z0) covers the (x, y) box from bb_min to bb_max
+    with the suggested values: step 0.25 m, 72 headings, 8 records, separations 1 m and 30 deg; without a box the grid is left empty."""
+    _fields_ = [("x0", C.c_float), ("y0", C.c_float), ("z0", C.c_float), ("step", C.c_float), ("nx", C.c_uint32), ("ny", C.c_uint32), ("n_yaw", C.c_uint32),
+                ("max_records", C.c_uint32), ("min_separation_xy", C.c_float), ("min_separation_yaw", C.c_float)]
+
+    @staticmethod
+    def defaults(bb_min=None, bb_max=None, z0=0.0, step=0.25):
+        cfg = SearchConfig(0.0, 0.0, float(z0), float(step), 0, 0, 72, 8, 1.0, math.radians(30.0))
+        if bb_min is not None and bb_max is not None:
+            cfg.x0, cfg.y0 = float(bb_min[0]), float(bb_min[1])
+            cfg.nx = int(math.floor((float(bb_max[0]) - float(bb_min[0])) / step)) + 1
+            cfg.ny = int(math.floor((float(bb_max[1]) - float(bb_min[1])) / step)) + 1
+        return cfg
+
+
+class _SearchResult(C.Structure):
+    _fields_ = [("n_candidates", C.c_uint64), ("n_valid", C.c_uint64), ("n_peaks", C.c_uint64), ("n_records", C.c_uint64)]
+
+
 class _SteinResult(C.Structure):
     _fields_ = [("bandwidth", C.c_float * 3), ("n_ref", C.c_uint32), ("n_blocked", C.c_uint32), ("rms_step_t", C.c_float), ("rms_step_r", C.c_float),
                 ("pad", C.c_float)]
@@ -195,7 +217,7 @@ EXPORTS = [
     "b2_pf_resample_kld", "b2_pf_cluster_stats", "b2_micp_pose_covariance", "b2_pf_recovery_reset", "b2_pf_recovery_observe",
     "b2_pf_recovery_inject", "b2_dfield_create", "b2_dfield_destroy", "b2_dfield_get_info", "b2_dfield_download", "b2_dfield_query",
     "b2_pf_sensor_update_field", "b2_pf_stein_update", "b2_pf_stein_slice_begin", "b2_pf_stein_slice_score", "b2_pf_stein_slice_move",
-    "b2_pf_stein_slice_result",
+    "b2_pf_stein_slice_result", "b2_pf_global_search",
 ]
 
 
@@ -1008,6 +1030,36 @@ class PCDSensorUpdaterB200:
                 self.steinScore, self.steinMove, self.steinResult, poses_local, dist, cfg.iterations, cfg.n_ref)
         finally:
             self.setStream(prev)
+
+    def globalSearch(self, field, Tsb, beams, config=None, surface=None, params: PFParams | None = None, scores=None):
+        """Where on the map does this scan fit best (b2_pf_global_search; SURVEY appendix M): every pose of `config`'s (x, y, yaw) grid (a
+        SearchConfig; default: SearchConfig.defaults() over the DistanceField `field`'s (x, y) box at z0 = 0) is scored as update() from the
+        field would score a particle there from {0, 0, 0}, the score array's local maxima are ranked, and those at least the config's
+        separations from a better one are kept.  `surface` (a SurfaceConfig) puts each candidate where projectToSurface would; one off the
+        surface scores -1.  `params`: the sensor model (default self.config).  `scores`: a float32 CUDA tensor of n_candidates elements that
+        receives every score in candidate order (x fastest, yaw slowest), the likelihood map.  Synchronises.  -> (result, records): a dict
+        (n_candidates, n_valid, n_peaks, n_records) and the kept peaks as a synth.SEARCH_RECORD_DTYPE array, records[0] the best."""
+        if not isinstance(field, DistanceField):
+            raise TypeError("expected a DistanceField")
+        cfg = config
+        if cfg is None:
+            inf = field.info()
+            hi = [inf["origin"][a] + (inf["dims"][a] - 1) * inf["resolution"] for a in range(2)]
+            cfg = SearchConfig.defaults(inf["origin"][:2], hi)
+        prm = params or self.config
+        pb, nb = _records(beams, 64, np.ascontiguousarray)
+        sp = None
+        if scores is not None:
+            sp, ns = _records(scores, 4)
+            want = int(cfg.nx) * int(cfg.ny) * int(cfg.n_yaw)
+            if ns != want:
+                raise ValueError(f"globalSearch: {want} candidates but {ns} scores")
+        recs = np.zeros(max(1, min(int(cfg.max_records), 64)), SEARCH_RECORD_DTYPE)
+        out = _SearchResult()
+        _chk(load_library().b2_pf_global_search(self._h, field._h, _p(_tf(Tsb)), pb if nb else None, C.c_uint32(nb), C.byref(prm), C.byref(cfg),
+                                                 None if surface is None else C.byref(surface), _p(recs), sp, C.byref(out)))
+        res = {k: int(getattr(out, k)) for k, _ in _SearchResult._fields_}
+        return res, recs[:res["n_records"]]
 
     def motionUpdate(self, particle_poses, particle_attrs, T_bnew_bold, forget_rate, check_collision=False):
         """TFMotionUpdaterGPU (rmcl_ros/src/rmcl/particle_motion.cu:11-46): in place on torch CUDA tensors.  check_collision adds the CPU

@@ -1952,6 +1952,7 @@ struct PfRecords {
     b2_recovery_result rec_res;                         // the result of an injection
     unsigned long long traffic;                         // remote bytes read by the p2p Gladiator kernel
     PfSteinState stein;                                 // the Stein step's result record and reduction tickets
+    PfSearchState search;                               // the global search's valid and peak counts
 };
 
 // The scratch below (partials, records, the resamplers' and the clusters' buffers) is shared by the entry points: a handle serves one call at
@@ -1996,6 +1997,10 @@ struct b2_pf {
     // floats per particle) and the block partials of the two grid reductions (one block per 256 particles of the whole set); the session
     DevBuf<SteinRef> d_stein_snap; DevBuf<PfBeam> d_stein_beams; DevBuf<float> d_stein_v; DevBuf<double> d_stein_part;
     PfSteinSession stein;
+    // global search (b2_pf_global_search), grown at its calls: the yaw table, the cells' surface probes, the scores (when the caller passes
+    // no array for them), the peaks' rank keys before and after the sort with the sort's temporary storage, the kept peaks and their records
+    DevBuf<float> d_search_yaw, d_search_scores; DevBuf<SearchCell> d_search_cells; DevBuf<unsigned long long> d_search_keys, d_search_keys2;
+    DevBuf<unsigned char> d_search_tmp; DevBuf<uint32_t> d_search_sel; DevBuf<b2_search_record> d_search_recs;
 };
 
 extern "C" int b2_pf_destroy(b2_pf* h);
@@ -2015,6 +2020,7 @@ static int pf_init(b2_pf* h)
     CU(cudaFuncSetAttribute(k_pf_update<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
     CU(cudaFuncSetAttribute(k_pf_update_field, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
     CU(cudaFuncSetAttribute(k_pf_stein_score, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
+    CU(cudaFuncSetAttribute(k_pf_search_score, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin - (int)B2_SEARCH_STATIC_SMEM));
     CU(cudaEventCreate(&h->ev_m0)); CU(cudaEventCreate(&h->ev_m1));
     { const char* e = getenv("B2_PF_MAP"); if (e) h->map_mode = std::min(3, std::max(0, atoi(e))); }
     return B2_OK;
@@ -2062,6 +2068,8 @@ extern "C" int b2_pf_destroy(b2_pf* h)
     h->d_cl_w.release(); h->d_cl_cnt.release(); h->d_cl_aux.release(); h->d_cl_slot.release(); h->d_cl_key.release(); h->d_cl_key2.release(); h->d_cl_idx.release();
     h->d_cl_idx2.release(); h->d_cl_poses.release(); h->d_cl_attrs.release();
     h->d_stein_snap.release(); h->d_stein_beams.release(); h->d_stein_v.release(); h->d_stein_part.release();
+    h->d_search_yaw.release(); h->d_search_scores.release(); h->d_search_cells.release(); h->d_search_keys.release(); h->d_search_keys2.release();
+    h->d_search_tmp.release(); h->d_search_sel.release(); h->d_search_recs.release();
     b2_mesh* map = h->map;
     delete h;
     (void)cudaGetLastError();
@@ -2582,6 +2590,113 @@ extern "C" int b2_pf_stein_update(b2_pf* h, const b2_dfield* f, b2_transform* po
         out_host->rms_step_t = r.n_steps ? (float)std::sqrt(r.sum_step_t2 / (double)r.n_steps) : 0.0f;
         out_host->rms_step_r = r.n_steps ? (float)std::sqrt(r.sum_step_r2 / (double)r.n_steps) : 0.0f;
     }
+    return B2_OK;
+}
+
+// Global search (kernels.cuh, SURVEY appendix M): the cells' surface probes, the scores, one pass for the peaks, the radix sort of their rank
+// keys, then the separation pass on the host over as many sorted keys as it needs (read back in chunks), and the kept peaks' records.
+static int surface_config_check(const b2_surface_config& c, const char* what, float* cos_max, float* tfar);
+extern "C" int b2_pf_global_search(b2_pf* h, const b2_dfield* f, const b2_transform* Tsb, const b2_range_meas* beams, uint32_t n_beams,
+                                   const b2_pf_params* prm, const b2_search_config* cfg, const b2_surface_config* surface,
+                                   b2_search_record* records_host, float* scores_dev, b2_search_result* out_host)
+{
+    // the arguments are checked before the handle: the checks need no device
+    NOTNULL(Tsb); NOTNULL(prm); NOTNULL(cfg); NOTNULL(records_host); NOTNULL(out_host);
+    if (n_beams) NOTNULL(beams);
+    const b2_search_config c = *cfg;
+    if (c.nx == 0 || c.ny == 0 || c.n_yaw == 0 || c.n_yaw > B2_SEARCH_MAX_YAW)
+        return fail(B2_ERR_INVALID, "global search: grid %u x %u x %u (each >= 1, n_yaw <= %u)", c.nx, c.ny, c.n_yaw, B2_SEARCH_MAX_YAW);
+    const uint64_t n_cand = (uint64_t)c.nx * c.ny * c.n_yaw;
+    if (n_cand > B2_SEARCH_MAX_CANDIDATES)
+        return fail(B2_ERR_INVALID, "global search: %llu candidates, at most 2^30", (unsigned long long)n_cand);
+    if (!(std::isfinite(c.step) && c.step > 0.0f)) return fail(B2_ERR_INVALID, "global search: step = %g must be finite and > 0", (double)c.step);
+    const float x1 = search_coord(c.x0, c.nx - 1, c.step), y1 = search_coord(c.y0, c.ny - 1, c.step);
+    if (!(std::isfinite(c.x0) && std::isfinite(c.y0) && std::isfinite(c.z0) && std::isfinite(x1) && std::isfinite(y1)))
+        return fail(B2_ERR_INVALID, "global search: the grid from (%g, %g, %g) to (%g, %g) is not finite", (double)c.x0, (double)c.y0, (double)c.z0, (double)x1, (double)y1);
+    if (c.max_records < 1 || c.max_records > B2_SEARCH_MAX_RECORDS)
+        return fail(B2_ERR_INVALID, "global search: max_records = %u must lie in [1, %u]", c.max_records, B2_SEARCH_MAX_RECORDS);
+    if (!(std::isfinite(c.min_separation_xy) && c.min_separation_xy >= 0.0f && std::isfinite(c.min_separation_yaw) && c.min_separation_yaw >= 0.0f))
+        return fail(B2_ERR_INVALID, "global search: separations (%g, %g) must be finite and >= 0", (double)c.min_separation_xy, (double)c.min_separation_yaw);
+    const float sq = prm->dist_sigma * prm->dist_sigma;
+    if (!(std::isfinite(prm->dist_sigma) && prm->dist_sigma > 0.0f && std::isfinite(sq) && sq > 0.0f))
+        return fail(B2_ERR_INVALID, "global search: dist_sigma = %g must be finite and > 0, and so must its square", (double)prm->dist_sigma);
+    b2_surface_config sc{};
+    float cos_max = 0.0f, tfar = 0.0f;
+    if (surface) { sc = *surface; RES(surface_config_check(sc, "global search", &cos_max, &tfar)); }
+    NOTNULL(f); NOTNULL(h);
+    if (f->map->device != h->map->device) return fail(B2_ERR_INVALID, "global search: the field is on device %d, the handle on device %d", f->map->device, h->map->device);
+    const size_t smem_max = (size_t)h->smem_optin - B2_SEARCH_STATIC_SMEM;
+    if (sizeof(float) * (size_t)n_beams > smem_max) return fail(B2_ERR_UNSUPPORTED, "global search: too many beams (%u)", n_beams);
+    CU(cudaSetDevice(h->map->device));
+    const uint32_t n = (uint32_t)n_cand, K = c.n_yaw, n_cells = c.nx * c.ny;
+    uint32_t ppb = B2_PF_BLOCK;
+    if (n_beams) {
+        RES(pf_prepare_beams(h, beams, n_beams, &ppb));
+        ppb = std::max<uint32_t>(1u, std::min<uint32_t>(ppb, (uint32_t)(smem_max / (sizeof(float) * (size_t)n_beams))));
+    }
+    // buffers: the yaw table, the scores unless the caller's array takes them, the cells with surface, the peaks (at most one per 2 x 2 x 2
+    // block of the grid: two neighbours are never both peaks)
+    const uint64_t cap = (uint64_t)((c.nx + 1) / 2) * ((c.ny + 1) / 2) * ((K + 1) / 2);
+    size_t sort_bytes = 0;
+    CU(cub::DeviceRadixSort::SortKeys(nullptr, sort_bytes, h->d_search_keys.p, h->d_search_keys2.p, (int)cap, 0, 64, h->stream));
+    RES(h->d_search_yaw.reserve(2 * (size_t)K));
+    if (!scores_dev) RES(h->d_search_scores.reserve(n));
+    if (surface) RES(h->d_search_cells.reserve(n_cells));
+    RES(h->d_search_keys.reserve(cap)); RES(h->d_search_keys2.reserve(cap)); RES(h->d_search_tmp.reserve(std::max<size_t>(sort_bytes, 16)));
+    RES(h->d_search_sel.reserve(B2_SEARCH_MAX_RECORDS)); RES(h->d_search_recs.reserve(B2_SEARCH_MAX_RECORDS));
+    float* scores = scores_dev ? scores_dev : h->d_search_scores.p;
+    std::vector<float> yaw(2 * (size_t)K);
+    for (uint32_t k = 0; k < K; k++) {
+        const double half = 0.5 * search_psi(k, K);
+        yaw[2 * k] = (float)std::sin(half); yaw[2 * k + 1] = (float)std::cos(half);
+    }
+    CU(cudaMemcpyAsync(h->d_search_yaw.p, yaw.data(), sizeof(float) * 2 * (size_t)K, cudaMemcpyHostToDevice, h->stream));
+    const SearchGrid g{c.x0, c.y0, c.z0, c.step, c.nx, c.ny, K, h->d_search_yaw.p};
+    if (surface) {
+        k_pf_search_cells<<<dfield_grid(h->n_sm, n_cells), 256, 0, h->stream>>>(h->map->view(), g, sc, cos_max, tfar, h->d_search_cells.p);
+        LAUNCHED();
+    }
+    k_pf_search_score<<<(n + ppb - 1) / ppb, B2_PF_BLOCK, sizeof(float) * (size_t)n_beams * ppb, h->stream>>>(
+        f->v, g, surface ? h->d_search_cells.p : nullptr, sc, n, *Tsb, h->d_beams.p, n_beams, *prm, ppb, scores);
+    LAUNCHED();
+    PfRecords* d = h->d_recs.p;
+    const PfRecords& hr = *h->h_recs;
+    CU(cudaMemsetAsync(&d->search, 0, sizeof(PfSearchState), h->stream));
+    k_pf_search_peaks<<<dfield_grid(h->n_sm, n), 256, 0, h->stream>>>(scores, c.nx, c.ny, K, n, h->d_search_keys.p, cap, &d->search);
+    LAUNCHED();
+    RES(pf_fetch(h, hr.search));
+    const uint64_t n_peaks = hr.search.n_peaks;
+    if (n_peaks > cap) return fail(B2_ERR_CUDA, "global search: %llu peaks, more than the %llu a grid of this size can hold", (unsigned long long)n_peaks, (unsigned long long)cap);
+    b2_search_result res = {n_cand, hr.search.n_valid, n_peaks, 0};
+    const unsigned long long* sorted = h->d_search_keys.p;
+    if (n_peaks > 1) {
+        CU(cub::DeviceRadixSort::SortKeys(h->d_search_tmp.p, sort_bytes, h->d_search_keys.p, h->d_search_keys2.p, (int)n_peaks, 0, 64, h->stream));
+        LAUNCHED();
+        sorted = h->d_search_keys2.p;
+    }
+    // the separation pass: keys read back in chunks that double, until max_records peaks are kept or none is left
+    uint32_t kept[B2_SEARCH_MAX_RECORDS], n_kept = 0;
+    std::vector<unsigned long long> chunk;
+    for (uint64_t at = 0, len = 1024; at < n_peaks && n_kept < c.max_records; at += len, len *= 2) {
+        const uint64_t m = std::min<uint64_t>(len, n_peaks - at);
+        chunk.resize(m);
+        CU(cudaMemcpyAsync(chunk.data(), sorted + at, sizeof(unsigned long long) * m, cudaMemcpyDeviceToHost, h->stream));
+        CU(cudaStreamSynchronize(h->stream));
+        for (uint64_t q = 0; q < m && n_kept < c.max_records; q++) {
+            const uint32_t cc = (uint32_t)chunk[q];
+            if (search_keep(g, cc, kept, n_kept, (double)c.min_separation_xy, (double)c.min_separation_yaw)) kept[n_kept++] = cc;
+        }
+    }
+    res.n_records = n_kept;
+    if (n_kept) {
+        CU(cudaMemcpyAsync(h->d_search_sel.p, kept, sizeof(uint32_t) * n_kept, cudaMemcpyHostToDevice, h->stream));
+        k_pf_search_records<<<1, B2_SEARCH_MAX_RECORDS, 0, h->stream>>>(g, surface ? h->d_search_cells.p : nullptr, sc, h->d_search_sel.p, n_kept, scores,
+                                                                       h->d_search_recs.p);
+        LAUNCHED();
+        CU(cudaMemcpyAsync(records_host, h->d_search_recs.p, sizeof(b2_search_record) * n_kept, cudaMemcpyDeviceToHost, h->stream));
+    }
+    CU(cudaStreamSynchronize(h->stream));
+    *out_host = res;
     return B2_OK;
 }
 

@@ -1452,7 +1452,9 @@ __global__ void __launch_bounds__(128) k_pf_motion(BvhView bvh, b2_transform* __
 // the smallest rotation also takes the body z-axis onto n); else it keeps its pose and gets the wall check's mark {0, 0, MAX_N_MEAS}.
 // The stamp and the rest of the attributes are left as they are.  cos_max = (float)cos((double)max_slope), tfar = probe_above + probe_below.
 // pf_surface_pose applies the rule to a pose in registers and reports the ground test; pf_surface_one applies it to a particle in memory.
-B2_DEV bool pf_surface_pose(const BvhView& bvh, Tf& T, const b2_surface_config& cfg, float cos_max, float tfar)
+// The rule is two steps: pf_surface_probe finds the ground point g and its upward normal n (it reads R only to test it for finiteness), and
+// pf_surface_place moves the pose onto them; the global search probes once per cell and places every heading of it.
+B2_DEV bool pf_surface_probe(const BvhView& bvh, const Tf& T, const b2_surface_config& cfg, float cos_max, float tfar, V3& g, V3& n)
 {
     const float oz = add(T.t.z, cfg.probe_above);
     HitRec h = trace_init(tfar);
@@ -1465,13 +1467,17 @@ B2_DEV bool pf_surface_pose(const BvhView& bvh, Tf& T, const b2_surface_config& 
         uint32_t nn = 0, nt = 0;
         trace_closest<false>(bvh, r, h, nn, nt);
     }
-    V3 n = mk3(0.0f, 0.0f, 0.0f);
+    n = mk3(0.0f, 0.0f, 0.0f);
     if (h.face != B2_NOFACE) {
         n = v_normalize(tri_ng(bvh, h.tri));
         if (n.z < 0.0f) n = v_neg(n);
     }
     if (!(h.face != B2_NOFACE && n.z >= cos_max)) return false;                       // no hit, too steep, or a NaN normal
-    const V3 g = mk3(T.t.x, T.t.y, sub(oz, h.t));
+    g = mk3(T.t.x, T.t.y, sub(oz, h.t));
+    return true;
+}
+B2_DEV Tf pf_surface_place(const Tf& T, V3 g, V3 n, const b2_surface_config& cfg)
+{
     Tf out;
     if (cfg.align) {
         const V3 a = q_rot(T.R, mk3(0.0f, 0.0f, 1.0f));
@@ -1489,7 +1495,13 @@ B2_DEV bool pf_surface_pose(const BvhView& bvh, Tf& T, const b2_surface_config& 
         out.R = T.R;
         out.t = mk3(g.x, g.y, add(g.z, cfg.base_height));
     }
-    T = out;
+    return out;
+}
+B2_DEV bool pf_surface_pose(const BvhView& bvh, Tf& T, const b2_surface_config& cfg, float cos_max, float tfar)
+{
+    V3 g, n;
+    if (!pf_surface_probe(bvh, T, cfg, cos_max, tfar, g, n)) return false;
+    T = pf_surface_place(T, g, n, cfg);
     return true;
 }
 // true iff the particle stood on ground and was moved; else it is marked
@@ -3081,6 +3093,175 @@ __global__ void __launch_bounds__(B2_STEIN_BLOCK) k_pf_stein_move(BvhView bvh, c
     st->rec.sum_step_t2 = tot[1];
     st->rec.sum_step_r2 = tot[2];
     st->ticket[1] = 0u;
+}
+#endif
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Global search (b2_pf_global_search; SURVEY appendix M): every candidate pose of an (x, y, yaw) grid scored as b2_pf_sensor_update_field
+// scores a particle, the peaks of the score array, their ranking and the separation pass.
+// ---------------------------------------------------------------------------------------------------------------------
+#define B2_SEARCH_MAX_YAW 32768u
+#define B2_SEARCH_MAX_RECORDS 64u
+#define B2_SEARCH_MAX_CANDIDATES (1u << 30)
+#define B2_SEARCH_PI 3.14159265358979323846
+#define B2_SEARCH_STATIC_SMEM 3072u      // k_pf_search_score's static shared memory (3712 B) beyond the 1 KiB the handle keeps free, rounded up
+// the grid; yaw: K entries (sin, cos) of psi_k / 2 from the host's FP64 libm, rounded to float, so that every candidate's R has the host's bits
+struct SearchGrid { float x0, y0, z0, step; uint32_t nx, ny, K; const float* yaw; };
+// one (i, j) cell's surface probe: the ground point g and its normal n, valid 0 where the rule finds no ground (32 B)
+struct SearchCell { float gx, gy, gz, valid, nx, ny, nz, pad; };
+struct PfSearchState { unsigned long long n_valid, n_peaks; };
+
+B2_DEV float search_coord(float o, uint32_t i, float step) { return add(o, mul((float)i, step)); }
+// psi_k = -pi + 2 pi k / K in double (the host's; the separation pass compares these)
+inline double search_psi(uint32_t k, uint32_t K) { return -B2_SEARCH_PI + 2.0 * B2_SEARCH_PI * (double)k / (double)K; }
+// candidate c's pose before the surface rule
+B2_DEV Tf search_pose(const SearchGrid& g, uint32_t c)
+{
+    const uint32_t i = c % g.nx, j = c / g.nx % g.ny, k = c / g.nx / g.ny;
+    Tf T;
+    T.R.x = 0.0f; T.R.y = 0.0f; T.R.z = ldg(g.yaw + 2 * k); T.R.w = ldg(g.yaw + 2 * k + 1);
+    T.t = mk3(search_coord(g.x0, i, g.step), search_coord(g.y0, j, g.step), g.z0);
+    return T;
+}
+// The surface rule's probe reads only t, so it runs once per cell (at R = identity; R is only tested for finiteness) and every heading is
+// placed on its result: the same bits as pf_surface_pose on each candidate.  The placement stays per candidate: with align 1 it rotates
+// a = R e_z onto n, and a is e_z only up to the rounding of sin^2 + cos^2 and the signs of zeros, which differ between headings.
+B2_DEV SearchCell search_cell(const BvhView& bvh, const SearchGrid& g, uint32_t cell, const b2_surface_config& cfg, float cos_max, float tfar)
+{
+    Tf T = tf_identity();
+    T.t = mk3(search_coord(g.x0, cell % g.nx, g.step), search_coord(g.y0, cell / g.nx, g.step), g.z0);
+    V3 p, n;
+    SearchCell s;
+    const bool ok = pf_surface_probe(bvh, T, cfg, cos_max, tfar, p, n);
+    s.gx = p.x; s.gy = p.y; s.gz = p.z; s.valid = ok ? 1.0f : 0.0f; s.nx = n.x; s.ny = n.y; s.nz = n.z; s.pad = 0.0f;
+    if (!ok) { s.gx = s.gy = s.gz = 0.0f; }
+    return s;
+}
+// candidate c's pose with the surface rule applied (cells nullable: no surface); false: off surface
+B2_DEV bool search_candidate(const SearchGrid& g, const SearchCell* cells, const b2_surface_config& cfg, uint32_t c, Tf& T)
+{
+    T = search_pose(g, c);
+    if (!cells) return true;
+    const SearchCell s = cells[c % (g.nx * g.ny)];
+    if (s.valid == 0.0f) return false;
+    T = pf_surface_place(T, mk3(s.gx, s.gy, s.gz), mk3(s.nx, s.ny, s.nz), cfg);
+    return true;
+}
+// the peak rule at candidate c of the score array s (SURVEY M3): valid, and ahead of every valid neighbour in (score descending, c ascending)
+B2_DEV bool search_is_peak(const float* s, uint32_t nx, uint32_t ny, uint32_t K, uint32_t c)
+{
+    const float sc = ldg(s + c);
+    if (!(sc >= 0.0f)) return false;
+    const uint32_t i = c % nx, j = c / nx % ny, k = c / nx / ny;
+    for (int dk = -1; dk <= 1; dk++) {
+        const uint32_t kk = (uint32_t)(((int64_t)k + dk + K) % K);
+        for (int dj = -1; dj <= 1; dj++) {
+            const int64_t jj = (int64_t)j + dj;
+            if (jj < 0 || jj >= (int64_t)ny) continue;
+            for (int di = -1; di <= 1; di++) {
+                const int64_t ii = (int64_t)i + di;
+                if (ii < 0 || ii >= (int64_t)nx) continue;
+                const uint32_t n = (kk * ny + (uint32_t)jj) * nx + (uint32_t)ii;
+                if (n == c) continue;
+                const float sn = ldg(s + n);
+                if (!(sn >= 0.0f)) continue;
+                if (!(sn < sc || (sn == sc && n > c))) return false;
+            }
+        }
+    }
+    return true;
+}
+// rank key: ascending order of keys = score descending (scores >= 0, so their bits order them), then c ascending
+B2_DEV unsigned long long search_key(float score, uint32_t c) { return ((unsigned long long)~f2u(score) << 32) | c; }
+// the separation pass's test of peak c against the kept ones: true iff no kept peak lies both within sep_xy (the grid positions' distance)
+// and within sep_yaw (the wrapped psi difference), strictly, in double
+inline bool search_keep(const SearchGrid& g, uint32_t c, const uint32_t* kept, uint32_t n_kept, double sep_xy, double sep_yaw)
+{
+    const uint32_t i = c % g.nx, j = c / g.nx % g.ny, k = c / g.nx / g.ny;
+    const double x = search_coord(g.x0, i, g.step), y = search_coord(g.y0, j, g.step), psi = search_psi(k, g.K);
+    for (uint32_t r = 0; r < n_kept; r++) {
+        const uint32_t q = kept[r], qi = q % g.nx, qj = q / g.nx % g.ny, qk = q / g.nx / g.ny;
+        const double dx = x - (double)search_coord(g.x0, qi, g.step), dy = y - (double)search_coord(g.y0, qj, g.step);
+        double dpsi = std::fabs(psi - search_psi(qk, g.K));
+        if (2.0 * B2_SEARCH_PI - dpsi < dpsi) dpsi = 2.0 * B2_SEARCH_PI - dpsi;
+        if (std::sqrt(dx * dx + dy * dy) < sep_xy && dpsi < sep_yaw) return false;
+    }
+    return true;
+}
+
+#ifdef __CUDACC__
+__global__ void __launch_bounds__(256) k_pf_search_cells(BvhView bvh, SearchGrid g, b2_surface_config cfg, float cos_max, float tfar, SearchCell* __restrict__ cells)
+{
+    const uint32_t n = g.nx * g.ny;
+    for (uint32_t c = blockIdx.x * blockDim.x + threadIdx.x; c < n; c += gridDim.x * blockDim.x) cells[c] = search_cell(bvh, g, c, cfg, cos_max, tfar);
+}
+// k_pf_update_field's layout over candidates: a block of ppb candidates, their poses (times Tsb) in shared memory, lanes over the beams of
+// one candidate, each evaluation at its beam's slot, then one thread per candidate merging from {0, 0, 0} in slot order
+__global__ void __launch_bounds__(B2_PF_BLOCK) k_pf_search_score(DfieldView f, SearchGrid g, const SearchCell* __restrict__ cells, b2_surface_config cfg,
+                                                              uint32_t n, b2_transform Tsb_val, const PfBeam* __restrict__ beams, uint32_t n_beams,
+                                                              b2_pf_params prm, uint32_t ppb, float* __restrict__ scores)
+{
+    extern __shared__ float s_eval[];            // [ppb][n_beams]
+    __shared__ Tf s_T[B2_PF_BLOCK];
+    __shared__ bool s_ok[B2_PF_BLOCK];
+    const uint32_t c0 = blockIdx.x * ppb, nc = min(ppb, n - c0);
+    if (threadIdx.x < nc) {
+        Tf T;
+        s_ok[threadIdx.x] = search_candidate(g, cells, cfg, c0 + threadIdx.x, T);
+        s_T[threadIdx.x] = tf_mul(T, tf_from_pod(Tsb_val));
+    }
+    __syncthreads();
+    float sigma_quad; double denom; pf_constants(prm, sigma_quad, denom);
+    const uint32_t total = nc * n_beams;
+    for (uint32_t w = threadIdx.x; w < total; w += blockDim.x) {
+        const uint32_t cl = w / n_beams, bi = w % n_beams;
+        if (!s_ok[cl]) continue;
+        const PfBeam b = beams[bi];
+        s_eval[cl * n_beams + b.slot] = pf_eval_field(f, s_T[cl], b, sigma_quad, denom);
+    }
+    __syncthreads();
+    if (threadIdx.x < nc) {
+        float s = -1.0f;
+        if (s_ok[threadIdx.x]) {
+            b2_gaussian1d lk; lk.mean = 0.0f; lk.sigma = 0.0f; lk.n_meas = 0u;
+            pf_merge(lk, s_eval + threadIdx.x * n_beams, n_beams);
+            s = lk.mean;
+        }
+        scores[c0 + threadIdx.x] = s;
+    }
+}
+// one pass over the score array: counts the valid candidates and appends every peak's rank key (at most cap; n_peaks counts them all)
+__global__ void __launch_bounds__(256) k_pf_search_peaks(const float* __restrict__ s, uint32_t nx, uint32_t ny, uint32_t K, uint32_t n,
+                                                         unsigned long long* __restrict__ keys, uint64_t cap, PfSearchState* __restrict__ st)
+{
+    for (uint32_t base = blockIdx.x * blockDim.x; base < n; base += gridDim.x * blockDim.x) {
+        const uint32_t c = base + threadIdx.x;
+        const bool valid = c < n && s[c] >= 0.0f;
+        const bool peak = valid && search_is_peak(s, nx, ny, K, c);
+        const uint32_t nv = __popc(__ballot_sync(0xffffffffu, valid)), pm = __ballot_sync(0xffffffffu, peak);
+        const uint32_t lane = threadIdx.x & 31u;
+        unsigned long long at = 0;
+        if (lane == 0) {
+            if (nv) atomicAdd(&st->n_valid, (unsigned long long)nv);
+            if (pm) at = atomicAdd(&st->n_peaks, (unsigned long long)__popc(pm));
+        }
+        at = __shfl_sync(0xffffffffu, at, 0) + __popc(pm & ((1u << lane) - 1u));
+        if (peak && at < cap) keys[at] = search_key(s[c], c);
+    }
+}
+// the records of the kept peaks, rank order
+__global__ void k_pf_search_records(SearchGrid g, const SearchCell* __restrict__ cells, b2_surface_config cfg, const uint32_t* __restrict__ sel, uint32_t m,
+                                    const float* __restrict__ scores, b2_search_record* __restrict__ out)
+{
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= m) return;
+    const uint32_t c = sel[r];
+    Tf T;
+    search_candidate(g, cells, cfg, c, T);
+    b2_search_record o;
+    o.pose.R.x = T.R.x; o.pose.R.y = T.R.y; o.pose.R.z = T.R.z; o.pose.R.w = T.R.w; o.pose.t.x = T.t.x; o.pose.t.y = T.t.y; o.pose.t.z = T.t.z; o.pose.stamp = 0u;
+    o.score = scores[c]; o.i = c % g.nx; o.j = c / g.nx % g.ny; o.k = c / g.nx / g.ny;
+    out[r] = o;
 }
 #endif
 

@@ -382,6 +382,9 @@ assert CLUSTER_RECORD_DTYPE.itemsize == 472
 CLUSTER_RESULT_DTYPE = np.dtype([("n_clusters", np.uint64), ("n_records", np.uint64), ("bins", np.uint64), ("n_clustered", np.uint64), ("weight_total", np.uint64),
                                  ("rounds", np.uint64), ("weight_sum", np.float64), ("weight_max", np.float64)])
 assert CLUSTER_RESULT_DTYPE.itemsize == 64
+# b2_search_record: what PCDSensorUpdaterB200.globalSearch returns per kept peak
+SEARCH_RECORD_DTYPE = np.dtype([("pose", TRANSFORM_DTYPE), ("score", np.float32), ("i", np.uint32), ("j", np.uint32), ("k", np.uint32)])
+assert SEARCH_RECORD_DTYPE.itemsize == 48
 
 
 def quat_from_rpy(roll, pitch, yaw):
