@@ -750,6 +750,44 @@ B2_API int b2_pf_global_search(b2_pf* h, const b2_dfield* f, const b2_transform*
                                b2_search_record* records_host, float* scores_dev /* nullable: n_candidates floats in c order */,
                                b2_search_result* out_host);
 
+/* b2_pf_global_search_bnb: b2_pf_global_search's records on grids too large or too fine to score exhaustively.  An exact branch and bound
+ * (Olson 2009's multi-resolution search; Hess et al. 2016's over a grid pyramid) over a quadtree of (i, j) per heading, each node bounded
+ * from a min-pooled pyramid of the field built at the call (SURVEY appendix N).
+ *  - Candidates, scores, surface rule, peaks, ranking, separation and records: appendix M's for the same cfg, with a 64-bit c = (k * ny + j)
+ *    * nx + i; nx and ny up to 2^24, n_yaw up to 32768, no cap on the number of candidates.
+ *  - records_host[r], r < n_records: the records of b2_pf_global_search whose score is >= tau = mul(min_ratio, s*), s* the best score of
+ *    the grid, in the same order, byte for byte (a prefix of them).  min_ratio 0 gives exactly b2_pf_global_search's records wherever that
+ *    call accepts the grid; min_ratio 1 only the records that share the best score.
+ *  - out_host: the counts of the search (nodes bounded per pass and per level, leaves scored, the last pass's peaks), s*, tau, the passes and
+ *    the tree depth.  A pruned search does not know n_valid or the number of peaks of the whole grid.
+ * Runs on the handle's stream and synchronises it; the particle set, the ray-mapping timers and the recovery record are untouched.
+ * Scratch (the handle's): the pyramid (288 B per allocated brick of the field, about 4.6 B per brick), the nodes of the tree pending at
+ * once, and about 29 B per candidate with score >= the last pass's threshold.  The passes stop once max_records peaks are kept or the
+ * threshold reaches tau, so with min_ratio 0 the last pass runs at threshold 0, bounds prune nothing and that set is every valid candidate,
+ * whenever the grid has fewer than max_records separated peaks above the earlier thresholds (a small map with max_records 64 and 1 m /
+ * 30 deg separations; flat scores from few beams or a scan that fits nowhere).  The call then costs what b2_pf_global_search costs, and a
+ * large grid fails with B2_ERR_OOM, or with B2_ERR_UNSUPPORTED above 2^31 - 1 such candidates; a min_ratio > 0 avoids it.  Failures
+ * (B2_ERR_OOM, B2_ERR_UNSUPPORTED, B2_ERR_CUDA) write nothing to records_host or out_host.
+ * Refused (B2_ERR_INVALID, no launch, nothing written): b2_pf_global_search's refusals, with nx or ny 0 or > 2^24 and n_yaw 0 or > 32768 for
+ * the grid and no limit on the product; min_ratio outside [0, 1] or NaN. */
+typedef struct {
+    uint64_t n_candidates;                    /* nx * ny * n_yaw */
+    uint64_t n_bounded;                       /* nodes bounded (levels >= 1), all passes */
+    uint64_t n_leaves;                        /* candidates scored exactly, all passes */
+    uint64_t n_peaks;                         /* peaks with score >= the last pass's threshold */
+    uint64_t n_records;
+    uint64_t n_bounded_pass[16];              /* nodes bounded in pass p (levels >= 1) */
+    uint64_t n_level[25];                     /* nodes of tree level l bounded (l >= 1) or scored (l = 0), all passes */
+    float best_score;                         /* s*; -1 when no candidate is valid */
+    float threshold;                          /* tau = mul(min_ratio, s*); -1 when no candidate is valid */
+    uint32_t n_passes;                        /* threshold passes run, <= 16 */
+    uint32_t depth;                           /* levels above the candidates: ceil(log2(max(nx, ny))) */
+} b2_search_bnb_result;                                                                                                   /* 384 B */
+typedef char b2_search_bnb_result_is_384_bytes[sizeof(b2_search_bnb_result) == 384 ? 1 : -1];
+B2_API int b2_pf_global_search_bnb(b2_pf* h, const b2_dfield* f, const b2_transform* Tsb, const b2_range_meas* beams_host, uint32_t n_beams,
+                                   const b2_pf_params* params, const b2_search_config* cfg, const b2_surface_config* surface /* nullable */,
+                                   float min_ratio, b2_search_record* records_host, b2_search_bnb_result* out_host);
+
 /* ---------------------------------------------------------------- introspection ------------------------------ */
 /* CUDA-event timing of the kernels inside b2_rcc_correct_once*(): when enabled, events are recorded on the handle's stream around the
  * find kernel and around the reduction/Umeyama kernels; b2_rcc_last_timing returns the two durations of the most recent call (ms). */

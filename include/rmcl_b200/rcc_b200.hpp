@@ -476,6 +476,20 @@ public:
         if (result) *result = r;
         return recs;
     }
+    // globalSearch's records on grids too large or too fine to score exhaustively (b2_pf_global_search_bnb; SURVEY appendix N): an exact
+    // branch and bound over a min-pooled pyramid of the field.  Returns globalSearch's records whose score is >= min_ratio times the best,
+    // in the same order (min_ratio 0: all of them); result (may be null) receives the search's counts.  Synchronises.
+    std::vector<b2_search_record> globalSearchBnB(const B200DistanceField& field, const b2_range_meas* beams, uint32_t n_beams, const b2_search_config& cfg,
+                                                  const b2_surface_config* surface = nullptr, float min_ratio = 0.0f, b2_search_bnb_result* result = nullptr)
+    {
+        std::vector<b2_search_record> recs(cfg.max_records >= 1 && cfg.max_records <= 64 ? cfg.max_records : 1);
+        b2_search_bnb_result r{};
+        b2_check(b2_pf_global_search_bnb(h_, field.handle(), reinterpret_cast<const b2_transform*>(&Tsb_), beams, n_beams, &config, &cfg, surface, min_ratio,
+                                         recs.data(), &r), "globalSearchBnB");
+        recs.resize(r.n_records);
+        if (result) *result = r;
+        return recs;
+    }
     // Stein variational steps toward the beams' likelihood over the field of setDistanceField (b2_pf_stein_update; SURVEY appendix L): in
     // place on the device poses, on the handle's stream; x, y and yaw move, z, roll, pitch and the attributes stay.  Throws without a field.
     // Returns the result record (a 32-byte read-back and a synchronise).  stein_config() gives the suggested values.

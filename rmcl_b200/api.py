@@ -11,7 +11,7 @@ import os
 import numpy as np
 
 from .synth import (CLUSTER_RECORD_DTYPE, CLUSTER_RESULT_DTYPE, CROSS_STATS_DTYPE, KLD_RESULT_DTYPE, PARTICLE_ATTR_DTYPE, PARTICLE_STATS_DTYPE, RANGE_MEAS_DTYPE,
-                    RECOVERY_RESULT_DTYPE, RECOVERY_STATE_DTYPE, RESIDUAL_RESULT_DTYPE, SEARCH_RECORD_DTYPE, TRANSFORM_DTYPE)
+                    RECOVERY_RESULT_DTYPE, RECOVERY_STATE_DTYPE, RESIDUAL_RESULT_DTYPE, SEARCH_BNB_RESULT_DTYPE, SEARCH_RECORD_DTYPE, TRANSFORM_DTYPE)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.environ.get("B2_LIB_PATH") or os.path.join(_HERE, "lib", "librmcl_b200.so")     # B2_LIB_PATH: experiment builds (scripts/)
@@ -217,7 +217,7 @@ EXPORTS = [
     "b2_pf_resample_kld", "b2_pf_cluster_stats", "b2_micp_pose_covariance", "b2_pf_recovery_reset", "b2_pf_recovery_observe",
     "b2_pf_recovery_inject", "b2_dfield_create", "b2_dfield_destroy", "b2_dfield_get_info", "b2_dfield_download", "b2_dfield_query",
     "b2_pf_sensor_update_field", "b2_pf_stein_update", "b2_pf_stein_slice_begin", "b2_pf_stein_slice_score", "b2_pf_stein_slice_move",
-    "b2_pf_stein_slice_result", "b2_pf_global_search",
+    "b2_pf_stein_slice_result", "b2_pf_global_search", "b2_pf_global_search_bnb",
 ]
 
 
@@ -1059,6 +1059,32 @@ class PCDSensorUpdaterB200:
         _chk(load_library().b2_pf_global_search(self._h, field._h, _p(_tf(Tsb)), pb if nb else None, C.c_uint32(nb), C.byref(prm), C.byref(cfg),
                                                  None if surface is None else C.byref(surface), _p(recs), sp, C.byref(out)))
         res = {k: int(getattr(out, k)) for k, _ in _SearchResult._fields_}
+        return res, recs[:res["n_records"]]
+
+    def globalSearchBnB(self, field, Tsb, beams, config=None, surface=None, params: PFParams | None = None, min_ratio=0.0):
+        """globalSearch's records on grids too large or too fine to score exhaustively (b2_pf_global_search_bnb; SURVEY appendix N): an exact
+        branch and bound over a quadtree per heading, bounded from a min-pooled pyramid of the field.  `field`, `Tsb`, `beams`, `config`,
+        `surface` and `params` as for globalSearch; the grid may hold more than 2^30 candidates (nx, ny up to 2^24).  The records are
+        globalSearch's records whose score is >= tau = min_ratio * s* (s* the best score of the grid), in the same order, byte for byte:
+        min_ratio 0 gives all of them, 1 those that share the best score.  Synchronises.  -> (result, records): a dict (n_candidates,
+        n_bounded, n_leaves, n_peaks, n_records, n_bounded_pass (one per pass), n_level (per tree level, 0 = leaves scored), best_score,
+        threshold, n_passes, depth; the fields of synth.SEARCH_BNB_RESULT_DTYPE, n_bounded_pass cut to n_passes) and the records as a
+        synth.SEARCH_RECORD_DTYPE array, records[0] the best."""
+        if not isinstance(field, DistanceField):
+            raise TypeError("expected a DistanceField")
+        cfg = config
+        if cfg is None:
+            inf = field.info()
+            hi = [inf["origin"][a] + (inf["dims"][a] - 1) * inf["resolution"] for a in range(2)]
+            cfg = SearchConfig.defaults(inf["origin"][:2], hi)
+        prm = params or self.config
+        pb, nb = _records(beams, 64, np.ascontiguousarray)
+        recs = np.zeros(max(1, min(int(cfg.max_records), 64)), SEARCH_RECORD_DTYPE)
+        out = np.zeros((), SEARCH_BNB_RESULT_DTYPE)
+        _chk(load_library().b2_pf_global_search_bnb(self._h, field._h, _p(_tf(Tsb)), pb if nb else None, C.c_uint32(nb), C.byref(prm), C.byref(cfg),
+                                                     None if surface is None else C.byref(surface), C.c_float(min_ratio), _p(recs), _p(out)))
+        res = {k: out[k].tolist() for k in SEARCH_BNB_RESULT_DTYPE.names}
+        res["n_bounded_pass"] = res["n_bounded_pass"][:res["n_passes"]]
         return res, recs[:res["n_records"]]
 
     def motionUpdate(self, particle_poses, particle_attrs, T_bnew_bold, forget_rate, check_collision=False):

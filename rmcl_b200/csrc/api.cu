@@ -3,6 +3,7 @@
 #include "kernels.cuh"
 #include "lbvh.cuh"
 #include <cub/device/device_scan.cuh>
+#include <cub/device/device_select.cuh>
 
 #include <algorithm>
 #include <atomic>
@@ -55,6 +56,19 @@ struct b2_mesh {
 
 template <typename T> struct DevBuf {
     T* p = nullptr; size_t cap = 0;
+    // reserve that keeps the first `keep` elements (copied on the stream, which it synchronises); grows at least twofold
+    int grow(size_t n, size_t keep, cudaStream_t s) {
+        if (n <= cap) return B2_OK;
+        n = n > 2 * cap ? n : 2 * cap;
+        T* q = nullptr;
+        cudaError_t e = cudaMalloc((void**)&q, sizeof(T) * n);
+        if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(B2_ERR_OOM, "cudaMalloc(%zu bytes) failed: %s", sizeof(T) * n, cudaGetErrorString(e)); }
+        if (keep) e = cudaMemcpyAsync(q, p, sizeof(T) * keep, cudaMemcpyDeviceToDevice, s);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        if (e != cudaSuccess) { cudaFree(q); return fail(B2_ERR_CUDA, "copy of %zu bytes failed: %s", sizeof(T) * keep, cudaGetErrorString(e)); }
+        if (p) cudaFree(p);
+        p = q; cap = n; return B2_OK;
+    }
     int reserve(size_t n) {
         if (n <= cap) return B2_OK;
         if (p) cudaFree(p);
@@ -2001,6 +2015,11 @@ struct b2_pf {
     // no array for them), the peaks' rank keys before and after the sort with the sort's temporary storage, the kept peaks and their records
     DevBuf<float> d_search_yaw, d_search_scores; DevBuf<SearchCell> d_search_cells; DevBuf<unsigned long long> d_search_keys, d_search_keys2;
     DevBuf<unsigned char> d_search_tmp; DevBuf<uint32_t> d_search_sel; DevBuf<b2_search_record> d_search_recs;
+    // branch-and-bound search (b2_pf_global_search_bnb), grown at its calls: the pyramid, the pending nodes of each tree level, a chunk's
+    // children or leaves with their flags, the candidates >= the threshold (L) and their sorted copies, the kept peaks
+    DevBuf<float> d_bnb_fine2, d_bnb_fine4, d_bnb_dense; DevBuf<uint64_t> d_bnb_nodes[B2_BNB_LEVELS]; DevBuf<uint64_t> d_bnb_child;
+    DevBuf<float> d_bnb_score; DevBuf<uint8_t> d_bnb_flag; DevBuf<uint64_t> d_bnb_lc, d_bnb_lc2; DevBuf<float> d_bnb_ls, d_bnb_ls2;
+    DevBuf<uint32_t> d_bnb_rank; DevBuf<unsigned long long> d_bnb_num; DevBuf<uint64_t> d_bnb_sel; DevBuf<float> d_bnb_sel_s;
 };
 
 extern "C" int b2_pf_destroy(b2_pf* h);
@@ -2021,6 +2040,8 @@ static int pf_init(b2_pf* h)
     CU(cudaFuncSetAttribute(k_pf_update_field, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
     CU(cudaFuncSetAttribute(k_pf_stein_score, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
     CU(cudaFuncSetAttribute(k_pf_search_score, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin - (int)B2_SEARCH_STATIC_SMEM));
+    CU(cudaFuncSetAttribute(k_pf_bnb_bound, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin - (int)B2_BNB_STATIC_SMEM));
+    CU(cudaFuncSetAttribute(k_pf_bnb_leaves, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin - (int)B2_BNB_STATIC_SMEM));
     CU(cudaEventCreate(&h->ev_m0)); CU(cudaEventCreate(&h->ev_m1));
     { const char* e = getenv("B2_PF_MAP"); if (e) h->map_mode = std::min(3, std::max(0, atoi(e))); }
     return B2_OK;
@@ -2070,6 +2091,9 @@ extern "C" int b2_pf_destroy(b2_pf* h)
     h->d_stein_snap.release(); h->d_stein_beams.release(); h->d_stein_v.release(); h->d_stein_part.release();
     h->d_search_yaw.release(); h->d_search_scores.release(); h->d_search_cells.release(); h->d_search_keys.release(); h->d_search_keys2.release();
     h->d_search_tmp.release(); h->d_search_sel.release(); h->d_search_recs.release();
+    h->d_bnb_fine2.release(); h->d_bnb_fine4.release(); h->d_bnb_dense.release(); for (auto& b : h->d_bnb_nodes) b.release();
+    h->d_bnb_child.release(); h->d_bnb_score.release(); h->d_bnb_flag.release(); h->d_bnb_lc.release(); h->d_bnb_lc2.release(); h->d_bnb_ls.release();
+    h->d_bnb_ls2.release(); h->d_bnb_rank.release(); h->d_bnb_num.release(); h->d_bnb_sel.release(); h->d_bnb_sel_s.release();
     b2_mesh* map = h->map;
     delete h;
     (void)cudaGetLastError();
@@ -2596,6 +2620,36 @@ extern "C" int b2_pf_stein_update(b2_pf* h, const b2_dfield* f, b2_transform* po
 // Global search (kernels.cuh, SURVEY appendix M): the cells' surface probes, the scores, one pass for the peaks, the radix sort of their rank
 // keys, then the separation pass on the host over as many sorted keys as it needs (read back in chunks), and the kept peaks' records.
 static int surface_config_check(const b2_surface_config& c, const char* what, float* cos_max, float* tfar);
+// the checks both searches make after the grid's size: the step and positions, the records and separations, the sensor model, the surface
+static int search_check(const b2_search_config& c, const b2_pf_params& prm, const b2_surface_config* surface, b2_surface_config* sc, float* cos_max, float* tfar)
+{
+    if (!(std::isfinite(c.step) && c.step > 0.0f)) return fail(B2_ERR_INVALID, "global search: step = %g must be finite and > 0", (double)c.step);
+    const float x1 = search_coord(c.x0, c.nx - 1, c.step), y1 = search_coord(c.y0, c.ny - 1, c.step);
+    if (!(std::isfinite(c.x0) && std::isfinite(c.y0) && std::isfinite(c.z0) && std::isfinite(x1) && std::isfinite(y1)))
+        return fail(B2_ERR_INVALID, "global search: the grid from (%g, %g, %g) to (%g, %g) is not finite", (double)c.x0, (double)c.y0, (double)c.z0, (double)x1, (double)y1);
+    if (c.max_records < 1 || c.max_records > B2_SEARCH_MAX_RECORDS)
+        return fail(B2_ERR_INVALID, "global search: max_records = %u must lie in [1, %u]", c.max_records, B2_SEARCH_MAX_RECORDS);
+    if (!(std::isfinite(c.min_separation_xy) && c.min_separation_xy >= 0.0f && std::isfinite(c.min_separation_yaw) && c.min_separation_yaw >= 0.0f))
+        return fail(B2_ERR_INVALID, "global search: separations (%g, %g) must be finite and >= 0", (double)c.min_separation_xy, (double)c.min_separation_yaw);
+    const float sq = prm.dist_sigma * prm.dist_sigma;
+    if (!(std::isfinite(prm.dist_sigma) && prm.dist_sigma > 0.0f && std::isfinite(sq) && sq > 0.0f))
+        return fail(B2_ERR_INVALID, "global search: dist_sigma = %g must be finite and > 0, and so must its square", (double)prm.dist_sigma);
+    if (surface) { *sc = *surface; RES(surface_config_check(*sc, "global search", cos_max, tfar)); }
+    return B2_OK;
+}
+// the yaw table of K headings (SearchGrid::yaw), uploaded on the handle's stream
+static int search_yaw(b2_pf* h, uint32_t K)
+{
+    RES(h->d_search_yaw.reserve(2 * (size_t)K));
+    std::vector<float> yaw(2 * (size_t)K);
+    for (uint32_t k = 0; k < K; k++) {
+        const double half = 0.5 * search_psi(k, K);
+        yaw[2 * k] = (float)std::sin(half); yaw[2 * k + 1] = (float)std::cos(half);
+    }
+    // from pageable memory: the copy has read the vector when it returns
+    CU(cudaMemcpyAsync(h->d_search_yaw.p, yaw.data(), sizeof(float) * 2 * (size_t)K, cudaMemcpyHostToDevice, h->stream));
+    return B2_OK;
+}
 extern "C" int b2_pf_global_search(b2_pf* h, const b2_dfield* f, const b2_transform* Tsb, const b2_range_meas* beams, uint32_t n_beams,
                                    const b2_pf_params* prm, const b2_search_config* cfg, const b2_surface_config* surface,
                                    b2_search_record* records_host, float* scores_dev, b2_search_result* out_host)
@@ -2609,20 +2663,9 @@ extern "C" int b2_pf_global_search(b2_pf* h, const b2_dfield* f, const b2_transf
     const uint64_t n_cand = (uint64_t)c.nx * c.ny * c.n_yaw;
     if (n_cand > B2_SEARCH_MAX_CANDIDATES)
         return fail(B2_ERR_INVALID, "global search: %llu candidates, at most 2^30", (unsigned long long)n_cand);
-    if (!(std::isfinite(c.step) && c.step > 0.0f)) return fail(B2_ERR_INVALID, "global search: step = %g must be finite and > 0", (double)c.step);
-    const float x1 = search_coord(c.x0, c.nx - 1, c.step), y1 = search_coord(c.y0, c.ny - 1, c.step);
-    if (!(std::isfinite(c.x0) && std::isfinite(c.y0) && std::isfinite(c.z0) && std::isfinite(x1) && std::isfinite(y1)))
-        return fail(B2_ERR_INVALID, "global search: the grid from (%g, %g, %g) to (%g, %g) is not finite", (double)c.x0, (double)c.y0, (double)c.z0, (double)x1, (double)y1);
-    if (c.max_records < 1 || c.max_records > B2_SEARCH_MAX_RECORDS)
-        return fail(B2_ERR_INVALID, "global search: max_records = %u must lie in [1, %u]", c.max_records, B2_SEARCH_MAX_RECORDS);
-    if (!(std::isfinite(c.min_separation_xy) && c.min_separation_xy >= 0.0f && std::isfinite(c.min_separation_yaw) && c.min_separation_yaw >= 0.0f))
-        return fail(B2_ERR_INVALID, "global search: separations (%g, %g) must be finite and >= 0", (double)c.min_separation_xy, (double)c.min_separation_yaw);
-    const float sq = prm->dist_sigma * prm->dist_sigma;
-    if (!(std::isfinite(prm->dist_sigma) && prm->dist_sigma > 0.0f && std::isfinite(sq) && sq > 0.0f))
-        return fail(B2_ERR_INVALID, "global search: dist_sigma = %g must be finite and > 0, and so must its square", (double)prm->dist_sigma);
     b2_surface_config sc{};
     float cos_max = 0.0f, tfar = 0.0f;
-    if (surface) { sc = *surface; RES(surface_config_check(sc, "global search", &cos_max, &tfar)); }
+    RES(search_check(c, *prm, surface, &sc, &cos_max, &tfar));
     NOTNULL(f); NOTNULL(h);
     if (f->map->device != h->map->device) return fail(B2_ERR_INVALID, "global search: the field is on device %d, the handle on device %d", f->map->device, h->map->device);
     const size_t smem_max = (size_t)h->smem_optin - B2_SEARCH_STATIC_SMEM;
@@ -2639,18 +2682,12 @@ extern "C" int b2_pf_global_search(b2_pf* h, const b2_dfield* f, const b2_transf
     const uint64_t cap = (uint64_t)((c.nx + 1) / 2) * ((c.ny + 1) / 2) * ((K + 1) / 2);
     size_t sort_bytes = 0;
     CU(cub::DeviceRadixSort::SortKeys(nullptr, sort_bytes, h->d_search_keys.p, h->d_search_keys2.p, (int)cap, 0, 64, h->stream));
-    RES(h->d_search_yaw.reserve(2 * (size_t)K));
     if (!scores_dev) RES(h->d_search_scores.reserve(n));
     if (surface) RES(h->d_search_cells.reserve(n_cells));
     RES(h->d_search_keys.reserve(cap)); RES(h->d_search_keys2.reserve(cap)); RES(h->d_search_tmp.reserve(std::max<size_t>(sort_bytes, 16)));
     RES(h->d_search_sel.reserve(B2_SEARCH_MAX_RECORDS)); RES(h->d_search_recs.reserve(B2_SEARCH_MAX_RECORDS));
     float* scores = scores_dev ? scores_dev : h->d_search_scores.p;
-    std::vector<float> yaw(2 * (size_t)K);
-    for (uint32_t k = 0; k < K; k++) {
-        const double half = 0.5 * search_psi(k, K);
-        yaw[2 * k] = (float)std::sin(half); yaw[2 * k + 1] = (float)std::cos(half);
-    }
-    CU(cudaMemcpyAsync(h->d_search_yaw.p, yaw.data(), sizeof(float) * 2 * (size_t)K, cudaMemcpyHostToDevice, h->stream));
+    RES(search_yaw(h, K));
     const SearchGrid g{c.x0, c.y0, c.z0, c.step, c.nx, c.ny, K, h->d_search_yaw.p};
     if (surface) {
         k_pf_search_cells<<<dfield_grid(h->n_sm, n_cells), 256, 0, h->stream>>>(h->map->view(), g, sc, cos_max, tfar, h->d_search_cells.p);
@@ -2694,6 +2731,236 @@ extern "C" int b2_pf_global_search(b2_pf* h, const b2_dfield* f, const b2_transf
                                                                        h->d_search_recs.p);
         LAUNCHED();
         CU(cudaMemcpyAsync(records_host, h->d_search_recs.p, sizeof(b2_search_record) * n_kept, cudaMemcpyDeviceToHost, h->stream));
+    }
+    CU(cudaStreamSynchronize(h->stream));
+    *out_host = res;
+    return B2_OK;
+}
+
+// Branch-and-bound search (kernels.cuh, SURVEY appendix N).  The pyramid is built per call.  A pass at threshold t walks the trees depth first
+// by chunks of at most B2_BNB_CHUNK nodes of one level, always the lowest level that has pending nodes, so that at most 4 chunks wait per
+// level: a chunk of level l >= 1 is bounded and its flagged children compacted (cub::DeviceSelect) into level l - 1; a chunk of leaves is
+// scored and its candidates with score >= t appended to L.  L is sorted by c, its peaks found through the rule over L, ranked by a stable
+// radix sort on the rank key with c as value, and separated on the host over as many as it needs.  Thresholds: N5.
+#define B2_BNB_CHUNK (1u << 20)
+extern "C" int b2_pf_global_search_bnb(b2_pf* h, const b2_dfield* f, const b2_transform* Tsb, const b2_range_meas* beams, uint32_t n_beams,
+                                       const b2_pf_params* prm, const b2_search_config* cfg, const b2_surface_config* surface, float min_ratio,
+                                       b2_search_record* records_host, b2_search_bnb_result* out_host)
+{
+    // the arguments are checked before the handle: the checks need no device
+    NOTNULL(Tsb); NOTNULL(prm); NOTNULL(cfg); NOTNULL(records_host); NOTNULL(out_host);
+    if (n_beams) NOTNULL(beams);
+    const b2_search_config c = *cfg;
+    if (c.nx == 0 || c.ny == 0 || c.n_yaw == 0 || c.nx > B2_BNB_MAX_AXIS || c.ny > B2_BNB_MAX_AXIS || c.n_yaw > B2_SEARCH_MAX_YAW)
+        return fail(B2_ERR_INVALID, "global search: grid %u x %u x %u (nx and ny in [1, 2^24], n_yaw in [1, %u])", c.nx, c.ny, c.n_yaw, B2_SEARCH_MAX_YAW);
+    b2_surface_config sc{};
+    float cos_max = 0.0f, tfar = 0.0f;
+    RES(search_check(c, *prm, surface, &sc, &cos_max, &tfar));
+    if (!(min_ratio >= 0.0f && min_ratio <= 1.0f)) return fail(B2_ERR_INVALID, "global search: min_ratio = %g must lie in [0, 1]", (double)min_ratio);
+    NOTNULL(f); NOTNULL(h);
+    if (f->map->device != h->map->device) return fail(B2_ERR_INVALID, "global search: the field is on device %d, the handle on device %d", f->map->device, h->map->device);
+    const size_t smem_max = (size_t)h->smem_optin - B2_BNB_STATIC_SMEM;
+    if (sizeof(float) * (size_t)n_beams > smem_max) return fail(B2_ERR_UNSUPPORTED, "global search: too many beams (%u)", n_beams);
+    CU(cudaSetDevice(h->map->device));
+    const uint32_t K = c.n_yaw;
+    const uint64_t n_cand = (uint64_t)c.nx * c.ny * K;
+    uint32_t ppb = B2_PF_BLOCK;
+    if (n_beams) {
+        RES(pf_prepare_beams(h, beams, n_beams, &ppb));
+        ppb = std::max<uint32_t>(1u, std::min<uint32_t>(ppb, (uint32_t)(smem_max / (sizeof(float) * (size_t)n_beams))));
+    }
+    RES(search_yaw(h, K));
+    const SearchGrid g{c.x0, c.y0, c.z0, c.step, c.nx, c.ny, K, h->d_search_yaw.p};
+
+    // the pyramid
+    const DfieldView& fv = f->v;
+    SearchPyr P{};
+    const uint64_t n_dense = pyr_levels(fv, P);
+    RES(h->d_bnb_fine2.reserve(std::max<uint64_t>(1, f->n_alloc * 64u))); RES(h->d_bnb_fine4.reserve(std::max<uint64_t>(1, f->n_alloc * 8u)));
+    RES(h->d_bnb_dense.reserve(n_dense));
+    P.fine2 = h->d_bnb_fine2.p; P.fine4 = h->d_bnb_fine4.p; P.dense = h->d_bnb_dense.p;
+    if (f->n_alloc) {
+        k_pf_bnb_pyr_fine2<<<dfield_grid(h->n_sm, f->n_alloc * 64u), 256, 0, h->stream>>>(fv, f->n_alloc * 64u, h->d_bnb_fine2.p);
+        LAUNCHED();
+        k_pf_bnb_pyr_fine4<<<dfield_grid(h->n_sm, f->n_alloc * 8u), 256, 0, h->stream>>>(h->d_bnb_fine2.p, f->n_alloc * 8u, h->d_bnb_fine4.p);
+        LAUNCHED();
+    }
+    k_pf_bnb_pyr_bricks<<<dfield_grid(h->n_sm, f->n_bricks), 256, 0, h->stream>>>(fv, h->d_bnb_fine4.p, f->n_bricks, h->d_bnb_dense.p);
+    LAUNCHED();
+    for (uint32_t L = 1; L < P.n_dense; L++) {
+        const uint32_t dx = pyr_dim(fv.bx, L), dy = pyr_dim(fv.by, L), dz = pyr_dim(fv.bz, L);
+        k_pf_bnb_pyr_up<<<dfield_grid(h->n_sm, (uint64_t)dx * dy * dz), 256, 0, h->stream>>>(h->d_bnb_dense.p + P.off[L - 1], pyr_dim(fv.bx, L - 1), pyr_dim(fv.by, L - 1),
+                                                                                         pyr_dim(fv.bz, L - 1), dx, dy, (uint64_t)dx * dy * dz, h->d_bnb_dense.p + P.off[L]);
+        LAUNCHED();
+    }
+
+    // the bound's constants (N1)
+    const SearchBnb sb = search_bnb_constants(c, *Tsb, surface ? &sc : nullptr, cos_max, tfar);
+    uint32_t depth = 0;
+    while ((1ull << depth) < std::max(c.nx, c.ny)) depth++;
+    const b2_transform Tsb_v = *Tsb;
+    const b2_pf_params pv = *prm;
+    const int surf = surface ? 1 : 0;
+    const BvhView bvh = h->map->view();
+    // the compactions' temporary storage: its size depends on the item type, so the larger of the u64 and the float selection
+    size_t sel_bytes = 0, sel_f_bytes = 0;
+    CU(cub::DeviceSelect::Flagged(nullptr, sel_bytes, h->d_bnb_child.p, h->d_bnb_flag.p, h->d_bnb_child.p, h->d_bnb_num.p, (int)(4u * B2_BNB_CHUNK), h->stream));
+    CU(cub::DeviceSelect::Flagged(nullptr, sel_f_bytes, h->d_bnb_score.p, h->d_bnb_flag.p, h->d_bnb_score.p, h->d_bnb_num.p, (int)(4u * B2_BNB_CHUNK), h->stream));
+    sel_bytes = std::max(sel_bytes, sel_f_bytes);
+    RES(h->d_bnb_child.reserve(4u * (size_t)B2_BNB_CHUNK)); RES(h->d_bnb_flag.reserve(4u * (size_t)B2_BNB_CHUNK));
+    RES(h->d_bnb_score.reserve(B2_BNB_CHUNK)); RES(h->d_bnb_num.reserve(1)); RES(h->d_search_tmp.reserve(std::max<size_t>(sel_bytes, 16)));
+    RES(h->d_bnb_sel.reserve(B2_SEARCH_MAX_RECORDS)); RES(h->d_bnb_sel_s.reserve(B2_SEARCH_MAX_RECORDS)); RES(h->d_search_recs.reserve(B2_SEARCH_MAX_RECORDS));
+    auto fetch_num = [&](unsigned long long* v) -> int {
+        CU(cudaMemcpyAsync(v, h->d_bnb_num.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+        CU(cudaStreamSynchronize(h->stream));
+        return B2_OK;
+    };
+
+    b2_search_bnb_result res{};
+    res.n_candidates = n_cand; res.depth = depth;
+    uint64_t kept_c[B2_SEARCH_MAX_RECORDS];
+    float kept_s[B2_SEARCH_MAX_RECORDS];
+    uint32_t n_kept = 0;
+    // one pass at threshold t: -> the number of candidates >= t (n_L) and, when there is one, the kept peaks and the best score
+    auto pass = [&](float t, uint64_t* n_L_out, float* best) -> int {
+        uint64_t cnt[B2_BNB_LEVELS] = {};
+        std::vector<uint64_t> roots(K);
+        for (uint32_t k = 0; k < K; k++) roots[k] = bnb_key(0u, 0u, k);
+        RES(h->d_bnb_nodes[depth].reserve(K));
+        CU(cudaMemcpyAsync(h->d_bnb_nodes[depth].p, roots.data(), sizeof(uint64_t) * K, cudaMemcpyHostToDevice, h->stream));
+        cnt[depth] = K;
+        uint64_t n_L = 0;
+        for (;;) {
+            int l = 0;
+            while (l <= (int)depth && cnt[l] == 0) l++;
+            if (l > (int)depth) break;
+            const uint32_t m = (uint32_t)std::min<uint64_t>(B2_BNB_CHUNK, cnt[l]);
+            cnt[l] -= m;
+            const uint64_t* nodes = h->d_bnb_nodes[l].p + cnt[l];
+            const uint32_t blocks = (m + ppb - 1) / ppb;
+            const size_t smem = sizeof(float) * (size_t)n_beams * ppb;
+            unsigned long long got = 0;
+            if (l > 0) {
+                RES(h->d_bnb_nodes[l - 1].reserve(4u * (size_t)m));
+                k_pf_bnb_bound<<<blocks, B2_PF_BLOCK, smem, h->stream>>>(fv, P, g, sb, (uint32_t)l, nodes, m, Tsb_v, h->d_beams.p, n_beams, pv, ppb, t,
+                                                                         h->d_bnb_child.p, h->d_bnb_flag.p);
+                LAUNCHED();
+                CU(cub::DeviceSelect::Flagged(h->d_search_tmp.p, sel_bytes, h->d_bnb_child.p, h->d_bnb_flag.p, h->d_bnb_nodes[l - 1].p, h->d_bnb_num.p,
+                                              (int)(4u * m), h->stream));
+                LAUNCHED();
+                RES(fetch_num(&got));
+                cnt[l - 1] = got;
+                res.n_level[l] += m; res.n_bounded += m; res.n_bounded_pass[res.n_passes] += m;
+            } else {
+                // the leaves' candidates go to the child buffer's first m entries, their scores and flags alongside
+                k_pf_bnb_leaves<<<blocks, B2_PF_BLOCK, smem, h->stream>>>(fv, bvh, g, sc, surf, cos_max, tfar, nodes, m, Tsb_v, h->d_beams.p, n_beams, pv, ppb,
+                                                                          t, h->d_bnb_child.p, h->d_bnb_score.p, h->d_bnb_flag.p);
+                LAUNCHED();
+                RES(h->d_bnb_lc.grow(n_L + m, n_L, h->stream)); RES(h->d_bnb_ls.grow(n_L + m, n_L, h->stream));
+                CU(cub::DeviceSelect::Flagged(h->d_search_tmp.p, sel_bytes, h->d_bnb_child.p, h->d_bnb_flag.p, h->d_bnb_lc.p + n_L, h->d_bnb_num.p, (int)m, h->stream));
+                LAUNCHED();
+                CU(cub::DeviceSelect::Flagged(h->d_search_tmp.p, sel_bytes, h->d_bnb_score.p, h->d_bnb_flag.p, h->d_bnb_ls.p + n_L, h->d_bnb_num.p, (int)m, h->stream));
+                LAUNCHED();
+                RES(fetch_num(&got));
+                n_L += got;
+                res.n_level[0] += m; res.n_leaves += m;
+                // cub's sorts and selections below count items in int
+                if (n_L > (uint64_t)INT32_MAX)
+                    return fail(B2_ERR_UNSUPPORTED, "global search: %llu candidates score >= the threshold %g, more than 2^31 - 1 (raise min_ratio)",
+                                (unsigned long long)n_L, (double)t);
+            }
+        }
+        *n_L_out = n_L;
+        n_kept = 0;
+        if (n_L == 0) return B2_OK;
+        // L sorted by c into (lc2, ls2); its peaks' c and rank keys compacted into (lc, ls as rank keys); sorted stably by rank into (ls2, lc2)
+        int end_bit = 1;
+        while (end_bit < 64 && (n_cand - 1) >> end_bit) end_bit++;
+        size_t sort_bytes = 0, sort2_bytes = 0;
+        RES(h->d_bnb_lc2.reserve(n_L)); RES(h->d_bnb_ls2.reserve(n_L)); RES(h->d_bnb_rank.reserve(n_L));
+        if (n_L > h->d_bnb_flag.cap) RES(h->d_bnb_flag.reserve(n_L));
+        uint32_t* rank1 = reinterpret_cast<uint32_t*>(h->d_bnb_ls.p);
+        uint32_t* rank2 = reinterpret_cast<uint32_t*>(h->d_bnb_ls2.p);
+        CU(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, h->d_bnb_lc.p, h->d_bnb_lc2.p, h->d_bnb_ls.p, h->d_bnb_ls2.p, (int)n_L, 0, end_bit, h->stream));
+        CU(cub::DeviceRadixSort::SortPairs(nullptr, sort2_bytes, h->d_bnb_rank.p, rank2, h->d_bnb_lc.p, h->d_bnb_lc2.p, (int)n_L, 0, 32, h->stream));
+        size_t sel2_bytes = 0, sel2_c_bytes = 0;
+        CU(cub::DeviceSelect::Flagged(nullptr, sel2_bytes, h->d_bnb_rank.p, h->d_bnb_flag.p, rank1, h->d_bnb_num.p, (int)n_L, h->stream));
+        CU(cub::DeviceSelect::Flagged(nullptr, sel2_c_bytes, h->d_bnb_lc2.p, h->d_bnb_flag.p, h->d_bnb_lc.p, h->d_bnb_num.p, (int)n_L, h->stream));
+        sel2_bytes = std::max(sel2_bytes, sel2_c_bytes);
+        RES(h->d_search_tmp.reserve(std::max({sort_bytes, sort2_bytes, sel2_bytes, sel_bytes, (size_t)16})));
+        CU(cub::DeviceRadixSort::SortPairs(h->d_search_tmp.p, sort_bytes, h->d_bnb_lc.p, h->d_bnb_lc2.p, h->d_bnb_ls.p, h->d_bnb_ls2.p, (int)n_L, 0, end_bit, h->stream));
+        LAUNCHED();
+        k_pf_bnb_peaks<<<dfield_grid(h->n_sm, n_L), 256, 0, h->stream>>>(h->d_bnb_lc2.p, h->d_bnb_ls2.p, n_L, c.nx, c.ny, K, h->d_bnb_flag.p, h->d_bnb_rank.p);
+        LAUNCHED();
+        CU(cub::DeviceSelect::Flagged(h->d_search_tmp.p, sel2_bytes, h->d_bnb_lc2.p, h->d_bnb_flag.p, h->d_bnb_lc.p, h->d_bnb_num.p, (int)n_L, h->stream));
+        LAUNCHED();
+        CU(cub::DeviceSelect::Flagged(h->d_search_tmp.p, sel2_bytes, h->d_bnb_rank.p, h->d_bnb_flag.p, rank1, h->d_bnb_num.p, (int)n_L, h->stream));
+        LAUNCHED();
+        unsigned long long n_peaks = 0;
+        RES(fetch_num(&n_peaks));
+        res.n_peaks = n_peaks;
+        const uint32_t* rk = rank1;
+        const uint64_t* pc = h->d_bnb_lc.p;
+        if (n_peaks > 1) {
+            CU(cub::DeviceRadixSort::SortPairs(h->d_search_tmp.p, sort2_bytes, rank1, rank2, h->d_bnb_lc.p, h->d_bnb_lc2.p, (int)n_peaks, 0, 32, h->stream));
+            LAUNCHED();
+            rk = rank2; pc = h->d_bnb_lc2.p;
+        }
+        // the separation pass: (rank, c) read back in chunks that double, until max_records peaks are kept or none is left
+        std::vector<uint32_t> ck_r;
+        std::vector<uint64_t> ck_c;
+        for (uint64_t at = 0, len = 1024; at < n_peaks && n_kept < c.max_records; at += len, len *= 2) {
+            const uint64_t q = std::min<uint64_t>(len, n_peaks - at);
+            ck_r.resize(q); ck_c.resize(q);
+            CU(cudaMemcpyAsync(ck_r.data(), rk + at, sizeof(uint32_t) * q, cudaMemcpyDeviceToHost, h->stream));
+            CU(cudaMemcpyAsync(ck_c.data(), pc + at, sizeof(uint64_t) * q, cudaMemcpyDeviceToHost, h->stream));
+            CU(cudaStreamSynchronize(h->stream));
+            if (at == 0) *best = u2f(~ck_r[0]);
+            for (uint64_t e = 0; e < q && n_kept < c.max_records; e++)
+                if (search_keep<uint64_t>(g, ck_c[e], kept_c, n_kept, (double)c.min_separation_xy, (double)c.min_separation_yaw)) {
+                    kept_c[n_kept] = ck_c[e]; kept_s[n_kept] = u2f(~ck_r[e]); n_kept++;
+                }
+        }
+        return B2_OK;
+    };
+
+    // the thresholds (N5): U f_q, f_q = (8 - q) / 8, until a pass finds a candidate, which gives s*; then max(tau, s* f_q) for the next q with
+    // s* f_q below the last threshold, until max_records peaks are kept or the threshold is tau
+    float denom_f = 0.0f;
+    { float sq; double denom; pf_constants(pv, sq, denom); denom_f = n_beams ? (float)(1.0 / denom) : 0.0f; }
+    float best = -1.0f, tau = -1.0f;
+    bool known = false;
+    for (uint32_t q = 1; q <= 8; q++) {
+        const float t = denom_f * ((float)(8u - q) / 8.0f);
+        uint64_t n_L = 0;
+        float b = -1.0f;
+        RES(pass(t, &n_L, &b));
+        res.n_passes++;
+        if (n_L) { best = b; tau = min_ratio * best; known = true; }
+        if (!known) continue;
+        float last = t;
+        uint32_t qb = 0;
+        while (n_kept < c.max_records && last > tau) {
+            do qb++; while (best * ((float)(8u - qb) / 8.0f) >= last);
+            const float tb = std::max(tau, best * ((float)(8u - qb) / 8.0f));
+            RES(pass(tb, &n_L, &b));
+            res.n_passes++;
+            last = tb;
+        }
+        break;
+    }
+    uint32_t n_rec = 0;
+    if (known) while (n_rec < n_kept && kept_s[n_rec] >= tau) n_rec++;
+    res.best_score = best; res.threshold = tau; res.n_records = n_rec;
+    if (n_rec) {
+        CU(cudaMemcpyAsync(h->d_bnb_sel.p, kept_c, sizeof(uint64_t) * n_rec, cudaMemcpyHostToDevice, h->stream));
+        CU(cudaMemcpyAsync(h->d_bnb_sel_s.p, kept_s, sizeof(float) * n_rec, cudaMemcpyHostToDevice, h->stream));
+        k_pf_bnb_records<<<1, B2_SEARCH_MAX_RECORDS, 0, h->stream>>>(bvh, g, sc, surf, cos_max, tfar, h->d_bnb_sel.p, h->d_bnb_sel_s.p, n_rec, h->d_search_recs.p);
+        LAUNCHED();
+        std::vector<b2_search_record> recs(n_rec);
+        CU(cudaMemcpyAsync(recs.data(), h->d_search_recs.p, sizeof(b2_search_record) * n_rec, cudaMemcpyDeviceToHost, h->stream));
+        CU(cudaStreamSynchronize(h->stream));
+        std::memcpy(records_host, recs.data(), sizeof(b2_search_record) * n_rec);
     }
     CU(cudaStreamSynchronize(h->stream));
     *out_host = res;

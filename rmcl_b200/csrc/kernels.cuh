@@ -1309,14 +1309,22 @@ B2_DEV float df_lookup_grad(const DfieldView& f, V3 p, V3& grad)
     return df_lerp(c0, c1, tz);
 }
 
-// Gaussian evaluation of one (particle, beam) pair from the field: the closest-point branch of pf_eval_one with e = field(q)
-B2_DEV float pf_eval_field(const DfieldView& f, Tf Tsm, const PfBeam& b, float sigma_quad, double denom)
+// Gaussian evaluation of one (particle, beam) pair from the field: the closest-point branch of pf_eval_one with e = field(q).  The beam's
+// end point q and the evaluation of an error are separate steps, so that the branch-and-bound search bounds both the same way.
+B2_DEV V3 pf_eval_point(const Tf& Tsm, const PfBeam& b)
 {
     const V3 orig_m = tf_apply(Tsm, mk3(b.ox, b.oy, b.oz));
     const V3 dir_m = q_rot(Tsm.R, mk3(b.dx, b.dy, b.dz));
-    const float error = df_lookup(f, v_add(orig_m, v_scale(dir_m, b.range)));
+    return v_add(orig_m, v_scale(dir_m, b.range));
+}
+B2_DEV float pf_eval_error(float error, float sigma_quad, double denom)
+{
     const float arg = dvd(dvd(-mul(error, error), sigma_quad), 2.0f);
     return (float)(exp((double)arg) / denom);
+}
+B2_DEV float pf_eval_field(const DfieldView& f, Tf Tsm, const PfBeam& b, float sigma_quad, double denom)
+{
+    return pf_eval_error(df_lookup(f, pf_eval_point(Tsm, b)), sigma_quad, denom);
 }
 
 #ifdef __CUDACC__
@@ -3114,22 +3122,22 @@ struct PfSearchState { unsigned long long n_valid, n_peaks; };
 B2_DEV float search_coord(float o, uint32_t i, float step) { return add(o, mul((float)i, step)); }
 // psi_k = -pi + 2 pi k / K in double (the host's; the separation pass compares these)
 inline double search_psi(uint32_t k, uint32_t K) { return -B2_SEARCH_PI + 2.0 * B2_SEARCH_PI * (double)k / (double)K; }
-// candidate c's pose before the surface rule
-B2_DEV Tf search_pose(const SearchGrid& g, uint32_t c)
+// candidate (i, j, k)'s pose before the surface rule; search_pose: candidate c's
+B2_DEV Tf search_pose_ijk(const SearchGrid& g, uint32_t i, uint32_t j, uint32_t k)
 {
-    const uint32_t i = c % g.nx, j = c / g.nx % g.ny, k = c / g.nx / g.ny;
     Tf T;
     T.R.x = 0.0f; T.R.y = 0.0f; T.R.z = ldg(g.yaw + 2 * k); T.R.w = ldg(g.yaw + 2 * k + 1);
     T.t = mk3(search_coord(g.x0, i, g.step), search_coord(g.y0, j, g.step), g.z0);
     return T;
 }
+B2_DEV Tf search_pose(const SearchGrid& g, uint32_t c) { return search_pose_ijk(g, c % g.nx, c / g.nx % g.ny, c / g.nx / g.ny); }
 // The surface rule's probe reads only t, so it runs once per cell (at R = identity; R is only tested for finiteness) and every heading is
 // placed on its result: the same bits as pf_surface_pose on each candidate.  The placement stays per candidate: with align 1 it rotates
 // a = R e_z onto n, and a is e_z only up to the rounding of sin^2 + cos^2 and the signs of zeros, which differ between headings.
-B2_DEV SearchCell search_cell(const BvhView& bvh, const SearchGrid& g, uint32_t cell, const b2_surface_config& cfg, float cos_max, float tfar)
+B2_DEV SearchCell search_cell_ij(const BvhView& bvh, const SearchGrid& g, uint32_t i, uint32_t j, const b2_surface_config& cfg, float cos_max, float tfar)
 {
     Tf T = tf_identity();
-    T.t = mk3(search_coord(g.x0, cell % g.nx, g.step), search_coord(g.y0, cell / g.nx, g.step), g.z0);
+    T.t = mk3(search_coord(g.x0, i, g.step), search_coord(g.y0, j, g.step), g.z0);
     V3 p, n;
     SearchCell s;
     const bool ok = pf_surface_probe(bvh, T, cfg, cos_max, tfar, p, n);
@@ -3137,50 +3145,75 @@ B2_DEV SearchCell search_cell(const BvhView& bvh, const SearchGrid& g, uint32_t 
     if (!ok) { s.gx = s.gy = s.gz = 0.0f; }
     return s;
 }
+B2_DEV SearchCell search_cell(const BvhView& bvh, const SearchGrid& g, uint32_t cell, const b2_surface_config& cfg, float cos_max, float tfar)
+{
+    return search_cell_ij(bvh, g, cell % g.nx, cell / g.nx, cfg, cos_max, tfar);
+}
+// the placement of a candidate's pose T on its cell's probe s; false: off surface (T unchanged)
+B2_DEV bool search_place(const SearchCell& s, const b2_surface_config& cfg, Tf& T)
+{
+    if (s.valid == 0.0f) return false;
+    T = pf_surface_place(T, mk3(s.gx, s.gy, s.gz), mk3(s.nx, s.ny, s.nz), cfg);
+    return true;
+}
 // candidate c's pose with the surface rule applied (cells nullable: no surface); false: off surface
 B2_DEV bool search_candidate(const SearchGrid& g, const SearchCell* cells, const b2_surface_config& cfg, uint32_t c, Tf& T)
 {
     T = search_pose(g, c);
     if (!cells) return true;
-    const SearchCell s = cells[c % (g.nx * g.ny)];
-    if (s.valid == 0.0f) return false;
-    T = pf_surface_place(T, mk3(s.gx, s.gy, s.gz), mk3(s.nx, s.ny, s.nz), cfg);
-    return true;
+    return search_place(cells[c % (g.nx * g.ny)], cfg, T);
 }
-// the peak rule at candidate c of the score array s (SURVEY M3): valid, and ahead of every valid neighbour in (score descending, c ascending)
-B2_DEV bool search_is_peak(const float* s, uint32_t nx, uint32_t ny, uint32_t K, uint32_t c)
+// the order of candidates (SURVEY M3): c is ahead of n iff score_n < score_c, or the same score and n > c
+template <class I> B2_DEV bool search_ahead(float sc, I c, float sn, I n) { return sn < sc || (sn == sc && n > c); }
+// the peak rule at candidate c of score sc (SURVEY M3): ahead of every valid neighbour; score_of(n) is a neighbour's score, < 0 when invalid
+template <class I, class S> B2_DEV bool search_peak_rule(I c, float sc, uint32_t nx, uint32_t ny, uint32_t K, S score_of)
 {
-    const float sc = ldg(s + c);
-    if (!(sc >= 0.0f)) return false;
-    const uint32_t i = c % nx, j = c / nx % ny, k = c / nx / ny;
+    const I i = c % nx, j = c / nx % ny, k = c / nx / ny;
     for (int dk = -1; dk <= 1; dk++) {
-        const uint32_t kk = (uint32_t)(((int64_t)k + dk + K) % K);
+        const I kk = (I)(((int64_t)k + dk + K) % K);
         for (int dj = -1; dj <= 1; dj++) {
             const int64_t jj = (int64_t)j + dj;
             if (jj < 0 || jj >= (int64_t)ny) continue;
             for (int di = -1; di <= 1; di++) {
                 const int64_t ii = (int64_t)i + di;
                 if (ii < 0 || ii >= (int64_t)nx) continue;
-                const uint32_t n = (kk * ny + (uint32_t)jj) * nx + (uint32_t)ii;
+                const I n = (kk * ny + (I)jj) * nx + (I)ii;
                 if (n == c) continue;
-                const float sn = ldg(s + n);
+                const float sn = score_of(n);
                 if (!(sn >= 0.0f)) continue;
-                if (!(sn < sc || (sn == sc && n > c))) return false;
+                if (!search_ahead(sc, c, sn, n)) return false;
             }
         }
     }
     return true;
 }
+// the peak rule at candidate c of the score array s: valid, and ahead of every valid neighbour
+B2_DEV bool search_is_peak(const float* s, uint32_t nx, uint32_t ny, uint32_t K, uint32_t c)
+{
+    const float sc = ldg(s + c);
+    if (!(sc >= 0.0f)) return false;
+    return search_peak_rule<uint32_t>(c, sc, nx, ny, K, [&](uint32_t n) { return ldg(s + n); });
+}
 // rank key: ascending order of keys = score descending (scores >= 0, so their bits order them), then c ascending
-B2_DEV unsigned long long search_key(float score, uint32_t c) { return ((unsigned long long)~f2u(score) << 32) | c; }
+B2_DEV uint32_t search_rank(float score) { return ~f2u(score); }
+B2_DEV unsigned long long search_key(float score, uint32_t c) { return ((unsigned long long)search_rank(score) << 32) | c; }
+// a kept peak's record
+B2_DEV b2_search_record search_record(const Tf& T, float score, uint32_t i, uint32_t j, uint32_t k)
+{
+    b2_search_record o;
+    o.pose.R.x = T.R.x; o.pose.R.y = T.R.y; o.pose.R.z = T.R.z; o.pose.R.w = T.R.w; o.pose.t.x = T.t.x; o.pose.t.y = T.t.y; o.pose.t.z = T.t.z; o.pose.stamp = 0u;
+    o.score = score; o.i = i; o.j = j; o.k = k;
+    return o;
+}
 // the separation pass's test of peak c against the kept ones: true iff no kept peak lies both within sep_xy (the grid positions' distance)
 // and within sep_yaw (the wrapped psi difference), strictly, in double
-inline bool search_keep(const SearchGrid& g, uint32_t c, const uint32_t* kept, uint32_t n_kept, double sep_xy, double sep_yaw)
+template <class I> inline bool search_keep(const SearchGrid& g, I c, const I* kept, uint32_t n_kept, double sep_xy, double sep_yaw)
 {
-    const uint32_t i = c % g.nx, j = c / g.nx % g.ny, k = c / g.nx / g.ny;
+    const uint32_t i = (uint32_t)(c % g.nx), j = (uint32_t)(c / g.nx % g.ny), k = (uint32_t)(c / g.nx / g.ny);
     const double x = search_coord(g.x0, i, g.step), y = search_coord(g.y0, j, g.step), psi = search_psi(k, g.K);
     for (uint32_t r = 0; r < n_kept; r++) {
-        const uint32_t q = kept[r], qi = q % g.nx, qj = q / g.nx % g.ny, qk = q / g.nx / g.ny;
+        const I q = kept[r];
+        const uint32_t qi = (uint32_t)(q % g.nx), qj = (uint32_t)(q / g.nx % g.ny), qk = (uint32_t)(q / g.nx / g.ny);
         const double dx = x - (double)search_coord(g.x0, qi, g.step), dy = y - (double)search_coord(g.y0, qj, g.step);
         double dpsi = std::fabs(psi - search_psi(qk, g.K));
         if (2.0 * B2_SEARCH_PI - dpsi < dpsi) dpsi = 2.0 * B2_SEARCH_PI - dpsi;
@@ -3258,10 +3291,310 @@ __global__ void k_pf_search_records(SearchGrid g, const SearchCell* __restrict__
     const uint32_t c = sel[r];
     Tf T;
     search_candidate(g, cells, cfg, c, T);
-    b2_search_record o;
-    o.pose.R.x = T.R.x; o.pose.R.y = T.R.y; o.pose.R.z = T.R.z; o.pose.R.w = T.R.w; o.pose.t.x = T.t.x; o.pose.t.y = T.t.y; o.pose.t.z = T.t.z; o.pose.stamp = 0u;
-    o.score = scores[c]; o.i = c % g.nx; o.j = c / g.nx % g.ny; o.k = c / g.nx / g.ny;
-    out[r] = o;
+    out[r] = search_record(T, scores[c], c % g.nx, c / g.nx % g.ny, c / g.nx / g.ny);
+}
+#endif
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Branch-and-bound global search (b2_pf_global_search_bnb; SURVEY appendix N): appendix M's candidates, scores, peaks and records, found
+// through a quadtree per heading whose nodes are bounded from a min-pooled pyramid of the field, by threshold passes.
+// TREE: a node of level l is (bi, bj, k): the cells i in [bi 2^l, min(nx, (bi + 1) 2^l)), likewise j, of heading k; key k << 48 | bj << 24
+//   | bi.  Level 0 nodes are candidates.
+// PYRAMID: below the brick, per allocated brick (slot), the min of the nodes of each of its 4^3 blocks of 2^3 cells (fine2, nodes 2a .. 2a + 2
+//   per axis) and of its 2^3 blocks of 4^3 cells (fine4); from the brick up, dense level L holds, per block of 2^L bricks per axis, the min
+//   over those bricks (trunc for an unallocated one): L = 0 one value per brick, then 2 x 2 x 2 mins, until one value.  Every entry is an
+//   exact min of stored node values (and trunc), so it is <= the lookup anywhere in the cells it covers (N2).
+// BOUND: per beam, the box the end point can reach from any valid candidate of the node (N1), the pyramid's min over the cells that box
+//   can touch lowered by the lerps' rounding (N2), evaluated one ulp up (N3), merged in slot order (N4): >= every valid candidate's score.
+// ---------------------------------------------------------------------------------------------------------------------
+#define B2_BNB_MAX_AXIS (1u << 24)
+#define B2_BNB_LEVELS 25                 // tree levels 0 .. 24
+#define B2_BNB_MAX_DENSE 24              // dense pyramid levels: a field has at most 2^21 bricks per axis
+#define B2_BNB_STATIC_SMEM 5120u         // k_pf_bnb_bound's static shared memory (5632 B) beyond the 1 KiB the handle keeps free, rounded up
+struct SearchPyr {
+    const float* fine2;                  // [slot][4][4][4]
+    const float* fine4;                  // [slot][2][2][2]
+    const float* dense;                  // the dense levels one after the other, level L at off[L], [z][y][x]
+    uint64_t off[B2_BNB_MAX_DENSE];
+    uint32_t n_dense;
+};
+// the bound's constants of a call (N1): the placed z range [zlo, zhi] before any tilt (z0 without surface), |R_sb|^2 and |t_sb| of the
+// sensor's mount, and with align 1 the tilt's reach coefficient and base_height (0 otherwise)
+struct SearchBnb { float zlo, zhi; double rsb2, tsb, tilt, base; };
+
+B2_DEV uint32_t pyr_dim(uint32_t b, uint32_t L) { return ((b - 1u) >> L) + 1u; }
+// the dense levels of field f's pyramid: P.n_dense and P.off; -> the number of dense entries
+inline uint64_t pyr_levels(const DfieldView& f, SearchPyr& P)
+{
+    P.n_dense = 1;
+    while (pyr_dim(f.bx, P.n_dense - 1) > 1u || pyr_dim(f.by, P.n_dense - 1) > 1u || pyr_dim(f.bz, P.n_dense - 1) > 1u) P.n_dense++;
+    uint64_t n = 0;
+    for (uint32_t L = 0; L < P.n_dense; L++) { P.off[L] = n; n += (uint64_t)pyr_dim(f.bx, L) * pyr_dim(f.by, L) * pyr_dim(f.bz, L); }
+    return n;
+}
+// the bound's constants of a call (N1); surface nullable; cos_max and tfar as surface_config_check gives them
+inline SearchBnb search_bnb_constants(const b2_search_config& c, const b2_transform& T, const b2_surface_config* surface, float cos_max, float tfar)
+{
+    SearchBnb sb{c.z0, c.z0, 0.0, 0.0, 0.0, 0.0};
+    sb.rsb2 = (double)T.R.x * T.R.x + (double)T.R.y * T.R.y + (double)T.R.z * T.R.z + (double)T.R.w * T.R.w;
+    sb.tsb = std::sqrt((double)T.t.x * T.t.x + (double)T.t.y * T.t.y + (double)T.t.z * T.t.z);
+    if (surface) {
+        const float oz = c.z0 + surface->probe_above;          // pf_surface_probe's origin; the ground lies at sub(oz, t), t in (0, tfar]
+        sb.zhi = oz + surface->base_height; sb.zlo = (oz - tfar) + surface->base_height;
+        sb.base = surface->base_height;
+        if (surface->align) {
+            const double theta = std::acos(std::fmin(1.0, (double)cos_max * (1.0 - 0x1p-20)));
+            sb.tilt = 2.0 * std::sin(0.5 * theta) * (1.0 + 0x1p-16) + 0x1p-16;
+        }
+    }
+    return sb;
+}
+B2_DEV uint64_t bnb_key(uint32_t bi, uint32_t bj, uint32_t k) { return ((uint64_t)k << 48) | ((uint64_t)bj << 24) | bi; }
+// min of the nodes [x0, x0 + w] x [y0, y0 + w] x [z0, z0 + w] (brick-local) of brick slot
+B2_DEV float pyr_nodes_min(const DfieldView& f, uint32_t slot, uint32_t x0, uint32_t y0, uint32_t z0, uint32_t w)
+{
+    const float* b = f.bricks + (size_t)slot * B2_DF_NODES;
+    float m = ldg(b + (z0 * 9u + y0) * 9u + x0);
+    for (uint32_t z = z0; z <= z0 + w; z++)
+        for (uint32_t y = y0; y <= y0 + w; y++)
+            for (uint32_t x = x0; x <= x0 + w; x++) m = fminf(m, ldg(b + (z * 9u + y) * 9u + x));
+    return m;
+}
+// entry e of a brick's fine2 (e = (z 4 + y) 4 + x), of its fine4 from fine2, of dense level 0 from fine4, of dense level L + 1 from L
+B2_DEV float pyr_fine2(const DfieldView& f, uint32_t slot, uint32_t e) { return pyr_nodes_min(f, slot, 2u * (e & 3u), 2u * (e >> 2 & 3u), 2u * (e >> 4), 2u); }
+B2_DEV float pyr_fine4(const float* fine2, uint32_t slot, uint32_t e)
+{
+    const uint32_t x = 2u * (e & 1u), y = 2u * (e >> 1 & 1u), z = 2u * (e >> 2);
+    float m = ldg(fine2 + (size_t)slot * 64u + (z * 4u + y) * 4u + x);
+    for (uint32_t d = 1; d < 8; d++) m = fminf(m, ldg(fine2 + (size_t)slot * 64u + ((z + (d >> 2)) * 4u + y + (d >> 1 & 1u)) * 4u + x + (d & 1u)));
+    return m;
+}
+B2_DEV float pyr_brick(const DfieldView& f, const float* fine4, uint64_t id)
+{
+    const uint32_t slot = ldg(f.index + id);
+    if (slot == B2_NOBRICK) return f.trunc;
+    float m = ldg(fine4 + (size_t)slot * 8u);
+    for (uint32_t d = 1; d < 8; d++) m = fminf(m, ldg(fine4 + (size_t)slot * 8u + d));
+    return m;
+}
+B2_DEV float pyr_up(const float* src, uint32_t sx, uint32_t sy, uint32_t sz, uint32_t dx, uint32_t dy, uint64_t id)
+{
+    const uint32_t x = (uint32_t)(id % dx), y = (uint32_t)(id / dx % dy), z = (uint32_t)(id / dx / dy);
+    float m = u2f(0x7f800000u);
+    for (uint32_t d = 0; d < 8; d++) {
+        const uint32_t xx = 2u * x + (d & 1u), yy = 2u * y + (d >> 1 & 1u), zz = 2u * z + (d >> 2);
+        if (xx < sx && yy < sy && zz < sz) m = fminf(m, ldg(src + ((size_t)zz * sy + yy) * sx + xx));
+    }
+    return m;
+}
+// min over the cells lo .. hi (per axis, within [0, dims - 2]) of the field's node values there, trunc for an unallocated brick: the entries
+// of the finest level at which the range spans at most two blocks per axis (2^3-cell blocks at the finest), at most eight
+B2_DEV float pyr_query(const SearchPyr& P, const DfieldView& f, const uint32_t lo[3], const uint32_t hi[3])
+{
+    uint32_t s = 1;
+    while (s < 2u + P.n_dense && ((hi[0] >> s) - (lo[0] >> s) > 1u || (hi[1] >> s) - (lo[1] >> s) > 1u || (hi[2] >> s) - (lo[2] >> s) > 1u)) s++;
+    float m = f.trunc;
+    for (uint32_t z = lo[2] >> s; z <= hi[2] >> s; z++)
+        for (uint32_t y = lo[1] >> s; y <= hi[1] >> s; y++)
+            for (uint32_t x = lo[0] >> s; x <= hi[0] >> s; x++) {
+                float v;
+                if (s >= 3u) {
+                    const uint32_t L = s - 3u;
+                    v = ldg(P.dense + P.off[L] + ((size_t)z * pyr_dim(f.by, L) + y) * pyr_dim(f.bx, L) + x);
+                } else {
+                    const uint32_t sh = 3u - s, msk = (1u << sh) - 1u;
+                    const uint32_t slot = ldg(f.index + ((size_t)(z >> sh) * f.by + (y >> sh)) * f.bx + (x >> sh));
+                    const uint32_t e = (((z & msk) << sh | (y & msk)) << sh) | (x & msk);
+                    v = slot == B2_NOBRICK ? f.trunc : ldg(s == 1u ? P.fine2 + (size_t)slot * 64u + e : P.fine4 + (size_t)slot * 8u + e);
+                }
+                m = fminf(m, v);
+            }
+    return m;
+}
+// the float nearest d from below / above
+B2_DEV float f_down(double d) { const float r = (float)d; return (double)r > d ? nextafterf(r, -u2f(0x7f800000u)) : r; }
+B2_DEV float f_up(double d) { const float r = (float)d; return (double)r < d ? nextafterf(r, u2f(0x7f800000u)) : r; }
+// N1 + N2: a lower bound of the field's value at every point of the box [lo, hi]: the lookup's grid coordinate is mul(sub(p, o), inv_h),
+// monotone in p, so the box's float bounds (rounded outwards) give the range of grid coordinates and of cells any point of it can reach
+B2_DEV float bnb_box_min(const SearchPyr& P, const DfieldView& f, const double lo[3], const double hi[3])
+{
+    const float o[3] = {f.ox, f.oy, f.oz};
+    const uint32_t d[3] = {f.dx, f.dy, f.dz};
+    uint32_t clo[3], chi[3];
+    for (int a = 0; a < 3; a++) {
+        const float glo = mul(sub(f_down(lo[a]), o[a]), f.inv_h), ghi = mul(sub(f_up(hi[a]), o[a]), f.inv_h);
+        if (!(ghi >= 0.0f && glo <= (float)(d[a] - 1u))) return f.trunc;                 // the whole box outside the field: trunc
+        auto cell = [](float g, uint32_t n) { const uint32_t c = (uint32_t)floorf(g); return c < n - 2u ? c : n - 2u; };
+        clo[a] = cell(fmaxf(glo, 0.0f), d[a]); chi[a] = cell(fminf(ghi, (float)(d[a] - 1u)), d[a]);
+    }
+    return pyr_query(P, f, clo, chi);
+}
+// N1 - N3 for one beam of a node: Tsm = the node's first candidate (i0, j0, k) at z = zhi, times Tsb; ext = the node's x and y extent
+// x(i1) - x(i0), y(j1) - y(j0); tmax bounds |t| of every candidate of the node
+B2_DEV float bnb_beam_bound(const DfieldView& f, const SearchPyr& P, const SearchBnb& sb, const Tf& Tsm, double ext_x, double ext_y, double tmax,
+                            const PfBeam& b, float sigma_quad, double denom)
+{
+    const double u = 0x1p-24;
+    const V3 q = pf_eval_point(Tsm, b);
+    const double A = sb.rsb2 * (sqrt((double)b.ox * b.ox + (double)b.oy * b.oy + (double)b.oz * b.oz) +
+                                sqrt((double)b.dx * b.dx + (double)b.dy * b.dy + (double)b.dz * b.dz) * fabs((double)b.range)) + sb.tsb;
+    const double m = 2.0 * (64.0 * 1.01 * u * A + 8.0 * u * tmax + 1e-37) + sb.tilt * (A + sb.base);
+    float e = 0.0f;                                                                     // no finite box: the bound of error 0
+    if (fabsf(q.x) < u2f(0x7f800000u) && fabsf(q.y) < u2f(0x7f800000u) && fabsf(q.z) < u2f(0x7f800000u) && m < 1e30) {
+        const double lo[3] = {(double)q.x - m, (double)q.y - m, (double)q.z + ((double)sb.zlo - (double)sb.zhi) - m};
+        const double hi[3] = {(double)q.x + ext_x + m, (double)q.y + ext_y + m, (double)q.z + m};
+        const float v = bnb_box_min(P, f, lo, hi);
+        e = v >= 0x1p-100f ? mul(v, 1.0f - 0x1p-20f) : 0.0f;                           // the lerps' rounding (N2)
+    }
+    return nextafterf(pf_eval_error(e, sigma_quad, denom), u2f(0x7f800000u));
+}
+// the node's first candidate before Tsb, its extents and tmax
+B2_DEV Tf bnb_node(const SearchGrid& g, const SearchBnb& sb, uint32_t level, uint64_t key, float ext[4])
+{
+    const uint32_t bi = (uint32_t)(key & 0xFFFFFFu), bj = (uint32_t)(key >> 24 & 0xFFFFFFu), k = (uint32_t)(key >> 48);
+    const uint32_t i0 = bi << level, j0 = bj << level;
+    const uint32_t i1 = (uint32_t)min((uint64_t)g.nx, ((uint64_t)bi + 1u) << level) - 1u, j1 = (uint32_t)min((uint64_t)g.ny, ((uint64_t)bj + 1u) << level) - 1u;
+    Tf T = search_pose_ijk(g, i0, j0, k);
+    T.t.z = sb.zhi;
+    ext[0] = search_coord(g.x0, i0, g.step); ext[1] = search_coord(g.x0, i1, g.step);
+    ext[2] = search_coord(g.y0, j0, g.step); ext[3] = search_coord(g.y0, j1, g.step);
+    return T;
+}
+B2_DEV double bnb_tmax(const SearchBnb& sb, const float ext[4])
+{
+    return fmax(fmax(fabs((double)ext[0]), fabs((double)ext[1])), fmax(fabs((double)ext[2]), fabs((double)ext[3]))) +
+           fmax(fabs((double)sb.zlo), fabs((double)sb.zhi)) + sb.base;
+}
+// candidate (i, j, k) with the surface rule (bvh nullable: no surface), probing its cell; false: off surface
+B2_DEV bool bnb_candidate(const BvhView* bvh, const SearchGrid& g, const b2_surface_config& cfg, float cos_max, float tfar, uint32_t i, uint32_t j, uint32_t k, Tf& T)
+{
+    T = search_pose_ijk(g, i, j, k);
+    if (!bvh) return true;
+    return search_place(search_cell_ij(*bvh, g, i, j, cfg, cos_max, tfar), cfg, T);
+}
+// score of candidate c among L's sorted candidates Lc (n of them), -1 when it is not there
+B2_DEV float bnb_find(const uint64_t* Lc, const float* Ls, uint64_t n, uint64_t c)
+{
+    uint64_t lo = 0, hi = n;
+    while (lo < hi) { const uint64_t mid = (lo + hi) / 2; if (ldg(Lc + mid) < c) lo = mid + 1; else hi = mid; }
+    return lo < n && ldg(Lc + lo) == c ? ldg(Ls + lo) : -1.0f;
+}
+
+#ifdef __CUDACC__
+__global__ void __launch_bounds__(256) k_pf_bnb_pyr_fine2(DfieldView f, uint64_t n, float* __restrict__ fine2)
+{
+    for (uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; t < n; t += (uint64_t)gridDim.x * blockDim.x) fine2[t] = pyr_fine2(f, (uint32_t)(t / 64u), (uint32_t)(t % 64u));
+}
+__global__ void __launch_bounds__(256) k_pf_bnb_pyr_fine4(const float* __restrict__ fine2, uint64_t n, float* __restrict__ fine4)
+{
+    for (uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; t < n; t += (uint64_t)gridDim.x * blockDim.x) fine4[t] = pyr_fine4(fine2, (uint32_t)(t / 8u), (uint32_t)(t % 8u));
+}
+__global__ void __launch_bounds__(256) k_pf_bnb_pyr_bricks(DfieldView f, const float* __restrict__ fine4, uint64_t n, float* __restrict__ dense)
+{
+    for (uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; t < n; t += (uint64_t)gridDim.x * blockDim.x) dense[t] = pyr_brick(f, fine4, t);
+}
+__global__ void __launch_bounds__(256) k_pf_bnb_pyr_up(const float* __restrict__ src, uint32_t sx, uint32_t sy, uint32_t sz, uint32_t dx, uint32_t dy, uint64_t n,
+                                                      float* __restrict__ dst)
+{
+    for (uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; t < n; t += (uint64_t)gridDim.x * blockDim.x) dst[t] = pyr_up(src, sx, sy, sz, dx, dy, t);
+}
+// k_pf_search_score's layout over the nodes of one level: per node its first candidate (times Tsb) and extents in shared memory, lanes over
+// the beams of one node, each beam's bound at its slot, one thread per node merging from {0, 0, 0} in slot order; a node whose bound is >= t
+// flags its children (those inside the grid) for the compaction
+__global__ void __launch_bounds__(B2_PF_BLOCK) k_pf_bnb_bound(DfieldView f, SearchPyr P, SearchGrid g, SearchBnb sb, uint32_t level, const uint64_t* __restrict__ nodes,
+                                                           uint32_t n, b2_transform Tsb_val, const PfBeam* __restrict__ beams, uint32_t n_beams, b2_pf_params prm,
+                                                           uint32_t ppb, float t, uint64_t* __restrict__ child, uint8_t* __restrict__ flag)
+{
+    extern __shared__ float s_eval[];            // [ppb][n_beams]
+    __shared__ Tf s_T[B2_PF_BLOCK];
+    __shared__ float s_ext[B2_PF_BLOCK][4];
+    const uint32_t c0 = blockIdx.x * ppb, nc = min(ppb, n - c0);
+    if (threadIdx.x < nc) s_T[threadIdx.x] = tf_mul(bnb_node(g, sb, level, nodes[c0 + threadIdx.x], s_ext[threadIdx.x]), tf_from_pod(Tsb_val));
+    __syncthreads();
+    float sigma_quad; double denom; pf_constants(prm, sigma_quad, denom);
+    const uint32_t total = nc * n_beams;
+    for (uint32_t w = threadIdx.x; w < total; w += blockDim.x) {
+        const uint32_t cl = w / n_beams, bi = w % n_beams;
+        const PfBeam b = beams[bi];
+        const float* e = s_ext[cl];
+        s_eval[cl * n_beams + b.slot] = bnb_beam_bound(f, P, sb, s_T[cl], (double)e[1] - (double)e[0], (double)e[3] - (double)e[2], bnb_tmax(sb, e), b,
+                                                       sigma_quad, denom);
+    }
+    __syncthreads();
+    if (threadIdx.x < nc) {
+        b2_gaussian1d lk; lk.mean = 0.0f; lk.sigma = 0.0f; lk.n_meas = 0u;
+        pf_merge(lk, s_eval + threadIdx.x * n_beams, n_beams);
+        const uint64_t key = nodes[c0 + threadIdx.x];
+        const uint32_t bi = (uint32_t)(key & 0xFFFFFFu), bj = (uint32_t)(key >> 24 & 0xFFFFFFu), k = (uint32_t)(key >> 48), cl = level - 1u;
+        for (uint32_t q = 0; q < 4; q++) {
+            const uint32_t ci = 2u * bi + (q & 1u), cj = 2u * bj + (q >> 1);
+            const size_t o = 4u * (size_t)(c0 + threadIdx.x) + q;
+            child[o] = bnb_key(ci, cj, k);
+            flag[o] = lk.mean >= t && ((uint64_t)ci << cl) < g.nx && ((uint64_t)cj << cl) < g.ny;
+        }
+    }
+}
+// the leaves: k_pf_search_score over a list of candidates, each probing its own cell with surface; flags the scores >= t
+__global__ void __launch_bounds__(B2_PF_BLOCK) k_pf_bnb_leaves(DfieldView f, BvhView bvh, SearchGrid g, b2_surface_config cfg, int surface, float cos_max, float tfar,
+                                                            const uint64_t* __restrict__ nodes, uint32_t n, b2_transform Tsb_val, const PfBeam* __restrict__ beams,
+                                                            uint32_t n_beams, b2_pf_params prm, uint32_t ppb, float t, uint64_t* __restrict__ cand,
+                                                            float* __restrict__ score, uint8_t* __restrict__ flag)
+{
+    extern __shared__ float s_eval[];            // [ppb][n_beams]
+    __shared__ Tf s_T[B2_PF_BLOCK];
+    __shared__ bool s_ok[B2_PF_BLOCK];
+    const uint32_t c0 = blockIdx.x * ppb, nc = min(ppb, n - c0);
+    if (threadIdx.x < nc) {
+        const uint64_t key = nodes[c0 + threadIdx.x];
+        const uint32_t i = (uint32_t)(key & 0xFFFFFFu), j = (uint32_t)(key >> 24 & 0xFFFFFFu), k = (uint32_t)(key >> 48);
+        Tf T;
+        s_ok[threadIdx.x] = bnb_candidate(surface ? &bvh : nullptr, g, cfg, cos_max, tfar, i, j, k, T);
+        s_T[threadIdx.x] = tf_mul(T, tf_from_pod(Tsb_val));
+        cand[c0 + threadIdx.x] = ((uint64_t)k * g.ny + j) * g.nx + i;
+    }
+    __syncthreads();
+    float sigma_quad; double denom; pf_constants(prm, sigma_quad, denom);
+    const uint32_t total = nc * n_beams;
+    for (uint32_t w = threadIdx.x; w < total; w += blockDim.x) {
+        const uint32_t cl = w / n_beams, bi = w % n_beams;
+        if (!s_ok[cl]) continue;
+        const PfBeam b = beams[bi];
+        s_eval[cl * n_beams + b.slot] = pf_eval_field(f, s_T[cl], b, sigma_quad, denom);
+    }
+    __syncthreads();
+    if (threadIdx.x < nc) {
+        float s = -1.0f;
+        if (s_ok[threadIdx.x]) {
+            b2_gaussian1d lk; lk.mean = 0.0f; lk.sigma = 0.0f; lk.n_meas = 0u;
+            pf_merge(lk, s_eval + threadIdx.x * n_beams, n_beams);
+            s = lk.mean;
+        }
+        score[c0 + threadIdx.x] = s;
+        flag[c0 + threadIdx.x] = s >= t;
+    }
+}
+// the peak rule over L (sorted by c): a neighbour missing from L scores < t <= the candidate's score, so it counts as behind it
+__global__ void __launch_bounds__(256) k_pf_bnb_peaks(const uint64_t* __restrict__ Lc, const float* __restrict__ Ls, uint64_t n, uint32_t nx, uint32_t ny, uint32_t K,
+                                                     uint8_t* __restrict__ flag, uint32_t* __restrict__ rank)
+{
+    for (uint64_t e = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; e < n; e += (uint64_t)gridDim.x * blockDim.x) {
+        const float sc = Ls[e];
+        flag[e] = search_peak_rule<uint64_t>(Lc[e], sc, nx, ny, K, [&](uint64_t c) { return bnb_find(Lc, Ls, n, c); });
+        rank[e] = search_rank(sc);
+    }
+}
+// the records of the kept peaks (candidates sel with scores sc), rank order.  Not k_pf_search_records: that kernel reads 32-bit c, the
+// cells' probes and the whole score array, none of which this search has; both build the record with search_record
+__global__ void k_pf_bnb_records(BvhView bvh, SearchGrid g, b2_surface_config cfg, int surface, float cos_max, float tfar, const uint64_t* __restrict__ sel,
+                                 const float* __restrict__ sc, uint32_t m, b2_search_record* __restrict__ out)
+{
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= m) return;
+    const uint64_t c = sel[r];
+    const uint32_t i = (uint32_t)(c % g.nx), j = (uint32_t)(c / g.nx % g.ny), k = (uint32_t)(c / g.nx / g.ny);
+    Tf T;
+    bnb_candidate(surface ? &bvh : nullptr, g, cfg, cos_max, tfar, i, j, k, T);
+    out[r] = search_record(T, sc[r], i, j, k);
 }
 #endif
 

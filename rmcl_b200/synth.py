@@ -385,6 +385,11 @@ assert CLUSTER_RESULT_DTYPE.itemsize == 64
 # b2_search_record: what PCDSensorUpdaterB200.globalSearch returns per kept peak
 SEARCH_RECORD_DTYPE = np.dtype([("pose", TRANSFORM_DTYPE), ("score", np.float32), ("i", np.uint32), ("j", np.uint32), ("k", np.uint32)])
 assert SEARCH_RECORD_DTYPE.itemsize == 48
+# b2_search_bnb_result: the counts of PCDSensorUpdaterB200.globalSearchBnB
+SEARCH_BNB_RESULT_DTYPE = np.dtype([("n_candidates", np.uint64), ("n_bounded", np.uint64), ("n_leaves", np.uint64), ("n_peaks", np.uint64), ("n_records", np.uint64),
+                                    ("n_bounded_pass", np.uint64, (16,)), ("n_level", np.uint64, (25,)), ("best_score", np.float32), ("threshold", np.float32),
+                                    ("n_passes", np.uint32), ("depth", np.uint32)])
+assert SEARCH_BNB_RESULT_DTYPE.itemsize == 384
 
 
 def quat_from_rpy(roll, pitch, yaw):
